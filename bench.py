@@ -38,7 +38,7 @@ ROW_BYTES = 64
 METRIC = "rows/s sorted (64B rows, u64 key)"
 ALGO_BYTES_PER_ROW_PASS = 24.0   # onesweep pass: read 8 B key + 4 B index, write the same
 ALGO_BYTES_PER_ROW_SORT = 332.0  # SURVEY §8(d): 8 + 8*24 + 4 + 2*64
-NVLINK_PEER_GBS = 770.0          # measured peer copy per direction per GPU on this pool (B200_PROFILING.md; 900 nominal)
+NVLINK_PEER_GBS = 450.0          # H100 SXM NVLink data sheet, per direction per GPU (not measured)
 MIN64 = -2**63
 
 
@@ -49,7 +49,7 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet HBM3 bandwidth (not measured)"
 
 
 class ClockSampler:
@@ -269,6 +269,47 @@ def verify_sort(out_flat, in_flat, row_bytes, key_cols, world=1, rank=0, dist=No
                     "checksum of whole rows, equal keys keep (source rank, position) order"}
 
 
+DUMP_SAMPLE_ROWS = 1 << 18   # 2^18 rows x 16 float64 halves = 32 MB; with positions and group samples at most 48 MB in all
+
+
+def _u32_halves(words):
+    """int64 tensor [..., k] -> float64 tensor [..., 2k] of its (low, high) 32-bit halves: exact in float64."""
+    import torch
+    lo = (words & 0xFFFFFFFF).to(torch.float64)
+    hi = ((words >> 32) & 0xFFFFFFFF).to(torch.float64)
+    return torch.stack([lo, hi], dim=-1).reshape(*words.shape[:-1], -1)
+
+
+def _sample_index(m, k, seed):
+    """Sorted positions of a fixed seeded sample of k of m rows (every row when m <= k)."""
+    if m <= k:
+        return np.arange(m, dtype=np.int64)
+    return np.sort(np.random.Generator(np.random.Philox(seed)).choice(m, k, replace=False)).astype(np.int64)
+
+
+def dump_outputs(out_dir, last, reduce_out, world, rank):
+    """Writes what the last timed step returned, as float64 .npy files: a fixed seeded sample of the sorted rows (each
+    64-bit word as its two 32-bit halves) with the sampled positions and, for the pipeline, a sample of the groups."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    suffix = f"_rank{rank}" if world > 1 else ""
+
+    def save(name, t):
+        np.save(os.path.join(out_dir, name + suffix + ".npy"), t.cpu().numpy().astype(np.float64, copy=False))
+
+    rows2d = last["out"].view(torch.int64).view(-1, ROW_BYTES // 8)
+    idx = _sample_index(rows2d.shape[0], DUMP_SAMPLE_ROWS, SEED + 7)
+    pos = torch.from_numpy(idx).to(rows2d.device)
+    save("sorted_rows_sample", _u32_halves(rows2d[pos]))
+    save("sorted_rows_sample_position", pos)
+    if "groups" in last:
+        g = int(last["groups"])
+        gpos = torch.from_numpy(_sample_index(g, DUMP_SAMPLE_ROWS, SEED + 8)).to(rows2d.device)
+        save("groups_sample_position", gpos)
+        for name in ("keys", "sums", "counts"):
+            save(f"groups_{name}_sample", _u32_halves(reduce_out[name][:g][gpos].unsqueeze(-1)))
+
+
 # ------------------------------------------------------------------------------------------------------------
 # GROUP BY (configs[3]) — secondary metric, with its own CPU baselines
 # ------------------------------------------------------------------------------------------------------------
@@ -475,7 +516,11 @@ def main():
                     help="N>1: ytgpu_shuffle_sort (default), the round-1 Python-driven peer scatter, or NCCL all_to_all_single")
     ap.add_argument("--groupby-rows", type=int, default=100_000_000)
     ap.add_argument("--dropin-rows", type=int, default=10_000_000, help="rows of the CreateSortingReader end-to-end leg (C++ adapter)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write a fixed sample of what the last timed step computed to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 0)
     if args.quick:
         args.no_variants = True
@@ -614,6 +659,8 @@ def main():
         parity["checks"]["reduce_keys_increasing"] = bool((gk[1:] > gk[:-1]).all()) if gk.numel() > 1 else True
         parity["ok"] = all(parity["checks"].values())
         del want_s, want_c, got_s, got_c
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, last, reduce_out, world, rank)
 
     # ---- key-distribution variants of the sort (SURVEY §8d C2) ----
     variants = None
@@ -673,43 +720,35 @@ def main():
         t, c = timers[name]
         return (t / c) if c else None
 
-    def kernel_roofline(name, bytes_per_row, avg_ms, launches_n, traffic_key, note, bound="hbm", rows_per_launch=n, peak_gbs=None):
+    def kernel_roofline(name, bytes_per_row, avg_ms, launches_n, note, bound="hbm", rows_per_launch=n, peak_gbs=None):
         pk = peak_gbs or peak
         ach = (bytes_per_row * rows_per_launch / (avg_ms / 1e3) / 1e9) if avg_ms else None
         return {"bound": bound, "kernel": name, "achieved": ach, "peak": pk, "unit": "GB/s", "frac": (ach / pk) if ach else None,
-                "peak_source": peak_src if bound == "hbm" else "measured peer copy per direction (B200_PROFILING.md)",
-                "traffic": traffic.get(traffic_key), "algorithmic_bytes_per_row": bytes_per_row, "avg_launch_ms": avg_ms,
+                "peak_source": peak_src if bound == "hbm" else "H100 SXM NVLink data sheet, per direction (not measured)",
+                "algorithmic_bytes_per_row": bytes_per_row, "avg_launch_ms": avg_ms,
                 "timed_launches": launches_n, "note": note}
 
-    traffic = {}
-    try:
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-    except Exception:
-        pass
     rows_local = parity["rows"] / world  # rows a rank sorts locally (== n up to the partition imbalance)
-    k_pass = kernel_roofline("onesweep_pass_kernel<256,16,3> (one 8-bit digit of (u64 key, u32 index) pairs)",
-                             ALGO_BYTES_PER_ROW_PASS, per_launch("radix_pass"), timers["radix_pass"][1], "onesweep_pass_kernel_bytes_per_launch",
-                             "traffic == algorithmic bytes; bound by issue slots (8-ballot ranking); 1.65x faster per pass than "
-                             "cub::DeviceRadixSort on the same GPU (profiles/r2_microbench.md)", rows_per_launch=rows_local)
+    k_pass = kernel_roofline("onesweep_pass_kernel<256,16,2> (one 8-bit digit of (u64 key, u32 index) pairs)",
+                             ALGO_BYTES_PER_ROW_PASS, per_launch("radix_pass"), timers["radix_pass"][1],
+                             "8-ballot ranking inside each warp", rows_per_launch=rows_local)
     k_gather = kernel_roofline("gather_rows_kernel (out[j] = rows[perm[j]], 64-byte rows)",
-                               132.0, per_launch("gather"), timers["gather"][1], "gather_rows_kernel_bytes_per_launch",
-                               "B200 DRAM reads 128 B per random 64 B access: real traffic 19.5 GB per launch = 70-77 % of the copy "
-                               "peak; grouping the reads by source chunk (random 64 B WRITES instead) measured slower "
-                               "(profiles/r2_microbench.md)", rows_per_launch=rows_local)
+                               132.0, per_launch("gather"), timers["gather"][1],
+                               "random 64 B row reads, sequential 64 B row writes", rows_per_launch=rows_local)
     kernels = {"radix_pass": k_pass, "row_gather": k_gather}
     if distributed and timers["scatter"][1]:
         off_rank = n * (world - 1) / world  # rows leaving the GPU per launch with balanced partitions
         kernels["peer_scatter"] = kernel_roofline(
             "scatter_stream_kernel (rows read sequentially, written to their slot in the destination GPU's receive buffer)",
-            float(ROW_BYTES), per_launch("scatter"), timers["scatter"][1], None,
-            "NVLink roofline: bytes that leave the GPU per launch / measured peer-copy bandwidth per direction; the HBM side "
+            float(ROW_BYTES), per_launch("scatter"), timers["scatter"][1],
+            "NVLink roofline: bytes that leave the GPU per launch / data-sheet NVLink bandwidth per direction; the HBM side "
             "(64 B read + 64 B/g local write per row) is far from its bound", bound="nvlink", rows_per_launch=off_rank, peak_gbs=NVLINK_PEER_GBS)
         kernels["partition_count"] = kernel_roofline(
             "partition_count_kernel (+3 scan launches): key -> partition index + per-tile counts, one pass over the rows",
-            68.0, per_launch("partition"), timers["partition"][1], None, "reads every 64 B row for its 8 B key")
+            68.0, per_launch("partition"), timers["partition"][1], "reads every 64 B row for its 8 B key")
     if args.workload == "pipeline" and timers["reduce"][1]:
         kernels["sorted_reduce"] = kernel_roofline("reduce_sorted_kernel (segmented SUM/COUNT over sorted rows, decoupled look-back)",
-                                                   64.0, per_launch("reduce"), timers["reduce"][1], None,
+                                                   64.0, per_launch("reduce"), timers["reduce"][1],
                                                    "one pass over the sorted rows; 24 B per group written", rows_per_launch=rows_local)
     dominant = max(kernels.values(), key=lambda k: (k["avg_launch_ms"] or 0) * (k["timed_launches"] or 0))
     roofline = dict(dominant)
@@ -755,7 +794,7 @@ def main():
         try:
             import subprocess
             if not os.path.exists(exe):
-                subprocess.check_call(["make", "-C", os.path.join(ROOT, "host")], stdout=subprocess.DEVNULL)
+                raise FileNotFoundError(f"{exe} is missing: build() makes it")
             r = subprocess.run([exe, str(args.dropin_rows)], capture_output=True, text=True, timeout=600)
             dropin = json.loads(r.stdout.strip().splitlines()[-1]) if r.returncode == 0 else {"error": (r.stderr or r.stdout)[-300:]}
         except Exception as ex:  # pragma: no cover
@@ -809,8 +848,8 @@ def bench_e2e(args, ctx, sorter, rows, key_cols, n, world, rank, local_rank, dev
     from ytsaurus_b200 import GpuContext
     nb = n * ROW_BYTES
     # N = 1: the job threads and their pinned buffers live on the GPU's own NUMA node for the length of this leg, as a job
-    # proxy pins its GPU slot (with the buffers on the other socket both copy directions share the socket link and two jobs
-    # in flight gain nothing: 239 vs 158 ms per step on the same kind of box).  N > 1: the ranks were bound at start-up.
+    # proxy pins its GPU slot (with the buffers on the other socket both copy directions share the socket link).  N > 1: the
+    # ranks were bound at start-up.
     numa_binding, saved_affinity = None, None
     if not distributed and not os.environ.get("YTGPU_BENCH_NO_NUMA"):
         saved_affinity = os.sched_getaffinity(0)
@@ -894,8 +933,7 @@ def _bench_e2e_bound(args, ctx, sorter, rows, key_cols, n, world, rank, local_ra
     if args.e2e_jobs > 1:
         # The same call from several sort jobs at once (one context + private stream + host thread each, as a node runs
         # several job slots): one job's sorted rows leave while the next job's input arrives.  Measured for 2..e2e_jobs jobs in
-        # flight; the best one is the headline.  (On the pool's B200 boxes the PCIe link moves ~54 GB/s one way and ~79 GB/s
-        # with both directions busy, so two jobs already sit at the link's duplex limit: 12.8 GB / 79 GB/s = 162 ms per step.)
+        # flight; the best one is the headline.
         ctxs = [GpuContext(local_rank, use_torch_stream=False) for _ in range(args.e2e_jobs)]
         outs = [hout_np] + [torch.empty(nb, dtype=torch.uint8).pin_memory().numpy() for _ in range(args.e2e_jobs - 1)]
         for j in range(args.e2e_jobs):  # warm-up: staging buffers and scratch of every context

@@ -1,4 +1,4 @@
-/* ytgpu.h — C ABI of the B200-native sort/shuffle + scan→filter→group-by hot path.
+/* ytgpu.h — C ABI of the H100-native sort/shuffle + scan→filter→group-by hot path.
  *
  * This is the drop-in boundary a YTsaurus job proxy / CHYT instance binds to
  * (INTEGRATION.md shows the C++ adapters).  Plain pointers and sizes only; no

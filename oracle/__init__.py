@@ -14,7 +14,6 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.path.join(_HERE, "libytoracle.so")
-_REF_PATH = os.path.join(_HERE, "_ref", "libfarmhash_ref.so")
 
 VALUE_DTYPE = np.dtype(
     [("id", "<u2"), ("type", "u1"), ("flags", "u1"), ("length", "<u4"), ("data", "<u8")]
@@ -28,17 +27,14 @@ T_STRING, T_ANY, T_COMPOSITE, T_MAX = 0x10, 0x11, 0x12, 0xEF
 
 
 def build(force: bool = False) -> None:
-    """Compile the oracle (and oracle/_ref when /root/reference is present)."""
+    """Compile the oracle."""
     if force or not os.path.exists(_LIB_PATH) or (
         os.path.getmtime(_LIB_PATH) < os.path.getmtime(os.path.join(_HERE, "yt_oracle.cpp"))
     ):
         subprocess.check_call(["make", "-C", _HERE, "libytoracle.so"])
-    if os.path.isdir("/root/reference") and (force or not os.path.exists(_REF_PATH)):
-        subprocess.check_call(["make", "-C", _HERE, "ref"])
 
 
 _lib = None
-_ref = None
 
 
 def lib() -> C.CDLL:
@@ -60,22 +56,6 @@ def lib() -> C.CDLL:
         _lib.yto_count_ones.restype = C.c_int64
         _lib.yto_bit_pack.restype = C.c_size_t
     return _lib
-
-
-def ref_lib():
-    """The reference's own FarmHash (oracle/_ref), or None when it was never built."""
-    global _ref
-    if _ref is None and os.path.exists(_REF_PATH):
-        _ref = C.CDLL(_REF_PATH)
-        _ref.ref_fingerprint64.restype = C.c_uint64
-        _ref.ref_fingerprint64.argtypes = [C.c_char_p, C.c_size_t]
-        _ref.ref_fingerprint_u64.restype = C.c_uint64
-        _ref.ref_fingerprint_u64.argtypes = [C.c_uint64]
-        _ref.ref_fingerprint_u128.restype = C.c_uint64
-        _ref.ref_fingerprint_u128.argtypes = [C.c_uint64, C.c_uint64]
-        _ref.ref_hash128to64.restype = C.c_uint64
-        _ref.ref_hash128to64.argtypes = [C.c_uint64, C.c_uint64]
-    return _ref
 
 
 class OracleError(RuntimeError):

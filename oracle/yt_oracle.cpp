@@ -8,10 +8,10 @@
 //
 // Parity pinning: the fingerprint / partitioner / compare / columnar functions
 // are checked against the golden vectors transcribed from the reference's own
-// unit tests (tests/golden/*.json) and against the reference's vendored FarmHash
-// compiled as-is into oracle/_ref (see oracle/Makefile).
+// unit tests (tests/golden/*.json), the FarmHash functions also against known
+// answers of the reference's vendored FarmHash (tests/golden/farmhash_fingerprints.json).
 //
-// All paths relative to /root/reference.
+// All paths relative to the reference tree's root.
 
 #include <algorithm>
 #include <atomic>
@@ -69,7 +69,7 @@ enum { ERR_OK = 0, ERR_UNSUPPORTED_TYPE = 1, ERR_BAD_ARGUMENT = 2, ERR_PARTITION
 // farmhash.h:158-181 (Fingerprint(u64), Fingerprint(u128)), farmhash.cc:408-578
 // (farmhashna::Hash64 == util::Fingerprint64, farmhash.cc:1957-1959).
 // Restated from the published algorithm; validated bit-for-bit against the
-// vendored source compiled into oracle/_ref/libfarmhash_ref.so.
+// vendored source (known answers in tests/golden/farmhash_fingerprints.json).
 // ---------------------------------------------------------------------------
 constexpr u64 K0 = 0xc3a5c85c97cb3127ULL;
 constexpr u64 K1 = 0xb492b66fbe98f273ULL;

@@ -1,5 +1,5 @@
-"""Pins the CPU oracle against the reference's own known-answer vectors (tests/golden) and against the
-reference's vendored FarmHash compiled as-is (oracle/_ref).  CPU only."""
+"""Pins the CPU oracle against the reference's own known-answer vectors (tests/golden), including known answers of
+the reference's vendored FarmHash.  CPU only."""
 import os
 import struct
 
@@ -39,20 +39,20 @@ def test_null_and_false_collide():
     assert fps[0] == fps[1] == 0
 
 
-@pytest.mark.skipif(oracle.ref_lib() is None, reason="oracle/_ref not built (no /root/reference)")
 def test_farmhash_restatement_matches_reference_build():
-    ref = oracle.ref_lib()
-    rng = np.random.default_rng(7)
-    for x in [0, 1, 42, 2**63, 2**64 - 1] + [int(v) for v in rng.integers(0, 2**63, 200)]:
-        assert oracle.farm_fingerprint_u64(x) == ref.ref_fingerprint_u64(x)
-    for _ in range(200):
-        lo, hi = (int(v) for v in rng.integers(0, 2**63, 2))
-        assert oracle.farm_fingerprint_u128(lo, hi) == ref.ref_fingerprint_u128(lo, hi)
-        assert oracle.lib().yto_hash128to64(lo, hi) == ref.ref_hash128to64(lo, hi)
-    # every length class of farmhashna::Hash64: 0, 1-3, 4-7, 8-16, 17-32, 33-64, >64 (incl. multiples of 64)
-    for n in list(range(0, 200)) + [255, 256, 257, 511, 512, 513, 1000, 4096, 65537]:
-        b = rng.integers(0, 256, n, dtype=np.uint8).tobytes()
-        assert oracle.farm_fingerprint_bytes(b) == ref.ref_fingerprint64(b, n), n
+    """The oracle's FarmHash against known answers of the reference's farmhash.cc (tests/golden)."""
+    from test_farmhash_vs_reference_build import det_bytes, golden, pattern_bytes
+    g = golden()
+    for x, want in g["fingerprint_u64"]:
+        assert oracle.farm_fingerprint_u64(int(x)) == int(want), x
+    for lo, hi, want in g["fingerprint_u128"]:
+        assert oracle.farm_fingerprint_u128(int(lo), int(hi)) == int(want), (lo, hi)
+    for lo, hi, want in g["hash128to64"]:
+        assert oracle.lib().yto_hash128to64(int(lo), int(hi)) == int(want), (lo, hi)
+    for n, want in g["fingerprint64_random_bytes"].items():
+        assert oracle.farm_fingerprint_bytes(det_bytes(int(n))) == int(want), n
+    for n, want in g["fingerprint64_pattern_bytes"].items():
+        assert oracle.farm_fingerprint_bytes(pattern_bytes(int(n))) == int(want), n
 
 
 def test_ordered_partitioner_golden(golden):

@@ -1,6 +1,6 @@
-"""ytsaurus_b200 — B200-native sort/shuffle + scan→filter→hash-aggregate hot path of YTsaurus.
+"""ytsaurus_b200 — H100-native sort/shuffle + scan→filter→hash-aggregate hot path of YTsaurus.
 
-The compute lives in hand-written CUDA (csrc/, sm_100a) behind the C ABI of include/ytgpu.h
+The compute lives in hand-written CUDA (csrc/, sm_90a) behind the C ABI of include/ytgpu.h
 (libytgpu.so).  This package is the thin host side: ctypes binding (capi), the flat row model
 (rowset), PyTorch-backed buffers/streams (runtime) and the in-box multi-GPU shuffle (shuffle).
 """

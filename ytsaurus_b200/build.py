@@ -1,4 +1,4 @@
-"""Builds libytgpu.so (hand-written CUDA for sm_100a + the C ABI) in-tree with nvcc."""
+"""Builds libytgpu.so (hand-written CUDA for sm_90a + the C ABI) in-tree with nvcc."""
 from __future__ import annotations
 
 import glob
@@ -13,7 +13,7 @@ OBJ = os.path.join(HERE, "_obj")
 LIB = os.path.join(HERE, "libytgpu.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-O2", "--expt-relaxed-constexpr", "-Xptxas", "-v",
 ]
 

@@ -1,4 +1,4 @@
-// common.cuh — shared device/host helpers for the ytgpu kernels (sm_100a).
+// common.cuh — shared device/host helpers for the ytgpu kernels (sm_90a).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -15,7 +15,7 @@ using u64 = uint64_t;
 using i32 = int32_t;
 using i64 = int64_t;
 
-constexpr int kNumSms = 148;  // B200: 2 dies x 74 SMs
+constexpr int kNumSms = 132;  // H100 SXM
 
 // Kernel classes for the per-context CUDA-event timers (ytgpu_context_kernel_ms).
 enum KernelClass { KC_RADIX_PASS = 0, KC_GATHER = 1, KC_EXTRACT = 2, KC_HISTOGRAM = 3, KC_PARTITION = 4,

@@ -392,8 +392,8 @@ __device__ __forceinline__ void onesweep_tile(const PassParams& P, const PassDes
 
     // ---- rank inside the warp: stable (item-major, then lane) ----
     // Peers with the same digit are found with 8 ballots (one per digit bit).  MATCH.ANY is NOT used:
-    // on B200 it costs ~2 SM-cycles per distinct value in the warp (~59 cycles for random 8-bit
-    // digits, scratch/match_bench.cu), the 8 ballots cost ~25.  The running per-digit counts of the
+    // its cost grows with the number of distinct values in the warp, and random 8-bit digits have
+    // many; the ballots cost the same on any data.  The running per-digit counts of the
     // warp live in its private shared histogram: every lane reads its bin (same-digit lanes broadcast),
     // the lowest lane of each digit group writes the bumped count back.
     u32 rank[ITEMS];
@@ -566,7 +566,9 @@ constexpr size_t pass_smem_bytes(int items) {
 }
 
 // Tuning variants of the pass kernel (items per thread, min resident CTAs per SM); YTGPU_SORT_VARIANT
-// selects one for experiments, the default is the best measured on B200 (profiles/).
+// selects one for experiments.  The default is the fastest measured on an H100 SXM (700 W power limit: 15.3 vs 18.0 ms per
+// 10^8-row sort for 16 items at 3 CTAs per SM): 2 CTAs per SM keep 128 registers without spills, where 3 CTAs per SM
+// (80 registers) spill to local memory.
 struct PassVariant {
     int items;
     int ctas_per_sm;
@@ -580,7 +582,7 @@ const PassVariant kVariants[] = {
     {12, 4, onesweep_pass_kernel<kSortThreads, 12, 4>},
     {20, 2, onesweep_pass_kernel<kSortThreads, 20, 2>},
 };
-constexpr int kDefaultVariant = 1;
+constexpr int kDefaultVariant = 0;
 
 const PassVariant& pass_variant(Context* ctx) {
     static const int v = [] {

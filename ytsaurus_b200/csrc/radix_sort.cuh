@@ -1,4 +1,4 @@
-// radix_sort.cuh — stable LSD radix sort of (multi-chunk u64 key, u32 row index) on one B200.
+// radix_sort.cuh — stable LSD radix sort of (multi-chunk u64 key, u32 row index) on one GPU.
 //
 // Single-pass-per-digit ("onesweep") design: one upfront histogram of every 8-bit digit of every key
 // chunk, then per digit ONE kernel that reads each (key, index) pair once and writes it once, using

@@ -3,7 +3,7 @@
 The reference materialises its shuffle through intermediate chunks: Partition jobs tag blocks with a
 partition index (yt/yt/ytlib/table_client/schemaless_chunk_writer.cpp:1604-1667), Sort jobs fetch the
 blocks of their partition over RPC (partition_chunk_reader.cpp:82-86), pivots come from sampled keys
-(yt/yt/server/controller_agent/helpers.cpp:263-425).  Inside one 8xB200 box the same structure is one
+(yt/yt/server/controller_agent/helpers.cpp:263-425).  Inside one 8-GPU box the same structure is one
 collective: every rank range-partitions its rows with the ordered partitioner (bit-identical partition
 indices), the per-destination slabs travel in one NCCL all_to_all_single, and each rank sorts what it
 received.  Rank r ends up with key range r, so the concatenation over ranks is globally sorted.
