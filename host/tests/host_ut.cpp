@@ -165,6 +165,33 @@ static void TestSortingReader() {
     EXPECT_TRUE(empty->Read() == nullptr);
 }
 
+// 1 KB string keys: the normalised key would exceed 256 bytes, the rowset sort refines by key words instead
+static void TestSortingReaderLongKeys() {
+    std::mt19937 rng(11);
+    const std::string prefix(1000, 'p');
+    std::vector<TUnversionedOwningRow> input;
+    for (int i = 0; i < 5000; ++i) {
+        std::string key = prefix.substr(0, 900 + rng() % 100);
+        for (int k = rng() % 40; k > 0; --k) key.push_back("ab\0"[rng() % 3]);
+        TUnversionedOwningRowBuilder b;
+        b.AddValue(MakeUnversionedStringValue(key));
+        b.AddValue(MakeUnversionedInt64Value(i));
+        input.push_back(b.FinishRow());
+    }
+    for (auto order : {ESortOrder::Ascending, ESortOrder::Descending}) {
+        std::vector<size_t> expect(input.size());
+        for (size_t i = 0; i < expect.size(); ++i) expect[i] = i;
+        std::stable_sort(expect.begin(), expect.end(), [&](size_t a, size_t b) {
+            int r = CompareValues(input[a][0], input[b][0]);
+            return (order == ESortOrder::Descending ? -r : r) < 0;
+        });
+        auto rows = ReadAll(CreateSortingReader(CreateInMemoryReader(input), TComparator({order})), 1000);
+        bool same = rows.size() == input.size();
+        for (size_t i = 0; same && i < rows.size(); ++i) same = rows[i][1].Data.Int64 == (int64_t)expect[i];
+        EXPECT_TRUE(same);
+    }
+}
+
 static void TestSortedMergingReader() {
     TComparator comparator({ESortOrder::Ascending, ESortOrder::Ascending});
     std::vector<ISchemalessMultiChunkReaderPtr> readers;
@@ -375,6 +402,7 @@ int main() {
         TestHash();
         TestColumnBased();
         TestSortingReader();
+        TestSortingReaderLongKeys();
         TestSortedMergingReader();
         TestSortedJoiningReader();
         TestPartitionMultiChunkWriter();

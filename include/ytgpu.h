@@ -81,7 +81,13 @@ void ytgpu_context_enable_timers(ytgpu_context* ctx, int enabled);
 int ytgpu_context_set_option(ytgpu_context* ctx, const char* name, int64_t value, ytgpu_error* err);
 /* Reads an option back, or one of the read-only counters:
  *   "last_merge_used_merge_path"  1 when the most recent ytgpu_merge_sorted_runs took the merge-path rounds, 0 when it
- *                                 sorted (many runs, an unsorted run, or the option switched off). */
+ *                                 sorted (many runs, an unsorted run, a key of more than 256 normalised bytes, or the
+ *                                 option switched off).
+ *   "last_sort_refine_rounds"     refinement rounds the most recent ytgpu_sort_rowset / ytgpu_merge_sorted_runs /
+ *                                 ytgpu_join_sorted_runs ran: >= 1 when its key did not fit the 256-byte normalised form
+ *                                 and took the width-free key words (the first round counts even when every key is
+ *                                 equal), 0 when it took the normalised-key path.
+ *   "last_sort_refine_rows.<r>"   rows that round r (from 0) of that call sorted (0 past its last round). */
 int ytgpu_context_get_option(ytgpu_context* ctx, const char* name, int64_t* value, ytgpu_error* err);
 
 /* Completion notification without blocking a thread: `fn(user)` runs on a driver thread once everything enqueued on the
@@ -161,7 +167,11 @@ typedef struct ytgpu_sort_spec {
  * factory sorting_reader.h:15-20) and TPartitionSortReader's bucket sort + merge
  * (partition_sort_reader.cpp:384-529).  The sort is STABLE (rows with equal keys keep input order),
  * which is one of the orders the reference's unstable std::sort may produce.
- * out_perm[i] = input index of the i-th output row. */
+ * out_perm[i] = input index of the i-th output row.
+ * Keys of any length: a key whose normalised form (strings padded to the longest one, or to the declared `width`) fits
+ * in 256 bytes is radix-sorted as such; a longer one is sorted by refinement rounds over width-free key words (see
+ * "last_sort_refine_rounds").  A string longer than a declared `width` is YTGPU_ERR_SCHEMA_VIOLATION on both paths;
+ * Any/Composite key values are YTGPU_ERR_UNSUPPORTED. */
 int ytgpu_sort_rowset(ytgpu_context* ctx, const ytgpu_rowset_view* in, const ytgpu_sort_spec* spec,
                       uint32_t* out_perm, ytgpu_value* out_values /* nullable: rows gathered in sorted order */,
                       int out_mem, ytgpu_error* err);
@@ -172,7 +182,8 @@ int ytgpu_sort_fixed_rows(ytgpu_context* ctx, const ytgpu_fixed_rows_view* in, c
 
 /* Replaces CreateSortedMergingReader (sorted_merging_reader.cpp:771-788; order = CompareStreams :395-409):
  * `in` is the concatenation of run_count sorted runs, run r = rows [run_offsets[r], run_offsets[r+1]).
- * Ties are broken by run index, then by position in the run. */
+ * Ties are broken by run index, then by position in the run.  Keys of any length, as ytgpu_sort_rowset; a key that does
+ * not fit the 256-byte normalised form always takes the stable sort of the concatenated runs. */
 int ytgpu_merge_sorted_runs(ytgpu_context* ctx, const ytgpu_rowset_view* in, const ytgpu_sort_spec* spec,
                             const uint64_t* run_offsets /* host */, uint32_t run_count, uint32_t* out_perm,
                             int out_mem, ytgpu_error* err);
@@ -184,7 +195,8 @@ int ytgpu_merge_sorted_runs(ytgpu_context* ctx, const ytgpu_rowset_view* in, con
  * :395-409; one index per stream, taken from its first row :101-104), so the adapters append that index as the last
  * key column.  The result is the stable order by all spec columns in which a foreign row survives iff its join key
  * occurs in the primary stream (:722-738: it equals the last primary key consumed or the next one).
- * out_perm (capacity row_count) receives the input indices of the emitted rows, *out_row_count (host) their number. */
+ * out_perm (capacity row_count) receives the input indices of the emitted rows, *out_row_count (host) their number.
+ * Keys of any length, as ytgpu_sort_rowset. */
 int ytgpu_join_sorted_runs(ytgpu_context* ctx, const ytgpu_rowset_view* in, const ytgpu_sort_spec* spec,
                            uint32_t join_key_column_count, const uint64_t* run_offsets /* host */, uint32_t run_count,
                            uint32_t* out_perm, uint64_t* out_row_count, int out_mem, ytgpu_error* err);

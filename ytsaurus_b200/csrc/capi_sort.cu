@@ -3,6 +3,7 @@
 
 #include "context.cuh"
 #include "keys.cuh"
+#include "long_keys.cuh"
 #include "merge.cuh"
 #include "radix_sort.cuh"
 #include "rows.cuh"
@@ -50,26 +51,40 @@ Status resolve_widths(Context* ctx, const ytgpu_sort_spec* spec, const ytgpu_val
 }
 
 // Stages a rowset on the device (HOST flavour), normalises its keys and sorts them: the pieces every rowset entry
-// point shares.  The buffers live as long as the object (the permutation refers to the scratch).
+// point shares.  The buffers live as long as the object (the permutation refers to the scratch).  Keys whose
+// fixed-width normalised form does not fit in kMaxKeyChunks chunks take the refinement sort of long_keys.cu instead.
 struct RowsetSort {
     DevBuf<ytgpu_value> vals_stage;
     DevBuf<u8> heap_stage;
     const ytgpu_value* vals = nullptr;
     const u8* heap = nullptr;
+    u32 vc = 0;
     KeyLayout L;
+    bool long_keys = false;
     ChunkSet chunks;
     SortScratch scratch;
+    DevBuf<u32> long_perm;
+    DevBuf<SortPlan> long_plan;  // all zero: the permutation is idx[0]
     PermRef perm;
 
     Status run(Context* ctx, const ytgpu_rowset_view* in, const ytgpu_sort_spec* spec) {
         YTGPU_TRY(prepare(ctx, in, spec));
         return sort(ctx, in->row_count);
     }
-    Status sort(Context* ctx, u64 n) { return radix_sort_keys(ctx, chunks.cptrs, (int)L.nchunks, n, &scratch, &perm); }
+    Status sort(Context* ctx, u64 n) {
+        if (!long_keys) return radix_sort_keys(ctx, chunks.cptrs, (int)L.nchunks, n, &scratch, &perm);
+        YTGPU_TRY(long_perm.allocate(ctx, n));
+        YTGPU_TRY(long_plan.allocate(ctx, 1));
+        YTGPU_CUDA_TRY(cudaMemsetAsync(long_plan.p, 0, sizeof(SortPlan), ctx->stream));
+        YTGPU_TRY(long_key_sort(ctx, L, vals, vc, heap, n, long_perm.p));
+        perm.plan = long_plan.p;
+        perm.idx[0] = perm.idx[1] = long_perm.p;
+        return Status{};
+    }
     // Staging + key normalisation only (the merge of sorted runs needs no sort).
     Status prepare(Context* ctx, const ytgpu_rowset_view* in, const ytgpu_sort_spec* spec) {
         const u64 n = in->row_count;
-        const u32 vc = in->value_count;
+        vc = in->value_count;
         vals = in->values;
         heap = in->string_heap;
         if (in->mem == YTGPU_MEM_HOST) {
@@ -83,7 +98,13 @@ struct RowsetSort {
         std::vector<ytgpu_key_column> cols;
         YTGPU_TRY(resolve_widths(ctx, spec, vals, vc, n, &cols));
         ytgpu_sort_spec rs{cols.data(), (u32)cols.size()};
-        YTGPU_TRY(build_key_layout(&rs, /*fixed_rows*/ false, /*force_type_byte*/ false, &L));
+        const Status s = build_key_layout(&rs, /*fixed_rows*/ false, /*force_type_byte*/ false, &L);
+        long_keys = s.code == YTGPU_ERR_UNSUPPORTED && L.nchunks > (u32)kMaxKeyChunks;
+        if (long_keys) {
+            YTGPU_TRY(check_long_keys(ctx, L, vals, vc, n));
+            return check_device_errors(ctx);
+        }
+        YTGPU_TRY(s);
         YTGPU_TRY(chunks.allocate(ctx, L.nchunks, n));
         YTGPU_TRY(normalize_rowset(ctx, L, vals, vc, heap, n, chunks.ptrs));
         YTGPU_TRY(check_device_errors(ctx));
@@ -96,6 +117,7 @@ Status sort_rowset_impl(Context* ctx, const ytgpu_rowset_view* in, const ytgpu_s
     if (!in || !spec || !spec->columns) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null argument");
     if (spec->column_count == 0 || spec->column_count > (u32)kMaxKeyColumns)
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "key column count must be in [1, %d]", kMaxKeyColumns);
+    ctx->last_sort_refine_rounds = 0;
     const u64 n = in->row_count;
     if (n == 0) return Status{};
     const u32 vc = in->value_count;
@@ -155,6 +177,19 @@ __global__ void join_heads_kernel(JoinPrefix P, const SortPlan* plan, const u32*
     head[j] = h;
 }
 
+// The same for keys that took the refinement sort: L holds the join key columns only.
+__global__ void join_heads_long_kernel(const KeyLayout L, const ytgpu_value* vals, u32 vc, const u8* heap, const SortPlan* plan,
+                                       const u32* pa, const u32* pb, u64 n, u64* head) {
+    const u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n) return;
+    u64 h = 1;
+    if (j > 0) {
+        const u32 r = perm_at(plan, pa, pb, j), q = perm_at(plan, pa, pb, j - 1);
+        h = key_first_diff(L, vals + (u64)r * vc, vals + (u64)q * vc, heap, 0) == kKeyEnd ? 0 : 1;
+    }
+    head[j] = h;
+}
+
 // gid (exclusive scan of head, so group of j = gid[j+1]-1 == gid[j] + head - 1): a primary row marks its group.
 __global__ void join_mark_kernel(const SortPlan* plan, const u32* pa, const u32* pb, u64 n, u64 primary_rows,
                                  const u64* scanned, const u64* total, u8* has_primary) {
@@ -186,14 +221,15 @@ Status join_sorted_impl(Context* ctx, const ytgpu_rowset_view* in, const ytgpu_s
                         u64 primary_rows, u32* out_perm, u64* out_count, int out_mem) {
     const u64 n = in->row_count;
     *out_count = 0;
+    ctx->last_sort_refine_rounds = 0;
     if (n == 0) return Status{};
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
     RowsetSort rs;
     YTGPU_TRY(rs.run(ctx, in, spec));
 
     JoinPrefix P{};
-    const u32 prefix_bytes = join_cols >= rs.L.ncols ? rs.L.total_bytes : rs.L.col[join_cols].byte_offset;
-    for (u32 c = 0; c < rs.L.nchunks; ++c) P.chunk[c] = rs.chunks.cptrs[c];
+    const u32 prefix_bytes = rs.long_keys ? 0 : (join_cols >= rs.L.ncols ? rs.L.total_bytes : rs.L.col[join_cols].byte_offset);
+    for (u32 c = 0; !rs.long_keys && c < rs.L.nchunks; ++c) P.chunk[c] = rs.chunks.cptrs[c];
     P.full_chunks = prefix_bytes / 8;
     const u32 rem = prefix_bytes % 8;
     P.tail_mask = rem ? ~0ull << (8 * (8 - rem)) : 0;
@@ -217,7 +253,13 @@ Status join_sorted_impl(Context* ctx, const ytgpu_rowset_view* in, const ytgpu_s
     }
     {
         KernelTimer t(ctx, KC_HISTOGRAM, 10);
-        join_heads_kernel<<<blocks, threads, 0, ctx->stream>>>(P, plan, pa, pb, n, head.p);
+        if (rs.long_keys) {
+            KeyLayout JL = rs.L;
+            JL.ncols = join_cols;
+            join_heads_long_kernel<<<blocks, threads, 0, ctx->stream>>>(JL, rs.vals, rs.vc, rs.heap, plan, pa, pb, n, head.p);
+        } else {
+            join_heads_kernel<<<blocks, threads, 0, ctx->stream>>>(P, plan, pa, pb, n, head.p);
+        }
         exclusive_scan_u64(ctx->stream, head.p, n, sums.p, totals.p);
         join_mark_kernel<<<blocks, threads, 0, ctx->stream>>>(plan, pa, pb, n, primary_rows, head.p, totals.p, has_primary.p);
         join_keep_kernel<<<blocks, threads, 0, ctx->stream>>>(plan, pa, pb, n, primary_rows, head.p, totals.p, has_primary.p, keep.p);
@@ -317,6 +359,7 @@ Status merge_sorted_runs_impl(Context* ctx, const ytgpu_rowset_view* in, const y
     if (!spec || !spec->columns || !out_perm) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null argument");
     if (spec->column_count == 0 || spec->column_count > (u32)kMaxKeyColumns)
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "key column count must be in [1, %d]", kMaxKeyColumns);
+    ctx->last_sort_refine_rounds = 0;
     const u64 n = in->row_count;
     if (n == 0) return Status{};
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
@@ -329,7 +372,7 @@ Status merge_sorted_runs_impl(Context* ctx, const ytgpu_rowset_view* in, const y
         dst = tmp.p;
     }
     bool merged = false;
-    if (ctx->opt_merge_path != 0)
+    if (ctx->opt_merge_path != 0 && !rs.long_keys)  // merge path compares normalised key chunks
         YTGPU_TRY(merge_sorted_key_runs(ctx, rs.chunks.cptrs, (int)rs.L.nchunks, n, run_offsets, run_count, dst, &merged));
     ctx->last_merge_used_merge_path = merged;
     if (!merged) {

@@ -202,7 +202,11 @@ int ytgpu_context_get_option(ytgpu_context* h, const char* name, int64_t* value,
     if (strcmp(name, "sort_hybrid") == 0) *value = c->opt_sort_hybrid;
     else if (strcmp(name, "merge_path") == 0) *value = c->opt_merge_path;
     else if (strcmp(name, "last_merge_used_merge_path") == 0) *value = c->last_merge_used_merge_path ? 1 : 0;
-    else return fill_error(err, make_status(YTGPU_ERR_INVALID_ARGUMENT, "unknown option '%s'", name));
+    else if (strcmp(name, "last_sort_refine_rounds") == 0) *value = c->last_sort_refine_rounds;
+    else if (strncmp(name, "last_sort_refine_rows.", 22) == 0) {
+        const size_t r = (size_t)strtoull(name + 22, nullptr, 10);
+        *value = r < c->last_sort_refine_rows.size() ? (int64_t)c->last_sort_refine_rows[r] : 0;
+    } else return fill_error(err, make_status(YTGPU_ERR_INVALID_ARGUMENT, "unknown option '%s'", name));
     return fill_error(err, Status{});
 }
 

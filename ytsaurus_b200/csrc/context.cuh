@@ -33,6 +33,8 @@ struct Context {
     u32 func_attrs_done = 0;
     int opt_merge_path = 1;    // ytgpu_merge_sorted_runs: 1 = merge-path rounds when the runs are few, 0 = always the stable sort
     bool last_merge_used_merge_path = false;
+    u32 last_sort_refine_rounds = 0;         // refinement rounds of the last rowset sort / merge / join (0: normalised keys)
+    std::vector<u64> last_sort_refine_rows;  // rows each of those rounds sorted
     int opt_sort_hybrid = -1;  // -1: environment default (YTGPU_SORT_HYBRID, on); 0/1: set through ytgpu_context_set_option
 
     Status alloc(void** p, size_t bytes) {

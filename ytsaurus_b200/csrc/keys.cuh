@@ -52,6 +52,7 @@ inline Status build_key_layout(const ytgpu_sort_spec* spec, bool fixed_rows, boo
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "key column count must be in [1, %d]", kMaxKeyColumns);
     L->ncols = spec->column_count;
     L->fixed_rows = fixed_rows;
+    L->nchunks = 0;  // > kMaxKeyChunks on return: every column was laid out, only the total width does not fit
     u32 off = 0;
     for (u32 c = 0; c < L->ncols; ++c) {
         const ytgpu_key_column& k = spec->columns[c];
@@ -186,6 +187,137 @@ __host__ __device__ inline u32 normalize_value(const KeyColLayout& c, const ytgp
     }
     w.zeros(c.payload_bytes - used);
     return err;
+}
+
+// ---- width-free key words (rowset keys whose fixed-width form exceeds kMaxKeyChunks chunks; long_keys.cu) ----
+// Column c of a row is the byte string E_c = [type byte] payload, the type byte under the same rule as above:
+//   Int64 / Uint64 / Double / Boolean payloads as above (8, 8, 8 and 1 bytes); Null and the sentinels: none;
+//   String of length L: L/7 + 1 blocks of 8 bytes, each 7 raw bytes (the last one zero-padded) and a tag byte = the
+//   number of raw bytes in the block, or 8 when the block is full and the string continues.  So "ab" < "ab\0" and
+//   "abcdefg" < "abcdefg\0" without padding to a width.
+// A descending column inverts every byte of E_c.  E_c is cut into big-endian u64 words from the column's own start;
+// the tail of the last word is zero padding, never inverted.  Every E_c is order-preserving and prefix-free (rows
+// whose words agree up to the end of one row's E_c end it at the same word), so comparing two rows word by word,
+// column after column, gives TComparator order.
+// A position in the word sequence of a row is a cursor (c << 32) | w; kKeyEnd = past the last column.
+constexpr u64 kKeyEnd = ~0ull;
+
+__host__ __device__ inline u64 key_cursor(u32 c, u32 w) { return ((u64)c << 32) | w; }
+
+// Type/schema errors of one key value (the checks normalize_value makes, with the string limit from the layout).
+__host__ __device__ inline u32 key_value_errors(const KeyColLayout& c, const ytgpu_value& v) {
+    u32 err = 0;
+    if (v.type == YTGPU_TYPE_ANY || v.type == YTGPU_TYPE_COMPOSITE) err |= DE_UNSUPPORTED_TYPE;
+    if (c.type != 0 && v.type != c.type && !(v.type == YTGPU_TYPE_NULL && c.has_type_byte)) err |= DE_SCHEMA_VIOLATION;
+    if (v.type == YTGPU_TYPE_STRING && v.length > c.width) err |= DE_STRING_TOO_LONG;
+    return err;
+}
+
+__host__ __device__ inline u32 key_string_blocks(u32 len) { return len / 7 + 1; }
+
+// Number of words of E_c.
+__host__ __device__ inline u32 key_col_words(const KeyColLayout& c, const ytgpu_value& v) {
+    u64 bytes = c.has_type_byte;
+    switch (v.type) {
+        case YTGPU_TYPE_INT64: case YTGPU_TYPE_UINT64: case YTGPU_TYPE_DOUBLE: bytes += 8; break;
+        case YTGPU_TYPE_BOOLEAN: bytes += 1; break;
+        case YTGPU_TYPE_STRING: bytes += 8ull * key_string_blocks(v.length); break;
+        default: break;
+    }
+    return (u32)((bytes + 7) / 8);
+}
+
+// Bytes [7k, 7k + 7) of a string of length len, zero-padded, as a 56-bit big-endian number.
+__host__ __device__ inline u64 key_string_raw7(const u8* s, u32 len, u32 k) {
+    u64 r = 0;
+    const u32 b0 = 7 * k;
+#pragma unroll
+    for (u32 i = 0; i < 7; ++i) r = (r << 8) | (b0 + i < len ? s[b0 + i] : 0);
+    return r;
+}
+
+__host__ __device__ inline u64 key_string_tag(u32 len, u32 k) {
+    return k + 1 < key_string_blocks(len) ? 8 : len - 7 * k;
+}
+
+// Word w (< key_col_words) of E_c.
+__host__ __device__ inline u64 key_col_word(const KeyColLayout& c, const ytgpu_value& v, const u8* heap, u32 w) {
+    const u32 tb = c.has_type_byte;
+    u64 word;
+    u32 bytes;  // meaningful bytes of this word (the rest is padding)
+    if (v.type == YTGPU_TYPE_STRING) {
+        const u8* s = heap + v.data;
+        const u32 nb = key_string_blocks(v.length);
+        if (!tb) {  // word w = block w
+            word = (key_string_raw7(s, v.length, w) << 8) | key_string_tag(v.length, w);
+            bytes = 8;
+        } else {    // word w = tag of block w-1 (or the type byte), then the raw bytes of block w
+            word = (w == 0 ? (u64)v.type : key_string_tag(v.length, w - 1)) << 56;
+            if (w < nb) word |= key_string_raw7(s, v.length, w);
+            bytes = w < nb ? 8 : 1;
+        }
+    } else {
+        u64 p = 0;
+        u32 pb = 0;
+        switch (v.type) {
+            case YTGPU_TYPE_INT64: p = v.data ^ 0x8000000000000000ull; pb = 8; break;
+            case YTGPU_TYPE_UINT64: p = v.data; pb = 8; break;
+            case YTGPU_TYPE_DOUBLE: p = normalize_double_bits(v.data); pb = 8; break;
+            case YTGPU_TYPE_BOOLEAN: p = (u64)((v.data & 0xff) != 0) << 56; pb = 1; break;
+            default: break;
+        }
+        // E_c = [type] p (pb bytes, left-aligned in p): at most 9 bytes, words 0 and 1
+        const u32 total = tb + pb;
+        if (tb) word = w == 0 ? ((u64)v.type << 56) | (p >> 8) : p << 56;
+        else word = p;
+        bytes = total - 8 * w < 8 ? total - 8 * w : 8;
+    }
+    const u64 mask = bytes >= 8 ? ~0ull : ~(~0ull >> (8 * bytes));
+    if (c.descending) word ^= mask;
+    return word & mask;
+}
+
+__host__ __device__ inline const ytgpu_value& key_value(const KeyColLayout& c, const ytgpu_value* row) {
+    return row[c.index];
+}
+
+// First cursor at or after `cur` where rows a and b differ (kKeyEnd: equal from there on).  A cursor past the end of
+// a column's words moves on to the next column.
+__host__ __device__ inline u64 key_first_diff(const KeyLayout& L, const ytgpu_value* a, const ytgpu_value* b,
+                                              const u8* heap, u64 cur) {
+    u32 w0 = (u32)cur;
+    for (u32 c = (u32)(cur >> 32); c < L.ncols; ++c, w0 = 0) {
+        const KeyColLayout& k = L.col[c];
+        const ytgpu_value va = key_value(k, a), vb = key_value(k, b);
+        const u32 na = key_col_words(k, va), nb = key_col_words(k, vb);
+        const u32 nw = na < nb ? na : nb;
+        for (u32 w = w0; w < nw; ++w)
+            if (key_col_word(k, va, heap, w) != key_col_word(k, vb, heap, w)) return key_cursor(c, w);
+        if (na != nb) return key_cursor(c, w0 > nw ? w0 : nw);
+    }
+    return kKeyEnd;
+}
+
+// Word at a cursor returned by key_first_diff (0 past the row's last word).
+__host__ __device__ inline u64 key_word_at(const KeyLayout& L, const ytgpu_value* row, const u8* heap, u64 cur) {
+    if (cur == kKeyEnd) return 0;
+    const KeyColLayout& k = L.col[(u32)(cur >> 32)];
+    const ytgpu_value v = key_value(k, row);
+    const u32 w = (u32)cur;
+    return w < key_col_words(k, v) ? key_col_word(k, v, heap, w) : 0;
+}
+
+// Three-way comparison of rows a and b, which are known to be equal before `cur`.
+__host__ __device__ inline int key_compare_from(const KeyLayout& L, const ytgpu_value* a, const ytgpu_value* b,
+                                                const u8* heap, u64 cur) {
+    const u64 d = key_first_diff(L, a, b, heap, cur);
+    if (d == kKeyEnd) return 0;
+    const KeyColLayout& k = L.col[(u32)(d >> 32)];
+    const ytgpu_value va = key_value(k, a), vb = key_value(k, b);
+    const u32 w = (u32)d;
+    const u32 na = key_col_words(k, va), nb = key_col_words(k, vb);
+    if (w >= na || w >= nb) return na < nb ? -1 : 1;  // a shorter E_c (cannot happen for prefix-free E_c)
+    return key_col_word(k, va, heap, w) < key_col_word(k, vb, heap, w) ? -1 : 1;
 }
 
 // Fixed-row column: raw little-endian scalar / exact-width string at a byte offset.
