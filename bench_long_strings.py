@@ -14,7 +14,14 @@ Per input: rows/s (median step; a host clock around the call, which reads the un
 the call ends synchronised), the refinement rounds and the rows each round sorted, and a parity check on the host (the
 result is a permutation; ~10^5 sampled adjacent pairs are ordered by the oracle's comparator, equal keys in input order).
 url_like also carries a CPU baseline: the oracle's SORT_STD (std::sort by the reference comparator, one thread) on its
-first 10^6 rows.  One JSON line on stdout, with the card's name and power limit.  Nothing is written to the source tree.
+first 10^6 rows.
+Partition leg (`partition` per input): ytgpu_partition_rowset with the ordered partitioner (DEVICE, index + histogram)
+for P = 8 and P = 1024 lower bounds.  Bound 0 is universal; bound j is the (j*m/P)-th key (prefix length 1, inclusive)
+of a seeded sample of m = 10^5 rows sorted by the oracle.  Per P: rows/s (median step, a host clock around the call and a
+device synchronise), `last_partition_key_words` (1: key words, 0: normalised keys), and parity of the sampled rows'
+indices with the oracle's TOrderedPartitioner.  url_like also carries a CPU baseline: the oracle's partitioner on its
+first 10^6 rows, one thread.
+One JSON line on stdout, with the card's name and power limit.  Nothing is written to the source tree.
 """
 from __future__ import annotations
 
@@ -106,6 +113,42 @@ def cpu_baseline(values_np, heap_np):
             "sample": f"first {len(values_np)} rows, the oracle's SORT_STD (std::sort by the reference comparator)"}
 
 
+def partition_leg(ctx, vals, heap, vals_np, heap_np, steps, warmup, cpu_baseline_rows=0):
+    """Ordered partitioning of the whole input for P = 8 and 1024 bounds taken from a sorted seeded sample."""
+    import oracle
+    from ytsaurus_b200 import capi
+    from ytsaurus_b200.rowset import Rowset, VALUE_DTYPE
+    n = len(vals_np)
+    sample = vals_np[_sample_index(n, 100_000, SEED + 1)]
+    m = len(sample)
+    perm, _ = oracle.sort_rows(sample, heap_np, 1, None, oracle.SORT_STABLE)
+    sorted_sample = sample[perm.astype(np.int64)]
+    out = {}
+    for P in (8, 1024):
+        bvals = np.concatenate([np.zeros((1, 2), dtype=VALUE_DTYPE), sorted_sample[[(j * m) // P for j in range(1, P)]]])
+        blen, binc = [0] + [1] * (P - 1), [1] * P
+        spec = ctx._partition_spec(capi.PARTITION_ORDERED, P, key_columns=[dict(index=0, type=0x10)],
+                                   bounds=Rowset(bvals, heap_np), bound_prefix_length=blen, bound_inclusive=binc)
+        times, idx = [], None
+        for step in range(warmup + steps):
+            t0 = time.perf_counter()
+            idx, _ = ctx.partition_rowset(vals, heap, spec)
+            ctx.synchronize()
+            if step >= warmup:
+                times.append(time.perf_counter() - t0)
+        r = {"partitions": P, "ms": [round(t * 1e3, 3) for t in times], "value": n / float(np.median(times)),
+             "unit": "rows/s", "key_words": ctx.get_option("last_partition_key_words")}
+        want, _ = oracle.partition_ordered(sample, heap_np, 1, None, bvals, heap_np, blen, binc)
+        got = idx.cpu().numpy()[_sample_index(n, 100_000, SEED + 1)]
+        r["parity_check"] = {"ok": bool((got == want).all()), "rows": int(m)}
+        if cpu_baseline_rows:
+            _, sec = oracle.partition_ordered(vals_np[:cpu_baseline_rows], heap_np, 1, None, bvals, heap_np, blen, binc)
+            r["cpu_baseline"] = {"value": cpu_baseline_rows / sec, "unit": "rows/s", "cores": 1,
+                                 "sample": f"first {cpu_baseline_rows} rows, the oracle's TOrderedPartitioner"}
+        out[f"P{P}"] = r
+    return out
+
+
 def _sample_index(m, k, seed):
     """Sorted positions of a fixed seeded sample of k of m rows (every row when m <= k)."""
     if m <= k:
@@ -179,6 +222,8 @@ def main():
             r["parity_check"] = parity_check(vals_np, heap_np, perm_np)
         if name == "url_like" and not args.no_cpu_baseline:
             r["cpu_baseline"] = cpu_baseline(vals_np[: min(n, 1_000_000)], heap_np)
+        r["partition"] = partition_leg(ctx, vals, heap, vals_np, heap_np, args.steps, args.warmup,
+                                       min(n, 1_000_000) if name == "url_like" and not args.no_cpu_baseline else 0)
         if args.dump_outputs:
             os.makedirs(args.dump_outputs, exist_ok=True)
             np.save(os.path.join(args.dump_outputs, f"{name}_perm_sample.npy"), perm_np[_sample_index(n, 100_000, SEED)].astype(np.float64))
@@ -189,7 +234,8 @@ def main():
     line = {"metric": "rows/s sorted (rowset [string key > 256 B, int64], ytgpu_sort_rowset DEVICE)",
             "value": results["url_like"]["value"], "unit": "rows/s", "config": {"rows": n, "steps": args.steps, "warmup": args.warmup},
             "device": name, "power_limit_w": power,
-            "parity_check": all(r.get("parity_check", {"ok": True})["ok"] for r in results.values()),
+            "parity_check": all(r.get("parity_check", {"ok": True})["ok"] and
+                                all(p["parity_check"]["ok"] for p in r["partition"].values()) for r in results.values()),
             "inputs": results}
     print(json.dumps(line), flush=True)
 

@@ -396,6 +396,75 @@ static void TestPartitionMultiChunkWriter() {
     ytgpu_context_destroy(ctx);
 }
 
+// 1 KB string keys and bounds: the ordered partitioner compares key words (the normalised key would exceed 256 bytes).
+// Every row written through the partition writer lands in the partition a CPU upper_bound over TestKey gives it.
+static void TestPartitionMultiChunkWriterLongKeys() {
+    std::mt19937 rng(13);
+    const std::string prefix(1000, 'p');
+    auto makeKey = [&] {
+        std::string key = prefix.substr(0, 900 + rng() % 100);
+        for (int k = rng() % 40; k > 0; --k) key.push_back("ab\0"[rng() % 3]);
+        return key;
+    };
+    std::vector<TUnversionedOwningRow> keep;
+    for (int i = 0; i < 3000; ++i) {
+        TUnversionedOwningRowBuilder b;
+        b.AddValue(MakeUnversionedStringValue(makeKey(), 0));
+        b.AddValue(MakeUnversionedInt64Value(i, 1));
+        keep.push_back(b.FinishRow());
+    }
+    std::vector<TUnversionedOwningRow> pivots;
+    for (int j = 0; j < 15; ++j) {
+        TUnversionedOwningRowBuilder b;
+        b.AddValue(MakeUnversionedStringValue(makeKey()));
+        pivots.push_back(b.FinishRow());
+    }
+    std::sort(pivots.begin(), pivots.end(), [](const auto& a, const auto& b) { return CompareValues(a[0], b[0]) < 0; });
+    std::vector<TOwningKeyBound> bounds{TOwningKeyBound::MakeUniversal(false)};
+    for (size_t j = 0; j < pivots.size(); ++j) bounds.push_back(TOwningKeyBound::FromRow(pivots[j], j % 3 != 0, false));
+    // TOrderedPartitioner::GetPartitionIndex (partitioner.cpp:41-57) on the CPU: upper_bound with !TestKey, minus one
+    auto testKey = [](const TUnversionedOwningRow& row, const TOwningKeyBound& bound) {
+        const int c = bound.Prefix.GetCount() ? CompareValues(row[0], bound.Prefix[0]) : 0;
+        return c > 0 || (c == 0 && bound.IsInclusive);
+    };
+    std::vector<int> expect;
+    for (auto& row : keep) {
+        auto it = std::upper_bound(bounds.begin(), bounds.end(), row, [&](const auto& r, const auto& b) { return !testKey(r, b); });
+        expect.push_back((int)(it - bounds.begin()) - 1);
+    }
+    struct TSink : IPartitionBlockSink {
+        std::vector<TPartitionBlock> Blocks;
+        bool WriteBlock(TPartitionBlock block) override {
+            Blocks.push_back(std::move(block));
+            return true;
+        }
+    };
+    auto sink = std::make_shared<TSink>();
+    TPartitionWriterConfig config;
+    config.BlockSize = 64 << 10;
+    config.MaxBufferSize = 256 << 10;
+    auto writer = CreatePartitionMultiChunkWriter(config, CreateOrderedPartitioner(bounds, TComparator({ESortOrder::Ascending})), sink);
+    for (size_t off = 0; off < keep.size(); off += 500) {
+        std::vector<TUnversionedRow> batch(keep.begin() + off, keep.begin() + std::min(keep.size(), off + 500));
+        (void)writer->Write(batch);
+    }
+    writer->Close();
+    ytgpu_context* ctx = nullptr;
+    ytgpu_error err{};
+    EXPECT_EQ(ytgpu_context_create(0, nullptr, &ctx, &err), (int)YTGPU_OK);
+    std::vector<int> got(keep.size(), -1);
+    for (auto& block : sink->Blocks) {
+        std::vector<ytgpu_value> values((size_t)block.RowCount * 2);
+        std::vector<uint32_t> counts((size_t)block.RowCount);
+        EXPECT_EQ(ytgpu_decode_horizontal_block(ctx, block.Data.data(), block.Data.size(), (uint32_t)block.RowCount, 2, values.data(),
+                                                counts.data(), YTGPU_MEM_HOST, &err), (int)YTGPU_OK);
+        for (int64_t r = 0; r < block.RowCount; ++r) got[(size_t)values[r * 2 + 1].data] = block.PartitionIndex;
+    }
+    EXPECT_TRUE(got == expect);
+    EXPECT_TRUE(std::set<int>(expect.begin(), expect.end()).size() > 8);  // the keys spread over the partitions
+    ytgpu_context_destroy(ctx);
+}
+
 int main() {
     try {
         TestOrdered();
@@ -406,6 +475,7 @@ int main() {
         TestSortedMergingReader();
         TestSortedJoiningReader();
         TestPartitionMultiChunkWriter();
+        TestPartitionMultiChunkWriterLongKeys();
     } catch (const std::exception& e) {
         std::fprintf(stderr, "unexpected exception: %s\n", e.what());
         return 100;

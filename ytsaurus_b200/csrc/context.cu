@@ -203,6 +203,7 @@ int ytgpu_context_get_option(ytgpu_context* h, const char* name, int64_t* value,
     else if (strcmp(name, "merge_path") == 0) *value = c->opt_merge_path;
     else if (strcmp(name, "last_merge_used_merge_path") == 0) *value = c->last_merge_used_merge_path ? 1 : 0;
     else if (strcmp(name, "last_sort_refine_rounds") == 0) *value = c->last_sort_refine_rounds;
+    else if (strcmp(name, "last_partition_key_words") == 0) *value = c->last_partition_key_words ? 1 : 0;
     else if (strncmp(name, "last_sort_refine_rows.", 22) == 0) {
         const size_t r = (size_t)strtoull(name + 22, nullptr, 10);
         *value = r < c->last_sort_refine_rows.size() ? (int64_t)c->last_sort_refine_rows[r] : 0;

@@ -35,6 +35,7 @@ struct Context {
     bool last_merge_used_merge_path = false;
     u32 last_sort_refine_rounds = 0;         // refinement rounds of the last rowset sort / merge / join (0: normalised keys)
     std::vector<u64> last_sort_refine_rows;  // rows each of those rounds sorted
+    bool last_partition_key_words = false;   // the last rowset ordered partitioning compared key words (keys over 256 B)
     int opt_sort_hybrid = -1;  // -1: environment default (YTGPU_SORT_HYBRID, on); 0/1: set through ytgpu_context_set_option
 
     Status alloc(void** p, size_t bytes) {

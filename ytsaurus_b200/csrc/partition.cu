@@ -179,6 +179,124 @@ __global__ void __launch_bounds__(256) partition_index_kernel(const PartParams P
     }
 }
 
+// ---- ordered partitioner over the width-free key words of keys.cuh (rowset keys whose fixed-width normalised form
+// does not fit in kMaxKeyChunks chunks) ----
+// Bound b compares its first plen[b] key columns; column c of it is the E_c words of the bound's value, at
+// words[col_off[b * (ncols + 1) + c] .. col_off[b * (ncols + 1) + c + 1]).  The key's words are computed from its values
+// and the heap as the probes need them: no per-row key is stored.
+struct WordBounds {
+    const u64* words;
+    const u64* col_off;   // [P][ncols + 1]
+    const u32* plen;      // [P] effective prefix length in columns
+    const u8* inclusive;  // [P] effective inclusiveness
+    u32 count;
+};
+
+constexpr u32 kHeadWords = 4;
+
+// Key column 0 and its first kHeadWords words, kept in registers: every probe of the binary search starts there.
+struct KeyHead {
+    ytgpu_value v0;
+    u32 n0;  // words of E_0
+    u64 w[kHeadWords];
+};
+
+__host__ __device__ __forceinline__ ytgpu_value key_load(const ytgpu_value* p) {
+#ifdef __CUDA_ARCH__
+    return load_value(p);
+#else
+    return *p;
+#endif
+}
+
+__host__ __device__ __forceinline__ KeyHead key_head(const KeyLayout& L, const ytgpu_value* row, const u8* heap) {
+    KeyHead h;
+    const KeyColLayout& k = L.col[0];
+    h.v0 = key_load(row + k.index);
+    h.n0 = key_col_words(k, h.v0);
+#pragma unroll
+    for (u32 w = 0; w < kHeadWords; ++w) h.w[w] = w < h.n0 ? key_col_word(k, h.v0, heap, w) : 0;
+    return h;
+}
+
+// Sign of (key - bound b) over the bound's effective prefix, column by column and word by word: TComparator::TestKey
+// (comparator.cpp:77-103) before the bound's inclusiveness is applied.
+__host__ __device__ __forceinline__ int compare_key_bound(const KeyLayout& L, const ytgpu_value* row, const u8* heap,
+                                                          const KeyHead& h, const WordBounds& B, u32 b) {
+    const u64* off = B.col_off + (u64)b * (L.ncols + 1);
+    const u32 plen = B.plen[b];
+    for (u32 c = 0; c < plen; ++c) {
+        const KeyColLayout& k = L.col[c];
+        const ytgpu_value v = c == 0 ? h.v0 : key_load(row + k.index);
+        const u32 nk = c == 0 ? h.n0 : key_col_words(k, v);
+        const u64* bw = B.words + off[c];
+        const u32 nb = (u32)(off[c + 1] - off[c]);
+        const u32 nw = nk < nb ? nk : nb;
+        u32 w = 0;
+        if (c == 0) {
+#pragma unroll
+            for (u32 i = 0; i < kHeadWords; ++i)
+                if (i < nw && h.w[i] != bw[i]) return h.w[i] < bw[i] ? -1 : 1;
+            w = kHeadWords;
+        }
+        for (; w < nw; ++w) {
+            const u64 kw = key_col_word(k, v, heap, w), x = bw[w];
+            if (kw != x) return kw < x ? -1 : 1;
+        }
+        if (nk != nb) return nk < nb ? -1 : 1;  // E_c is prefix-free: equal words up to here mean equal lengths
+    }
+    return 0;
+}
+
+// std::upper_bound(bounds, key, !TestKey) - 1   (partitioner.cpp:46-56), over key words.
+__host__ __device__ __forceinline__ i32 ordered_index_words(const KeyLayout& L, const ytgpu_value* row, const u8* heap,
+                                                            const WordBounds& B) {
+    const KeyHead h = key_head(L, row, heap);
+    u32 lo = 0, cnt = B.count;
+    while (cnt > 0) {
+        const u32 step = cnt >> 1, mid = lo + step;
+        const int cmp = compare_key_bound(L, row, heap, h, B, mid);
+        if (cmp > 0 || (cmp == 0 && B.inclusive[mid])) {
+            lo = mid + 1;
+            cnt -= step + 1;
+        } else {
+            cnt = step;
+        }
+    }
+    return (i32)lo - 1;
+}
+
+// The same outputs and error bits as partition_index_kernel<false> for YTGPU_PARTITION_ORDERED.
+__global__ void __launch_bounds__(256) partition_words_kernel(const PartParams P, const WordBounds B) {
+    extern __shared__ u32 s_hist[];
+    const bool smem_hist = P.histogram && P.partition_count <= (u32)kMaxSmemPartitions;
+    if (smem_hist) {
+        for (u32 i = threadIdx.x; i < P.partition_count; i += blockDim.x) s_hist[i] = 0;
+        __syncthreads();
+    }
+    u32 err = 0;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < P.n; i += (u64)gridDim.x * blockDim.x) {
+        const ytgpu_value* row = P.values + i * P.value_count;
+        for (u32 c = 0; c < P.layout.ncols; ++c) err |= key_value_errors(P.layout.col[c], load_value(row + P.layout.col[c].index));
+        i32 idx = ordered_index_words(P.layout, row, P.heap, B);
+        if (idx < 0) { err |= DE_PART_OUT_OF_BOUNDS; idx = 0; }
+        if (P.out_index) P.out_index[i] = idx;
+        if (P.out_chunk) P.out_chunk[i] = (u64)(u32)idx;
+        if (P.histogram) {
+            if (smem_hist) atomicAdd(&s_hist[idx], 1u);
+            else atomicAdd(&P.histogram[idx], 1ull);
+        }
+    }
+    if (err) atomicOr(P.err_word, err);
+    if (smem_hist) {
+        __syncthreads();
+        for (u32 i = threadIdx.x; i < P.partition_count; i += blockDim.x) {
+            u32 c = s_hist[i];
+            if (c) atomicAdd(&P.histogram[i], (unsigned long long)c);
+        }
+    }
+}
+
 // ---- host side: lower bounds -> normalised bytes (same encoding as the keys) ----
 struct HostBounds {
     std::vector<u64> words;
@@ -288,21 +406,70 @@ Status normalize_bounds(const ytgpu_partition_spec* spec, const KeyLayout& L, Ho
     return Status{};
 }
 
+// ---- host side: lower bounds -> key words (keys.cuh; the encoder the keys use) ----
+struct HostWordBounds {
+    std::vector<u64> words, col_off;
+    std::vector<u32> plen;
+    std::vector<u8> inclusive;
+    WordBounds view() const { return WordBounds{words.data(), col_off.data(), plen.data(), inclusive.data(), (u32)plen.size()}; }
+};
+
+// The rules of normalize_bounds that do not depend on a width.  A bound string needs no width: prefix-free words order
+// it against keys of any length.
+Status encode_bounds_words(const ytgpu_partition_spec* spec, const KeyLayout& L, HostWordBounds* hb) {
+    const u32 P = (u32)spec->partition_count;
+    hb->words.clear();
+    hb->col_off.clear();
+    hb->plen.assign(P, 0);
+    hb->inclusive.assign(P, 0);
+    for (u32 b = 0; b < P; ++b) {
+        u32 plen = spec->bound_prefix_length ? spec->bound_prefix_length[b] : 0;
+        if (plen > L.ncols || plen > spec->bound_value_count)
+            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "Comparator is used with longer key bound (bound %u has %u values, comparator length %u)", b, plen, L.ncols);
+        bool incl = spec->bound_inclusive ? spec->bound_inclusive[b] != 0 : true;
+        u32 eff = plen;
+        hb->col_off.push_back(hb->words.size());
+        for (u32 c = 0; c < plen; ++c) {
+            const KeyColLayout& kc = L.col[c];
+            const ytgpu_value& v = spec->bounds[(size_t)b * spec->bound_value_count + c];
+            if (v.type == YTGPU_TYPE_ANY || v.type == YTGPU_TYPE_COMPOSITE)
+                return make_status(YTGPU_ERR_UNSUPPORTED, "partition bound %u holds an Any/Composite value", b);
+            if (!kc.has_type_byte && v.type != kc.type) {
+                // every key equal to the bound so far holds the declared type here: type order decides
+                eff = c;
+                incl = ((int)kc.type > (int)v.type ? 1 : -1) * (kc.descending ? -1 : 1) > 0;
+                break;
+            }
+            for (u32 w = 0, nw = key_col_words(kc, v); w < nw; ++w) hb->words.push_back(key_col_word(kc, v, spec->bounds_heap, w));
+            hb->col_off.push_back(hb->words.size());
+        }
+        hb->col_off.resize((size_t)(b + 1) * (L.ncols + 1), hb->words.size());
+        hb->plen[b] = eff;
+        hb->inclusive[b] = incl ? 1 : 0;
+    }
+    if (hb->words.empty()) hb->words.push_back(0);  // every bound universal: keep the upload non-empty
+    return Status{};
+}
+
 struct PartitionRun {
     DevBuf<u64> bwords;
-    DevBuf<u32> bnbytes;
+    DevBuf<u32> bnbytes;     // key-word bounds: effective prefix length in columns
     DevBuf<u8> bincl;
+    DevBuf<u64> boff;        // key-word bounds: per-column word offsets
+    bool key_words = false;  // the layout does not fit kMaxKeyChunks: partition_words_kernel over `wbounds`
+    WordBounds wbounds{};
     DevBuf<unsigned long long> hist;
     DevBuf<i32> index;
     DevBuf<u64> chunk;
 };
 
-Status launch_partition(Context* ctx, PartParams& P, bool fixed) {
+Status launch_partition(Context* ctx, PartParams& P, bool fixed, const WordBounds* words = nullptr) {
     if (P.n == 0) return Status{};
     KernelTimer t(ctx, KC_PARTITION);
     u32 blocks = (u32)std::min<u64>((P.n + 255) / 256, (u64)kNumSms * 8);
     size_t smem = (P.histogram && P.partition_count <= (u32)kMaxSmemPartitions) ? (size_t)P.partition_count * 4 : 0;
-    if (fixed) partition_index_kernel<true><<<blocks, 256, smem, ctx->stream>>>(P);
+    if (words) partition_words_kernel<<<blocks, 256, smem, ctx->stream>>>(P, *words);
+    else if (fixed) partition_index_kernel<true><<<blocks, 256, smem, ctx->stream>>>(P);
     else partition_index_kernel<false><<<blocks, 256, smem, ctx->stream>>>(P);
     YTGPU_CUDA_TRY(cudaGetLastError());
     return Status{};
@@ -333,9 +500,27 @@ Status prepare_params(Context* ctx, const ytgpu_partition_spec* spec, bool fixed
             }
         }
         ytgpu_sort_spec ks{cols.data(), (u32)cols.size()};
-        YTGPU_TRY(build_key_layout(&ks, fixed, false, &P->layout));
+        const Status s = build_key_layout(&ks, fixed, false, &P->layout);
+        run->key_words = !fixed && s.code == YTGPU_ERR_UNSUPPORTED && P->layout.nchunks > (u32)kMaxKeyChunks;
+        if (!run->key_words) YTGPU_TRY(s);
         if (!spec->bounds && spec->partition_count > 1)
             return make_status(YTGPU_ERR_INVALID_ARGUMENT, "ordered partitioner needs bounds");
+        if (run->key_words) {
+            HostWordBounds hw;
+            YTGPU_TRY(encode_bounds_words(spec, P->layout, &hw));
+            const u32 Pn = P->partition_count;
+            YTGPU_TRY(run->bwords.allocate(ctx, hw.words.size()));
+            YTGPU_TRY(run->boff.allocate(ctx, hw.col_off.size()));
+            YTGPU_TRY(run->bnbytes.allocate(ctx, Pn));
+            YTGPU_TRY(run->bincl.allocate(ctx, Pn));
+            YTGPU_CUDA_TRY(cudaMemcpyAsync(run->bwords.p, hw.words.data(), hw.words.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+            YTGPU_CUDA_TRY(cudaMemcpyAsync(run->boff.p, hw.col_off.data(), hw.col_off.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+            YTGPU_CUDA_TRY(cudaMemcpyAsync(run->bnbytes.p, hw.plen.data(), Pn * 4, cudaMemcpyHostToDevice, ctx->stream));
+            YTGPU_CUDA_TRY(cudaMemcpyAsync(run->bincl.p, hw.inclusive.data(), Pn, cudaMemcpyHostToDevice, ctx->stream));
+            YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));  // hw goes out of scope
+            run->wbounds = WordBounds{run->bwords.p, run->boff.p, run->bnbytes.p, run->bincl.p, Pn};
+            return Status{};
+        }
         HostBounds hb;
         YTGPU_TRY(normalize_bounds(spec, P->layout, &hb));
         const u32 Pn = P->partition_count;
@@ -373,6 +558,7 @@ Status finish_outputs(Context* ctx, PartitionRun& run, u64 n, u32 Pn, i32* out_i
 Status partition_rowset_impl(Context* ctx, const ytgpu_rowset_view* in, const ytgpu_partition_spec* spec,
                              i32* out_index, u64* out_histogram, int out_mem, ytgpu_value* out_slab_values = nullptr,
                              u32* out_slab_perm = nullptr) {
+    ctx->last_partition_key_words = false;
     if (!in) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null rowset");
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
     const u64 n = in->row_count;
@@ -391,6 +577,7 @@ Status partition_rowset_impl(Context* ctx, const ytgpu_rowset_view* in, const yt
     PartParams P;
     PartitionRun run;
     YTGPU_TRY(prepare_params(ctx, spec, false, in->value_count, vals, n, &P, &run));
+    ctx->last_partition_key_words = run.key_words;
     P.values = vals;
     P.value_count = in->value_count;
     P.heap = heap;
@@ -414,7 +601,7 @@ Status partition_rowset_impl(Context* ctx, const ytgpu_rowset_view* in, const yt
         YTGPU_TRY(run.chunk.allocate(ctx, n));
         P.out_chunk = run.chunk.p;
     }
-    YTGPU_TRY(launch_partition(ctx, P, false));
+    YTGPU_TRY(launch_partition(ctx, P, false, run.key_words ? &run.wbounds : nullptr));
     if (slabs) {
         // variable-length rows: the 16-byte values of a row are fixed width and the strings stay where they are (their
         // offsets still point into the input heap), so the slab scatter is the fixed-row one over value_count * 16 bytes
@@ -645,6 +832,21 @@ int ytgpu_hostcheck_partition_ordered(const ytgpu_value* values, uint32_t value_
         }
         out_index[i] = (i32)lo - 1;
     }
+    return YTGPU_OK;
+}
+
+// The key-word partitioner (the bound encoding and the __host__ __device__ search partition_words_kernel runs) for keys
+// of any width, the ones that fit the normalised form included.  out_index[i] = -1 for a key below the first bound.
+int ytgpu_hostcheck_partition_ordered_words(const ytgpu_value* values, uint32_t value_count, const uint8_t* heap, uint64_t n,
+                                            const ytgpu_partition_spec* spec, int32_t* out_index) {
+    KeyLayout L;
+    Status s = build_key_layout(&spec->key, false, false, &L);
+    if (!s.ok() && !(s.code == YTGPU_ERR_UNSUPPORTED && L.nchunks > (u32)kMaxKeyChunks)) return s.code;
+    HostWordBounds hb;
+    s = encode_bounds_words(spec, L, &hb);
+    if (!s.ok()) return s.code;
+    const WordBounds B = hb.view();
+    for (u64 i = 0; i < n; ++i) out_index[i] = ordered_index_words(L, values + i * value_count, heap, B);
     return YTGPU_OK;
 }
 
