@@ -342,13 +342,19 @@ public:
                          const IUnversionedRowsetWriterPtr& writer) override {
         TQueryStatistics stats;
         if (query.GroupColumns.empty() || query.GroupColumns.size() > 8) throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "1..8 group items");
-        // the columns the query touches, each flattened once: 64-bit payloads + a null bitmap
+        // the columns the query touches, each flattened once: 64-bit payloads + a null bitmap, or (strings) one heap with
+        // starts, lengths and a null bytemap
         struct TFlatColumn {
             int Position;
             EValueType Type = EValueType::Null;
             std::vector<uint64_t> Values;
             std::vector<uint8_t> Nulls;  // bitmap
             bool AnyNull = false;
+            std::string Heap;
+            std::vector<uint64_t> Starts;
+            std::vector<uint32_t> Lengths;
+            std::vector<uint8_t> NullBytes;
+            std::string_view StringAt(uint64_t row) const { return std::string_view(Heap.data() + Starts[row], Lengths[row]); }
         };
         std::vector<TFlatColumn> columns;
         auto columnIndex = [&](int position) {
@@ -374,23 +380,44 @@ public:
                 const size_t base = c.Values.size();
                 c.Values.resize(base + rows.size());
                 c.Nulls.resize((base + rows.size() + 7) / 8, 0);
+                c.NullBytes.resize(base + rows.size(), 0);
                 for (size_t i = 0; i < rows.size(); ++i) {
                     const auto& v = rows[i][c.Position];
                     if (v.Type == EValueType::Null) {
                         c.Nulls[(base + i) >> 3] |= (uint8_t)(1u << ((base + i) & 7));
+                        c.NullBytes[base + i] = 1;
                         c.AnyNull = true;
                         continue;
                     }
-                    if (v.Type != EValueType::Int64 && v.Type != EValueType::Uint64 && v.Type != EValueType::Double && v.Type != EValueType::Boolean)
-                        throw TErrorException(YTGPU_ERR_UNSUPPORTED, "GROUP BY columns must be fixed-width scalars on the GPU path");
+                    if (v.Type != EValueType::Int64 && v.Type != EValueType::Uint64 && v.Type != EValueType::Double && v.Type != EValueType::Boolean &&
+                        v.Type != EValueType::String)
+                        throw TErrorException(YTGPU_ERR_UNSUPPORTED, "GROUP BY columns must be fixed-width scalars or strings on the GPU path");
                     if (c.Type == EValueType::Null) c.Type = v.Type;
                     else if (c.Type != v.Type) throw TErrorException(YTGPU_ERR_SCHEMA_VIOLATION, "Column changes its value type");
+                    if (v.Type == EValueType::String) {
+                        if (c.Starts.size() < base + rows.size()) {
+                            c.Starts.resize(base + rows.size(), 0);
+                            c.Lengths.resize(base + rows.size(), 0);
+                        }
+                        c.Starts[base + i] = c.Heap.size();
+                        c.Lengths[base + i] = v.Length;
+                        c.Heap.append(v.Data.String, v.Length);
+                        continue;
+                    }
                     c.Values[base + i] = v.Type == EValueType::Boolean ? (v.Data.Boolean ? 1 : 0) : v.Data.Uint64;
                 }
             }
             stats.RowsRead += (int64_t)rows.size();
         }
         const uint64_t n = (uint64_t)stats.RowsRead;
+        if (whereIndex >= 0 && columns[whereIndex].Type == EValueType::String)
+            throw TErrorException(YTGPU_ERR_UNSUPPORTED, "the WHERE column (position " + std::to_string(query.WhereColumn) +
+                                                             ") holds strings: string predicates are not on the GPU path");
+        for (size_t a = 0; a < query.AggregateItems.size(); ++a) {
+            const auto f = query.AggregateItems[a].Function;
+            if ((f == EAggregateFunction::Sum || f == EAggregateFunction::Avg) && columns[aggIndex[a]].Type == EValueType::String)
+                throw TErrorException(YTGPU_ERR_UNSUPPORTED, "sum / avg of a string column");
+        }
         std::vector<TUnversionedOwningRow> owned;
         if (n > 0) {
             auto view = [&](const TFlatColumn& c) {
@@ -405,13 +432,46 @@ public:
                 v.mem = YTGPU_MEM_HOST;
                 return v;
             };
+            // scalar columns are value columns, string columns follow them as string columns of the call
+            std::vector<int> argIndex(columns.size());
             std::vector<ytgpu_column_view> keyViews, valueViews;
-            for (int k : keyIndex) keyViews.push_back(view(columns[k]));
-            for (const auto& c : columns) valueViews.push_back(view(c));  // value column i == flattened column i
+            std::vector<ytgpu_string_column> stringViews;
+            for (auto& c : columns) {
+                if (c.Type != EValueType::String) continue;
+                c.Starts.resize(n, 0);
+                c.Lengths.resize(n, 0);
+                stringViews.push_back(ytgpu_string_column{reinterpret_cast<const uint8_t*>(c.Heap.data()), c.Heap.size(), c.Starts.data(),
+                                                          c.Lengths.data(), c.NullBytes.data(), n, YTGPU_MEM_HOST, 0});
+            }
+            for (size_t i = 0, s = 0; i < columns.size(); ++i) {
+                if (columns[i].Type == EValueType::String) {
+                    argIndex[i] = -1 - (int)s++;
+                } else {
+                    argIndex[i] = (int)valueViews.size();
+                    valueViews.push_back(view(columns[i]));
+                }
+            }
+            for (auto& a : argIndex)
+                if (a < 0) a = (int)valueViews.size() + (-1 - a);
+            for (int k : keyIndex) {
+                auto& c = columns[k];
+                if (c.Type == EValueType::String) {  // a string group item: canonical row ids (the first row of every value)
+                    ytgpu_error err{};
+                    if (ytgpu_string_value_ids(GetGpuContext(), reinterpret_cast<const uint8_t*>(c.Heap.data()), c.Heap.size(), c.Starts.data(),
+                                               c.Lengths.data(), c.NullBytes.data(), n, c.Values.data(), nullptr, YTGPU_MEM_HOST, &err) != YTGPU_OK)
+                        ThrowFrom(err);
+                    auto ids = view(c);
+                    ids.value_type = (uint8_t)EValueType::Uint64;
+                    keyViews.push_back(ids);
+                } else {
+                    keyViews.push_back(view(c));
+                }
+            }
             std::vector<ytgpu_aggregate> aggregates;
             for (size_t a = 0; a < query.AggregateItems.size(); ++a) {
                 static const int ops[] = {YTGPU_AGG_SUM, YTGPU_AGG_MIN, YTGPU_AGG_MAX, YTGPU_AGG_COUNT, YTGPU_AGG_AVG, YTGPU_AGG_ARGMIN, YTGPU_AGG_ARGMAX, YTGPU_AGG_FIRST};
-                aggregates.push_back(ytgpu_aggregate{ops[(int)query.AggregateItems[a].Function], aggIndex[a], byIndex[a], 0});
+                aggregates.push_back(ytgpu_aggregate{ops[(int)query.AggregateItems[a].Function], argIndex[aggIndex[a]],
+                                                     byIndex[a] >= 0 ? argIndex[byIndex[a]] : -1, 0});
             }
             const size_t nk = keyViews.size(), na = aggregates.size();
             uint64_t cap = std::min<uint64_t>(n, 1 << 16);
@@ -425,16 +485,19 @@ public:
                 ytgpu_groupby_multi_result res{0, cap, pk.data(), pkn.data(), pv.data(), pvn.data(), nullptr, nullptr};
                 ytgpu_predicate pred{CmpOf(query.WhereOp), 0, query.WhereConstant.Data.Uint64};
                 ytgpu_error err{};
-                const int code = ytgpu_scan_filter_groupby_multi(GetGpuContext(), keyViews.data(), (uint32_t)nk, valueViews.data(),
-                                                                 (uint32_t)valueViews.size(), aggregates.data(), (uint32_t)na,
-                                                                 whereIndex >= 0 ? &pred : nullptr, whereIndex, 0, &res, YTGPU_MEM_HOST, &err);
+                const int code = ytgpu_scan_filter_groupby_multi_strings(
+                    GetGpuContext(), keyViews.data(), (uint32_t)nk, valueViews.data(), (uint32_t)valueViews.size(), aggregates.data(),
+                    (uint32_t)na, whereIndex >= 0 ? &pred : nullptr, whereIndex >= 0 ? argIndex[whereIndex] : -1, 0, &res, YTGPU_MEM_HOST,
+                    stringViews.data(), (uint32_t)stringViews.size(), &err);
                 if (code == YTGPU_ERR_INVALID_ARGUMENT && res.group_count > cap) {  // more groups than the first guess
                     cap = res.group_count;
                     continue;
                 }
                 if (code != YTGPU_OK) ThrowFrom(err);
-                auto make = [](EValueType type, uint64_t bits, bool null, int id) {
+                // a string result (and a string key) is the index of a row that holds it
+                auto make = [&](const TFlatColumn* strings, EValueType type, uint64_t bits, bool null, int id) {
                     if (null) return MakeUnversionedNullValue(id);
+                    if (strings) return MakeUnversionedStringValue(strings->StringAt(bits), id);
                     switch (type) {
                         case EValueType::Uint64: return MakeUnversionedUint64Value(bits, id);
                         case EValueType::Double: { double d; std::memcpy(&d, &bits, 8); return MakeUnversionedDoubleValue(d, id); }
@@ -442,16 +505,18 @@ public:
                         default: return MakeUnversionedInt64Value((int64_t)bits, id);
                     }
                 };
+                auto stringsOf = [&](int index) { return columns[index].Type == EValueType::String ? &columns[index] : nullptr; };
                 owned.reserve(res.group_count);
                 for (uint64_t g = 0; g < res.group_count; ++g) {  // already in first-seen order
                     TUnversionedOwningRowBuilder b;
                     int id = 0;
-                    for (size_t k = 0; k < nk; ++k, ++id) b.AddValue(make(columns[keyIndex[k]].Type, keys[k][g], keyNull[k][g], id));
+                    for (size_t k = 0; k < nk; ++k, ++id)
+                        b.AddValue(make(stringsOf(keyIndex[k]), columns[keyIndex[k]].Type, keys[k][g], keyNull[k][g], id));
                     for (size_t a = 0; a < na; ++a, ++id) {
                         const auto f = query.AggregateItems[a].Function;
                         const EValueType type = f == EAggregateFunction::Count ? EValueType::Int64
                             : f == EAggregateFunction::Avg ? EValueType::Double : columns[aggIndex[a]].Type;
-                        b.AddValue(make(type, values[a][g], valueNull[a][g], id));
+                        b.AddValue(make(f == EAggregateFunction::Count ? nullptr : stringsOf(aggIndex[a]), type, values[a][g], valueNull[a][g], id));
                     }
                     owned.push_back(b.FinishRow());
                 }

@@ -120,8 +120,10 @@ struct IEvaluator {
     virtual ~IEvaluator() = default;
     virtual TQueryStatistics Run(const TGroupQuery& query, const ISchemalessMultiChunkReaderPtr& reader,
                                  const IUnversionedRowsetWriterPtr& writer) = 0;
-    //! The same for TMultiGroupQuery: one ytgpu_scan_filter_groupby_multi call over all rows the reader yields (at most
-    //! 2^30 per query fragment).  Columns must be Int64 / Uint64 / Double / Boolean (or Null).
+    //! The same for TMultiGroupQuery: one ytgpu_scan_filter_groupby_multi_strings call over all rows the reader yields (at
+    //! most 2^30 per query fragment).  Every column holds one type of Int64 / Uint64 / Double / Boolean / String (or Null);
+    //! a string group item goes through ytgpu_string_value_ids, and min / max / first / count / argmin / argmax take string
+    //! arguments.  sum / avg of a string column and a string WHERE column throw YTGPU_ERR_UNSUPPORTED.
     virtual TQueryStatistics Run(const TMultiGroupQuery& query, const ISchemalessMultiChunkReaderPtr& reader,
                                  const IUnversionedRowsetWriterPtr& writer) = 0;
 };

@@ -521,7 +521,8 @@ typedef enum ytgpu_agg_op {
 
 typedef struct ytgpu_aggregate {
     int32_t op;         /* ytgpu_agg_op */
-    int32_t column;     /* index into value_columns: the aggregated (argmin / argmax: the returned) column */
+    int32_t column;     /* index into value_columns (++ string_columns, see ytgpu_scan_filter_groupby_multi_strings):
+                           the aggregated (argmin / argmax: the returned) column */
     int32_t by_column;  /* argmin / argmax: the column that is minimised / maximised */
     int32_t reserved;
 } ytgpu_aggregate;
@@ -544,6 +545,45 @@ int ytgpu_scan_filter_groupby_multi(ytgpu_context* ctx, const ytgpu_column_view*
                                     const ytgpu_aggregate* aggregates, uint32_t aggregate_count,
                                     const ytgpu_predicate* predicate, int32_t predicate_column, uint64_t group_count_hint,
                                     ytgpu_groupby_multi_result* out, int out_mem, ytgpu_error* err);
+
+/* A flat string column, as ytgpu_extract_column, ytgpu_string_value_ids and ytgpu_encode_string_column take it: value i is
+ * the lengths[i] bytes at heap + starts[i]; a NULL row (null_bytemap[i] != 0) ignores its start and length. */
+typedef struct ytgpu_string_column {
+    const uint8_t* heap;          /* string bytes */
+    uint64_t heap_bytes;
+    const uint64_t* starts;       /* row_count entries: byte offset of the value in heap */
+    const uint32_t* lengths;      /* row_count entries */
+    const uint8_t* null_bytemap;  /* nullable; 1 = NULL (start / length ignored) */
+    uint64_t row_count;
+    int32_t mem;                  /* ytgpu_mem of every pointer above */
+    int32_t reserved;
+} ytgpu_string_column;
+
+/* ytgpu_scan_filter_groupby_multi with string-valued aggregates (YT QL's min / max / first / argmin / argmax / count over
+ * strings: builtin_function_types.cpp:201-254, the string branches of engine/udf/min.c and max.c,
+ * builtin_function_profiler.cpp:1442-1482).  An aggregate's `column` and `by_column` index value_columns ++ string_columns:
+ * index value_count + i is string_columns[i].  The predicate column must be a value column; a string GROUP BY key is passed
+ * as the ids of ytgpu_string_value_ids in key_columns.  Strings are ordered as in QL: unsigned bytes over the common prefix,
+ * then the shorter value first.  Over a string column:
+ *   MIN / MAX  skip NULLs, NULL without values
+ *   COUNT      number of non-NULL values
+ *   FIRST      the first non-NULL value
+ *   ARGMIN / ARGMAX  `column`, `by_column` or both may be strings; the first row (smallest index) that attains the bound wins
+ *   SUM / AVG  YTGPU_ERR_UNSUPPORTED
+ * A string-valued result (MIN, MAX, FIRST of a string column; ARGMIN / ARGMAX whose `column` is a string) is a ROW INDEX:
+ * values[a][g] is the row that holds the group's result (read starts / lengths there); value_null as for scalars.  For
+ * MIN / MAX it is the smallest row index that holds the value, so the output is deterministic.
+ * INVALID_ARGUMENT: a string column whose row_count differs from the key columns, a null starts / lengths, a null heap
+ * with heap_bytes > 0, a mem that is neither DEVICE nor HOST, a
+ * non-NULL value whose [start, start + length) leaves the heap (checked on the device for the columns the aggregates
+ * read; no byte outside the heap is read).  With string_count = 0 this is ytgpu_scan_filter_groupby_multi. */
+int ytgpu_scan_filter_groupby_multi_strings(ytgpu_context* ctx, const ytgpu_column_view* key_columns, uint32_t key_count,
+                                            const ytgpu_column_view* value_columns, uint32_t value_count,
+                                            const ytgpu_aggregate* aggregates, uint32_t aggregate_count,
+                                            const ytgpu_predicate* predicate, int32_t predicate_column,
+                                            uint64_t group_count_hint, ytgpu_groupby_multi_result* out, int out_mem,
+                                            const ytgpu_string_column* string_columns, uint32_t string_count,
+                                            ytgpu_error* err);
 
 /* ---- segmented SUM / COUNT over rows ALREADY SORTED by the group key (the aggregate stage after a sort) ----
  * Consecutive rows with equal keys form a group; no hash table.  Replaces the per-group accumulation of a GROUP BY

@@ -56,6 +56,7 @@ enum DevErr : u32 {
     DE_TABLE_FULL = 1u << 7,
     DE_PEER_TIMEOUT = 1u << 8,       // a peer GPU did not reach the in-box shuffle's barrier in time
     DE_BAD_PARTITION_INDEX = 1u << 9,  // caller-supplied partition index outside [0, partition_count)
+    DE_STRING_OUT_OF_HEAP = 1u << 10,  // a string value's [start, start + length) leaves its heap
 };
 
 struct Context;  // context.cu

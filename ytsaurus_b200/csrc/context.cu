@@ -65,6 +65,7 @@ Status check_device_errors(Context* ctx) {
         return make_status(YTGPU_ERR_CUDA, "in-box shuffle: a peer GPU did not reach the barrier within 20 s (a rank failed or never made the call)");
     if (e & DE_BAD_PARTITION_INDEX)
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "partition index outside [0, partition_count) or partition row counts that disagree with it");
+    if (e & DE_STRING_OUT_OF_HEAP) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "a string value runs past the end of its heap");
     return make_status(YTGPU_ERR_CUDA, "unknown device error word 0x%x", e);
 }
 

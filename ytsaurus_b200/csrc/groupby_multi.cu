@@ -14,13 +14,16 @@
 //   2. accumulate: one pass per aggregate over its value column, atomics on per-slot state.  min / max move one way, so a
 //      plain read that already bounds the value skips the atomic; argmin / argmax / first select a ROW (atomicMin of the
 //      row index among the rows that attain the bound), the value is gathered at the end — exactly the reference's
-//      "the first row wins a tie" (strict comparison in UpdateAggregateValue).
+//      "the first row wins a tie" (strict comparison in UpdateAggregateValue).  An aggregate over a string column (or
+//      argmin / argmax by one) takes mg_accumulate_strings_kernel instead: it selects the row lock-free with a CAS on
+//      the slot's row, comparing strings by the width-free key words of keys.cuh.
 //   3. emit: occupied slots are compacted and ordered by first row == QL's first-seen order (InsertGroupRow appends new
 //      groups), keys are decoded from the group's first row, states are finalised (avg = sum / count as double).
 #include <vector>
 
 #include "columnar.cuh"
 #include "context.cuh"
+#include "keys.cuh"
 #include "radix_sort.cuh"
 
 using namespace ytgpu;
@@ -360,6 +363,158 @@ __global__ void __launch_bounds__(512) mg_accumulate_kernel(int op, int phase, c
     }
 }
 
+// ---- string-valued aggregates (MIN / MAX / FIRST / COUNT / ARGMIN / ARGMAX with a string column or by_column) ----
+struct StringDev {
+    const u8* heap;
+    u64 heap_bytes;
+    const u64* starts;
+    const u32* lengths;
+    const u8* nulls;  // nullable bytemap
+    u32 present;      // 0: the argument is a scalar ColumnDev
+};
+
+// Value i of a string argument: false for NULL; a value that leaves the heap sets the error bit and counts as absent, so
+// no later read goes outside the heap.
+__device__ __forceinline__ bool string_at(const StringDev& c, u64 i, ytgpu_value* v, u32* bad) {
+    if (c.nulls && c.nulls[i]) return false;
+    const u64 s = c.starts[i];
+    const u32 l = c.lengths[i];
+    if (s > c.heap_bytes || (u64)l > c.heap_bytes - s) {
+        *bad = 1;
+        return false;
+    }
+    v->type = YTGPU_TYPE_STRING;
+    v->length = l;
+    v->data = s;
+    return true;
+}
+
+__device__ __forceinline__ ytgpu_value string_of(const StringDev& c, u64 row) {
+    ytgpu_value v{};
+    v.type = YTGPU_TYPE_STRING;
+    v.length = c.lengths[row];
+    v.data = c.starts[row];
+    return v;
+}
+
+// QL string order through the width-free key words of keys.cuh (a one-column, required, ascending String key): the order
+// the long-key sort and the ordered partitioner already use.  Words are prefix-free, so the first differing word decides.
+__device__ __forceinline__ int string_compare(const u8* heap, const ytgpu_value& a, const ytgpu_value& b) {
+    KeyColLayout L{};
+    L.type = YTGPU_TYPE_STRING;
+    const u32 na = key_string_blocks(a.length), nb = key_string_blocks(b.length);
+    const u32 nw = na < nb ? na : nb;
+    for (u32 w = 0; w < nw; ++w) {
+        const u64 x = key_col_word(L, a, heap, w), y = key_col_word(L, b, heap, w);
+        if (x != y) return x < y ? -1 : 1;
+    }
+    return 0;
+}
+
+// The selection key of MIN / MAX (the string column itself) or ARGMIN / ARGMAX (by_column, string or scalar).
+struct Selector {
+    ColumnDev by;
+    StringDev bs;
+    bool larger;  // MAX / ARGMAX
+    // (key(a), a) better than (key(b), b): a smaller (larger) key, the smaller row on equal keys.  b holds a selected row,
+    // whose value was checked when it was installed.
+    __device__ __forceinline__ bool better(u64 a, u64 b) const {
+        int c;
+        if (bs.present) {
+            c = string_compare(bs.heap, string_of(bs, a), string_of(bs, b));
+        } else {
+            bool nul;
+            const u64 ea = minmax_encode(by.value_type, decode_at(by, (i64)a, &nul));
+            const u64 eb = minmax_encode(by.value_type, decode_at(by, (i64)b, &nul));
+            c = ea < eb ? -1 : (ea > eb ? 1 : 0);
+        }
+        if (larger) c = -c;
+        return c < 0 || (c == 0 && a < b);
+    }
+};
+
+// Lock-free selection: install `cand` while it beats the holder.  A CAS fails only because another thread installed a
+// better row; the inputs are immutable, so comparing against the winner again is enough.
+__device__ __forceinline__ void select_row(unsigned long long* state, u64 cand, const Selector& sel) {
+    u64 cur = __ldcg(state);
+    while (cur == ~0ull || sel.better(cand, cur)) {
+        const u64 old = atomicCAS(state, (unsigned long long)cur, (unsigned long long)cand);
+        if (old == cur) return;
+        cur = old;
+    }
+}
+
+// Step 2 for an aggregate over a string column or by a string column.  State: S.row (selected row, ~0 = none) or, for
+// COUNT, S.nn.  Every non-NULL string of the arguments is bounds-checked, including rows the predicate dropped.
+__global__ void __launch_bounds__(256) mg_accumulate_strings_kernel(int op, const ColumnDev col, const StringDev cs, const ColumnDev by,
+                                                                    const StringDev bs, u64 n, const u32* __restrict__ slot_of_row,
+                                                                    AggState S, u32* err_word) {
+    const bool arg = op == YTGPU_AGG_ARGMIN || op == YTGPU_AGG_ARGMAX;
+    Selector sel;
+    sel.larger = op == YTGPU_AGG_MAX || op == YTGPU_AGG_ARGMAX;
+    if (arg) {
+        sel.by = by;
+        sel.bs = bs;
+    } else {  // MIN / MAX select by the column itself
+        sel.by = col;
+        sel.bs = cs;
+    }
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    const u64 trips = (n + stride - 1) / stride;  // the same for every thread: the warp collectives see whole warps
+    u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    u32 bad = 0;
+    for (u64 t = 0; t < trips; ++t, i += stride) {
+        const bool in = i < n;
+        const u32 slot = in ? slot_of_row[i] : kNoSlot;
+        bool have = false;
+        if (in) {
+            ytgpu_value v;
+            bool nul = true;
+            if (cs.present) have = string_at(cs, i, &v, &bad);
+            else {
+                decode_at(col, (i64)i, &nul);
+                have = !nul;
+            }
+            if (arg) {  // both arguments must be non-null (builtin_function_profiler.cpp:1304-1309)
+                bool bhave;
+                if (bs.present) bhave = string_at(bs, i, &v, &bad);
+                else {
+                    decode_at(by, (i64)i, &nul);
+                    bhave = !nul;
+                }
+                have = have && bhave;
+            }
+        }
+        have = have && slot != kNoSlot;
+        const u32 slot0 = __shfl_sync(0xffffffffu, slot, 0);
+        const bool uniform = __all_sync(0xffffffffu, slot == slot0) && slot0 != kNoSlot;  // sorted / clustered keys
+        if (op == YTGPU_AGG_COUNT) {
+            if (uniform) {
+                const u32 cnt = __popc(__ballot_sync(0xffffffffu, have));
+                if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(&S.nn[slot], (unsigned long long)cnt);
+            } else if (have) {
+                atomicAdd(&S.nn[slot], 1ull);
+            }
+            continue;
+        }
+        if (op == YTGPU_AGG_FIRST) {
+            if (have && i < __ldcg(&S.row[slot])) atomicMin(&S.row[slot], (unsigned long long)i);
+            continue;
+        }
+        u64 cand = have ? i : ~0ull;
+        if (uniform) {  // the warp's best row first: one CAS loop per warp instead of 32 on one address
+#pragma unroll
+            for (int d = 16; d > 0; d >>= 1) {
+                const u64 o = __shfl_xor_sync(0xffffffffu, cand, d);
+                if (o != ~0ull && (cand == ~0ull || sel.better(o, cand))) cand = o;
+            }
+            if ((threadIdx.x & 31) != 0) cand = ~0ull;
+        }
+        if (cand != ~0ull) select_row(&S.row[slot], cand, sel);
+    }
+    if (bad) atomicOr(err_word, (u32)DE_STRING_OUT_OF_HEAP);
+}
+
 // Step 3a: occupied slots -> (first row, slot) pairs, order arbitrary (one atomicAdd per warp).
 __global__ void __launch_bounds__(256) mg_compact_kernel(const u32* rep, u64 cap, const unsigned long long* first, u64* out_first,
                                                          u32* out_slot, u32* counter) {
@@ -404,15 +559,22 @@ __global__ void __launch_bounds__(256) mg_emit_keys_kernel(const KeyColumns K, c
     if (out_first) out_first[o] = row;
 }
 
-// Step 3c: one aggregate's result column.
+// Step 3c: one aggregate's result column.  row_result: a string-valued result, written as the selected row.
 __global__ void __launch_bounds__(256) mg_finalize_kernel(int op, const ColumnDev col, u8 by_type, u64 g, const u32* slot_sorted, AggState S,
-                                                          u64* out_value, u8* out_null) {
+                                                          u64* out_value, u8* out_null, bool row_result) {
     const u64 o = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (o >= g) return;
     const u32 slot = slot_sorted[o];
     const u8 vtype = col.value_type;
     u64 v = 0;
     bool nul = false;
+    if (row_result) {
+        v = S.row[slot];
+        nul = v == ~0ull;
+        out_value[o] = nul ? 0 : v;
+        out_null[o] = nul ? 1 : 0;
+        return;
+    }
     switch (op) {
         case YTGPU_AGG_SUM:
             nul = S.nn[slot] == 0;
@@ -459,11 +621,53 @@ __global__ void __launch_bounds__(256) mg_finalize_kernel(int op, const ColumnDe
 
 bool aggregatable_type(u8 t) { return t == YTGPU_TYPE_INT64 || t == YTGPU_TYPE_UINT64 || t == YTGPU_TYPE_DOUBLE || t == YTGPU_TYPE_BOOLEAN; }
 
+// A string column on the device (HOST inputs are uploaded).
+struct StagedStrings {
+    StringDev dev{};
+    DevBuf<u8> heap, nulls;
+    DevBuf<u64> starts;
+    DevBuf<u32> lengths;
+};
+
+Status stage_strings(Context* ctx, const ytgpu_string_column& c, StagedStrings* s) {
+    StringDev& d = s->dev;
+    d.heap_bytes = c.heap_bytes;
+    d.present = 1;
+    if (c.mem != YTGPU_MEM_HOST) {
+        d.heap = c.heap;
+        d.starts = c.starts;
+        d.lengths = c.lengths;
+        d.nulls = c.null_bytemap;
+        return Status{};
+    }
+    const u64 n = c.row_count;
+    YTGPU_TRY(s->heap.allocate(ctx, c.heap_bytes));
+    YTGPU_TRY(copy_in(ctx, s->heap.p, c.heap, c.heap_bytes, YTGPU_MEM_HOST));
+    YTGPU_TRY(s->starts.allocate(ctx, n));
+    YTGPU_TRY(copy_in(ctx, s->starts.p, c.starts, n * 8, YTGPU_MEM_HOST));
+    YTGPU_TRY(s->lengths.allocate(ctx, n));
+    YTGPU_TRY(copy_in(ctx, s->lengths.p, c.lengths, n * 4, YTGPU_MEM_HOST));
+    d.heap = s->heap.p;
+    d.starts = s->starts.p;
+    d.lengths = s->lengths.p;
+    d.nulls = nullptr;
+    if (c.null_bytemap) {
+        YTGPU_TRY(s->nulls.allocate(ctx, n));
+        YTGPU_TRY(copy_in(ctx, s->nulls.p, c.null_bytemap, n, YTGPU_MEM_HOST));
+        d.nulls = s->nulls.p;
+    }
+    return Status{};
+}
+
 Status groupby_multi_impl(Context* ctx, const ytgpu_column_view* key_columns, u32 key_count, const ytgpu_column_view* value_columns,
                           u32 value_count, const ytgpu_aggregate* aggregates, u32 aggregate_count, const ytgpu_predicate* pred,
-                          int32_t pred_column, u64 hint, ytgpu_groupby_multi_result* out, int out_mem) {
-    if (!key_columns || !out || (aggregate_count && !aggregates) || (value_count && !value_columns))
+                          int32_t pred_column, u64 hint, ytgpu_groupby_multi_result* out, int out_mem,
+                          const ytgpu_string_column* string_columns, u32 string_count) {
+    if (!key_columns || !out || (aggregate_count && !aggregates) || (value_count && !value_columns) || (string_count && !string_columns))
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null argument");
+    // aggregate arguments index value_columns ++ string_columns
+    const u64 columns_total = (u64)value_count + string_count;
+    auto is_string = [&](int32_t c) { return (u32)c >= value_count; };
     if (key_count == 0 || key_count > (u32)kMaxGroupKeys)
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "key column count must be in [1, %d]", kMaxGroupKeys);
     if (aggregate_count > (u32)kMaxAggregates) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "at most %d aggregates", kMaxAggregates);
@@ -474,6 +678,14 @@ Status groupby_multi_impl(Context* ctx, const ytgpu_column_view* key_columns, u3
         if ((u64)key_columns[k].value_count != n) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "key columns differ in length");
     for (u32 v = 0; v < value_count; ++v)
         if ((u64)value_columns[v].value_count != n) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "value column %u differs in length", v);
+    for (u32 s = 0; s < string_count; ++s) {
+        const ytgpu_string_column& S = string_columns[s];
+        if (S.row_count != n) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "string column %u differs in length", s);
+        if ((S.heap_bytes && !S.heap) || !S.starts || !S.lengths)  // an empty heap (all "" / NULL) is never read
+            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "string column %u: null heap, starts or lengths", s);
+        if (S.mem != YTGPU_MEM_DEVICE && S.mem != YTGPU_MEM_HOST)
+            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "string column %u: mem must be YTGPU_MEM_DEVICE or YTGPU_MEM_HOST", s);
+    }
     if (n > (1ull << 30)) return make_status(YTGPU_ERR_UNSUPPORTED, "at most 2^30 rows per call (slots and rows are 32-bit)");
     const int op = pred ? pred->op : YTGPU_CMP_NONE;
     if (op != YTGPU_CMP_NONE && (pred_column < 0 || (u32)pred_column >= value_count))
@@ -481,15 +693,20 @@ Status groupby_multi_impl(Context* ctx, const ytgpu_column_view* key_columns, u3
     for (u32 a = 0; a < aggregate_count; ++a) {
         const ytgpu_aggregate& A = aggregates[a];
         if (A.op < YTGPU_AGG_SUM || A.op > YTGPU_AGG_FIRST) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "aggregate %u: unknown op %d", a, A.op);
-        if (A.column < 0 || (u32)A.column >= value_count) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "aggregate %u: column out of range", a);
-        const u8 t = value_columns[A.column].value_type;
-        if (!aggregatable_type(t)) return make_status(YTGPU_ERR_UNSUPPORTED, "aggregate %u: value type 0x%x is not a fixed-width scalar", a, t);
-        if ((A.op == YTGPU_AGG_SUM || A.op == YTGPU_AGG_AVG) && t == YTGPU_TYPE_BOOLEAN)
-            return make_status(YTGPU_ERR_UNSUPPORTED, "aggregate %u: sum / avg need int64, uint64 or double", a);
+        if (A.column < 0 || (u64)A.column >= columns_total) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "aggregate %u: column out of range", a);
+        if (is_string(A.column)) {
+            if (A.op == YTGPU_AGG_SUM || A.op == YTGPU_AGG_AVG)
+                return make_status(YTGPU_ERR_UNSUPPORTED, "aggregate %u: sum / avg over a string column", a);
+        } else {
+            const u8 t = value_columns[A.column].value_type;
+            if (!aggregatable_type(t)) return make_status(YTGPU_ERR_UNSUPPORTED, "aggregate %u: value type 0x%x is not a fixed-width scalar", a, t);
+            if ((A.op == YTGPU_AGG_SUM || A.op == YTGPU_AGG_AVG) && t == YTGPU_TYPE_BOOLEAN)
+                return make_status(YTGPU_ERR_UNSUPPORTED, "aggregate %u: sum / avg need int64, uint64 or double", a);
+        }
         if (A.op == YTGPU_AGG_ARGMIN || A.op == YTGPU_AGG_ARGMAX) {
-            if (A.by_column < 0 || (u32)A.by_column >= value_count)
+            if (A.by_column < 0 || (u64)A.by_column >= columns_total)
                 return make_status(YTGPU_ERR_INVALID_ARGUMENT, "aggregate %u: by_column out of range", a);
-            if (!aggregatable_type(value_columns[A.by_column].value_type))
+            if (!is_string(A.by_column) && !aggregatable_type(value_columns[A.by_column].value_type))
                 return make_status(YTGPU_ERR_UNSUPPORTED, "aggregate %u: by_column is not a fixed-width scalar", a);
         }
     }
@@ -505,6 +722,8 @@ Status groupby_multi_impl(Context* ctx, const ytgpu_column_view* key_columns, u3
         K.col[k] = sk[k].dev;
     }
     for (u32 v = 0; v < value_count; ++v) YTGPU_TRY(stage_column(ctx, &value_columns[v], &sv[v]));
+    std::vector<StagedStrings> ss(string_count);
+    for (u32 s = 0; s < string_count; ++s) YTGPU_TRY(stage_strings(ctx, string_columns[s], &ss[s]));
     bool keys_direct = true;  // plain 64-bit key vectors: the probe compares with one load per column
     for (u32 k = 0; k < key_count; ++k)
         keys_direct = keys_direct && is_direct64(sk[k].dev) && sk[k].dev.base == 0 && !sk[k].dev.zigzag;
@@ -564,8 +783,35 @@ Status groupby_multi_impl(Context* ctx, const ytgpu_column_view* key_columns, u3
     // step 2
     std::vector<DevBuf<unsigned long long>> acc(aggregate_count), nn(aggregate_count), rows(aggregate_count);
     std::vector<AggState> states(aggregate_count);
+    bool any_strings = false;
     for (u32 a = 0; a < aggregate_count; ++a) {
         const ytgpu_aggregate& A = aggregates[a];
+        const bool arg = A.op == YTGPU_AGG_ARGMIN || A.op == YTGPU_AGG_ARGMAX;
+        if (is_string(A.column) || (arg && is_string(A.by_column))) {
+            // string state: the selected row, or the non-NULL count
+            AggState S{nullptr, nullptr, nullptr};
+            if (A.op == YTGPU_AGG_COUNT) {
+                YTGPU_TRY(nn[a].allocate(ctx, cap));
+                YTGPU_CUDA_TRY(cudaMemsetAsync(nn[a].p, 0, cap * 8, ctx->stream));
+                S.nn = nn[a].p;
+            } else {
+                YTGPU_TRY(rows[a].allocate(ctx, cap));
+                YTGPU_CUDA_TRY(cudaMemsetAsync(rows[a].p, 0xff, cap * 8, ctx->stream));
+                S.row = rows[a].p;
+            }
+            states[a] = S;
+            const bool col_str = is_string(A.column), by_str = arg && is_string(A.by_column);
+            const ColumnDev col = col_str ? ColumnDev{} : sv[A.column].dev;
+            const StringDev cs = col_str ? ss[A.column - value_count].dev : StringDev{};
+            const ColumnDev by = arg && !by_str ? sv[A.by_column].dev : ColumnDev{};
+            const StringDev bs = by_str ? ss[A.by_column - value_count].dev : StringDev{};
+            KernelTimer t(ctx, KC_GROUPBY);
+            mg_accumulate_strings_kernel<<<all_rows_blocks, threads, 0, ctx->stream>>>(A.op, col, cs, by, bs, n, slot_of_row.p, S,
+                                                                                      ctx->dev_err);
+            YTGPU_CUDA_TRY(cudaGetLastError());
+            any_strings = true;
+            continue;
+        }
         const bool select_row = A.op == YTGPU_AGG_ARGMIN || A.op == YTGPU_AGG_ARGMAX || A.op == YTGPU_AGG_FIRST;
         const bool need_acc = A.op != YTGPU_AGG_COUNT && A.op != YTGPU_AGG_FIRST;
         AggState S{nullptr, nullptr, nullptr};
@@ -587,7 +833,6 @@ Status groupby_multi_impl(Context* ctx, const ytgpu_column_view* key_columns, u3
         }
         states[a] = S;
         const ColumnDev col = sv[A.column].dev;
-        const bool arg = A.op == YTGPU_AGG_ARGMIN || A.op == YTGPU_AGG_ARGMAX;
         const ColumnDev by = arg ? sv[A.by_column].dev : ColumnDev{};
         KernelTimer t(ctx, KC_GROUPBY, arg ? 2 : 1);
         const u32 slots = cap <= (u64)kSmemSlots ? (u32)cap : 0xffffffffu;
@@ -600,6 +845,7 @@ Status groupby_multi_impl(Context* ctx, const ytgpu_column_view* key_columns, u3
         if (arg) mg_accumulate_kernel<<<row_blocks, acc_threads, 0, ctx->stream>>>(A.op, 1, col, by, n, slots, slot_of_row.p, S);
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
+    if (any_strings) YTGPU_TRY(check_device_errors(ctx));  // a string that leaves its heap
 
     // step 3
     const u64 max_groups = std::min<u64>(n, cap);
@@ -666,7 +912,9 @@ Status groupby_multi_impl(Context* ctx, const ytgpu_column_view* key_columns, u3
             dn = tvn[a].p;
         }
         const ytgpu_aggregate& A = aggregates[a];
-        mg_finalize_kernel<<<gblocks, threads, 0, ctx->stream>>>(A.op, sv[A.column].dev, 0, g, slot_sorted.p, states[a], dv, dn);
+        const bool row_result = is_string(A.column) && A.op != YTGPU_AGG_COUNT;
+        const ColumnDev col = is_string(A.column) ? ColumnDev{} : sv[A.column].dev;
+        mg_finalize_kernel<<<gblocks, threads, 0, ctx->stream>>>(A.op, col, 0, g, slot_sorted.p, states[a], dv, dn, row_result);
         ctx->count_launch();
         if (host) {
             YTGPU_TRY(copy_out(ctx, out->values[a], dv, g * 8, YTGPU_MEM_HOST));
@@ -694,10 +942,21 @@ int ytgpu_scan_filter_groupby_multi(ytgpu_context* h, const ytgpu_column_view* k
                                     const ytgpu_column_view* value_columns, uint32_t value_count, const ytgpu_aggregate* aggregates,
                                     uint32_t aggregate_count, const ytgpu_predicate* predicate, int32_t predicate_column,
                                     uint64_t group_count_hint, ytgpu_groupby_multi_result* out, int out_mem, ytgpu_error* err) {
+    return ytgpu_scan_filter_groupby_multi_strings(h, key_columns, key_count, value_columns, value_count, aggregates, aggregate_count,
+                                                   predicate, predicate_column, group_count_hint, out, out_mem, nullptr, 0, err);
+}
+
+int ytgpu_scan_filter_groupby_multi_strings(ytgpu_context* h, const ytgpu_column_view* key_columns, uint32_t key_count,
+                                            const ytgpu_column_view* value_columns, uint32_t value_count,
+                                            const ytgpu_aggregate* aggregates, uint32_t aggregate_count,
+                                            const ytgpu_predicate* predicate, int32_t predicate_column, uint64_t group_count_hint,
+                                            ytgpu_groupby_multi_result* out, int out_mem, const ytgpu_string_column* string_columns,
+                                            uint32_t string_count, ytgpu_error* err) {
     if (!h) return fill_error(err, make_status(YTGPU_ERR_INVALID_ARGUMENT, "null context"));
     CtxLock lock(h);
     return fill_error(err, groupby_multi_impl(as_context(h), key_columns, key_count, value_columns, value_count, aggregates,
-                                              aggregate_count, predicate, predicate_column, group_count_hint, out, out_mem));
+                                              aggregate_count, predicate, predicate_column, group_count_hint, out, out_mem,
+                                              string_columns, string_count));
 }
 
 }  // extern "C"

@@ -40,6 +40,27 @@ def _ptr_mem(x):
     return a.ctypes.data, capi.MEM_HOST
 
 
+def _string_column(heap, starts, lengths, nulls=None) -> capi.StringColumn:
+    """ytgpu_string_column over a heap of bytes, 8-byte starts, 4-byte lengths and a 1-byte null map (or None), all numpy
+    arrays or all CUDA tensors."""
+    def check(x, what, size):
+        if _is_tensor(x):
+            ok = x.dim() == 1 and x.element_size() == size and not x.dtype.is_floating_point and x.dtype != torch.bool
+        else:
+            ok = isinstance(x, np.ndarray) and x.ndim == 1 and x.dtype.itemsize == size and x.dtype.kind in "iu"
+        if not ok:
+            raise ValueError(f"string column {what} must be a 1-D array of {size}-byte integers")
+        return _ptr_mem(x)
+    hp, mem = check(heap, "heap", 1)
+    parts = [check(starts, "starts", 8), check(lengths, "lengths", 4)] + ([check(nulls, "nulls", 1)] if nulls is not None else [])
+    if any(m != mem for _, m in parts):
+        raise ValueError("heap, starts, lengths and nulls of a string column must all be host arrays or all device tensors")
+    n = len(starts)
+    if len(lengths) != n or (nulls is not None and len(nulls) != n):
+        raise ValueError("starts, lengths and nulls of a string column differ in length")
+    return capi.StringColumn(hp, len(heap), parts[0][0], parts[1][0], parts[2][0] if nulls is not None else None, n, mem, 0)
+
+
 class GpuContext:
     """One per device/stream; wraps ytgpu_context (explicit, no thread-local state).
 
@@ -729,12 +750,17 @@ class GpuContext:
 
 
     def scan_filter_groupby_multi(self, key_cols, value_cols, aggregates, predicate=None, predicate_column: int = -1,
-                                  group_count_hint: int = 0, capacity: int | None = None):
+                                  group_count_hint: int = 0, capacity: int | None = None, string_columns=()):
         """GROUP BY key tuple with a list of aggregates [(op, column[, by_column])] ->
-        dict(keys=[...], key_null=[...], values=[...], value_null=[...], count, first_row), first-seen order."""
+        dict(keys=[...], key_null=[...], values=[...], value_null=[...], count, first_row), first-seen order.
+        string_columns: (heap, starts, lengths, nulls or None) per column; aggregate column len(value_cols) + i is string
+        column i, and a string-valued result is the index of the row that holds it."""
         kviews = [c.view() for c in key_cols]
         vviews = [c.view() for c in value_cols]
         mem = kviews[0].mem
+        sarr = (capi.StringColumn * max(len(string_columns), 1))()
+        for i, column in enumerate(string_columns):
+            sarr[i] = _string_column(*column)
         n = key_cols[0].value_count
         if capacity is None:
             capacity = max(n, 1)
@@ -760,10 +786,14 @@ class GpuContext:
             op, const = predicate
             pred = capi.Predicate(op, 0, const & 0xFFFFFFFFFFFFFFFF)
         err = capi.Error()
-        capi.check(self.lib.ytgpu_scan_filter_groupby_multi(
-            self.handle, C.cast(karr, C.c_void_p), len(kviews), C.cast(varr, C.c_void_p), len(vviews), C.cast(aggs, C.c_void_p),
-            len(aggregates), C.cast(C.pointer(pred), C.c_void_p) if pred is not None else None, predicate_column,
-            group_count_hint, C.byref(res), mem, C.byref(err)), err)
+        args = [self.handle, C.cast(karr, C.c_void_p), len(kviews), C.cast(varr, C.c_void_p), len(vviews), C.cast(aggs, C.c_void_p),
+                len(aggregates), C.cast(C.pointer(pred), C.c_void_p) if pred is not None else None, predicate_column,
+                group_count_hint, C.byref(res), mem]
+        if string_columns:
+            code = self.lib.ytgpu_scan_filter_groupby_multi_strings(*args, C.cast(sarr, C.c_void_p), len(string_columns), C.byref(err))
+        else:
+            code = self.lib.ytgpu_scan_filter_groupby_multi(*args, C.byref(err))
+        capi.check(code, err)
         g = int(res.group_count)
         return dict(keys=[k[:g] for k in keys], key_null=[k[:g] for k in kn], values=[v[:g] for v in vals],
                     value_null=[v[:g] for v in vn], count=counts[:g], first_row=first[:g])
