@@ -31,9 +31,6 @@ Status gather_rows(Context* ctx, const u8* in_dev, const PermRef& perm, u8* out_
 // chunk[i] = (u64)(u32)index[i]: a partition index array as a radix-sort key chunk.
 Status widen_index(Context* ctx, const i32* index_dev, u64 n, u64* chunk_dev);
 
-// Same with a plain permutation array.
-Status gather_rows_plain(Context* ctx, const u8* in_dev, const u32* perm_dev, u8* out_dev, u64 n, u32 row_bytes);
-
 // The whole fixed-row sort (capi_sort.cu): key extraction -> radix sort -> row gather / permutation.  Used by the
 // C ABI entry point and by the in-box shuffle's local sort.
 Status sort_fixed_rows_impl(Context* ctx, const ytgpu_fixed_rows_view* in, const ytgpu_sort_spec* spec, u8* out_rows,
