@@ -391,18 +391,31 @@ struct PassParams {
     int shift;     // of the digit in the key (pair) or in the packed word (32 + 8 k in the k-th packed pass)
     u32 n;
     u32 prefix_sel, prefix_mask;  // packed: SortPlan::prefix_sel / prefix_mask
+    int copy16;                   // packed: chunk and key buffers are 16-byte aligned (a chunk may start at any word)
 };
 
-template <bool PACKED>
-constexpr size_t kElemBytes = PACKED ? 8 : 12;
+// Element region of a tile's shared memory: packed, the staged input words and the tile-sorted words (TILE each); pair,
+// the tile-sorted keys and row indices (the input keys are held in registers).
+constexpr size_t tile_elem_bytes(int items, bool packed) { return (size_t)kSortThreads * items * (packed ? 2 * 8 : 12); }
+
+// + the warp histograms [WARPS][256], the digit offsets [256], the global bases [256] and 16 words of scratch
+constexpr size_t pass_smem_bytes(int items, bool packed) {
+    return tile_elem_bytes(items, packed) + (size_t)(kSortThreads / 32) * kRadix * 4 + 2 * kRadix * 4 + 16 * 4;
+}
+
+__device__ __forceinline__ void cp_async_u64(u64* dst, const u64* src) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" :: "r"((u32)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 template <int THREADS, int ITEMS, bool FULL, bool PACKED>
 __device__ __forceinline__ void onesweep_tile(const PassParams& P, const PassDesc pd, const u32 tile, unsigned char* smem_raw) {
     constexpr int WARPS = THREADS / 32;
     constexpr int TILE = THREADS * ITEMS;
-    u64* s_keys = reinterpret_cast<u64*>(smem_raw);                      // TILE keys / packed words
-    u32* s_vals = reinterpret_cast<u32*>(smem_raw + (size_t)TILE * 8);   // TILE row indices (pair format)
-    u32* s_hist = reinterpret_cast<u32*>(smem_raw + (size_t)TILE * kElemBytes<PACKED>);  // [WARPS][256]
+    u64* s_in = reinterpret_cast<u64*>(smem_raw);                         // packed: TILE words as loaded (warp-striped)
+    u64* s_keys = PACKED ? s_in + TILE : reinterpret_cast<u64*>(smem_raw);  // TILE keys / packed words, tile-sorted
+    u32* s_vals = reinterpret_cast<u32*>(smem_raw + (size_t)TILE * 8);      // pair: TILE row indices, tile-sorted
+    u32* s_hist = reinterpret_cast<u32*>(smem_raw + tile_elem_bytes(ITEMS, PACKED));  // [WARPS][256]
     u32* s_excl = s_hist + WARPS * kRadix;                      // [256]
     u32* s_gbase = s_excl + kRadix;                             // [256]
     u32* s_misc = s_gbase + kRadix;                             // [0..7] warp totals, [8] tile id
@@ -426,10 +439,37 @@ __device__ __forceinline__ void onesweep_tile(const PassParams& P, const PassDes
             asm volatile("prefetch.global.L2 [%0];" :: "l"(ibase + off));
     }
 
-    // ---- load keys, warp-striped: item i of lane l sits at warp_base + i*32 + l ----
-    const u32 wbase = base + warp * (32 * ITEMS) + lane;
-    u64 key[ITEMS];
-    if (!PACKED && pd.src_kind == 1) {
+    // ---- load the tile, warp-striped: item i of lane l is element warp_slot + i*32 + l of the tile ----
+    // Packed: the words are staged in shared memory with cp.async.  Kept there until they are written out instead of
+    // occupying 2 registers per item, they free the registers for more items per tile.  Each warp copies its own slice,
+    // so the cp.async.wait_all and __syncwarp below are all the synchronisation the copies need.  16-byte copies that
+    // bypass L1 take the packed pass from 0.96 to 0.89 ms (16 items at 3 CTAs per SM) against 8-byte copies through L1;
+    // the 8-byte copies remain for buffers that are not 16-byte aligned.  Pair: the keys are loaded into registers
+    // (staging keys and row indices with 8- and 4-byte copies measured slower: 1.32 vs 1.29 ms per pass).
+    const u32 wslot = warp * (32 * ITEMS) + lane;
+    const u32 wbase = base + wslot;
+    u64 key[PACKED ? 1 : ITEMS];
+    if constexpr (PACKED) {
+        static_assert(ITEMS % 2 == 0, "16-byte copies of 8-byte words");
+        if (P.copy16) {
+            // the warp's slice of the tile is contiguous: 16-byte copies that bypass L1, lane l copies bytes 16 (l + 32 k)
+            const u32 wfirst = base + warp * (32 * ITEMS);
+            u64* sdst = s_in + warp * (32 * ITEMS);
+#pragma unroll
+            for (int k = 0; k < ITEMS / 2; ++k) {
+                const u32 e = 2 * (lane + 32 * k);
+                if (FULL || wfirst + e < P.n) {
+                    const u32 bytes = (FULL || wfirst + e + 1 < P.n) ? 16 : 8;
+                    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" :: "r"((u32)__cvta_generic_to_shared(sdst + e)),
+                                 "l"(kin + wfirst + e), "r"(bytes) : "memory");
+                }
+            }
+        } else {
+#pragma unroll
+            for (int i = 0; i < ITEMS; ++i)
+                if (FULL || wbase + i * 32 < P.n) cp_async_u64(s_in + wslot + i * 32, kin + wbase + i * 32);
+        }
+    } else if (pd.src_kind == 1) {
         u32 src[ITEMS];
 #pragma unroll
         for (int i = 0; i < ITEMS; ++i) {
@@ -447,44 +487,82 @@ __device__ __forceinline__ void onesweep_tile(const PassParams& P, const PassDes
             u32 pos = wbase + i * 32;
             key[i] = (FULL || pos < P.n) ? ld_stream_u64(kin + pos) : ~0ull;
         }
-        if (PACKED && pd.src_kind == 0) {  // key -> (prefix << 32) | row index
-#pragma unroll
-            for (int i = 0; i < ITEMS; ++i) {
-                const u32 pref = __byte_perm((u32)key[i], (u32)(key[i] >> 32), P.prefix_sel) & P.prefix_mask;
-                key[i] = ((u64)pref << 32) | (wbase + i * 32);
-            }
-        }
     }
+    // the warp's private histogram is cleared while the loads are in flight
+    u32* wh = s_hist + warp * kRadix;
+    reinterpret_cast<uint4*>(wh)[lane] = make_uint4(0, 0, 0, 0);
+    reinterpret_cast<uint4*>(wh)[lane + 32] = make_uint4(0, 0, 0, 0);
+    // Element i of this lane.  The first packed pass builds the word (prefix << 32) | row index from the chunk's key.
+    // Packed items past the end of a partial tile read stale words: they are masked out of the ranking and never written.
+    auto elem = [&](int i) -> u64 {
+        if constexpr (PACKED) {
+            const u64 v = s_in[wslot + i * 32];
+            if (pd.src_kind != 0) return v;
+            const u32 pref = __byte_perm((u32)v, (u32)(v >> 32), P.prefix_sel) & P.prefix_mask;
+            return ((u64)pref << 32) | (wbase + i * 32);
+        } else {
+            return key[i];
+        }
+    };
+    if (PACKED) cp_async_wait_all();
+    __syncwarp();  // every lane's copies and histogram clear
 
     // ---- rank inside the warp: stable (item-major, then lane) ----
     // Peers with the same digit are found with 8 ballots (one per digit bit).  MATCH.ANY is NOT used:
     // its cost grows with the number of distinct values in the warp, and random 8-bit digits have
-    // many; the ballots cost the same on any data.  The running per-digit counts of the
-    // warp live in its private shared histogram: every lane reads its bin (same-digit lanes broadcast),
-    // the lowest lane of each digit group writes the bumped count back.
-    u32 rank[ITEMS];
-    u32* wh = s_hist + warp * kRadix;
+    // many; the ballots cost the same on any data.  The running per-digit counts of the warp live in its
+    // private shared histogram.
+    u32 m[ITEMS];  // peer mask, then rank inside the warp
     const u32 lt = lanemask_lt();
-#pragma unroll
-    for (int i = 0; i < ITEMS; ++i) {
-        const u32 d = (u32)(key[i] >> shift) & 0xff;
-        u32 m = 0xffffffffu;
+    auto peers = [&](u32 d, int i) -> u32 {
+        u32 mm = 0xffffffffu;
 #pragma unroll
         for (int b = 0; b < kRadixBits; ++b) {
             const bool bit = (d >> b) & 1;
             const u32 v = __ballot_sync(0xffffffffu, bit);
-            m &= bit ? v : ~v;
+            mm &= bit ? v : ~v;
         }
-        bool valid = true;
-        if (!FULL) {
-            valid = wbase + i * 32 < P.n;
-            m &= __ballot_sync(0xffffffffu, valid);
+        if (!FULL) mm &= __ballot_sync(0xffffffffu, wbase + i * 32 < P.n);
+        return mm;
+    };
+    if constexpr (PACKED) {
+        // Every item's peer mask is computed first (the ballots of different items are independent).  Then the lowest
+        // lane of each digit group adds the group's size to the bin with one shared atomic, and the group reads the old
+        // count from it with a shuffle, so no item waits for the previous item's load-store round trip.
+        u32 dig[(ITEMS + 3) / 4] = {};  // the items' digits, four per word
+#pragma unroll
+        for (int i = 0; i < ITEMS; ++i) {
+            const u32 d = (u32)(elem(i) >> shift) & 0xff;
+            dig[i / 4] |= d << (8 * (i % 4));
+            m[i] = peers(d, i);
         }
-        const u32 prev = wh[d];
-        __syncwarp();
-        if (valid && (m & lt) == 0) wh[d] = prev + __popc(m);
-        rank[i] = prev + __popc(m & lt);
-        __syncwarp();
+        u32 prev[ITEMS];
+#pragma unroll
+        for (int i = 0; i < ITEMS; ++i) {
+            const u32 d = (dig[i / 4] >> (8 * (i % 4))) & 0xff;
+            prev[i] = 0;
+            if ((FULL || wbase + i * 32 < P.n) && (m[i] & lt) == 0) prev[i] = atomicAdd(&wh[d], (u32)__popc(m[i]));
+            // The leaders of consecutive items are different lanes, and only this barrier orders their shared accesses
+            // (PTX memory model): without it item i+1's add to a bin could be performed before item i's, and equal
+            // digits would no longer be ranked item-major, i.e. the sort would lose its stability.
+            __syncwarp();
+        }
+#pragma unroll
+        for (int i = 0; i < ITEMS; ++i) m[i] = __shfl_sync(0xffffffffu, prev[i], __ffs(m[i]) - 1) + __popc(m[i] & lt);
+    } else {
+        // Pair format (keys in registers): every lane reads its bin (same-digit lanes broadcast), the lowest lane of each
+        // digit group writes the bumped count back.  The shared atomics above measured slower here (1.304 vs 1.297 ms
+        // per pass of the composite workload).
+#pragma unroll
+        for (int i = 0; i < ITEMS; ++i) {
+            const u32 d = (u32)(key[i] >> shift) & 0xff;
+            const u32 mm = peers(d, i);
+            const u32 prev = wh[d];
+            __syncwarp();
+            if ((FULL || wbase + i * 32 < P.n) && (mm & lt) == 0) wh[d] = prev + __popc(mm);
+            m[i] = prev + __popc(mm & lt);
+            __syncwarp();
+        }
     }
     __syncthreads();
 
@@ -512,6 +590,7 @@ __device__ __forceinline__ void onesweep_tile(const PassParams& P, const PassDes
     // status word costs an L2 round trip, so a tile typically has to add the partial counts of ~10
     // predecessors.  Instead of spinning, one status load is kept in flight while the keys and row
     // indices are scattered into shared memory; whatever is left is finished by the loop after them.
+    // (Loading the words of 4 predecessors at a time measured slower: 1.00 vs 0.94 ms per packed pass.)
     u32 lb_excl = 0;
     i32 lb_tile = (i32)tile - 1;
     bool lb_done = tile == 0;
@@ -530,14 +609,17 @@ __device__ __forceinline__ void onesweep_tile(const PassParams& P, const PassDes
         }
     };
 
-    // ---- keys and row indices -> shared memory in tile-sorted order ----
+    // ---- keys and row indices -> shared memory in tile-sorted order (the row index of a packed word travels inside it) ----
 #pragma unroll
     for (int i = 0; i < ITEMS; ++i) {
         if ((i & 3) == 0) lb_issue();
-        const u32 d = (u32)(key[i] >> shift) & 0xff;
-        const u32 lp = wh[d] + rank[i];
-        rank[i] = lp;
-        if (FULL || (wbase + i * 32 < P.n)) s_keys[lp] = key[i];
+        const u32 pos = wbase + i * 32;
+        if (FULL || pos < P.n) {
+            const u64 w = elem(i);
+            const u32 lp = wh[(u32)(w >> shift) & 0xff] + m[i];
+            m[i] = lp;
+            s_keys[lp] = w;
+        }
         if ((i & 3) == 3) lb_consume();
     }
     if (PACKED) {
@@ -547,7 +629,7 @@ __device__ __forceinline__ void onesweep_tile(const PassParams& P, const PassDes
         for (int i = 0; i < ITEMS; ++i) {
             if ((i & 3) == 0) lb_issue();
             const u32 pos = wbase + i * 32;
-            if (FULL || pos < P.n) s_vals[rank[i]] = pos;
+            if (FULL || pos < P.n) s_vals[m[i]] = pos;
             if ((i & 3) == 3) lb_consume();
         }
     } else {
@@ -564,7 +646,7 @@ __device__ __forceinline__ void onesweep_tile(const PassParams& P, const PassDes
 #pragma unroll
             for (int i = 0; i < VB; ++i) {
                 const u32 pos = wbase + (b0 + i) * 32;
-                if (FULL || pos < P.n) s_vals[rank[b0 + i]] = v[i];
+                if (FULL || pos < P.n) s_vals[m[b0 + i]] = v[i];
             }
             lb_consume();
         }
@@ -603,8 +685,7 @@ __global__ void __launch_bounds__(THREADS, MINB) onesweep_pass_kernel(const Pass
     constexpr int TILE = THREADS * ITEMS;
     static_assert(THREADS == 256, "digit phase assumes one thread per bin");
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    u32* s_hist = reinterpret_cast<u32*>(smem_raw + (size_t)TILE * kElemBytes<PACKED>);
-    u32* s_misc = s_hist + WARPS * kRadix + 2 * kRadix;
+    u32* s_misc = reinterpret_cast<u32*>(smem_raw + tile_elem_bytes(ITEMS, PACKED)) + WARPS * kRadix + 2 * kRadix;
 
     if (P.schedule == 1 && !P.plan->fallback) return;
     const PassDesc pd = P.schedule == 1 ? P.plan->pass_b[P.plan_index] : P.plan->pass[P.plan_index];
@@ -619,8 +700,6 @@ __global__ void __launch_bounds__(THREADS, MINB) onesweep_pass_kernel(const Pass
     const bool persistent = gridDim.x < tiles;
     for (;;) {
         if (threadIdx.x == 0) s_misc[8] = atomicAdd(P.counter, 1u);
-#pragma unroll
-        for (int i = threadIdx.x; i < WARPS * kRadix; i += THREADS) s_hist[i] = 0;
         __syncthreads();
         const u32 tile = s_misc[8];
         if (tile >= tiles) break;
@@ -636,17 +715,18 @@ __global__ void materialize_perm_kernel(const SortPlan* plan, const u32* a, cons
         dst[i] = perm_at(plan, a, b, i);
 }
 
-constexpr size_t pass_smem_bytes(int items, bool packed) {
-    return (size_t)kSortThreads * items * (packed ? kElemBytes<true> : kElemBytes<false>) + (size_t)(kSortThreads / 32) * kRadix * 4 +
-           2 * kRadix * 4 + 16 * 4;
-}
-
 // Tuning variants of the pass kernel (items per thread, min resident CTAs per SM), one table per element format;
 // YTGPU_SORT_VARIANT / YTGPU_SORT_PACKED_VARIANT select one for experiments.  The defaults are the fastest measured on
 // an H100 SXM at a 700 W power limit.  Pair format (15.3 vs 18.0 ms per 10^8-row sort for 16 items at 3 CTAs per SM):
 // 2 CTAs per SM keep 128 registers without spills, where 3 CTAs per SM (80 registers) spill to local memory.  Packed
 // format (mean pass launch over a 10^8-row sort, 4 packed passes): 16 items at 2 CTAs per SM 0.95 ms, 125 registers, no
 // spills; 10 at 3 (80 registers, no spills) 1.05 ms; 12 at 3 (12 B spilled) 0.98 ms; 8 at 4 (16 B spilled) 1.16 ms.
+// With the packed tile staged in shared memory and ranked by shared atomics (H100 80GB HBM3, 400 W power limit; the
+// register-held kernel's 16 items at 2 CTAs: 0.98-0.99 ms on that card).  8-byte copies through L1: 16 items at 3 CTAs
+// per SM 0.94-0.96 ms (80 registers, 74 KB of shared memory); 16 at 2 1.03 ms (127 registers); 12 at 3 1.01 ms (80
+// registers); 8 at 4 1.18 ms (64 registers); 24 at 2 0.95 ms.  16-byte copies bypassing L1: 24 items at 2 CTAs per SM
+// 0.87-0.89 ms (128 registers, 106 KB of shared memory); 16 at 3 0.89-0.90 ms (80 registers); 20 at 2 0.93 ms (128
+// registers).  None of them spills.
 struct PassVariant {
     int items;
     int ctas_per_sm;
@@ -657,12 +737,10 @@ struct PassVariant {
 #define YTGPU_PASS_VARIANT(items, ctas, packed) \
     { items, ctas, pass_smem_bytes(items, packed), onesweep_pass_kernel<kSortThreads, items, ctas, packed> }
 const PassVariant kVariants[] = {
-    YTGPU_PASS_VARIANT(16, 2, false), YTGPU_PASS_VARIANT(16, 3, false), YTGPU_PASS_VARIANT(12, 3, false),
-    YTGPU_PASS_VARIANT(8, 4, false),  YTGPU_PASS_VARIANT(12, 4, false), YTGPU_PASS_VARIANT(20, 2, false),
+    YTGPU_PASS_VARIANT(16, 2, false),
 };
 const PassVariant kPackedVariants[] = {
-    YTGPU_PASS_VARIANT(16, 2, true), YTGPU_PASS_VARIANT(10, 3, true), YTGPU_PASS_VARIANT(12, 3, true),
-    YTGPU_PASS_VARIANT(8, 4, true),
+    YTGPU_PASS_VARIANT(24, 2, true),
 };
 #undef YTGPU_PASS_VARIANT
 constexpr int kDefaultVariant = 0;
@@ -799,6 +877,7 @@ Status radix_sort_chunks(Context* ctx, const u64* const* chunks, int nchunks, u6
         P.n = (u32)n;
         P.prefix_sel = hp.prefix_sel;
         P.prefix_mask = hp.prefix_mask;
+        P.copy16 = (((uintptr_t)chunk | (uintptr_t)P.keys[0] | (uintptr_t)P.keys[1]) & 15) == 0;
         v.kernel<<<v.tiles(n), kSortThreads, v.smem, st>>>(P);
     };
     SortPlan hp{};  // host copy of the plan (read_plan only)
