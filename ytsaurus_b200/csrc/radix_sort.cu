@@ -103,13 +103,19 @@ __global__ void __launch_bounds__(256) plan_kernel(u32* hist, int nchunks, u32 n
                                                    int allow_packed) {
     __shared__ u32 s_warp_tot[8];
     __shared__ u8 s_active[kMaxKeyChunks * kPassesPerChunk];
+    __shared__ u8 s_skewed[kPassesPerChunk];
     const int total = nchunks * kPassesPerChunk;
     for (int rp = 0; rp < total; ++rp) {
         u32 c = hist[rp * kRadix + threadIdx.x];
         int full = __syncthreads_or(c == n);
+        // a bin with more than twice its uniform share: > 2 n / 256 rows (see the three-pass schedule below)
+        const int skewed = nchunks == 1 ? __syncthreads_or(c > (n >> 7)) : 0;
         u32 ex = block_exclusive_scan_256(c, s_warp_tot);
         hist[rp * kRadix + threadIdx.x] = ex;
-        if (threadIdx.x == 0) s_active[rp] = !full;
+        if (threadIdx.x == 0) {
+            s_active[rp] = !full;
+            if (nchunks == 1) s_skewed[rp] = (u8)skewed;
+        }
     }
     __syncthreads();
     if (threadIdx.x != 0) return;
@@ -119,7 +125,7 @@ __global__ void __launch_bounds__(256) plan_kernel(u32* hist, int nchunks, u32 n
     plan->final_idx_b = 2;
     plan->active_passes_b = 0;
     plan->final_key = plan->final_key_b = 2;
-    plan->packed = plan->prefix_sel = plan->prefix_mask = 0;
+    plan->packed = plan->prefix_sel = plan->prefix_mask = plan->run_shift = 0;
     u32 final_key = 2;
     if (nchunks == 1) {
         int act[kPassesPerChunk], m = 0;
@@ -134,13 +140,21 @@ __global__ void __launch_bounds__(256) plan_kernel(u32* hist, int nchunks, u32 n
         const int* sched = hybrid ? act + (m - need) : act;  // scheduled digits, least significant first
         const int t = hybrid ? need : m;
         const bool packed = allow_packed && t >= 1 && t <= 4;
+        // Three of four: prefix byte 0 is in every packed word already, so the passes sort bytes 1-3 only and
+        // tie_fix_runs_kernel orders each run of equal 24-bit prefixes by the whole prefix (and the full key where
+        // prefixes tie).  n <= 2^27 keeps the mean run at <= 8 rows.  A sorted digit with a bin of more than twice its
+        // uniform share means clustered keys, whose long runs would mix different keys: those keep the fourth pass.
+        // (For uniform keys the largest of 256 bins of >= 2^20 rows is within a few percent of n / 256.)
+        bool skip_byte0 = hybrid && packed && need == 4 && n <= (1u << 27);
+        for (int k = 1; k < need && skip_byte0; ++k) skip_byte0 = !s_skewed[sched[k]];
+        const int skip = skip_byte0 ? 1 : 0;
         if (hybrid) {
-            build_schedule(plan->pass, sched, need, packed, &plan->final_idx, &final_key);
+            build_schedule(plan->pass, sched + skip, need - skip, packed, &plan->final_idx, &final_key);
             build_schedule(plan->pass_b, act, m, !keep_keys, &plan->final_idx_b, &plan->final_key_b);
             plan->hybrid = 1;
             plan->hybrid_shift = 8u * (u32)sched[0];
             plan->final_key_a = plan->pass[act[m - 1]].key_dst;
-            plan->active_passes = (u32)need;
+            plan->active_passes = (u32)(need - skip);
             plan->active_passes_b = (u32)m;
         } else {
             build_schedule(plan->pass, act, m, !keep_keys, &plan->final_idx, &plan->final_key);
@@ -154,6 +168,7 @@ __global__ void __launch_bounds__(256) plan_kernel(u32* hist, int nchunks, u32 n
             plan->prefix_sel = sel;
             plan->prefix_mask = t == 4 ? 0xffffffffu : (1u << (8 * t)) - 1;
             plan->pass[sched[t - 1]].write_prefix = hybrid ? 1 : 0;
+            plan->run_shift = 8u * (u32)skip;
         }
         return;
     }
@@ -208,7 +223,7 @@ struct HybridSummary {
 };
 
 // Sorted words the hybrid tail reads: the prefix-sorted keys (pair format; prefix = word >> hybrid_shift) or the u32
-// prefixes the last packed pass wrote (prefix = word).  Full keys: the word itself, or chunk[idx[j]].
+// prefixes the last packed pass wrote (prefix = word >> run_shift).  Full keys: the word itself, or chunk[idx[j]].
 template <bool PACKED>
 struct TailWords {
     const u64* keys;
@@ -217,7 +232,7 @@ struct TailWords {
     __device__ __forceinline__ TailWords(const SortPlan* plan, const u64* keys0, const u64* keys1, const u32* idx0, const u32* idx1) {
         keys = plan->final_key_a ? keys1 : keys0;
         pre = plan->final_idx ? idx0 : idx1;
-        shift = PACKED ? 0 : plan->hybrid_shift;
+        shift = PACKED ? plan->run_shift : plan->hybrid_shift;
     }
     __device__ __forceinline__ u64 operator[](u32 j) const { return PACKED ? (u64)pre[j] : keys[j]; }
 };
@@ -282,6 +297,171 @@ __global__ void __launch_bounds__(256) tie_fix_kernel(SortPlan* plan, const u64*
             }
             idx[i + b] = v;
         }
+    }
+}
+
+// Hybrid tail of the packed three-pass schedule (run_shift == 8).  The passes sorted prefix bytes 1-3 only, so nearly
+// every row sits in a run of equal 24-bit prefixes (n / 2^24 rows on average), still in input order.  A block owns the
+// runs that START in its tile of kRunTile positions and stages the prefixes and row indices of the tile, with 32
+// positions more on each side (a short run has at most kMaxTieRun rows), in shared memory.  Each warp walks the runs
+// that start in its eighth of the tile in windows of up to 32 positions that end where a run ends, and ranks every row
+// inside its run by (prefix byte 0, position) with 8 ballots, one per bit of the byte: that rank is its slot.  Rows whose
+// whole prefixes are equal get adjacent slots, and only they read their full keys chunk[idx] to be ordered (stable
+// insertion sort per group).  The row indices are read once and written back once, coalesced, per tile.  Long runs are
+// left as they are, registered by their first row and marked where a row's key differs from its left neighbour's, as
+// tie_fix_kernel does.  Only positions of short runs owned by a block are written, and a long run is never written, so
+// blocks that read their neighbours' positions (halos) see either a value they ignore or a final one.
+constexpr int kRunTile = 1984;                 // positions owned by a block (a multiple of 32 and of 8)
+constexpr int kRunSpan = kRunTile + 64;        // staged: local position l is global position tile * kRunTile - 32 + l
+constexpr int kRunWords = kRunSpan / 32;
+constexpr int kRunItems = kRunSpan / 256;
+constexpr u32 kNoSlot = 0xffffffffu;
+
+__global__ void __launch_bounds__(256) tie_fix_runs_kernel(const u64* __restrict__ chunk, const u32* __restrict__ pre, u32* idx,
+                                                           u32 n, u32* __restrict__ mixedmask, u32* __restrict__ longlist,
+                                                           HybridSummary* sum) {
+    __shared__ u32 s_comp[kRunSpan];      // (prefix << 24) | l: prefix byte 0 on top
+    __shared__ u32 s_idx[kRunSpan];       // row indices in position order
+    __shared__ u32 s_out[kRunSpan];       // the staged prefixes; then row indices in slot order, kNoSlot: not written
+    __shared__ u32 s_head[kRunWords];     // bit l: position l starts a run (positions outside [0, n) are runs of one)
+    __shared__ u32 s_ties[kRunSpan / 2];  // groups of equal prefixes: first slot | length << 16
+    __shared__ u32 s_nties, s_long;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int base = (int)blockIdx.x * kRunTile - 32;  // n < 2^30
+    if (tid == 0) s_nties = s_long = 0;
+    {
+        u32 p[kRunItems], x[kRunItems];
+#pragma unroll
+        for (int it = 0; it < kRunItems; ++it) {
+            const int g = base + it * 256 + tid;
+            const bool in = g >= 0 && g < (int)n;
+            p[it] = in ? pre[g] : 0;
+            x[it] = in ? idx[g] : 0;
+        }
+#pragma unroll
+        for (int it = 0; it < kRunItems; ++it) {
+            s_out[it * 256 + tid] = p[it];
+            s_idx[it * 256 + tid] = x[it];
+        }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int it = 0; it < kRunItems; ++it) {
+        const int l = it * 256 + tid, g = base + l;
+        const u32 p = s_out[l];
+        // Local position 0 counts as a head: a run through it that reaches position 32 or later has > 32 rows anyway.
+        const bool head = l == 0 || g <= 0 || g >= (int)n || ((p ^ s_out[l - 1]) >> 8) != 0;
+        const u32 hb = __ballot_sync(0xffffffffu, head);
+        if (lane == 0) s_head[l >> 5] = hb;
+        s_comp[l] = (p << 24) | l;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int it = 0; it < kRunItems; ++it) s_out[it * 256 + tid] = kNoSlot;
+    // first head at or after local position x (kRunSpan if none)
+    auto next_head = [&](int x) -> int {
+        if (x >= kRunSpan) return kRunSpan;
+        int w = x >> 5;
+        u32 m = s_head[w] & (0xffffffffu << (x & 31));
+        while (m == 0) {
+            if (++w == kRunWords) return kRunSpan;
+            m = s_head[w];
+        }
+        return w * 32 + __ffs(m) - 1;
+    };
+    if (tid == 0 && next_head(33) - (31 - __clz(s_head[0])) > kMaxTieRun && !(s_head[1] & 1))
+        s_long = 1;  // the run through position 32 started in the previous tile and is long
+    __syncthreads();
+
+    const u32 lt_mask = lanemask_lt();
+    {
+        const int rs = 32 + warp * (kRunTile / 8), re = rs + kRunTile / 8;
+        int ws = next_head(rs);
+        while (ws < re) {  // warp-uniform: ws is a head
+            // heads at positions ws .. ws + 32 (bit 0: ws itself)
+            const u64 win = ((((u64)s_head[(ws >> 5) + 1] << 32) | s_head[ws >> 5]) >> (ws & 31)) & ((2ull << 32) - 1);
+            const u64 later = win & ~1ull;
+            if (later == 0) {  // a run of more than kMaxTieRun rows: left to classify_long_runs_kernel
+                if (lane == 0) s_long = 1;
+                ws = next_head(ws + kMaxTieRun + 1);
+                continue;
+            }
+            // the window ends at its last head, or at the first head of the next warp's runs
+            int len = 63 - __clzll(later);
+            if (re - ws <= kMaxTieRun) {
+                const u64 beyond = later >> (re - ws);
+                if (beyond) len = re - ws + __ffsll(beyond) - 1;
+            }
+            const u32 hb = (u32)win;
+            const bool act = lane < len;
+            const u32 c = act ? s_comp[ws + lane] : 0;
+            const int start = 31 - __clz(hb & (0xffffffffu >> (31 - lane)));
+            const u32 after = hb & (0xfffffffeu << lane);
+            const int end = after ? __ffs(after) - 1 : 32;
+            // rank inside the run [start, end) by byte 0, MSB first, then by position
+            u32 lt = 0, eq = (0xffffffffu >> (32 - end)) & (0xffffffffu << start);
+#pragma unroll
+            for (int b = 7; b >= 0; --b) {
+                const bool bit = (c >> (24 + b)) & 1;
+                const u32 v = __ballot_sync(0xffffffffu, bit);
+                if (bit) {
+                    lt |= eq & ~v;
+                    eq &= v;
+                } else {
+                    eq &= ~v;
+                }
+            }
+            if (act && end - start >= 2) {
+                const int first = ws + start + __popc(lt);  // slot of the first row with this prefix
+                s_out[first + __popc(eq & lt_mask)] = s_idx[ws + lane];
+                if (__popc(eq) > 1 && (eq & lt_mask) == 0) s_ties[atomicAdd(&s_nties, 1u)] = (u32)first | ((u32)__popc(eq) << 16);
+            }
+            ws += len;
+        }
+    }
+    __syncthreads();
+
+    // equal prefixes: stable insertion sort by the full key
+    for (u32 t = tid; t < s_nties; t += 256) {
+        const u32 q = s_ties[t] & 0xffff, e = q + (s_ties[t] >> 16);
+        for (u32 a = q + 1; a < e; ++a) {
+            const u32 x = s_out[a];
+            const u64 k = chunk[x];
+            u32 b = a;
+            while (b > q && chunk[s_out[b - 1]] > k) {
+                s_out[b] = s_out[b - 1];
+                --b;
+            }
+            s_out[b] = x;
+        }
+    }
+    if (s_long) {
+        // Long runs: register each by its first row, and mark every position whose key differs from its left
+        // neighbour's.  A position's run [ph, nh) comes from the head bits of its word and the two around it.
+#pragma unroll 1
+        for (int it = 0; it < kRunItems; ++it) {
+            const int l = it * 256 + tid, w = l >> 5, g = base + l;
+            if (w == 0 || l >= 32 + kRunTile) continue;  // warp-uniform
+            const u64 below = (((u64)s_head[w] << 32) | s_head[w - 1]) & (~0ull >> (31 - lane));
+            const u64 above = (((u64)s_head[w + 1] << 32) | s_head[w]) & (~0ull << (lane + 1));
+            const int ph = w * 32 - 32 + 63 - __clzll(below), nh = w * 32 + __ffsll(above) - 1;
+            const bool is_long = below == 0 || above == 0 || nh - ph > kMaxTieRun;
+            const bool head = (s_head[w] >> lane) & 1;
+            if (head && is_long && g < (int)n) longlist[atomicAdd(&sum->long_count, 1u)] = (u32)g;
+            const bool differs = !head && is_long && g < (int)n &&
+                                 (((s_comp[l] ^ s_comp[l - 1]) >> 24) != 0 || chunk[s_idx[l]] != chunk[s_idx[l - 1]]);
+            const u32 mixed = __ballot_sync(0xffffffffu, differs);
+            if (lane == 0 && g < (int)n) mixedmask[g >> 5] = mixed;
+        }
+    } else if (tid < kRunTile / 32) {
+        const int g = base + 32 + tid * 32;
+        if (g < (int)n) mixedmask[g >> 5] = 0;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int it = 0; it < kRunItems; ++it) {
+        const int q = it * 256 + tid;
+        if (s_out[q] != kNoSlot) idx[base + q] = s_out[q];
     }
 }
 
@@ -890,8 +1070,9 @@ Status radix_sort_chunks(Context* ctx, const u64* const* chunks, int nchunks, u6
         int k = 0;
         for (int p = 0; p < kPassesPerChunk; ++p) {
             if (!hp.pass[p].active) continue;
-            // packed: the k-th pass sorts by prefix byte k, i.e. bits 32 + 8k of the word
-            launch_pass(hp.packed ? *pk : *pv, chunks[0], 0, p, k, p, hp.packed ? 32 + k * kRadixBits : p * kRadixBits, hp);
+            // packed: the k-th pass sorts by prefix byte k, or k + 1 when byte 0 is left to the tail (run_shift == 8)
+            const int shift = hp.packed ? 32 + (int)hp.run_shift + k * kRadixBits : p * kRadixBits;
+            launch_pass(hp.packed ? *pk : *pv, chunks[0], 0, p, k, p, shift, hp);
             ++k;
         }
     } else {
@@ -914,10 +1095,18 @@ Status radix_sort_chunks(Context* ctx, const u64* const* chunks, int nchunks, u6
         {
             KernelTimer t(ctx, KC_HISTOGRAM, 2);
             const u32 blocks = (u32)std::min<u64>((n + 255) / 256, (u64)kNumSms * 8);
-            auto tie_fix = hp.packed ? tie_fix_kernel<true> : tie_fix_kernel<false>;
             auto classify = hp.packed ? classify_long_runs_kernel<true> : classify_long_runs_kernel<false>;
-            tie_fix<<<blocks, 256, 0, st>>>(s->plan.p, chunks[0], s->keys[0].p, s->keys[1].p, s->idx[0].p, s->idx[1].p, (u32)n, mixedmask.p,
-                                            longlist.p, summary.p);
+            if (hp.run_shift) {
+                // the prefixes are in the permutation buffer the last pass did not write
+                u32* idx = s->idx[hp.final_idx].p;
+                const u32* pre = s->idx[hp.final_idx ^ 1].p;
+                tie_fix_runs_kernel<<<(u32)((n + kRunTile - 1) / kRunTile), 256, 0, st>>>(chunks[0], pre, idx, (u32)n, mixedmask.p,
+                                                                                         longlist.p, summary.p);
+            } else {
+                auto tie_fix = hp.packed ? tie_fix_kernel<true> : tie_fix_kernel<false>;
+                tie_fix<<<blocks, 256, 0, st>>>(s->plan.p, chunks[0], s->keys[0].p, s->keys[1].p, s->idx[0].p, s->idx[1].p, (u32)n,
+                                                mixedmask.p, longlist.p, summary.p);
+            }
             classify<<<kNumSms * 4, 256, 0, st>>>(s->plan.p, s->keys[0].p, s->keys[1].p, s->idx[0].p, s->idx[1].p, (u32)n, mixedmask.p,
                                                   longlist.p, summary.p, mixedlist.p);
         }

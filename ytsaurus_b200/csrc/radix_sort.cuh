@@ -51,11 +51,14 @@ struct SortPlan {
     u32 final_key_b;    // ... of schedule `pass_b`
     // Packed format (single-chunk sorts of >= 2^18 rows whose scheduled digits fit in 32 bits, not keep_keys): the
     // passes of `pass` move one u64 per row, (prefix << 32) | row index, where prefix byte k is the key digit of the k-th
-    // scheduled pass (least significant first).  The last pass writes the row indices to idx[final_idx] and, for the
+    // scheduled digit (least significant first).  The last pass writes the row indices to idx[final_idx] and, for the
     // hybrid schedule, the prefixes to idx[final_idx ^ 1].
     u32 packed;
     u32 prefix_sel;   // __byte_perm selector over the key's two halves: nibble k = key digit of prefix byte k
     u32 prefix_mask;  // prefix bytes in use
+    // Packed hybrid schedule: 8 when the passes sort prefix bytes 1-3 only and leave byte 0 to the hybrid tail, else 0.
+    // Rows with equal (prefix >> run_shift) form one run for the tail.
+    u32 run_shift;
 };
 
 // Buffer holding the sorted keys of a keep_keys sort (0/1 = work buffer, 2 = the input chunk: no pass moved data).
