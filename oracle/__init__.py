@@ -441,9 +441,11 @@ def groupby_min_max(keys, vals, val_type, key_null=None, val_null=None, filt=Non
 AGG_SUM, AGG_MIN, AGG_MAX, AGG_COUNT, AGG_AVG, AGG_ARGMIN, AGG_ARGMAX, AGG_FIRST = range(8)
 
 
-def groupby_multi(keys, key_nulls, vals, val_nulls, val_types, aggregates, filt=None):
+def groupby_multi(keys, key_nulls, vals, val_nulls, val_types, aggregates, filt=None, style=MINMAX_QL):
     """QL GROUP BY over a key tuple with a list of aggregates [(op, column[, by_column])], first-seen order.
-    keys / vals: lists of uint64 arrays (bit patterns); *_nulls: lists of uint8 bytemaps or None; val_types: EValueType codes."""
+    keys / vals: lists of uint64 arrays (bit patterns); *_nulls: lists of uint8 bytemaps or None; val_types: EValueType codes.
+    style: the order of MIN / MAX / ARGMIN / ARGMAX — MINMAX_QL (QL's comparisons, `state >= new` for min) or MINMAX_YQL
+    (AggLess: NaN the biggest value, of equal values the first stays)."""
     n = len(keys[0])
     nk, nv, na = len(keys), len(vals), len(aggregates)
     keys = [np.ascontiguousarray(k, dtype=np.uint64) for k in keys]
@@ -467,7 +469,7 @@ def groupby_multi(keys, key_nulls, vals, val_nulls, val_types, aggregates, filt=
     g = C.c_size_t(0)
     _chk(lib().yto_groupby_multi(ptrs(keys), ptrs(key_nulls), C.c_uint32(nk), ptrs(vals), ptrs(val_nulls), _p(vt), C.c_uint32(nv),
                                  _p(op), _p(col), _p(by), C.c_uint32(na), _p(f) if f is not None else None, C.c_size_t(n),
-                                 ptrs(ok), ptrs(okn), ptrs(ov), ptrs(ovn), _p(counts), _p(first), C.byref(g)), "groupby_multi")
+                                 C.c_int(style), ptrs(ok), ptrs(okn), ptrs(ov), ptrs(ovn), _p(counts), _p(first), C.byref(g)), "groupby_multi")
     g = g.value
     return dict(keys=[k[:g] for k in ok], key_null=[k[:g] for k in okn], values=[v[:g] for v in ov],
                 value_null=[v[:g] for v in ovn], count=counts[:g], first_row=first[:g])

@@ -1730,21 +1730,33 @@ int yto_groupby_min_max(const u64* keys, const u8* key_null, const u64* vals, co
 //                 (builtin_function_profiler.cpp:1442-1482)
 //   op 7 first = the first non-null value (registry.cpp:3642-3663)
 // val_type per value column: EValueType code (int64 / uint64 / double / boolean).
+// style: the order of min / max / argmin / argmax, as in yto_groupby_min_max —
+//   1 (QL):  the comparisons above on the raw values; next to a NaN both `state >= new` and `state < new` are false, so
+//            the result depends on the row order;
+//   0 (YQL): AggLess, NaN the biggest value, of equal values the first stays — the order-free total order the GPU kernels
+//            implement.
 // ---------------------------------------------------------------------------
 int yto_groupby_multi(const u64* const* keys, const u8* const* key_null, u32 nk, const u64* const* vals,
                       const u8* const* val_null, const u8* val_type, u32 nv, const i32* agg_op, const i32* agg_col,
-                      const i32* agg_by, u32 na, const u8* filter, size_t n, u64* const* out_keys, u8* const* out_key_null,
-                      u64* const* out_vals, u8* const* out_val_null, u64* out_counts, u64* out_first, size_t* ngroups) {
+                      const i32* agg_by, u32 na, const u8* filter, size_t n, int style, u64* const* out_keys,
+                      u8* const* out_key_null, u64* const* out_vals, u8* const* out_val_null, u64* out_counts, u64* out_first,
+                      size_t* ngroups) {
     (void)nv;
     struct AggSt { bool has = false; u64 bits = 0; u64 by = 0; u64 count = 0; };
     struct Group { size_t first; u64 count = 0; std::vector<AggSt> st; };
     using Key = std::vector<u64>;  // (null mask, words...)
     std::map<Key, size_t> index;
     std::vector<Group> groups;
-    auto less_typed = [](u8 t, u64 a, u64 b) {
+    auto less_typed = [style](u8 t, u64 a, u64 b) {
         if (t == T_INT64) return (i64)a < (i64)b;
-        if (t == T_DOUBLE) return as_double(a) < as_double(b);
+        if (t == T_DOUBLE) return style == 0 ? agg_less_bits(T_DOUBLE, a, b) : as_double(a) < as_double(b);
         return a < b;  // uint64, boolean
+    };
+    // min replaces when state >= new (QL), when new < state (YQL: the first of equal values stays)
+    auto min_replaces = [&](u8 t, u64 state, u64 v) {
+        if (style == 0) return less_typed(t, v, state);
+        if (t == T_DOUBLE) return as_double(state) >= as_double(v);
+        return !less_typed(t, state, v);
     };
     for (size_t i = 0; i < n; ++i) {
         if (filter && !filter[i]) continue;
@@ -1781,7 +1793,7 @@ int yto_groupby_multi(const u64* const* keys, const u8* const* key_null, u32 nk,
                     S.count++;
                     break;
                 case 1:
-                    if (!S.has || !less_typed(t, S.bits, v)) S.bits = v;
+                    if (!S.has || min_replaces(t, S.bits, v)) S.bits = v;
                     S.has = true;
                     break;
                 case 2:

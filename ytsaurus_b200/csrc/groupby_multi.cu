@@ -216,6 +216,12 @@ struct AggState {
     unsigned long long* row;  // selected row (argmin / argmax / first)
 };
 
+// The order of an argmin / argmax `by` value: its MIN / MAX word with -0.0 taken as +0.0, so the two zeros tie and the
+// first row wins, as QL's strict `new.by < state.by` has it.
+__device__ __forceinline__ u64 by_encode(u8 vtype, u64 bits) {
+    return minmax_encode(vtype, vtype == YTGPU_TYPE_DOUBLE && bits == 0x8000000000000000ull ? 0 : bits);
+}
+
 // Step 2.  phase 1 is the row selection of argmin / argmax (the bound is final after phase 0).
 __global__ void __launch_bounds__(512) mg_accumulate_kernel(int op, int phase, const ColumnDev col, const ColumnDev by, u64 n, u32 slots,
                                                             const u32* __restrict__ slot_of_row, AggState S) {
@@ -322,7 +328,7 @@ __global__ void __launch_bounds__(512) mg_accumulate_kernel(int op, int phase, c
                     bool bnul;
                     const u64 bv = decode_at(by, (i64)i, &bnul);
                     if (!bnul) {
-                        const u64 e = minmax_encode(by.value_type, bv);
+                        const u64 e = by_encode(by.value_type, bv);
                         if (phase == 0) {
                             if (op == YTGPU_AGG_ARGMIN) {
                                 if (e < __ldcg(&S.acc[slot])) atomicMin(&S.acc[slot], (unsigned long long)e);
@@ -424,8 +430,8 @@ struct Selector {
             c = string_compare(bs.heap, string_of(bs, a), string_of(bs, b));
         } else {
             bool nul;
-            const u64 ea = minmax_encode(by.value_type, decode_at(by, (i64)a, &nul));
-            const u64 eb = minmax_encode(by.value_type, decode_at(by, (i64)b, &nul));
+            const u64 ea = by_encode(by.value_type, decode_at(by, (i64)a, &nul));
+            const u64 eb = by_encode(by.value_type, decode_at(by, (i64)b, &nul));
             c = ea < eb ? -1 : (ea > eb ? 1 : 0);
         }
         if (larger) c = -c;
