@@ -306,16 +306,23 @@ Status sort_fixed_rows_impl(Context* ctx, const ytgpu_fixed_rows_view* in, const
     YTGPU_TRY(chunks.allocate(ctx, L.nchunks, n));
     SortScratch scratch;
     PermRef perm;
-    YTGPU_TRY(prepare_histogram(ctx, (int)L.nchunks, &scratch));
-    YTGPU_TRY(normalize_fixed_rows(ctx, L, rows, n, rb, chunks.ptrs, scratch.hist.p, &scratch.hist_precomputed));
-    YTGPU_TRY(radix_sort_keys(ctx, chunks.cptrs, (int)L.nchunks, n, &scratch, &perm));
+    u8* dst = out_rows;
     if (out_rows) {
-        u8* dst = out_rows;
         if (out_mem == YTGPU_MEM_HOST) {
             YTGPU_TRY(out_stage.allocate(ctx, n * rb));
             dst = out_stage.p;
         }
-        YTGPU_TRY(gather_rows(ctx, rows, perm, dst, n, rb));
+        // the sort may move the rows itself (three-pass schedule); then the permutation is written only if wanted
+        scratch.gather.rows = rows;
+        scratch.gather.out = dst;
+        scratch.gather.row_bytes = rb;
+        scratch.gather.want_perm = out_perm != nullptr;
+    }
+    YTGPU_TRY(prepare_histogram(ctx, (int)L.nchunks, &scratch));
+    YTGPU_TRY(normalize_fixed_rows(ctx, L, rows, n, rb, chunks.ptrs, scratch.hist.p, &scratch.hist_precomputed));
+    YTGPU_TRY(radix_sort_keys(ctx, chunks.cptrs, (int)L.nchunks, n, &scratch, &perm));
+    if (out_rows) {
+        if (!scratch.rows_gathered) YTGPU_TRY(gather_rows(ctx, rows, perm, dst, n, rb));
         if (out_mem == YTGPU_MEM_HOST) YTGPU_TRY(copy_out(ctx, out_rows, dst, n * rb, YTGPU_MEM_HOST));
     }
     if (out_perm) {

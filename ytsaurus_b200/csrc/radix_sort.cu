@@ -10,6 +10,7 @@
 #include <vector>
 
 #include "radix_sort.cuh"
+#include "rows.cuh"
 
 namespace ytgpu {
 namespace {
@@ -311,21 +312,52 @@ __global__ void __launch_bounds__(256) tie_fix_kernel(SortPlan* plan, const u64*
 // left as they are, registered by their first row and marked where a row's key differs from its left neighbour's, as
 // tie_fix_kernel does.  Only positions of short runs owned by a block are written, and a long run is never written, so
 // blocks that read their neighbours' positions (halos) see either a value they ignore or a final one.
+//
+// GATHER: the block also moves the rows, out[j] = rows[idx[j]] for every position j it owns, so the sort's caller needs
+// no separate gather and, unless it wants the permutation (write_idx), the row indices are not written back at all.
+// Every position is owned by exactly one block:
+//   * the positions of the short runs that start in the block's tile, halo positions after the tile included;
+//   * the runs of one row and the long-run positions that lie inside the tile (a long run is gathered in input order;
+//     the mixed ones are sorted on the side afterwards and their positions gathered again);
+//   * but not the positions at the start of the tile that belong to a short run that began in the previous tile: that
+//     block owns them.
+// A block sees the run through the tile's first position the way the previous block sees it (both find its end, and
+// its start when the run has <= 32 rows), so they agree on whether it is short.
 constexpr int kRunTile = 1984;                 // positions owned by a block (a multiple of 32 and of 8)
 constexpr int kRunSpan = kRunTile + 64;        // staged: local position l is global position tile * kRunTile - 32 + l
 constexpr int kRunWords = kRunSpan / 32;
 constexpr int kRunItems = kRunSpan / 256;
 constexpr u32 kNoSlot = 0xffffffffu;
+constexpr int kTailGatherUnroll = 4;  // 16-byte granules in flight per thread in the gathering tail
 
-__global__ void __launch_bounds__(256) tie_fix_runs_kernel(const u64* __restrict__ chunk, const u32* __restrict__ pre, u32* idx,
-                                                           u32 n, u32* __restrict__ mixedmask, u32* __restrict__ longlist,
-                                                           HybridSummary* sum) {
+// Rows the gathering tail moves: gr 16-byte granules per row.  Granule q of a block's span belongs to position
+// q / gr = (2q * gr_magic) >> 32 with gr_magic = ceil(2^31 / gr): with gr_magic = (2^31 + e) / gr, e < gr, that is exact
+// while q e < 2^31, so for the span's kRunSpan * gr granules up to gr = kTailGatherMaxGranules.  (A u32 division or a
+// 64-bit multiply needs more registers than 8 blocks per SM leave: either spilled.)
+constexpr u32 kTailGatherMaxGranules = 1024;  // rows of up to 16 KB
+struct TailGather {
+    const uint4* rows;
+    uint4* out;
+    u32 gr, gr_magic;
+    int write_idx;  // also write the final row indices back (the caller consumes the permutation)
+};
+
+__device__ __forceinline__ u32 granule_row(u32 q, const TailGather& G) { return __umulhi(q << 1, G.gr_magic); }
+
+// 8 resident blocks per SM (26.3 KB of shared memory and 32 registers each, no spills): when gathering, with 4 granules
+// in flight per thread, that matches the memory-level parallelism of gather_rows_kernel.
+template <bool GATHER>
+__global__ void __launch_bounds__(256, 8) tie_fix_runs_kernel(const u64* __restrict__ chunk, const u32* __restrict__ pre,
+                                                                           u32* idx, u32 n, u32* __restrict__ mixedmask,
+                                                                           u32* __restrict__ longlist, HybridSummary* sum,
+                                                                           const TailGather G) {
     __shared__ u32 s_comp[kRunSpan];      // (prefix << 24) | l: prefix byte 0 on top
     __shared__ u32 s_idx[kRunSpan];       // row indices in position order
     __shared__ u32 s_out[kRunSpan];       // the staged prefixes; then row indices in slot order, kNoSlot: not written
     __shared__ u32 s_head[kRunWords];     // bit l: position l starts a run (positions outside [0, n) are runs of one)
-    __shared__ u32 s_ties[kRunSpan / 2];  // groups of equal prefixes: first slot | length << 16
+    __shared__ u16 s_ties[kRunSpan / 2];  // groups of equal prefixes: first slot | (length - 1) << 11
     __shared__ u32 s_nties, s_long;
+    __shared__ int s_first;               // first position of the tile that is not part of a short run of the previous tile
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int base = (int)blockIdx.x * kRunTile - 32;  // n < 2^30
     if (tid == 0) s_nties = s_long = 0;
@@ -369,8 +401,14 @@ __global__ void __launch_bounds__(256) tie_fix_runs_kernel(const u64* __restrict
         }
         return w * 32 + __ffs(m) - 1;
     };
-    if (tid == 0 && next_head(33) - (31 - __clz(s_head[0])) > kMaxTieRun && !(s_head[1] & 1))
-        s_long = 1;  // the run through position 32 started in the previous tile and is long
+    if (tid == 0) {
+        // the run through position 32 started in the previous tile: long, or short and owned by the previous block
+        const int nh = next_head(33);
+        const bool crosses = !(s_head[1] & 1);
+        const bool long_cross = crosses && nh - (31 - __clz(s_head[0])) > kMaxTieRun;
+        if (long_cross) s_long = 1;
+        s_first = crosses && !long_cross ? nh : 32;
+    }
     __syncthreads();
 
     const u32 lt_mask = lanemask_lt();
@@ -414,7 +452,7 @@ __global__ void __launch_bounds__(256) tie_fix_runs_kernel(const u64* __restrict
             if (act && end - start >= 2) {
                 const int first = ws + start + __popc(lt);  // slot of the first row with this prefix
                 s_out[first + __popc(eq & lt_mask)] = s_idx[ws + lane];
-                if (__popc(eq) > 1 && (eq & lt_mask) == 0) s_ties[atomicAdd(&s_nties, 1u)] = (u32)first | ((u32)__popc(eq) << 16);
+                if (__popc(eq) > 1 && (eq & lt_mask) == 0) s_ties[atomicAdd(&s_nties, 1u)] = (u16)(first | ((__popc(eq) - 1) << 11));
             }
             ws += len;
         }
@@ -423,7 +461,7 @@ __global__ void __launch_bounds__(256) tie_fix_runs_kernel(const u64* __restrict
 
     // equal prefixes: stable insertion sort by the full key
     for (u32 t = tid; t < s_nties; t += 256) {
-        const u32 q = s_ties[t] & 0xffff, e = q + (s_ties[t] >> 16);
+        const u32 q = s_ties[t] & 0x7ff, e = q + (s_ties[t] >> 11) + 1;
         for (u32 a = q + 1; a < e; ++a) {
             const u32 x = s_out[a];
             const u64 k = chunk[x];
@@ -458,10 +496,46 @@ __global__ void __launch_bounds__(256) tie_fix_runs_kernel(const u64* __restrict
         if (g < (int)n) mixedmask[g >> 5] = 0;
     }
     __syncthreads();
+    if constexpr (GATHER) {
+        // granule q of the span is granule q % gr of position q / gr: consecutive threads read and write whole rows
+        const int lo = s_first, hi = min(32 + kRunTile, (int)n - base);
+        const u32 total = (u32)kRunSpan * G.gr;  // a multiple of 256 * kTailGatherUnroll: every step is whole
+        static_assert(kRunSpan % (256 * kTailGatherUnroll) == 0, "whole gather steps");
+        const long long out0 = (long long)base * G.gr;
+        for (u32 q0 = tid; q0 < total; q0 += 256 * kTailGatherUnroll) {
+            uint4 v[kTailGatherUnroll];
+            bool ok[kTailGatherUnroll];
 #pragma unroll
-    for (int it = 0; it < kRunItems; ++it) {
-        const int q = it * 256 + tid;
-        if (s_out[q] != kNoSlot) idx[base + q] = s_out[q];
+            for (int k = 0; k < kTailGatherUnroll; ++k) {
+                const u32 q = q0 + k * 256;
+                const u32 l = granule_row(q, G);
+                u32 r = s_out[l];
+                if (r == kNoSlot && (int)l >= lo && (int)l < hi) r = s_idx[l];
+                ok[k] = r != kNoSlot;
+                if (ok[k]) v[k] = ld_stream_u128(G.rows + (u64)r * G.gr + (q - l * G.gr));
+            }
+#pragma unroll
+            for (int k = 0; k < kTailGatherUnroll; ++k)
+                if (ok[k]) st_stream_u128(G.out + (out0 + q0 + k * 256), v[k]);
+        }
+    }
+    if (!GATHER || G.write_idx) {
+#pragma unroll
+        for (int it = 0; it < kRunItems; ++it) {
+            const int q = it * 256 + tid;
+            if (s_out[q] != kNoSlot) idx[base + q] = s_out[q];
+        }
+    }
+}
+
+// Rows at the positions of the mixed long runs again, once sort_mixed_runs has rewritten their row indices.
+__global__ void __launch_bounds__(256) regather_rows_kernel(const u32* __restrict__ pos, u32 m, const u32* __restrict__ idx,
+                                                            const TailGather G) {
+    const u64 total = (u64)m * G.gr;
+    for (u64 q = (u64)blockIdx.x * blockDim.x + threadIdx.x; q < total; q += (u64)gridDim.x * blockDim.x) {
+        const u64 k = q / G.gr;
+        const u32 g = (u32)(q - k * G.gr), j = pos[k];
+        st_stream_u128(G.out + (u64)j * G.gr + g, ld_stream_u128(G.rows + (u64)idx[j] * G.gr + g));
     }
 }
 
@@ -940,6 +1014,8 @@ std::pair<const PassVariant*, const PassVariant*> pass_variants(Context* ctx) {
     if (!(ctx->func_attrs_done & FA_SORT_PASS)) {  // per device (the attribute belongs to the current device's function)
         for (const PassVariant* x : {&kVariants[v], &kPackedVariants[pv]})
             cudaFuncSetAttribute(x->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)x->smem);
+        // 8 gathering tail blocks per SM need the largest shared-memory carveout
+        cudaFuncSetAttribute(tie_fix_runs_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
         ctx->func_attrs_done |= FA_SORT_PASS;
     }
     return {&kVariants[v], &kPackedVariants[pv]};
@@ -951,8 +1027,9 @@ std::pair<const PassVariant*, const PassVariant*> pass_variants(Context* ctx) {
 // to a side buffer in run order, sorted by the full key with the plain schedule, and written back — the k-th smallest
 // side element belongs at the k-th marked position because runs are ordered by prefix, i.e. by key.  Packed format
 // (packed_chunk != nullptr): the keys are read from the chunk through the permutation, only the permutation is written.
+// regather: the gathering tail moved the rows already; those of the re-sorted positions are moved again.
 static Status sort_mixed_runs(Context* ctx, SortScratch* s, const HybridSummary& hs, const MixedRun* mixedlist_dev,
-                              const u64* packed_chunk) {
+                              const u64* packed_chunk, const TailGather* regather) {
     cudaStream_t st = ctx->stream;
     const u32 w = hs.mixed_count;
     std::vector<MixedRun> runs(w);
@@ -988,6 +1065,11 @@ static Status sort_mixed_runs(Context* ctx, SortScratch* s, const HybridSummary&
                                                                                                               total, side_key.p, side_idx.p,
                                                                                                               side_pos.p, keys, idx);
     ctx->count_launch();
+    if (regather) {
+        KernelTimer t(ctx, KC_GATHER);
+        regather_rows_kernel<<<(u32)std::min<u64>(((u64)total * regather->gr + 255) / 256, (u64)kNumSms * 16), 256, 0, st>>>(side_pos.p, total,
+                                                                                                                       idx, *regather);
+    }
     YTGPU_CUDA_TRY(cudaGetLastError());
     YTGPU_CUDA_TRY(cudaStreamSynchronize(st));  // `host` / `runs` back the asynchronous upload
     return Status{};
@@ -1082,8 +1164,20 @@ Status radix_sort_chunks(Context* ctx, const u64* const* chunks, int nchunks, u6
                 launch_pass(*pv, chunks[r], 0, r * kPassesPerChunk + p, p, r * kPassesPerChunk + p, p * kRadixBits, hp);
         }
     }
+    s->rows_gathered = false;
     if (hp.hybrid) {
-        // hybrid tail: order the short runs of equal prefixes, classify the long ones
+        // hybrid tail: order the short runs of equal prefixes, classify the long ones.  The three-pass packed schedule's
+        // tail also moves the rows when the caller asked for them (SortScratch::gather).
+        const bool gather = s->gather.rows && hp.packed && hp.run_shift == 8 && s->gather.row_bytes / 16 <= kTailGatherMaxGranules;
+        TailGather tg{};
+        if (gather) {
+            const u32 gr = s->gather.row_bytes / 16;
+            tg.rows = reinterpret_cast<const uint4*>(s->gather.rows);
+            tg.out = reinterpret_cast<uint4*>(s->gather.out);
+            tg.gr_magic = (u32)(((1ull << 31) + gr - 1) / gr);
+            tg.gr = gr;
+            tg.write_idx = s->gather.want_perm ? 1 : 0;
+        }
         DevBuf<u32> mixedmask, longlist;
         DevBuf<HybridSummary> summary;
         DevBuf<MixedRun> mixedlist;
@@ -1093,20 +1187,27 @@ Status radix_sort_chunks(Context* ctx, const u64* const* chunks, int nchunks, u6
         YTGPU_TRY(mixedlist.allocate(ctx, kMixedCap));
         YTGPU_CUDA_TRY(cudaMemsetAsync(summary.p, 0, sizeof(HybridSummary), st));
         {
-            KernelTimer t(ctx, KC_HISTOGRAM, 2);
             const u32 blocks = (u32)std::min<u64>((n + 255) / 256, (u64)kNumSms * 8);
             auto classify = hp.packed ? classify_long_runs_kernel<true> : classify_long_runs_kernel<false>;
             if (hp.run_shift) {
                 // the prefixes are in the permutation buffer the last pass did not write
                 u32* idx = s->idx[hp.final_idx].p;
                 const u32* pre = s->idx[hp.final_idx ^ 1].p;
-                tie_fix_runs_kernel<<<(u32)((n + kRunTile - 1) / kRunTile), 256, 0, st>>>(chunks[0], pre, idx, (u32)n, mixedmask.p,
-                                                                                         longlist.p, summary.p);
+                const u32 tail_blocks = (u32)((n + kRunTile - 1) / kRunTile);
+                if (gather) {
+                    KernelTimer t(ctx, KC_GATHER);
+                    tie_fix_runs_kernel<true><<<tail_blocks, 256, 0, st>>>(chunks[0], pre, idx, (u32)n, mixedmask.p, longlist.p, summary.p, tg);
+                } else {
+                    KernelTimer t(ctx, KC_HISTOGRAM);
+                    tie_fix_runs_kernel<false><<<tail_blocks, 256, 0, st>>>(chunks[0], pre, idx, (u32)n, mixedmask.p, longlist.p, summary.p, tg);
+                }
             } else {
+                KernelTimer t(ctx, KC_HISTOGRAM);
                 auto tie_fix = hp.packed ? tie_fix_kernel<true> : tie_fix_kernel<false>;
                 tie_fix<<<blocks, 256, 0, st>>>(s->plan.p, chunks[0], s->keys[0].p, s->keys[1].p, s->idx[0].p, s->idx[1].p, (u32)n,
                                                 mixedmask.p, longlist.p, summary.p);
             }
+            KernelTimer t(ctx, KC_HISTOGRAM);
             classify<<<kNumSms * 4, 256, 0, st>>>(s->plan.p, s->keys[0].p, s->keys[1].p, s->idx[0].p, s->idx[1].p, (u32)n, mixedmask.p,
                                                   longlist.p, summary.p, mixedlist.p);
         }
@@ -1123,11 +1224,19 @@ Status radix_sort_chunks(Context* ctx, const u64* const* chunks, int nchunks, u6
                 YTGPU_CUDA_TRY(cudaMemsetAsync(s->status.p, 0, (size_t)kPassesPerChunk * tiles * kRadix * 4, st));
                 for (int p = 0; p < kPassesPerChunk; ++p)
                     if (hp.pass_b[p].active) launch_pass(*pv, chunks[0], 1, p, p, total_passes + p, p * kRadixBits, hp);
+                if (gather) {  // the rows the tail moved are in the wrong order: all of them again
+                    PermRef full;
+                    full.plan = s->plan.p;
+                    full.idx[0] = s->idx[0].p;
+                    full.idx[1] = s->idx[1].p;
+                    YTGPU_TRY(gather_rows(ctx, s->gather.rows, full, s->gather.out, n, s->gather.row_bytes));
+                }
                 YTGPU_CUDA_TRY(cudaStreamSynchronize(st));  // `one` lives on this stack frame
             } else {
-                YTGPU_TRY(sort_mixed_runs(ctx, s, hs, mixedlist.p, hp.packed ? chunks[0] : nullptr));
+                YTGPU_TRY(sort_mixed_runs(ctx, s, hs, mixedlist.p, hp.packed ? chunks[0] : nullptr, gather ? &tg : nullptr));
             }
         }
+        s->rows_gathered = gather;
     }
     YTGPU_CUDA_TRY(cudaGetLastError());
     YTGPU_CUDA_TRY(cudaMemcpyAsync(ctx->host_err + 1, &s->plan.p->active_passes, 4, cudaMemcpyDeviceToHost, st));

@@ -82,6 +82,14 @@ __device__ __forceinline__ u32 perm_at(const SortPlan* plan, const u32* a, const
     return f == 2 ? (u32)i : (f == 0 ? a[i] : b[i]);
 }
 
+// Fixed rows the sort may move itself: out[j] = rows[perm[j]].
+struct RowGatherRequest {
+    const u8* rows = nullptr;  // device, row_bytes apart; nullptr: no request
+    u8* out = nullptr;         // device, n * row_bytes
+    u32 row_bytes = 0;         // a multiple of 16
+    bool want_perm = true;     // the caller reads the permutation as well
+};
+
 struct SortScratch {
     DevBuf<u64> keys[2];
     DevBuf<u32> idx[2];
@@ -92,6 +100,10 @@ struct SortScratch {
     bool hist_precomputed = false;  // the caller filled `hist` (see prepare_histogram / hist_accumulate)
     bool keep_keys = false;         // the final pass writes the keys too: keys[plan_final_key()] holds them sorted
     bool no_hybrid = false;         // always the plain schedule (side sorts)
+    // The three-pass packed hybrid schedule moves the requested rows in its tail and sets rows_gathered; every other
+    // schedule leaves the gather to the caller.  With rows_gathered and !gather.want_perm the permutation is NOT complete.
+    RowGatherRequest gather;
+    bool rows_gathered = false;
 };
 
 // Shared-memory digit histogram of one key chunk: 8 digits x 256 bins.  Warp-uniform digits (constant
