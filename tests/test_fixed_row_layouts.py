@@ -323,6 +323,20 @@ def test_prefix_sort_tie_run_limit(ctx, run, n):
         assert passes == 9
 
 
+@pytest.mark.gpu
+def test_prefix_sort_clustered_prefix_chunk_takes_its_complete_schedule(ctx):
+    # The prefix chunk's three most significant bytes (integer bytes 4, 3, 2) take four values: its hybrid sort (3 passes)
+    # leaves four long runs that mix keys and sorts the chunk again with every active byte (8 passes).  Rows with equal
+    # prefixes (groups of 8) differ in the 9th byte: the tie fix orders them through the keys of that second sort.
+    n = 2**18
+    rng = np.random.default_rng(94)
+    rows = _prefix_rows(rng, 5, 4, n)
+    rows[:, 2:5] = rng.integers(0, 256, (4, 3), dtype=np.uint8)[rng.integers(0, 4, n)]
+    rows = _groups_of(rng, rows, 8)
+    assert _active_bytes(rows, _PREFIX_COLS) == 9
+    assert _sort_and_check(ctx, rows, _PREFIX_ROW_BYTES, _PREFIX_COLS) == 3 + 8
+
+
 # ---- 4. single-chunk sorts of >= 2^18 rows: packed onesweep tile edges (6144 items per tile) ----
 _TILE = 6144
 _PACKED_SIZES = [2**18, 43 * _TILE, 43 * _TILE + 1, 43 * _TILE + 769, 300_001]

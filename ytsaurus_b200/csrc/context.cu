@@ -149,8 +149,8 @@ double ytgpu_context_kernel_ms(ytgpu_context* h, int which, uint64_t* launches) 
     if (which < 0 || which >= KC_COUNT) return 0.0;
     c->collect_timers();
     if (which == KC_RADIX_PASS || which == KC_PASS_SKIPPED) {
-        // Pass launches are timed one by one; launches of skipped digits / the unarmed fallback schedule exit at
-        // once.  A launch counts as "active" when it ran at least a fifth as long as the longest one.
+        // Pass launches are timed one by one; launches of skipped digits exit at once.  A launch counts as "active"
+        // when it ran at least a fifth as long as the longest one.
         float mx = 0;
         for (float f : c->pass_ms) mx = f > mx ? f : mx;
         double act = 0, skip = 0;
@@ -178,7 +178,7 @@ void ytgpu_context_reset_timers(ytgpu_context* h) {
 uint64_t ytgpu_context_last_sort_passes(ytgpu_context* h) {
     Context* c = reinterpret_cast<Context*>(h);
     cudaStreamSynchronize(c->stream);
-    return c->host_err[1] + (c->host_err[3] ? c->host_err[2] : 0);
+    return c->host_err[1] + c->last_sort_hybrid_passes;
 }
 
 int ytgpu_context_set_option(ytgpu_context* h, const char* name, int64_t value, ytgpu_error* err) {

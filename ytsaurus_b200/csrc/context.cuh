@@ -36,7 +36,10 @@ struct Context {
     u32 last_sort_refine_rounds = 0;         // refinement rounds of the last rowset sort / merge / join (0: normalised keys)
     std::vector<u64> last_sort_refine_rows;  // rows each of those rounds sorted
     bool last_partition_key_words = false;   // the last rowset ordered partitioning compared key words (keys over 256 B)
-    int opt_sort_hybrid = -1;  // -1: environment default (YTGPU_SORT_HYBRID, on); 0/1: set through ytgpu_context_set_option
+    int opt_sort_hybrid = 1;   // set through ytgpu_context_set_option
+    // Passes of a hybrid schedule whose sort then found clustered keys and sorted them again: the last sort's pass count
+    // is these plus the re-sort's (host_err[1]).
+    u32 last_sort_hybrid_passes = 0;
 
     Status alloc(void** p, size_t bytes) {
         if (bytes == 0) bytes = 16;

@@ -29,7 +29,7 @@ __global__ void __launch_bounds__(256) scatter_rows_to_peers_kernel(const uint4*
     for (u32 i = threadIdx.x; i <= parts; i += blockDim.x) s_start[i] = start[i];
     for (u32 i = threadIdx.x; i < parts; i += blockDim.x) s_dest[i] = dest[i];
     __syncthreads();
-    const u32 f = plan_final_idx(plan);
+    const u32 f = plan->final_idx;
     const u32* perm = f == 1 ? pb : pa;
     const u64 total = n * gr;
     const u64 stride = (u64)gridDim.x * blockDim.x;

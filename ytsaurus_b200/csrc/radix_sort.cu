@@ -5,7 +5,6 @@
 //   10k-bucket std::sort + heap merge yt/yt/ytlib/table_client/partition_sort_reader.cpp:461-529
 // with a stable radix sort over order-preserving normalised keys (keys.cuh).
 #include <algorithm>
-#include <cstdlib>
 #include <utility>
 #include <vector>
 
@@ -56,7 +55,7 @@ __global__ void __launch_bounds__(kHistThreads) histogram_kernel(const u64* __re
 }
 
 // ---------------------------------------------------------------------------------------------
-// Plan: turns counts into exclusive digit offsets, finds skippable digits, and fixes the buffer
+// Plan: turns the counts into exclusive digit offsets, finds skippable digits, and fixes the buffer
 // ping-pong schedule for every (chunk, digit) pass.  One block of 256 threads.
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ u32 block_exclusive_scan_256(u32 v, u32* s_warp_tot) {
@@ -100,8 +99,8 @@ __device__ void build_schedule(PassDesc* descs, const int* sel, int nsel, bool m
 }
 
 // allow_packed: single-chunk sort of >= kHybridMinRows rows that only consumes the permutation.
-__global__ void __launch_bounds__(256) plan_kernel(u32* hist, int nchunks, u32 n, SortPlan* plan, int allow_hybrid, int keep_keys,
-                                                   int allow_packed) {
+__global__ void __launch_bounds__(256) plan_kernel(const u32* hist, u32* offsets, int nchunks, u32 n, SortPlan* plan, int allow_hybrid,
+                                                   int keep_keys, int allow_packed) {
     __shared__ u32 s_warp_tot[8];
     __shared__ u8 s_active[kMaxKeyChunks * kPassesPerChunk];
     __shared__ u8 s_skewed[kPassesPerChunk];
@@ -112,7 +111,7 @@ __global__ void __launch_bounds__(256) plan_kernel(u32* hist, int nchunks, u32 n
         // a bin with more than twice its uniform share: > 2 n / 256 rows (see the three-pass schedule below)
         const int skewed = nchunks == 1 ? __syncthreads_or(c > (n >> 7)) : 0;
         u32 ex = block_exclusive_scan_256(c, s_warp_tot);
-        hist[rp * kRadix + threadIdx.x] = ex;
+        offsets[rp * kRadix + threadIdx.x] = ex;
         if (threadIdx.x == 0) {
             s_active[rp] = !full;
             if (nchunks == 1) s_skewed[rp] = (u8)skewed;
@@ -121,11 +120,8 @@ __global__ void __launch_bounds__(256) plan_kernel(u32* hist, int nchunks, u32 n
     __syncthreads();
     if (threadIdx.x != 0) return;
     for (int rp = 0; rp < total; ++rp) plan->pass[rp] = PassDesc{};
-    for (int p = 0; p < kPassesPerChunk; ++p) plan->pass_b[p] = PassDesc{};
-    plan->hybrid = plan->fallback = plan->hybrid_shift = plan->final_key_a = 0;
-    plan->final_idx_b = 2;
-    plan->active_passes_b = 0;
-    plan->final_key = plan->final_key_b = 2;
+    plan->hybrid = plan->hybrid_shift = plan->final_key_a = 0;
+    plan->final_key = 2;
     plan->packed = plan->prefix_sel = plan->prefix_mask = plan->run_shift = 0;
     u32 final_key = 2;
     if (nchunks == 1) {
@@ -151,12 +147,10 @@ __global__ void __launch_bounds__(256) plan_kernel(u32* hist, int nchunks, u32 n
         const int skip = skip_byte0 ? 1 : 0;
         if (hybrid) {
             build_schedule(plan->pass, sched + skip, need - skip, packed, &plan->final_idx, &final_key);
-            build_schedule(plan->pass_b, act, m, !keep_keys, &plan->final_idx_b, &plan->final_key_b);
             plan->hybrid = 1;
             plan->hybrid_shift = 8u * (u32)sched[0];
             plan->final_key_a = plan->pass[act[m - 1]].key_dst;
             plan->active_passes = (u32)(need - skip);
-            plan->active_passes_b = (u32)m;
         } else {
             build_schedule(plan->pass, act, m, !keep_keys, &plan->final_idx, &plan->final_key);
             plan->active_passes = (u32)m;
@@ -209,7 +203,8 @@ __global__ void __launch_bounds__(256) plan_kernel(u32* hist, int nchunks, u32 n
 //     EQUAL keys (duplicates, "maniac" keys) has no such position and is already in its final stable order.
 // classify_long_runs_kernel then finds each long run's end and looks for a marked position inside it: runs that mix
 // different keys go to the mixed list.  The host reads the summary once and either is done, re-sorts the few mixed runs
-// in a side buffer (sort_mixed_runs), or — clustered keys: many / very long mixed runs — runs the complete LSD schedule.
+// in a side buffer (sort_mixed_runs), or — clustered keys: many / very long mixed runs — sorts the chunk again with the
+// plain schedule.
 constexpr int kMaxTieRun = 32;
 constexpr u32 kMixedCap = 16384;       // mixed long runs handled individually; more = clustered keys = complete schedule
 constexpr u64 kHybridMinRows = 1u << 18;  // smaller sorts are launch bound: plain schedule, no host round trip
@@ -640,9 +635,8 @@ struct PassParams {
     u32* status;            // [tiles][256] look-back words, zeroed
     u32* counter;           // dynamic tile id, zeroed
     const SortPlan* plan;
-    int plan_index;
-    int schedule;  // 0: plan->pass[plan_index]; 1: plan->pass_b[plan_index], runs only when plan->fallback
-    int shift;     // of the digit in the key (pair) or in the packed word (32 + 8 k in the k-th packed pass)
+    int plan_index;  // into plan->pass
+    int shift;       // of the digit in the key (pair) or in the packed word (32 + 8 k in the k-th packed pass)
     u32 n;
     u32 prefix_sel, prefix_mask;  // packed: SortPlan::prefix_sel / prefix_mask
     int copy16;                   // packed: chunk and key buffers are 16-byte aligned (a chunk may start at any word)
@@ -941,27 +935,17 @@ __global__ void __launch_bounds__(THREADS, MINB) onesweep_pass_kernel(const Pass
     extern __shared__ __align__(16) unsigned char smem_raw[];
     u32* s_misc = reinterpret_cast<u32*>(smem_raw + tile_elem_bytes(ITEMS, PACKED)) + WARPS * kRadix + 2 * kRadix;
 
-    if (P.schedule == 1 && !P.plan->fallback) return;
-    const PassDesc pd = P.schedule == 1 ? P.plan->pass_b[P.plan_index] : P.plan->pass[P.plan_index];
+    const PassDesc pd = P.plan->pass[P.plan_index];
     if (!pd.active) return;
-    // One tile per CTA.  (A persistent variant — 3 CTAs per SM looping over an atomic tile counter — measured 8 %
-    // slower on the active passes: 6.51 vs 5.96 ms for 8 passes over 10^8 rows; hardware CTA launch is cheaper
-    // than the extra barrier per tile.)  Tile ids still come from the atomic counter so that they are handed
+    // One tile per CTA, one CTA per tile.  (A persistent variant — 3 CTAs per SM looping over an atomic tile counter —
+    // measured 8 % slower on the active passes: 6.51 vs 5.96 ms for 8 passes over 10^8 rows; hardware CTA launch is
+    // cheaper than the extra barrier per tile.)  Tile ids still come from the atomic counter so that they are handed
     // out in start order, which the decoupled look-back relies on.
-    // The rarely armed fallback schedule is launched with a small persistent grid (gridDim < tiles) so that its
-    // eight normally idle launches cost a few microseconds instead of `tiles` empty CTAs each.
-    const u32 tiles = (u32)(((u64)P.n + TILE - 1) / TILE);
-    const bool persistent = gridDim.x < tiles;
-    for (;;) {
-        if (threadIdx.x == 0) s_misc[8] = atomicAdd(P.counter, 1u);
-        __syncthreads();
-        const u32 tile = s_misc[8];
-        if (tile >= tiles) break;
-        if ((u64)(tile + 1) * TILE <= (u64)P.n) onesweep_tile<THREADS, ITEMS, true, PACKED>(P, pd, tile, smem_raw);
-        else onesweep_tile<THREADS, ITEMS, false, PACKED>(P, pd, tile, smem_raw);
-        if (!persistent) break;
-        __syncthreads();  // everyone is done with this tile's shared memory
-    }
+    if (threadIdx.x == 0) s_misc[8] = atomicAdd(P.counter, 1u);
+    __syncthreads();
+    const u32 tile = s_misc[8];
+    if ((u64)(tile + 1) * TILE <= (u64)P.n) onesweep_tile<THREADS, ITEMS, true, PACKED>(P, pd, tile, smem_raw);
+    else onesweep_tile<THREADS, ITEMS, false, PACKED>(P, pd, tile, smem_raw);
 }
 
 __global__ void materialize_perm_kernel(const SortPlan* plan, const u32* a, const u32* b, u64 n, u32* dst) {
@@ -969,9 +953,8 @@ __global__ void materialize_perm_kernel(const SortPlan* plan, const u32* a, cons
         dst[i] = perm_at(plan, a, b, i);
 }
 
-// Tuning variants of the pass kernel (items per thread, min resident CTAs per SM), one table per element format;
-// YTGPU_SORT_VARIANT / YTGPU_SORT_PACKED_VARIANT select one for experiments.  The defaults are the fastest measured on
-// an H100 SXM at a 700 W power limit.  Pair format (15.3 vs 18.0 ms per 10^8-row sort for 16 items at 3 CTAs per SM):
+// Shapes of the pass kernel (items per thread, min resident CTAs per SM), one per element format: the fastest measured
+// on an H100 SXM at a 700 W power limit.  Pair format (15.3 vs 18.0 ms per 10^8-row sort for 16 items at 3 CTAs per SM):
 // 2 CTAs per SM keep 128 registers without spills, where 3 CTAs per SM (80 registers) spill to local memory.  Packed
 // format (mean pass launch over a 10^8-row sort, 4 packed passes): 16 items at 2 CTAs per SM 0.95 ms, 125 registers, no
 // spills; 10 at 3 (80 registers, no spills) 1.05 ms; 12 at 3 (12 B spilled) 0.98 ms; 8 at 4 (16 B spilled) 1.16 ms.
@@ -981,44 +964,45 @@ __global__ void materialize_perm_kernel(const SortPlan* plan, const u32* a, cons
 // registers); 8 at 4 1.18 ms (64 registers); 24 at 2 0.95 ms.  16-byte copies bypassing L1: 24 items at 2 CTAs per SM
 // 0.87-0.89 ms (128 registers, 106 KB of shared memory); 16 at 3 0.89-0.90 ms (80 registers); 20 at 2 0.93 ms (128
 // registers).  None of them spills.
-struct PassVariant {
+struct PassKernel {
     int items;
-    int ctas_per_sm;
     size_t smem;
     void (*kernel)(const PassParams);
     u32 tiles(u64 n) const { return (u32)((n + (u64)kSortThreads * items - 1) / ((u64)kSortThreads * items)); }
 };
-#define YTGPU_PASS_VARIANT(items, ctas, packed) \
-    { items, ctas, pass_smem_bytes(items, packed), onesweep_pass_kernel<kSortThreads, items, ctas, packed> }
-const PassVariant kVariants[] = {
-    YTGPU_PASS_VARIANT(16, 2, false),
-};
-const PassVariant kPackedVariants[] = {
-    YTGPU_PASS_VARIANT(24, 2, true),
-};
-#undef YTGPU_PASS_VARIANT
-constexpr int kDefaultVariant = 0;
-constexpr int kDefaultPackedVariant = 0;
+#define YTGPU_PASS_KERNEL(items, ctas, packed) \
+    { items, pass_smem_bytes(items, packed), onesweep_pass_kernel<kSortThreads, items, ctas, packed> }
+const PassKernel kPairPass = YTGPU_PASS_KERNEL(16, 2, false);
+const PassKernel kPackedPass = YTGPU_PASS_KERNEL(24, 2, true);
+#undef YTGPU_PASS_KERNEL
 
-template <size_t N>
-int variant_from_env(const char* name, const PassVariant (&)[N], int dflt) {
-    const char* e = getenv(name);
-    const int x = e ? atoi(e) : dflt;
-    return x >= 0 && x < (int)N ? x : dflt;
+void set_sort_func_attrs(Context* ctx) {
+    if (ctx->func_attrs_done & FA_SORT_PASS) return;  // per device (the attribute belongs to the current device's function)
+    for (const PassKernel* x : {&kPairPass, &kPackedPass})
+        cudaFuncSetAttribute(x->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)x->smem);
+    // 8 gathering tail blocks per SM need the largest shared-memory carveout
+    cudaFuncSetAttribute(tie_fix_runs_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
+    ctx->func_attrs_done |= FA_SORT_PASS;
 }
 
-// -> {pair variant, packed variant}
-std::pair<const PassVariant*, const PassVariant*> pass_variants(Context* ctx) {
-    static const int v = variant_from_env("YTGPU_SORT_VARIANT", kVariants, kDefaultVariant);
-    static const int pv = variant_from_env("YTGPU_SORT_PACKED_VARIANT", kPackedVariants, kDefaultPackedVariant);
-    if (!(ctx->func_attrs_done & FA_SORT_PASS)) {  // per device (the attribute belongs to the current device's function)
-        for (const PassVariant* x : {&kVariants[v], &kPackedVariants[pv]})
-            cudaFuncSetAttribute(x->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)x->smem);
-        // 8 gathering tail blocks per SM need the largest shared-memory carveout
-        cudaFuncSetAttribute(tie_fix_runs_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
-        ctx->func_attrs_done |= FA_SORT_PASS;
-    }
-    return {&kVariants[v], &kPackedVariants[pv]};
+// Checks the arguments and, unless the caller filled `hist`, computes the digit counts of every chunk.
+Status sort_setup(Context* ctx, const u64* const* chunks, int nchunks, u64 n, SortScratch* s) {
+    if (nchunks < 1 || nchunks > kMaxKeyChunks)
+        return make_status(YTGPU_ERR_UNSUPPORTED, "normalised key of %d bytes exceeds the %d-byte limit",
+                           nchunks * 8, kMaxKeyChunks * 8);
+    if (n >= (1ull << 30))
+        return make_status(YTGPU_ERR_UNSUPPORTED, "row count %llu exceeds 2^30-1 rows per sort call",
+                           (unsigned long long)n);
+    YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (s->hist_precomputed) return Status{};
+    YTGPU_TRY(prepare_histogram(ctx, nchunks, s));
+    KernelTimer t(ctx, KC_HISTOGRAM, nchunks);
+    const u64 per_block = (u64)kHistThreads * kHistItems;
+    const u32 blocks = (u32)std::min<u64>((n + per_block - 1) / per_block, (u64)kNumSms * 4);
+    for (int c = 0; c < nchunks; ++c)
+        histogram_kernel<<<blocks, kHistThreads, 0, ctx->stream>>>(chunks[c], n, s->hist.p + (size_t)c * kPassesPerChunk * kRadix);
+    s->hist_precomputed = true;
+    return Status{};
 }
 
 }  // namespace
@@ -1077,51 +1061,34 @@ static Status sort_mixed_runs(Context* ctx, SortScratch* s, const HybridSummary&
 
 Status radix_sort_chunks(Context* ctx, const u64* const* chunks, int nchunks, u64 n, SortScratch* s,
                          PermRef* out) {
-    if (nchunks < 1 || nchunks > kMaxKeyChunks)
-        return make_status(YTGPU_ERR_UNSUPPORTED, "normalised key of %d bytes exceeds the %d-byte limit",
-                           nchunks * 8, kMaxKeyChunks * 8);
-    if (n >= (1ull << 30))
-        return make_status(YTGPU_ERR_UNSUPPORTED, "row count %llu exceeds 2^30-1 rows per sort call",
-                           (unsigned long long)n);
+    YTGPU_TRY(sort_setup(ctx, chunks, nchunks, n, s));
+    set_sort_func_attrs(ctx);
     cudaStream_t st = ctx->stream;
-    YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
-    const auto variants = pass_variants(ctx);
-    const PassVariant* pv = variants.first;   // pair format
-    const PassVariant* pk = variants.second;  // packed format
-    const u32 tiles = std::max(pv->tiles(n), pk->tiles(n));  // look-back rows per pass, enough for either format
+    const u32 tiles = std::max(kPairPass.tiles(n), kPackedPass.tiles(n));  // look-back rows per pass, enough for either format
     const int total_passes = nchunks * kPassesPerChunk;
 
     YTGPU_TRY(s->keys[0].allocate(ctx, n));
     YTGPU_TRY(s->keys[1].allocate(ctx, n));
     YTGPU_TRY(s->idx[0].allocate(ctx, n));
     YTGPU_TRY(s->idx[1].allocate(ctx, n));
-    if (!s->hist_precomputed) YTGPU_TRY(prepare_histogram(ctx, nchunks, s));
+    YTGPU_TRY(s->offsets.allocate(ctx, (size_t)total_passes * kRadix));
     YTGPU_TRY(s->status.allocate(ctx, (size_t)kPassesPerChunk * tiles * kRadix));
-    YTGPU_TRY(s->counters.allocate(ctx, (size_t)total_passes + kPassesPerChunk));
+    YTGPU_TRY(s->counters.allocate(ctx, (size_t)total_passes));
     YTGPU_TRY(s->plan.allocate(ctx, 1));
 
-    YTGPU_CUDA_TRY(cudaMemsetAsync(s->counters.p, 0, ((size_t)total_passes + kPassesPerChunk) * 4, st));
-    static const int env_hybrid = [] { const char* e = getenv("YTGPU_SORT_HYBRID"); return e ? atoi(e) : 1; }();
-    const int allow_hybrid = (ctx->opt_sort_hybrid >= 0 ? ctx->opt_sort_hybrid : env_hybrid) && !s->no_hybrid && n >= kHybridMinRows;
+    YTGPU_CUDA_TRY(cudaMemsetAsync(s->counters.p, 0, (size_t)total_passes * 4, st));
+    const int allow_hybrid = ctx->opt_sort_hybrid && !s->no_hybrid && n >= kHybridMinRows;
 
-    if (!s->hist_precomputed) {
-        KernelTimer t(ctx, KC_HISTOGRAM, nchunks);
-        u64 per_block = (u64)kHistThreads * kHistItems;
-        u32 blocks = (u32)std::min<u64>((n + per_block - 1) / per_block, (u64)kNumSms * 4);
-        for (int c = 0; c < nchunks; ++c)
-            histogram_kernel<<<blocks, kHistThreads, 0, st>>>(chunks[c], n, s->hist.p + (size_t)c * kPassesPerChunk * kRadix);
-    }
     // Single-chunk sorts of >= kHybridMinRows rows read the plan back: the host launches only the active passes, in the
     // plan's element format.  Smaller sorts stay free of host round trips and launch every digit's pass (inactive ones
     // return at once).
     const bool read_plan = nchunks == 1 && n >= kHybridMinRows;
-    plan_kernel<<<1, 256, 0, st>>>(s->hist.p, nchunks, (u32)n, s->plan.p, allow_hybrid, s->keep_keys ? 1 : 0,
+    plan_kernel<<<1, 256, 0, st>>>(s->hist.p, s->offsets.p, nchunks, (u32)n, s->plan.p, allow_hybrid, s->keep_keys ? 1 : 0,
                                    read_plan && !s->keep_keys ? 1 : 0);
     ctx->count_launch();
 
-    // plan_index: into plan->pass (schedule 0) or plan->pass_b (schedule 1); slot: the pass's look-back status rows
-    auto launch_pass = [&](const PassVariant& v, const u64* chunk, int schedule, int plan_index, int slot, int counter, int shift,
-                           const SortPlan& hp) {
+    // plan_index: into plan->pass; slot: the pass's look-back status rows
+    auto launch_pass = [&](const PassKernel& v, const u64* chunk, int plan_index, int slot, int counter, int shift, const SortPlan& hp) {
         KernelTimer t(ctx, KC_RADIX_PASS);
         PassParams P;
         P.chunk = chunk;
@@ -1129,12 +1096,11 @@ Status radix_sort_chunks(Context* ctx, const u64* const* chunks, int nchunks, u6
         P.keys[1] = s->keys[1].p;
         P.idx[0] = s->idx[0].p;
         P.idx[1] = s->idx[1].p;
-        P.digit_base = s->hist.p + (size_t)plan_index * kRadix;
+        P.digit_base = s->offsets.p + (size_t)plan_index * kRadix;
         P.status = s->status.p + (size_t)slot * tiles * kRadix;
         P.counter = s->counters.p + counter;
         P.plan = s->plan.p;
         P.plan_index = plan_index;
-        P.schedule = schedule;
         P.shift = shift;
         P.n = (u32)n;
         P.prefix_sel = hp.prefix_sel;
@@ -1154,14 +1120,14 @@ Status radix_sort_chunks(Context* ctx, const u64* const* chunks, int nchunks, u6
             if (!hp.pass[p].active) continue;
             // packed: the k-th pass sorts by prefix byte k, or k + 1 when byte 0 is left to the tail (run_shift == 8)
             const int shift = hp.packed ? 32 + (int)hp.run_shift + k * kRadixBits : p * kRadixBits;
-            launch_pass(hp.packed ? *pk : *pv, chunks[0], 0, p, k, p, shift, hp);
+            launch_pass(hp.packed ? kPackedPass : kPairPass, chunks[0], p, k, p, shift, hp);
             ++k;
         }
     } else {
         for (int r = nchunks - 1; r >= 0; --r) {
             YTGPU_CUDA_TRY(cudaMemsetAsync(s->status.p, 0, (size_t)kPassesPerChunk * tiles * kRadix * 4, st));
             for (int p = 0; p < kPassesPerChunk; ++p)
-                launch_pass(*pv, chunks[r], 0, r * kPassesPerChunk + p, p, r * kPassesPerChunk + p, p * kRadixBits, hp);
+                launch_pass(kPairPass, chunks[r], r * kPassesPerChunk + p, p, r * kPassesPerChunk + p, p * kRadixBits, hp);
         }
     }
     s->rows_gathered = false;
@@ -1218,30 +1184,22 @@ Status radix_sort_chunks(Context* ctx, const u64* const* chunks, int nchunks, u6
         YTGPU_CUDA_TRY(cudaStreamSynchronize(st));
         if (hs.hybrid && hs.mixed_count > 0) {
             if (hs.mixed_count > kMixedCap || hs.mixed_elems > n / 8) {
-                // clustered keys: the complete LSD schedule (pass_b) from the chunk
-                const u32 one = 1;
-                YTGPU_CUDA_TRY(cudaMemcpyAsync(&s->plan.p->fallback, &one, 4, cudaMemcpyHostToDevice, st));
-                YTGPU_CUDA_TRY(cudaMemsetAsync(s->status.p, 0, (size_t)kPassesPerChunk * tiles * kRadix * 4, st));
-                for (int p = 0; p < kPassesPerChunk; ++p)
-                    if (hp.pass_b[p].active) launch_pass(*pv, chunks[0], 1, p, p, total_passes + p, p * kRadixBits, hp);
-                if (gather) {  // the rows the tail moved are in the wrong order: all of them again
-                    PermRef full;
-                    full.plan = s->plan.p;
-                    full.idx[0] = s->idx[0].p;
-                    full.idx[1] = s->idx[1].p;
-                    YTGPU_TRY(gather_rows(ctx, s->gather.rows, full, s->gather.out, n, s->gather.row_bytes));
-                }
-                YTGPU_CUDA_TRY(cudaStreamSynchronize(st));  // `one` lives on this stack frame
-            } else {
-                YTGPU_TRY(sort_mixed_runs(ctx, s, hs, mixedlist.p, hp.packed ? chunks[0] : nullptr, gather ? &tg : nullptr));
+                // Clustered keys: the chunk is sorted again with the plain schedule over every active digit, from the
+                // counts still in `hist`.  The re-sort allocates the other buffers of `s` again: the stream-ordered pool
+                // hands back the blocks just freed, so the peak footprint does not grow.  It leaves the rows to the
+                // caller (rows_gathered = false), so rows the tail moved in the wrong order are gathered again.
+                s->no_hybrid = true;
+                YTGPU_TRY(radix_sort_chunks(ctx, chunks, 1, n, s, out));
+                ctx->last_sort_hybrid_passes = hp.active_passes;  // after the re-sort, whose own accounting clears it
+                return Status{};
             }
+            YTGPU_TRY(sort_mixed_runs(ctx, s, hs, mixedlist.p, hp.packed ? chunks[0] : nullptr, gather ? &tg : nullptr));
         }
         s->rows_gathered = gather;
     }
     YTGPU_CUDA_TRY(cudaGetLastError());
     YTGPU_CUDA_TRY(cudaMemcpyAsync(ctx->host_err + 1, &s->plan.p->active_passes, 4, cudaMemcpyDeviceToHost, st));
-    YTGPU_CUDA_TRY(cudaMemcpyAsync(ctx->host_err + 2, &s->plan.p->active_passes_b, 4, cudaMemcpyDeviceToHost, st));
-    YTGPU_CUDA_TRY(cudaMemcpyAsync(ctx->host_err + 3, &s->plan.p->fallback, 4, cudaMemcpyDeviceToHost, st));
+    ctx->last_sort_hybrid_passes = 0;
     out->plan = s->plan.p;
     out->idx[0] = s->idx[0].p;
     out->idx[1] = s->idx[1].p;
@@ -1345,7 +1303,7 @@ __global__ void __launch_bounds__(256) deep_tie_fix_kernel(const SortPlan* plan,
     if (sel->complete) return;
     const u32 fk = plan_final_key(plan);
     const u64* keys = fk == 2 ? chunk_h : (fk ? keys1 : keys0);
-    const u32 fi = plan_final_idx(plan);
+    const u32 fi = plan->final_idx;
     u32* idx = fi ? idx1 : idx0;  // fi == 2 (identity, no pass ran) means every prefix is equal: handled as one long run
     const u32 lane = threadIdx.x & 31;
     for (u64 base = (u64)blockIdx.x * blockDim.x; base < n; base += (u64)gridDim.x * blockDim.x) {
@@ -1392,24 +1350,10 @@ __global__ void __launch_bounds__(256) deep_tie_fix_kernel(const SortPlan* plan,
 }  // namespace
 
 Status radix_sort_keys(Context* ctx, const u64* const* chunks, int nchunks, u64 n, SortScratch* s, PermRef* out) {
-    static const int env_prefix = [] { const char* e = getenv("YTGPU_SORT_PREFIX_CHUNK"); return e ? atoi(e) : 1; }();
-    if (nchunks == 1 || n < 2 || !env_prefix) return radix_sort_chunks(ctx, chunks, nchunks, n, s, out);
-    if (nchunks < 1 || nchunks > kMaxKeyChunks)
-        return make_status(YTGPU_ERR_UNSUPPORTED, "normalised key of %d bytes exceeds the %d-byte limit", nchunks * 8, kMaxKeyChunks * 8);
-    if (n >= (1ull << 30))
-        return make_status(YTGPU_ERR_UNSUPPORTED, "row count %llu exceeds 2^30-1 rows per sort call", (unsigned long long)n);
-    cudaStream_t st = ctx->stream;
-    YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (nchunks == 1 || n < 2) return radix_sort_chunks(ctx, chunks, nchunks, n, s, out);
     // 1. raw digit counts of every chunk (the complete schedule needs them as well)
-    if (!s->hist_precomputed) {
-        YTGPU_TRY(prepare_histogram(ctx, nchunks, s));
-        KernelTimer t(ctx, KC_HISTOGRAM, nchunks);
-        const u64 per_block = (u64)kHistThreads * kHistItems;
-        const u32 blocks = (u32)std::min<u64>((n + per_block - 1) / per_block, (u64)kNumSms * 4);
-        for (int c = 0; c < nchunks; ++c)
-            histogram_kernel<<<blocks, kHistThreads, 0, st>>>(chunks[c], n, s->hist.p + (size_t)c * kPassesPerChunk * kRadix);
-        s->hist_precomputed = true;
-    }
+    YTGPU_TRY(sort_setup(ctx, chunks, nchunks, n, s));
+    cudaStream_t st = ctx->stream;
     // 2. prefix chunk of the 8 most significant active bytes + its histogram
     DevBuf<PrefixSel> sel;
     DevBuf<u64> hchunk;

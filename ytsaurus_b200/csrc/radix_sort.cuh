@@ -38,17 +38,12 @@ struct SortPlan {
     u32 final_idx;  // 0/1 = permutation buffer holding the result, 2 = identity
     u32 active_passes;
     // Hybrid schedule for single-chunk keys (see radix_sort.cu): `pass` then only covers the most significant
-    // active digits, tie_fix_kernel orders the short runs of equal prefixes, and `pass_b` is the complete LSD
-    // schedule that runs only if a run was too long (fallback != 0).
-    PassDesc pass_b[kPassesPerChunk];
-    u32 final_idx_b;
-    u32 active_passes_b;
+    // active digits and the hybrid tail orders the runs of equal prefixes.  When the tail finds clustered keys the
+    // host sorts the chunk again with the plain schedule, which replaces this plan.
     u32 hybrid;
     u32 hybrid_shift;   // keys with equal (key >> hybrid_shift) form one run after the hybrid passes
     u32 final_key_a;    // work buffer holding the keys after the hybrid passes
-    u32 fallback;
-    u32 final_key;      // keep_keys sorts: buffer holding the sorted keys of schedule `pass` (0/1, 2 = the chunk itself)
-    u32 final_key_b;    // ... of schedule `pass_b`
+    u32 final_key;      // keep_keys sorts: buffer holding the sorted keys (0/1, 2 = the chunk itself)
     // Packed format (single-chunk sorts of >= 2^18 rows whose scheduled digits fit in 32 bits, not keep_keys): the
     // passes of `pass` move one u64 per row, (prefix << 32) | row index, where prefix byte k is the key digit of the k-th
     // scheduled digit (least significant first).  The last pass writes the row indices to idx[final_idx] and, for the
@@ -63,12 +58,7 @@ struct SortPlan {
 
 // Buffer holding the sorted keys of a keep_keys sort (0/1 = work buffer, 2 = the input chunk: no pass moved data).
 __device__ __forceinline__ u32 plan_final_key(const SortPlan* plan) {
-    if (plan->fallback) return plan->final_key_b;
     return plan->hybrid ? plan->final_key_a : plan->final_key;
-}
-
-__device__ __forceinline__ u32 plan_final_idx(const SortPlan* plan) {
-    return plan->fallback ? plan->final_idx_b : plan->final_idx;
 }
 
 // Result handle: the permutation lives in idx[plan->final_idx] (or is the identity).
@@ -78,7 +68,7 @@ struct PermRef {
 };
 
 __device__ __forceinline__ u32 perm_at(const SortPlan* plan, const u32* a, const u32* b, u64 i) {
-    u32 f = plan_final_idx(plan);
+    u32 f = plan->final_idx;
     return f == 2 ? (u32)i : (f == 0 ? a[i] : b[i]);
 }
 
@@ -90,16 +80,20 @@ struct RowGatherRequest {
     bool want_perm = true;     // the caller reads the permutation as well
 };
 
+// Serves ONE sort of one set of keys: the sort records state in it (hist_precomputed, and no_hybrid after a re-sort of
+// clustered keys), so a second sort of different keys needs a fresh SortScratch.
 struct SortScratch {
     DevBuf<u64> keys[2];
     DevBuf<u32> idx[2];
-    DevBuf<u32> hist;      // [chunks*8][256] -> exclusive digit offsets
+    DevBuf<u32> hist;      // [chunks*8][256] digit counts
+    DevBuf<u32> offsets;   // [chunks*8][256] exclusive digit offsets (plan_kernel)
     DevBuf<u32> status;    // [8][tiles][256] look-back words for one round
     DevBuf<u32> counters;  // [chunks*8] dynamic tile counters
     DevBuf<SortPlan> plan;
-    bool hist_precomputed = false;  // the caller filled `hist` (see prepare_histogram / hist_accumulate)
+    bool hist_precomputed = false;  // `hist` holds the keys' counts: filled by the caller (see prepare_histogram /
+                                    // hist_accumulate) or by the sort itself, so that a re-sort of the keys reuses them
     bool keep_keys = false;         // the final pass writes the keys too: keys[plan_final_key()] holds them sorted
-    bool no_hybrid = false;         // always the plain schedule (side sorts)
+    bool no_hybrid = false;         // always the plain schedule (side sorts, re-sorts of clustered keys)
     // The three-pass packed hybrid schedule moves the requested rows in its tail and sets rows_gathered; every other
     // schedule leaves the gather to the caller.  With rows_gathered and !gather.want_perm the permutation is NOT complete.
     RowGatherRequest gather;

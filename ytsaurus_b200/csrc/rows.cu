@@ -188,7 +188,7 @@ __global__ void __launch_bounds__(256) gather_rows_kernel(const uint4* __restric
                                                           const u32* __restrict__ pa, const u32* __restrict__ pb,
                                                           uint4* __restrict__ out, u64 n, u32 gr, u32 gr_shift) {
     const u64 total = n * gr;
-    const u32 f = plan_final_idx(plan);
+    const u32 f = plan->final_idx;
     const u32* perm = f == 1 ? pb : pa;
     const u64 stride = (u64)gridDim.x * blockDim.x;
     u64 q0 = (u64)blockIdx.x * blockDim.x + threadIdx.x;
