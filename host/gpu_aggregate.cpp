@@ -372,6 +372,16 @@ public:
             byIndex.push_back(arg ? columnIndex(item.ByColumn) : -1);
         }
         const int whereIndex = query.WhereOp != EBinaryOp::None ? columnIndex(query.WhereColumn) : -1;
+        if (query.Where && query.WhereOp != EBinaryOp::None)
+            throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "a query has either Where or WhereColumn / WhereOp");
+        std::vector<int> filterIndex, filterIndex2;  // flattened columns of the expression's leaves
+        if (query.Where) {
+            for (const auto& node : query.Where->Nodes) {
+                const bool leaf = node.Op != EFilterOp::And && node.Op != EFilterOp::Or && node.Op != EFilterOp::Not;
+                filterIndex.push_back(leaf ? columnIndex(node.Column) : -1);
+                filterIndex2.push_back(node.Op == EFilterOp::CompareColumns ? columnIndex(node.Column2) : -1);
+            }
+        }
         std::vector<IUnversionedRowBatchPtr> keep;
         while (auto batch = reader->Read()) {  // ScanOpHelper (cg_routines/registry.cpp:315-438)
             if (batch->IsEmpty()) continue;
@@ -451,6 +461,95 @@ public:
                     valueViews.push_back(view(columns[i]));
                 }
             }
+            int predicateColumn = whereIndex;
+            std::vector<uint8_t> selection;  // the WHERE expression's bitmap: one more BOOLEAN value column
+            if (query.Where) {
+                const int scalarCount = (int)valueViews.size();
+                auto callIndex = [&](int i) { return argIndex[i] >= 0 ? argIndex[i] : scalarCount + (-1 - argIndex[i]); };
+                std::vector<ytgpu_filter_node> program;
+                std::vector<uint64_t> lists;
+                std::string constants;
+                auto addString = [&](const std::string& b) {
+                    const uint64_t off = constants.size();
+                    constants += b;
+                    return off;
+                };
+                for (size_t k = 0; k < query.Where->Nodes.size(); ++k) {
+                    const TFilterNode& node = query.Where->Nodes[k];
+                    ytgpu_filter_node f{(int32_t)node.Op, 0, -1, -1, 0, 0, 0};
+                    if (filterIndex[k] < 0) {
+                        program.push_back(f);
+                        continue;
+                    }
+                    const TFlatColumn& c = columns[filterIndex[k]];
+                    f.column = callIndex(filterIndex[k]);
+                    const bool noValues = c.Type == EValueType::Null ||
+                                          (node.Op == EFilterOp::CompareColumns && columns[filterIndex2[k]].Type == EValueType::Null);
+                    auto typed = [&](const TFilterConstant& v) {
+                        if (v.Type != c.Type)
+                            throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "WHERE node " + std::to_string(k) + ": the constant's type differs from column " +
+                                                                                  std::to_string(node.Column) + "'s");
+                    };
+                    if (noValues && node.Op != EFilterOp::IsNull && node.Op != EFilterOp::IsNotNull) {
+                        // a column without a value: every comparison, IN and prefix test is NULL, as COMPARE over it is
+                        f.op = YTGPU_FILTER_COMPARE;
+                        f.cmp = YTGPU_CMP_EQ;
+                        f.column = callIndex(c.Type == EValueType::Null ? filterIndex[k] : filterIndex2[k]);
+                        program.push_back(f);
+                        continue;
+                    }
+                    switch (node.Op) {
+                        case EFilterOp::Compare:
+                            typed(node.Constant);
+                            f.cmp = CmpOf(node.Cmp);
+                            if (c.Type == EValueType::String) {
+                                f.constant = addString(node.Constant.Bytes);
+                                f.length = (uint32_t)node.Constant.Bytes.size();
+                            } else {
+                                f.constant = node.Constant.Bits;
+                            }
+                            break;
+                        case EFilterOp::CompareColumns:
+                            f.cmp = CmpOf(node.Cmp);
+                            f.column2 = callIndex(filterIndex2[k]);
+                            break;
+                        case EFilterOp::StartsWith:
+                            typed(node.Constant);
+                            f.constant = addString(node.Constant.Bytes);
+                            f.length = (uint32_t)node.Constant.Bytes.size();
+                            break;
+                        case EFilterOp::In:
+                            f.constant = lists.size();
+                            f.length = (uint32_t)node.List.size();
+                            for (const auto& v : node.List) {
+                                typed(v);
+                                lists.push_back(c.Type == EValueType::String ? (addString(v.Bytes) << 32) | v.Bytes.size() : v.Bits);
+                            }
+                            break;
+                        default:
+                            break;
+                    }
+                    program.push_back(f);
+                }
+                selection.assign((n + 63) / 64 * 8, 0);
+                uint64_t selected = 0;
+                ytgpu_error err{};
+                if (ytgpu_evaluate_filter(GetGpuContext(), valueViews.data(), (uint32_t)valueViews.size(), stringViews.data(),
+                                          (uint32_t)stringViews.size(), program.data(), (uint32_t)program.size(), lists.data(), lists.size(),
+                                          reinterpret_cast<const uint8_t*>(constants.data()), constants.size(), selection.data(), nullptr,
+                                          nullptr, 0, &selected, YTGPU_MEM_HOST, &err) != YTGPU_OK)
+                    ThrowFrom(err);
+                ytgpu_column_view v{};
+                v.value_count = (int64_t)n;
+                v.value_type = (uint8_t)EValueType::Boolean;
+                v.has_values = 1;
+                v.bit_width = 1;
+                v.values = selection.data();
+                v.values_count = n;
+                v.mem = YTGPU_MEM_HOST;
+                predicateColumn = (int)valueViews.size();
+                valueViews.push_back(v);
+            }
             for (auto& a : argIndex)
                 if (a < 0) a = (int)valueViews.size() + (-1 - a);
             for (int k : keyIndex) {
@@ -484,10 +583,12 @@ public:
                 for (size_t a = 0; a < na; ++a) { pv.push_back(values[a].data()); pvn.push_back(valueNull[a].data()); }
                 ytgpu_groupby_multi_result res{0, cap, pk.data(), pkn.data(), pv.data(), pvn.data(), nullptr, nullptr};
                 ytgpu_predicate pred{CmpOf(query.WhereOp), 0, query.WhereConstant.Data.Uint64};
+                if (query.Where) pred = ytgpu_predicate{YTGPU_CMP_EQ, 0, 1};
+                const int predArg = query.Where ? predicateColumn : (whereIndex >= 0 ? argIndex[whereIndex] : -1);
                 ytgpu_error err{};
                 const int code = ytgpu_scan_filter_groupby_multi_strings(
                     GetGpuContext(), keyViews.data(), (uint32_t)nk, valueViews.data(), (uint32_t)valueViews.size(), aggregates.data(),
-                    (uint32_t)na, whereIndex >= 0 ? &pred : nullptr, whereIndex >= 0 ? argIndex[whereIndex] : -1, 0, &res, YTGPU_MEM_HOST,
+                    (uint32_t)na, predArg >= 0 ? &pred : nullptr, predArg, 0, &res, YTGPU_MEM_HOST,
                     stringViews.data(), (uint32_t)stringViews.size(), &err);
                 if (code == YTGPU_ERR_INVALID_ARGUMENT && res.group_count > cap) {  // more groups than the first guess
                     cap = res.group_count;

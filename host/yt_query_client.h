@@ -100,12 +100,69 @@ struct TAggregateItem {
     int Column = 0;     // position of the argument in the input rows (argmin / argmax: the returned column)
     int ByColumn = -1;  // argmin / argmax: the minimised / maximised column
 };
+//! A WHERE expression of AND / OR / NOT over comparisons, IN lists, NULL tests and prefix tests, evaluated on the GPU
+//! (ytgpu_evaluate_filter: the semantics, three-valued logic included, are in include/ytgpu.h).  Nodes are in postfix
+//! order; columns are positions in the input rows.  A constant has the column's type (a mistyped constant is
+//! INVALID_ARGUMENT); string constants and IN lists are owned by the expression.
+enum class EFilterOp { Compare = 1, CompareColumns = 2, In = 3, StartsWith = 4, IsNull = 5, IsNotNull = 6, And = 7, Or = 8, Not = 9 };
+struct TFilterConstant {
+    EValueType Type = EValueType::Null;
+    uint64_t Bits = 0;    // Int64 / Uint64 / Double bit pattern, Boolean 0 / 1
+    std::string Bytes;    // String
+    static TFilterConstant Of(const TUnversionedValue& v) {
+        TFilterConstant c;
+        c.Type = v.Type;
+        if (v.Type == EValueType::String) c.Bytes.assign(v.Data.String, v.Length);
+        else if (v.Type == EValueType::Boolean) c.Bits = v.Data.Boolean ? 1 : 0;
+        else c.Bits = v.Data.Uint64;
+        return c;
+    }
+};
+struct TFilterNode {
+    EFilterOp Op = EFilterOp::Compare;
+    EBinaryOp Cmp = EBinaryOp::None;       // Compare, CompareColumns
+    int Column = -1;                       // leaves
+    int Column2 = -1;                      // CompareColumns
+    TFilterConstant Constant;              // Compare; StartsWith: the prefix (a String)
+    std::vector<TFilterConstant> List;     // In
+};
+struct TFilterExpression {
+    std::vector<TFilterNode> Nodes;
+    TFilterExpression& Compare(int column, EBinaryOp cmp, const TUnversionedValue& v) {
+        Nodes.push_back({EFilterOp::Compare, cmp, column, -1, TFilterConstant::Of(v), {}});
+        return *this;
+    }
+    TFilterExpression& CompareColumns(int column, EBinaryOp cmp, int column2) {
+        Nodes.push_back({EFilterOp::CompareColumns, cmp, column, column2, {}, {}});
+        return *this;
+    }
+    TFilterExpression& In(int column, const std::vector<TUnversionedValue>& values) {
+        TFilterNode n{EFilterOp::In, EBinaryOp::None, column, -1, {}, {}};
+        for (const auto& v : values) n.List.push_back(TFilterConstant::Of(v));
+        Nodes.push_back(std::move(n));
+        return *this;
+    }
+    TFilterExpression& StartsWith(int column, const std::string& prefix) {
+        TFilterConstant c;
+        c.Type = EValueType::String;
+        c.Bytes = prefix;
+        Nodes.push_back({EFilterOp::StartsWith, EBinaryOp::None, column, -1, c, {}});
+        return *this;
+    }
+    TFilterExpression& IsNull(int column) { Nodes.push_back({EFilterOp::IsNull, EBinaryOp::None, column, -1, {}, {}}); return *this; }
+    TFilterExpression& IsNotNull(int column) { Nodes.push_back({EFilterOp::IsNotNull, EBinaryOp::None, column, -1, {}, {}}); return *this; }
+    TFilterExpression& And() { Nodes.push_back({EFilterOp::And, EBinaryOp::None, -1, -1, {}, {}}); return *this; }
+    TFilterExpression& Or() { Nodes.push_back({EFilterOp::Or, EBinaryOp::None, -1, -1, {}, {}}); return *this; }
+    TFilterExpression& Not() { Nodes.push_back({EFilterOp::Not, EBinaryOp::None, -1, -1, {}, {}}); return *this; }
+};
+
 struct TMultiGroupQuery {
     std::vector<int> GroupColumns;               // positions of the group items in the input rows (1..8)
     std::vector<TAggregateItem> AggregateItems;
     int WhereColumn = -1;                        // position of the filtered column (must be an aggregate / by argument)
     EBinaryOp WhereOp = EBinaryOp::None;
     TUnversionedValue WhereConstant{};
+    std::optional<TFilterExpression> Where;      // a general WHERE expression; not together with WhereOp
 };
 
 struct TQueryStatistics {

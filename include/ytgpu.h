@@ -585,6 +585,84 @@ int ytgpu_scan_filter_groupby_multi_strings(ytgpu_context* ctx, const ytgpu_colu
                                             const ytgpu_string_column* string_columns, uint32_t string_count,
                                             ytgpu_error* err);
 
+/* ---- WHERE expressions: a selection over several columns ----
+ * The filter of YT QL's ScanOpHelper / FilterOpHelper (the WHERE clause compiled by the query evaluator) and of
+ * ClickHouse's FilterTransform, for expressions built of comparisons, IN lists, NULL tests and prefix tests joined by
+ * AND / OR / NOT.  A filter is a PROGRAM of nodes in POSTFIX order; a row is selected iff the program evaluates to TRUE
+ * under three-valued (Kleene) logic:
+ *   COMPARE(column, cmp, constant)        NULL if the value is NULL; otherwise the comparison of the built-in predicate:
+ *                                         INT64 signed, UINT64 unsigned, DOUBLE by IEEE (a NaN operand makes every op false
+ *                                         except NE; -0.0 == +0.0), BOOLEAN 0 < 1.  STRING: unsigned bytes over the common
+ *                                         prefix, then the shorter value first (QL's string order).
+ *   COMPARE_COLUMNS(column, cmp, column2) NULL if either value is NULL, otherwise as above.  Both columns have the same
+ *                                         type (both strings, or the same value_type).
+ *   IN(column, list)                      NULL if the value is NULL; TRUE if it equals an entry by the EQ rule above (a NaN
+ *                                         entry never matches), else FALSE.  The list holds no NULL: write
+ *                                         is_null(c) OR c IN (...) instead.
+ *   STARTS_WITH(column, prefix)           string columns only (QL is_prefix, ClickHouse startsWith): NULL if the value is
+ *                                         NULL, else whether its first len(prefix) bytes are the prefix.  An empty prefix
+ *                                         matches every non-NULL value.
+ *   IS_NULL(column), IS_NOT_NULL(column)  never NULL.  NULL is what the group-by calls take as NULL: a dictionary index of
+ *                                         0, a null bit or Arrow validity bit, has_values = 0; the null bytemap of a string
+ *                                         column.
+ *   AND, OR, NOT                          Kleene: F AND x = F, T OR x = T, NOT N = N; every other combination with a NULL
+ *                                         operand is NULL.
+ * A one-node COMPARE program selects exactly the rows the built-in ytgpu_predicate passes.  These NULL rules are the
+ * SQL ones; they were not checked against YT QL's own evaluator.
+ *
+ * Node fields by op:
+ *   column     index into columns ++ string_columns (column_count + i is string_columns[i]), as ytgpu_aggregate::column
+ *   cmp        ytgpu_cmp_op, LT .. NE (COMPARE, COMPARE_COLUMNS)
+ *   column2    COMPARE_COLUMNS: the right-hand column
+ *   constant   COMPARE on a scalar column: the bit pattern in the column's type (length must be 0);
+ *              COMPARE / STARTS_WITH on a string column: byte offset of the constant in string_constants, `length` bytes;
+ *              IN: index of the first entry in list_values, `length` entries.  A scalar column's entries are bit patterns
+ *              in its type; a string column's are (offset << 32) | length into string_constants.
+ * Limits: 1 .. 64 nodes and a stack depth of at most 16; at most 65536 IN entries over all IN nodes of a call; at most
+ * 1 MiB of string_constants; fewer than 2^32 rows, and every column (value_count) and string column (row_count) holds
+ * the same number of rows.  Scalar columns are INT64, UINT64, DOUBLE or BOOLEAN.
+ * Outputs, each nullable, in out_mem:
+ *   out_bitmap   8 * ceil(n / 64) bytes; bit i (LSB first) = row i selected, the bits past n zero.  So
+ *                {value_type = BOOLEAN, bit_width = 1, has_values = 1, values = out_bitmap, values_count = n, value_count = n}
+ *                is a column the GROUP BY calls aggregate the selected rows of with the predicate {YTGPU_CMP_EQ, 1}.
+ *   out_bytemap  n bytes of 0 / 1: ClickHouse's IColumn::Filter, also the filter_hint of the string column conversion.
+ *   out_rows     the selected row indexes in ascending order, rows_capacity entries.
+ *   *out_selected (host) the number of selected rows; always written when the call gets that far.
+ * Launches: without out_rows one evaluation kernel and one read of the count and the error word; with out_rows four
+ * more (an exclusive scan of the per-32-row counts and the row write).  HOST inputs are copied to the device first.
+ * YTGPU_ERR_INVALID_ARGUMENT: a malformed program (stack underflow, other than one value left, an unknown op or cmp, a
+ * column out of range), STARTS_WITH or a non-zero `length` on a scalar column, COMPARE_COLUMNS over different types, a
+ * constant or list range outside its buffer, a limit above, rows_capacity below the selected count (the count is still in
+ * *out_selected), a non-NULL string that leaves its heap (checked on the device for the string columns the program reads;
+ * no byte outside the heap is read).  YTGPU_ERR_UNSUPPORTED: a scalar column of another type. */
+typedef enum ytgpu_filter_op {
+    YTGPU_FILTER_COMPARE = 1, YTGPU_FILTER_COMPARE_COLUMNS = 2, YTGPU_FILTER_IN = 3, YTGPU_FILTER_STARTS_WITH = 4,
+    YTGPU_FILTER_IS_NULL = 5, YTGPU_FILTER_IS_NOT_NULL = 6, YTGPU_FILTER_AND = 7, YTGPU_FILTER_OR = 8, YTGPU_FILTER_NOT = 9
+} ytgpu_filter_op;
+
+#define YTGPU_FILTER_MAX_NODES 64
+#define YTGPU_FILTER_MAX_DEPTH 16
+#define YTGPU_FILTER_MAX_IN_ENTRIES 65536
+#define YTGPU_FILTER_MAX_STRING_CONSTANT_BYTES (1u << 20)
+
+typedef struct ytgpu_filter_node {
+    int32_t op;         /* ytgpu_filter_op */
+    int32_t cmp;        /* ytgpu_cmp_op: COMPARE, COMPARE_COLUMNS */
+    int32_t column;     /* index into columns ++ string_columns */
+    int32_t column2;    /* COMPARE_COLUMNS */
+    uint64_t constant;  /* see above */
+    uint32_t length;    /* string constant: bytes; IN: number of entries */
+    uint32_t reserved;
+} ytgpu_filter_node;
+
+int ytgpu_evaluate_filter(ytgpu_context* ctx, const ytgpu_column_view* columns, uint32_t column_count,
+                          const ytgpu_string_column* string_columns, uint32_t string_count,
+                          const ytgpu_filter_node* program /* host */, uint32_t node_count,
+                          const uint64_t* list_values /* host */, uint64_t list_value_count,
+                          const uint8_t* string_constants /* host */, uint64_t string_constant_bytes,
+                          uint8_t* out_bitmap, uint8_t* out_bytemap, uint32_t* out_rows, uint64_t rows_capacity,
+                          uint64_t* out_selected /* host */, int out_mem, ytgpu_error* err);
+
 /* ---- segmented SUM / COUNT over rows ALREADY SORTED by the group key (the aggregate stage after a sort) ----
  * Consecutive rows with equal keys form a group; no hash table.  Replaces the per-group accumulation of a GROUP BY
  * over a sorted stream / a sorted reduce (yt/yt/library/query/engine/cg_routines/registry.cpp:1838-1920 for the

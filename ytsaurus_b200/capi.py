@@ -113,7 +113,7 @@ EXPORTED_SYMBOLS = [
     "ytgpu_scatter_rows_to_peers", "ytgpu_shuffle_create", "ytgpu_shuffle_connect", "ytgpu_shuffle_sort",
     "ytgpu_shuffle_destroy", "ytgpu_reduce_sorted_fixed_rows", "ytgpu_context_set_option", "ytgpu_context_notify", "ytgpu_decode_horizontal_block", "ytgpu_encode_horizontal_block",
     "ytgpu_decode_column", "ytgpu_decode_string_offsets", "ytgpu_decode_string_pointers_and_lengths", "ytgpu_scan_filter_groupby", "ytgpu_scan_filter_groupby_multi",
-    "ytgpu_scan_filter_groupby_multi_strings",
+    "ytgpu_scan_filter_groupby_multi_strings", "ytgpu_evaluate_filter",
     "ytgpu_convert_integer_column", "ytgpu_encode_integer_column", "ytgpu_encode_double_column", "ytgpu_encode_boolean_column", "ytgpu_encode_string_column", "ytgpu_decode_string_segment", "ytgpu_string_value_ids", "ytgpu_extract_column",
     "ytgpu_block_agg_state_init", "ytgpu_block_combine_all",
     "ytgpu_build_bitmap_from_flags", "ytgpu_build_bytemap_from_flags", "ytgpu_count_flags", "ytgpu_build_dictionary_indexes",
@@ -154,6 +154,16 @@ class Aggregate(C.Structure):
 class StringColumn(C.Structure):
     _fields_ = [("heap", C.c_void_p), ("heap_bytes", C.c_uint64), ("starts", C.c_void_p), ("lengths", C.c_void_p),
                 ("null_bytemap", C.c_void_p), ("row_count", C.c_uint64), ("mem", C.c_int32), ("reserved", C.c_int32)]
+
+
+(FILTER_COMPARE, FILTER_COMPARE_COLUMNS, FILTER_IN, FILTER_STARTS_WITH, FILTER_IS_NULL, FILTER_IS_NOT_NULL, FILTER_AND, FILTER_OR,
+ FILTER_NOT) = range(1, 10)
+FILTER_MAX_NODES, FILTER_MAX_DEPTH, FILTER_MAX_IN_ENTRIES, FILTER_MAX_STRING_CONSTANT_BYTES = 64, 16, 65536, 1 << 20
+
+
+class FilterNode(C.Structure):
+    _fields_ = [("op", C.c_int32), ("cmp", C.c_int32), ("column", C.c_int32), ("column2", C.c_int32), ("constant", C.c_uint64),
+                ("length", C.c_uint32), ("reserved", C.c_uint32)]
 
 
 class GroupByMultiResult(C.Structure):
@@ -227,6 +237,9 @@ def load() -> C.CDLL:
     lib.ytgpu_scan_filter_groupby_multi_strings.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p,
                                                             C.c_uint32, C.c_void_p, C.c_int32, C.c_uint64, C.POINTER(GroupByMultiResult),
                                                             C.c_int, C.c_void_p, C.c_uint32, C.POINTER(Error)]
+    lib.ytgpu_evaluate_filter.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p,
+                                          C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64,
+                                          C.POINTER(C.c_uint64), C.c_int, C.POINTER(Error)]
     lib.ytgpu_partition_rowset.argtypes = [C.c_void_p, C.POINTER(RowsetView), C.POINTER(PartitionSpec), C.c_void_p,
                                            C.c_void_p, C.c_int, C.POINTER(Error)]
     lib.ytgpu_partition_rowset_slabs.argtypes = [C.c_void_p, C.POINTER(RowsetView), C.POINTER(PartitionSpec), C.c_void_p, C.c_void_p,

@@ -1,0 +1,562 @@
+// filter.cu — WHERE expressions over several columns: AND / OR / NOT of comparisons, IN lists, NULL tests and string
+// prefix tests, evaluated into a selection bitmap / bytemap / row list (ytgpu_evaluate_filter, semantics in ytgpu.h).
+//
+// One pass over the rows, separate from the aggregation: the result bitmap has the layout of a BOOLEAN column with
+// bit_width 1, so ytgpu_scan_filter_groupby_multi[_strings] aggregates the selected rows through its existing {EQ, 1}
+// predicate, and no aggregation kernel changes.  The kernel is an interpreter of a postfix program:
+//   * one thread per row and 32 consecutive rows per warp, so direct columns load coalesced and the 32-row result is one
+//     __ballot_sync word of the bitmap (whole words, no atomics);
+//   * every lane runs the same node, so the interpreter loop does not diverge; the program, the referenced columns' views,
+//     the head of the (sorted) IN lists and of the string constants are staged in shared memory once per CTA, the rest of
+//     the lists and constants is read through __ldg;
+//   * the truth stack is two bits per entry (bit 0 TRUE, bit 1 FALSE, neither NULL) in one 32-bit register: 16 entries,
+//     Kleene AND / OR / NOT are two bit operations each, and nothing goes to local memory;
+//   * an RLE column finds its run from a hint that lane 0 finds once per 32 rows (rle_pos_from, as groupby_multi).
+#include <algorithm>
+#include <cstring>
+#include <string>
+#include <vector>
+
+#include "columnar.cuh"
+#include "context.cuh"
+#include "scan.cuh"
+#include "strings.cuh"
+
+using namespace ytgpu;
+
+namespace {
+
+constexpr int kFilterThreads = 256;
+constexpr u32 kStagedListEntries = 1024;  // IN entries kept in shared memory per CTA (8 KB)
+constexpr u32 kStagedConstBytes = 4096;   // bytes of string constants kept in shared memory per CTA
+constexpr u32 kMaxFilterColumns = 2 * YTGPU_FILTER_MAX_NODES;  // distinct columns one program can reference
+
+// T = 1, F = 2, NULL = 0 (bit 0: the value is TRUE, bit 1: it is FALSE)
+constexpr u32 kTrue = 1, kFalse = 2, kNull = 0;
+
+struct NodeDev {
+    u8 op;
+    u8 cmp;
+    u8 is_string;  // the node's column(s) are string columns: col / col2 index the string table
+    u8 pad;
+    u16 col, col2;  // compact column tables (referenced columns only)
+    u32 length;     // string constant bytes / IN entries
+    u64 constant;   // scalar constant bits / string constant offset / first IN entry (in the sorted list)
+};
+static_assert(sizeof(NodeDev) == 24, "NodeDev layout");
+
+struct FilterArgs {
+    const NodeDev* nodes;
+    u32 node_count;
+    u32 scalar_count, string_count;
+    const ColumnDev* scalars;
+    const StringDev* strings;
+    const u64* lists;  // sorted IN entries (scalars: minmax order words; strings: (offset << 32) | length)
+    u32 list_count, staged_list;
+    const u8* consts;
+    u32 const_bytes, staged_const;
+    u64 n;
+    u32* bitmap;         // 2 * ceil(n / 64) words of 32 bits
+    u8* bytemap;         // nullable
+    u64* word_counts;    // nullable: popcount of every 32-bit bitmap word (for the row list)
+    u32 bytemap_vec;     // the bytemap is 16-byte aligned: whole 32-row groups are written as two 16-byte stores
+    unsigned long long* result;  // [0] selected count, [1] error bits
+};
+
+// A value canonicalised for the IN search: -0.0 becomes +0.0 (the EQ rule says they are equal).
+__host__ __device__ __forceinline__ u64 in_key(u8 vtype, u64 bits) {
+    if (vtype == YTGPU_TYPE_DOUBLE && bits == 0x8000000000000000ull) bits = 0;
+    return minmax_encode(vtype, bits);
+}
+
+__device__ __forceinline__ bool cmp_holds(int op, int c) {
+    switch (op) {
+        case YTGPU_CMP_LT: return c < 0;
+        case YTGPU_CMP_LE: return c <= 0;
+        case YTGPU_CMP_GT: return c > 0;
+        case YTGPU_CMP_GE: return c >= 0;
+        case YTGPU_CMP_EQ: return c == 0;
+        default: return c != 0;
+    }
+}
+
+__device__ __forceinline__ u64 load_list(const FilterArgs& A, const u64* s_list, u64 k) {
+    return k < A.staged_list ? s_list[k] : __ldg(A.lists + k);
+}
+
+// The constant bytes [off, off + len) as a (heap, value) pair: the shared-memory copy when it holds them.
+__device__ __forceinline__ const u8* const_heap(const FilterArgs& A, const u8* s_const, u64 off, u32 len) {
+    return off + len <= A.staged_const ? s_const : A.consts;
+}
+
+// Scalar value of row i of a column; lane 0 finds the run of the warp's first row for an RLE column (uniform branch: every
+// lane evaluates the same node).
+__device__ __forceinline__ u64 scalar_value(const ColumnDev& c, u64 i, u64 warp_row, bool live, bool* nul) {
+    u64 hint = kNoRleHint;
+    if (c.rle && c.has_values) {
+        u64 h = 0;
+        if ((threadIdx.x & 31) == 0) h = rle_pos(c.rle, c.rle_count, (u64)c.start + warp_row);
+        hint = __shfl_sync(0xffffffffu, h, 0);
+    }
+    *nul = true;
+    if (!live) return 0;
+    return decode_at(c, (i64)i, nul, hint);
+}
+
+__global__ void __launch_bounds__(kFilterThreads) filter_kernel(const FilterArgs A) {
+    extern __shared__ __align__(16) unsigned char smem[];
+    NodeDev* s_nodes = reinterpret_cast<NodeDev*>(smem);
+    ColumnDev* s_scalars = reinterpret_cast<ColumnDev*>(s_nodes + A.node_count);
+    StringDev* s_strings = reinterpret_cast<StringDev*>(s_scalars + A.scalar_count);
+    u64* s_list = reinterpret_cast<u64*>(s_strings + A.string_count);
+    u8* s_const = reinterpret_cast<u8*>(s_list + A.staged_list);
+    {
+        const u32* src = reinterpret_cast<const u32*>(A.nodes);
+        u32* dst = reinterpret_cast<u32*>(s_nodes);
+        for (u32 k = threadIdx.x; k < A.node_count * (u32)(sizeof(NodeDev) / 4); k += blockDim.x) dst[k] = src[k];
+        src = reinterpret_cast<const u32*>(A.scalars);
+        dst = reinterpret_cast<u32*>(s_scalars);
+        for (u32 k = threadIdx.x; k < A.scalar_count * (u32)(sizeof(ColumnDev) / 4); k += blockDim.x) dst[k] = src[k];
+        src = reinterpret_cast<const u32*>(A.strings);
+        dst = reinterpret_cast<u32*>(s_strings);
+        for (u32 k = threadIdx.x; k < A.string_count * (u32)(sizeof(StringDev) / 4); k += blockDim.x) dst[k] = src[k];
+        for (u32 k = threadIdx.x; k < A.staged_list; k += blockDim.x) s_list[k] = A.lists[k];
+        for (u32 k = threadIdx.x; k < A.staged_const; k += blockDim.x) s_const[k] = A.consts[k];
+    }
+    __syncthreads();
+
+    const u32 lane = threadIdx.x & 31;
+    const u64 words = (A.n + 63) / 64 * 2;  // 32-row groups, the last 64-bit word of the bitmap included
+    const u64 warps = (u64)gridDim.x * (blockDim.x >> 5);
+    u32 bad = 0;
+    u64 selected = 0;
+    for (u64 w = (u64)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); w < words; w += warps) {
+        const u64 row0 = w * 32;
+        const u64 i = row0 + lane;
+        const bool live = i < A.n;
+        u32 stack = 0;
+#pragma unroll 1
+        for (u32 k = 0; k < A.node_count; ++k) {
+            const NodeDev nd = s_nodes[k];
+            u32 r;
+            if (nd.op == YTGPU_FILTER_AND || nd.op == YTGPU_FILTER_OR) {
+                const u32 a = stack & 3, b = (stack >> 2) & 3;
+                stack >>= 4;
+                r = nd.op == YTGPU_FILTER_AND ? ((a & b & 1) | ((a | b) & 2)) : (((a | b) & 1) | (a & b & 2));
+            } else if (nd.op == YTGPU_FILTER_NOT) {
+                const u32 a = stack & 3;
+                stack >>= 2;
+                r = ((a & 1) << 1) | (a >> 1);
+            } else if (nd.is_string) {
+                const StringDev& sc = s_strings[nd.col];
+                ytgpu_value v{};
+                const bool have = live && string_at(sc, i, &v, &bad);
+                if (nd.op == YTGPU_FILTER_IS_NULL) r = have || !live ? kFalse : kTrue;
+                else if (nd.op == YTGPU_FILTER_IS_NOT_NULL) r = have ? kTrue : kFalse;
+                else if (!have) r = kNull;
+                else if (nd.op == YTGPU_FILTER_COMPARE_COLUMNS) {
+                    const StringDev& sc2 = s_strings[nd.col2];
+                    ytgpu_value v2{};
+                    r = string_at(sc2, i, &v2, &bad) ? (cmp_holds(nd.cmp, string_compare2(sc.heap, v, sc2.heap, v2)) ? kTrue : kFalse)
+                                                      : kNull;
+                } else if (nd.op == YTGPU_FILTER_COMPARE) {
+                    ytgpu_value c{};
+                    c.type = YTGPU_TYPE_STRING;
+                    c.length = nd.length;
+                    c.data = nd.constant;
+                    r = cmp_holds(nd.cmp, string_compare2(sc.heap, v, const_heap(A, s_const, nd.constant, nd.length), c)) ? kTrue : kFalse;
+                } else if (nd.op == YTGPU_FILTER_STARTS_WITH) {
+                    bool ok = v.length >= nd.length;
+                    const u8* p = const_heap(A, s_const, nd.constant, nd.length) + nd.constant;
+                    const u8* s = sc.heap + v.data;
+                    for (u32 b = 0; ok && b < nd.length; ++b) ok = s[b] == p[b];
+                    r = ok ? kTrue : kFalse;
+                } else {  // IN: binary search over the sorted entries
+                    u64 lo = nd.constant, cnt = nd.length;
+                    while (cnt > 0) {
+                        const u64 half = cnt >> 1, mid = lo + half;
+                        const u64 e = load_list(A, s_list, mid);
+                        ytgpu_value c{};
+                        c.type = YTGPU_TYPE_STRING;
+                        c.length = (u32)e;
+                        c.data = e >> 32;
+                        if (string_compare2(sc.heap, v, const_heap(A, s_const, c.data, c.length), c) > 0) {
+                            lo = mid + 1;
+                            cnt -= half + 1;
+                        } else {
+                            cnt = half;
+                        }
+                    }
+                    r = kFalse;
+                    if (lo < nd.constant + nd.length) {
+                        const u64 e = load_list(A, s_list, lo);
+                        ytgpu_value c{};
+                        c.type = YTGPU_TYPE_STRING;
+                        c.length = (u32)e;
+                        c.data = e >> 32;
+                        if (string_compare2(sc.heap, v, const_heap(A, s_const, c.data, c.length), c) == 0) r = kTrue;
+                    }
+                }
+            } else {
+                const ColumnDev& c = s_scalars[nd.col];
+                bool nul;
+                const u64 v = scalar_value(c, i, row0, live, &nul);
+                if (nd.op == YTGPU_FILTER_IS_NULL) r = nul && live ? kTrue : kFalse;
+                else if (nd.op == YTGPU_FILTER_IS_NOT_NULL) r = nul ? kFalse : kTrue;
+                else if (nd.op == YTGPU_FILTER_COMPARE_COLUMNS) {
+                    bool nul2;
+                    const u64 v2 = scalar_value(s_scalars[nd.col2], i, row0, live, &nul2);
+                    r = nul || nul2 ? kNull : (passes(nd.cmp, c.value_type, v, v2) ? kTrue : kFalse);
+                } else if (nul) r = kNull;
+                else if (nd.op == YTGPU_FILTER_COMPARE) r = passes(nd.cmp, c.value_type, v, nd.constant) ? kTrue : kFalse;
+                else {  // IN: lower bound of the value's order word, then the EQ rule on the entry found
+                    const u64 key = in_key(c.value_type, v);
+                    u64 lo = nd.constant, cnt = nd.length;
+                    while (cnt > 0) {
+                        const u64 half = cnt >> 1, mid = lo + half;
+                        if (load_list(A, s_list, mid) < key) {
+                            lo = mid + 1;
+                            cnt -= half + 1;
+                        } else {
+                            cnt = half;
+                        }
+                    }
+                    r = lo < nd.constant + nd.length &&
+                                passes(YTGPU_CMP_EQ, c.value_type, v, minmax_decode(c.value_type, load_list(A, s_list, lo)))
+                            ? kTrue : kFalse;
+                }
+            }
+            stack = (stack << 2) | r;
+        }
+        const bool sel = live && (stack & 3) == kTrue;
+        const u32 m = __ballot_sync(0xffffffffu, sel);
+        if (lane == 0) {
+            A.bitmap[w] = m;
+            if (A.word_counts) A.word_counts[w] = (u64)__popc(m);
+        }
+        selected += (u64)__popc(m);
+        if (A.bytemap) {
+            if (A.bytemap_vec && row0 + 32 <= A.n) {
+                if (lane < 2) {  // 16 rows per lane: bit b of the ballot becomes byte b
+                    u32 q[4];
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        const u32 b = (m >> (16 * lane + 4 * j)) & 0xF;
+                        q[j] = (b & 1) | ((b & 2) << 7) | ((b & 4) << 14) | ((b & 8) << 21);
+                    }
+                    *reinterpret_cast<uint4*>(A.bytemap + row0 + 16 * lane) = make_uint4(q[0], q[1], q[2], q[3]);
+                }
+            } else if (live) {
+                A.bytemap[i] = sel ? 1 : 0;
+            }
+        }
+    }
+    if (lane == 0 && selected) atomicAdd(&A.result[0], (unsigned long long)selected);
+    if (bad) atomicOr(&A.result[1], (unsigned long long)DE_STRING_OUT_OF_HEAP);
+}
+
+// out_rows[scan[w] + rank of the bit] = row, for every set bit of bitmap word w.
+__global__ void __launch_bounds__(kFilterThreads) filter_rows_kernel(const u32* __restrict__ bitmap, const u64* __restrict__ offsets,
+                                                                     u64 words, u32* out_rows) {
+    const u32 lane = threadIdx.x & 31;
+    const u64 warps = (u64)gridDim.x * (blockDim.x >> 5);
+    for (u64 w = (u64)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); w < words; w += warps) {
+        const u32 m = bitmap[w];
+        if ((m >> lane) & 1) out_rows[offsets[w] + __popc(m & lanemask_lt())] = (u32)(w * 32 + lane);
+    }
+}
+
+// ---- host ----
+struct Checked {
+    std::vector<NodeDev> nodes;
+    std::vector<u64> lists;   // sorted entries of every IN node, node by node
+    std::vector<int> scalar_of, string_of;  // caller column -> compact table slot (-1: not referenced)
+    std::vector<u32> scalar_cols, string_cols;  // compact slot -> caller column
+};
+
+bool is_filter_type(u8 t) {
+    return t == YTGPU_TYPE_INT64 || t == YTGPU_TYPE_UINT64 || t == YTGPU_TYPE_DOUBLE || t == YTGPU_TYPE_BOOLEAN;
+}
+
+Status check_program(const ytgpu_column_view* columns, u32 column_count, u32 string_count, const ytgpu_filter_node* program,
+                     u32 node_count, const u64* list_values, u64 list_value_count, const u8* consts, u64 const_bytes,
+                     Checked* out) {
+    if (node_count == 0 || node_count > (u32)YTGPU_FILTER_MAX_NODES)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "a filter program has 1 .. %d nodes", YTGPU_FILTER_MAX_NODES);
+    if (!program) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null program");
+    if (const_bytes > (u64)YTGPU_FILTER_MAX_STRING_CONSTANT_BYTES)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "at most %u bytes of string constants", YTGPU_FILTER_MAX_STRING_CONSTANT_BYTES);
+    if (const_bytes && !consts) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null string_constants");
+    if (list_value_count && !list_values) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null list_values");
+    const u64 total = (u64)column_count + string_count;
+    out->scalar_of.assign(column_count, -1);
+    out->string_of.assign(string_count, -1);
+    auto slot = [&](u32 c) -> u16 {
+        if (c < column_count) {
+            if (out->scalar_of[c] < 0) {
+                out->scalar_of[c] = (int)out->scalar_cols.size();
+                out->scalar_cols.push_back(c);
+            }
+            return (u16)out->scalar_of[c];
+        }
+        const u32 s = c - column_count;
+        if (out->string_of[s] < 0) {
+            out->string_of[s] = (int)out->string_cols.size();
+            out->string_cols.push_back(s);
+        }
+        return (u16)out->string_of[s];
+    };
+    auto string_range_ok = [&](u64 off, u64 len) { return off <= const_bytes && len <= const_bytes - off; };
+    u64 in_entries = 0;
+    int depth = 0;
+    for (u32 k = 0; k < node_count; ++k) {
+        const ytgpu_filter_node& N = program[k];
+        NodeDev d{};
+        d.op = (u8)N.op;
+        const bool leaf = N.op >= YTGPU_FILTER_COMPARE && N.op <= YTGPU_FILTER_IS_NOT_NULL;
+        if (!leaf && N.op != YTGPU_FILTER_AND && N.op != YTGPU_FILTER_OR && N.op != YTGPU_FILTER_NOT)
+            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: unknown op %d", k, N.op);
+        if (!leaf) {
+            const int pops = N.op == YTGPU_FILTER_NOT ? 1 : 2;
+            if (depth < pops) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: stack underflow", k);
+            depth -= pops - 1;
+            out->nodes.push_back(d);
+            continue;
+        }
+        if (N.column < 0 || (u64)N.column >= total) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: column %d out of range", k, N.column);
+        const bool str = (u32)N.column >= column_count;
+        const u8 vtype = str ? (u8)YTGPU_TYPE_STRING : columns[N.column].value_type;
+        if (!str && !is_filter_type(vtype))
+            return make_status(YTGPU_ERR_UNSUPPORTED, "node %u: column %d has value type 0x%x (INT64, UINT64, DOUBLE or BOOLEAN)", k,
+                               N.column, vtype);
+        d.is_string = str;
+        d.col = slot((u32)N.column);
+        if (N.op == YTGPU_FILTER_COMPARE || N.op == YTGPU_FILTER_COMPARE_COLUMNS) {
+            if (N.cmp < YTGPU_CMP_LT || N.cmp > YTGPU_CMP_NE) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: unknown cmp %d", k, N.cmp);
+            d.cmp = (u8)N.cmp;
+        }
+        switch (N.op) {
+            case YTGPU_FILTER_COMPARE:
+                if (str && !string_range_ok(N.constant, N.length))
+                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: string constant outside string_constants", k);
+                if (!str && N.length) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: a string constant on a scalar column", k);
+                d.constant = N.constant;
+                d.length = N.length;
+                break;
+            case YTGPU_FILTER_STARTS_WITH:
+                if (!str) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: STARTS_WITH on a scalar column", k);
+                if (!string_range_ok(N.constant, N.length))
+                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: prefix outside string_constants", k);
+                d.constant = N.constant;
+                d.length = N.length;
+                break;
+            case YTGPU_FILTER_COMPARE_COLUMNS: {
+                if (N.column2 < 0 || (u64)N.column2 >= total)
+                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: column2 %d out of range", k, N.column2);
+                const bool str2 = (u32)N.column2 >= column_count;
+                if (str != str2 || (!str && columns[N.column2].value_type != vtype))
+                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: COMPARE_COLUMNS over different types", k);
+                d.col2 = slot((u32)N.column2);
+                break;
+            }
+            case YTGPU_FILTER_IN: {
+                if (N.constant > list_value_count || (u64)N.length > list_value_count - N.constant)
+                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: IN list outside list_values", k);
+                in_entries += N.length;
+                if (in_entries > (u64)YTGPU_FILTER_MAX_IN_ENTRIES)
+                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "at most %d IN entries per call", YTGPU_FILTER_MAX_IN_ENTRIES);
+                const u64* e = list_values + N.constant;
+                std::vector<u64> sorted;
+                sorted.reserve(N.length);
+                if (str) {
+                    for (u32 j = 0; j < N.length; ++j) {
+                        if (!string_range_ok(e[j] >> 32, e[j] & 0xffffffffu))
+                            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: IN entry %u outside string_constants", k, j);
+                        sorted.push_back(e[j]);
+                    }
+                    auto bytes = [&](u64 x) { return std::string(reinterpret_cast<const char*>(consts) + (x >> 32), (size_t)(x & 0xffffffffu)); };
+                    std::sort(sorted.begin(), sorted.end(), [&](u64 a, u64 b) { return bytes(a) < bytes(b); });  // unsigned bytes
+                } else {
+                    for (u32 j = 0; j < N.length; ++j) {
+                        const u64 x = e[j];
+                        if (vtype == YTGPU_TYPE_DOUBLE && (x & 0x7fffffffffffffffull) > 0x7ff0000000000000ull) continue;  // NaN never matches
+                        sorted.push_back(in_key(vtype, x));
+                    }
+                    std::sort(sorted.begin(), sorted.end());
+                }
+                d.constant = out->lists.size();
+                d.length = (u32)sorted.size();
+                out->lists.insert(out->lists.end(), sorted.begin(), sorted.end());
+                break;
+            }
+            default:  // IS_NULL / IS_NOT_NULL
+                break;
+        }
+        if (++depth > YTGPU_FILTER_MAX_DEPTH)
+            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: stack deeper than %d", k, YTGPU_FILTER_MAX_DEPTH);
+        out->nodes.push_back(d);
+    }
+    if (depth != 1) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "the program leaves %d values on the stack, not 1", depth);
+    return Status{};
+}
+
+Status evaluate_filter_impl(Context* ctx, const ytgpu_column_view* columns, u32 column_count, const ytgpu_string_column* string_columns,
+                            u32 string_count, const ytgpu_filter_node* program, u32 node_count, const u64* list_values,
+                            u64 list_value_count, const u8* consts, u64 const_bytes, u8* out_bitmap, u8* out_bytemap, u32* out_rows,
+                            u64 rows_capacity, u64* out_selected, int out_mem) {
+    if ((column_count && !columns) || (string_count && !string_columns)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null columns");
+    if (column_count + (u64)string_count == 0) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "no columns");
+    if (out_mem != YTGPU_MEM_DEVICE && out_mem != YTGPU_MEM_HOST)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "out_mem must be YTGPU_MEM_DEVICE or YTGPU_MEM_HOST");
+    const u64 n = column_count ? (u64)columns[0].value_count : string_columns[0].row_count;
+    for (u32 c = 0; c < column_count; ++c)
+        if (columns[c].value_count < 0 || (u64)columns[c].value_count != n)
+            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "column %u differs in length", c);
+    for (u32 s = 0; s < string_count; ++s) {
+        const ytgpu_string_column& S = string_columns[s];
+        if (S.row_count != n) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "string column %u differs in length", s);
+        if ((S.heap_bytes && !S.heap) || (n && (!S.starts || !S.lengths)))  // an empty column reads nothing
+            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "string column %u: null heap, starts or lengths", s);
+        if (S.mem != YTGPU_MEM_DEVICE && S.mem != YTGPU_MEM_HOST)
+            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "string column %u: mem must be YTGPU_MEM_DEVICE or YTGPU_MEM_HOST", s);
+    }
+    if (n >= (1ull << 32)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "fewer than 2^32 rows per call");
+    Checked P;
+    YTGPU_TRY(check_program(columns, column_count, string_count, program, node_count, list_values, list_value_count, consts, const_bytes, &P));
+    if (P.scalar_cols.size() + P.string_cols.size() > kMaxFilterColumns)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "too many columns");  // unreachable: 64 nodes reference at most 128
+    YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (out_selected) *out_selected = 0;
+    if (n == 0) return Status{};
+
+    // columns the program reads, in compact order
+    std::vector<StagedColumn> sc(P.scalar_cols.size());
+    std::vector<ColumnDev> hc(P.scalar_cols.size());
+    for (size_t k = 0; k < sc.size(); ++k) {
+        YTGPU_TRY(stage_column(ctx, &columns[P.scalar_cols[k]], &sc[k]));
+        hc[k] = sc[k].dev;
+    }
+    std::vector<StagedStrings> ss(P.string_cols.size());
+    std::vector<StringDev> hs(P.string_cols.size());
+    for (size_t k = 0; k < ss.size(); ++k) {
+        YTGPU_TRY(stage_strings(ctx, string_columns[P.string_cols[k]], &ss[k]));
+        hs[k] = ss[k].dev;
+    }
+
+    // one upload: nodes | scalar views | string views | sorted lists | string constants, then the outputs' scratch
+    const size_t nodes_b = P.nodes.size() * sizeof(NodeDev), scal_b = hc.size() * sizeof(ColumnDev), str_b = hs.size() * sizeof(StringDev);
+    const size_t list_b = P.lists.size() * 8, const_b = (size_t)const_bytes;
+    auto up16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
+    const size_t o_scal = up16(nodes_b), o_str = o_scal + up16(scal_b), o_list = o_str + up16(str_b), o_const = o_list + up16(list_b);
+    const size_t blob_b = o_const + up16(const_b);
+    std::vector<u8> blob(blob_b, 0);
+    if (nodes_b) memcpy(blob.data(), P.nodes.data(), nodes_b);
+    if (scal_b) memcpy(blob.data() + o_scal, hc.data(), scal_b);
+    if (str_b) memcpy(blob.data() + o_str, hs.data(), str_b);
+    if (list_b) memcpy(blob.data() + o_list, P.lists.data(), list_b);
+    if (const_b) memcpy(blob.data() + o_const, consts, const_b);
+    DevBuf<u8> dblob;
+    YTGPU_TRY(dblob.allocate(ctx, blob_b));
+    YTGPU_CUDA_TRY(cudaMemcpyAsync(dblob.p, blob.data(), blob_b, cudaMemcpyHostToDevice, ctx->stream));
+
+    const u64 words = (n + 63) / 64 * 2;  // 32-bit bitmap words
+    const bool host = out_mem == YTGPU_MEM_HOST;
+    DevBuf<u32> tbitmap;
+    DevBuf<u8> tbytemap;
+    DevBuf<u64> word_counts, scan_sums, scan_total;
+    DevBuf<unsigned long long> result;
+    u32* dbitmap = reinterpret_cast<u32*>(out_bitmap);
+    if (!out_bitmap || host) {
+        YTGPU_TRY(tbitmap.allocate(ctx, words));
+        dbitmap = tbitmap.p;
+    }
+    u8* dbytemap = out_bytemap;
+    if (out_bytemap && host) {
+        YTGPU_TRY(tbytemap.allocate(ctx, n));
+        dbytemap = tbytemap.p;
+    }
+    if (out_rows) YTGPU_TRY(word_counts.allocate(ctx, words));
+    YTGPU_TRY(result.allocate(ctx, 2));
+    YTGPU_CUDA_TRY(cudaMemsetAsync(result.p, 0, 16, ctx->stream));
+
+    FilterArgs A{};
+    A.nodes = reinterpret_cast<const NodeDev*>(dblob.p);
+    A.node_count = (u32)P.nodes.size();
+    A.scalars = reinterpret_cast<const ColumnDev*>(dblob.p + o_scal);
+    A.scalar_count = (u32)hc.size();
+    A.strings = reinterpret_cast<const StringDev*>(dblob.p + o_str);
+    A.string_count = (u32)hs.size();
+    A.lists = reinterpret_cast<const u64*>(dblob.p + o_list);
+    A.list_count = (u32)P.lists.size();
+    A.staged_list = std::min<u32>(A.list_count, kStagedListEntries);
+    A.consts = dblob.p + o_const;
+    A.const_bytes = (u32)const_bytes;
+    A.staged_const = std::min<u32>(A.const_bytes, kStagedConstBytes);
+    A.n = n;
+    A.bitmap = dbitmap;
+    A.bytemap = dbytemap;
+    A.word_counts = out_rows ? word_counts.p : nullptr;
+    A.bytemap_vec = dbytemap && (reinterpret_cast<uintptr_t>(dbytemap) & 15) == 0;
+    A.result = result.p;
+    // shared memory in the kernel's order; every part is a multiple of 8 bytes (NodeDev 24, ColumnDev / StringDev 8-aligned)
+    const size_t smem = nodes_b + scal_b + str_b + (size_t)A.staged_list * 8 + A.staged_const;
+    static_assert(sizeof(ColumnDev) % 8 == 0 && sizeof(StringDev) % 8 == 0, "shared-memory layout");
+    const u64 warps = words;
+    const u32 blocks = (u32)std::max<u64>(1, std::min<u64>((warps * 32 + kFilterThreads - 1) / kFilterThreads, (u64)kNumSms * 8));
+    {
+        KernelTimer t(ctx, KC_DECODE);
+        filter_kernel<<<blocks, kFilterThreads, smem, ctx->stream>>>(A);
+        YTGPU_CUDA_TRY(cudaGetLastError());
+    }
+    unsigned long long res[2] = {0, 0};  // the one host read: selected count and error bits
+    YTGPU_CUDA_TRY(cudaMemcpyAsync(res, result.p, 16, cudaMemcpyDeviceToHost, ctx->stream));
+    YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    if (res[1] & DE_STRING_OUT_OF_HEAP)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "a string value of a filter column leaves its heap");
+    const u64 selected = res[0];
+    if (out_selected) *out_selected = selected;
+    if (out_rows && selected > rows_capacity)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "%llu rows selected, rows_capacity is %llu", (unsigned long long)selected,
+                           (unsigned long long)rows_capacity);
+
+    DevBuf<u32> trows;
+    if (out_rows && selected) {
+        u32* drows = out_rows;
+        if (host) {
+            YTGPU_TRY(trows.allocate(ctx, selected));
+            drows = trows.p;
+        }
+        YTGPU_TRY(scan_sums.allocate(ctx, scan_block_count(words)));
+        YTGPU_TRY(scan_total.allocate(ctx, 1));
+        {
+            KernelTimer t(ctx, KC_DECODE, 4);
+            exclusive_scan_u64(ctx->stream, word_counts.p, words, scan_sums.p, scan_total.p);
+            filter_rows_kernel<<<blocks, kFilterThreads, 0, ctx->stream>>>(dbitmap, word_counts.p, words, drows);
+            YTGPU_CUDA_TRY(cudaGetLastError());
+        }
+        if (host) YTGPU_TRY(copy_out(ctx, out_rows, drows, selected * 4, YTGPU_MEM_HOST));
+    }
+    if (host && out_bitmap) YTGPU_TRY(copy_out(ctx, out_bitmap, dbitmap, words * 4, YTGPU_MEM_HOST));
+    if (host && out_bytemap) YTGPU_TRY(copy_out(ctx, out_bytemap, dbytemap, n, YTGPU_MEM_HOST));
+    if (host) YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return Status{};
+}
+
+}  // namespace
+
+extern "C" {
+
+int ytgpu_evaluate_filter(ytgpu_context* h, const ytgpu_column_view* columns, uint32_t column_count,
+                          const ytgpu_string_column* string_columns, uint32_t string_count, const ytgpu_filter_node* program,
+                          uint32_t node_count, const uint64_t* list_values, uint64_t list_value_count,
+                          const uint8_t* string_constants, uint64_t string_constant_bytes, uint8_t* out_bitmap,
+                          uint8_t* out_bytemap, uint32_t* out_rows, uint64_t rows_capacity, uint64_t* out_selected, int out_mem,
+                          ytgpu_error* err) {
+    if (!h) return fill_error(err, make_status(YTGPU_ERR_INVALID_ARGUMENT, "null context"));
+    CtxLock lock(h);
+    return fill_error(err, evaluate_filter_impl(as_context(h), columns, column_count, string_columns, string_count, program, node_count,
+                                                list_values, list_value_count, string_constants, string_constant_bytes, out_bitmap,
+                                                out_bytemap, out_rows, rows_capacity, out_selected, out_mem));
+}
+
+}  // extern "C"

@@ -25,6 +25,7 @@
 #include "context.cuh"
 #include "keys.cuh"
 #include "radix_sort.cuh"
+#include "strings.cuh"
 
 using namespace ytgpu;
 
@@ -370,53 +371,6 @@ __global__ void __launch_bounds__(512) mg_accumulate_kernel(int op, int phase, c
 }
 
 // ---- string-valued aggregates (MIN / MAX / FIRST / COUNT / ARGMIN / ARGMAX with a string column or by_column) ----
-struct StringDev {
-    const u8* heap;
-    u64 heap_bytes;
-    const u64* starts;
-    const u32* lengths;
-    const u8* nulls;  // nullable bytemap
-    u32 present;      // 0: the argument is a scalar ColumnDev
-};
-
-// Value i of a string argument: false for NULL; a value that leaves the heap sets the error bit and counts as absent, so
-// no later read goes outside the heap.
-__device__ __forceinline__ bool string_at(const StringDev& c, u64 i, ytgpu_value* v, u32* bad) {
-    if (c.nulls && c.nulls[i]) return false;
-    const u64 s = c.starts[i];
-    const u32 l = c.lengths[i];
-    if (s > c.heap_bytes || (u64)l > c.heap_bytes - s) {
-        *bad = 1;
-        return false;
-    }
-    v->type = YTGPU_TYPE_STRING;
-    v->length = l;
-    v->data = s;
-    return true;
-}
-
-__device__ __forceinline__ ytgpu_value string_of(const StringDev& c, u64 row) {
-    ytgpu_value v{};
-    v.type = YTGPU_TYPE_STRING;
-    v.length = c.lengths[row];
-    v.data = c.starts[row];
-    return v;
-}
-
-// QL string order through the width-free key words of keys.cuh (a one-column, required, ascending String key): the order
-// the long-key sort and the ordered partitioner already use.  Words are prefix-free, so the first differing word decides.
-__device__ __forceinline__ int string_compare(const u8* heap, const ytgpu_value& a, const ytgpu_value& b) {
-    KeyColLayout L{};
-    L.type = YTGPU_TYPE_STRING;
-    const u32 na = key_string_blocks(a.length), nb = key_string_blocks(b.length);
-    const u32 nw = na < nb ? na : nb;
-    for (u32 w = 0; w < nw; ++w) {
-        const u64 x = key_col_word(L, a, heap, w), y = key_col_word(L, b, heap, w);
-        if (x != y) return x < y ? -1 : 1;
-    }
-    return 0;
-}
-
 // The selection key of MIN / MAX (the string column itself) or ARGMIN / ARGMAX (by_column, string or scalar).
 struct Selector {
     ColumnDev by;
@@ -626,44 +580,6 @@ __global__ void __launch_bounds__(256) mg_finalize_kernel(int op, const ColumnDe
 }
 
 bool aggregatable_type(u8 t) { return t == YTGPU_TYPE_INT64 || t == YTGPU_TYPE_UINT64 || t == YTGPU_TYPE_DOUBLE || t == YTGPU_TYPE_BOOLEAN; }
-
-// A string column on the device (HOST inputs are uploaded).
-struct StagedStrings {
-    StringDev dev{};
-    DevBuf<u8> heap, nulls;
-    DevBuf<u64> starts;
-    DevBuf<u32> lengths;
-};
-
-Status stage_strings(Context* ctx, const ytgpu_string_column& c, StagedStrings* s) {
-    StringDev& d = s->dev;
-    d.heap_bytes = c.heap_bytes;
-    d.present = 1;
-    if (c.mem != YTGPU_MEM_HOST) {
-        d.heap = c.heap;
-        d.starts = c.starts;
-        d.lengths = c.lengths;
-        d.nulls = c.null_bytemap;
-        return Status{};
-    }
-    const u64 n = c.row_count;
-    YTGPU_TRY(s->heap.allocate(ctx, c.heap_bytes));
-    YTGPU_TRY(copy_in(ctx, s->heap.p, c.heap, c.heap_bytes, YTGPU_MEM_HOST));
-    YTGPU_TRY(s->starts.allocate(ctx, n));
-    YTGPU_TRY(copy_in(ctx, s->starts.p, c.starts, n * 8, YTGPU_MEM_HOST));
-    YTGPU_TRY(s->lengths.allocate(ctx, n));
-    YTGPU_TRY(copy_in(ctx, s->lengths.p, c.lengths, n * 4, YTGPU_MEM_HOST));
-    d.heap = s->heap.p;
-    d.starts = s->starts.p;
-    d.lengths = s->lengths.p;
-    d.nulls = nullptr;
-    if (c.null_bytemap) {
-        YTGPU_TRY(s->nulls.allocate(ctx, n));
-        YTGPU_TRY(copy_in(ctx, s->nulls.p, c.null_bytemap, n, YTGPU_MEM_HOST));
-        d.nulls = s->nulls.p;
-    }
-    return Status{};
-}
 
 Status groupby_multi_impl(Context* ctx, const ytgpu_column_view* key_columns, u32 key_count, const ytgpu_column_view* value_columns,
                           u32 value_count, const ytgpu_aggregate* aggregates, u32 aggregate_count, const ytgpu_predicate* pred,

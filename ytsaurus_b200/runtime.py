@@ -798,6 +798,56 @@ class GpuContext:
         return dict(keys=[k[:g] for k in keys], key_null=[k[:g] for k in kn], values=[v[:g] for v in vals],
                     value_null=[v[:g] for v in vn], count=counts[:g], first_row=first[:g])
 
+    def evaluate_filter(self, columns, string_columns=(), program=(), list_values=(), string_constants=b"",
+                        want_bitmap: bool = True, want_bytemap: bool = True, want_rows: bool = True,
+                        rows_capacity: int | None = None):
+        """WHERE expression (ytgpu_evaluate_filter) -> dict(bitmap, bytemap, rows, count).
+        columns: Column objects; string_columns: (heap, starts, lengths, nulls or None) per column, node column
+        len(columns) + i naming string column i.  program: postfix nodes, each a capi.FilterNode or a tuple
+        (op, cmp, column, column2, constant, length).  list_values: IN entries (uint64 bit patterns; for a string column
+        (offset << 32) | length into string_constants).  The outputs are in the inputs' memory flavour: bitmap
+        8 * ceil(n / 64) bytes, bytemap n bytes, rows uint32 (int32 on the device) trimmed to the count; an output not
+        wanted is None."""
+        views = [c.view() for c in columns]
+        sarr = (capi.StringColumn * max(len(string_columns), 1))()
+        for i, column in enumerate(string_columns):
+            sarr[i] = _string_column(*column)
+        if views:
+            mem, n = views[0].mem, int(views[0].value_count)
+        elif string_columns:
+            mem, n = sarr[0].mem, int(sarr[0].row_count)
+        else:
+            raise ValueError("evaluate_filter needs at least one column")
+        carr = (capi.ColumnView * max(len(views), 1))(*views)
+        nodes = (capi.FilterNode * max(len(program), 1))()
+        for i, node in enumerate(program):
+            if isinstance(node, capi.FilterNode):
+                nodes[i] = node
+            else:
+                op, cmp, column, column2, constant, length = (tuple(node) + (0,) * 6)[:6]
+                nodes[i] = capi.FilterNode(op, cmp, column, column2, int(constant) & 0xFFFFFFFFFFFFFFFF, length, 0)
+        lv = np.ascontiguousarray(np.asarray(list_values, dtype=np.uint64).reshape(-1))
+        sc = np.frombuffer(bytes(string_constants), dtype=np.uint8) if len(string_constants) else np.zeros(0, np.uint8)
+        words = (n + 63) // 64
+        bitmap = self._out((words * 8,), np.uint8, mem) if want_bitmap else None
+        bytemap = self._out((n,), np.uint8, mem) if want_bytemap else None
+        if rows_capacity is None:
+            rows_capacity = n
+        rows = self._out((max(rows_capacity, 1),), np.uint32, mem) if want_rows else None
+        selected = C.c_uint64(0)
+        err = capi.Error()
+        code = self.lib.ytgpu_evaluate_filter(self.handle, C.cast(carr, C.c_void_p), len(views), C.cast(sarr, C.c_void_p),
+                                              len(string_columns), C.cast(nodes, C.c_void_p), len(program),
+                                              lv.ctypes.data if lv.size else None, lv.size, sc.ctypes.data if sc.size else None,
+                                              sc.size, _ptr_mem(bitmap)[0], _ptr_mem(bytemap)[0], _ptr_mem(rows)[0], rows_capacity,
+                                              C.byref(selected), mem, C.byref(err))
+        count = int(selected.value)
+        if code != capi.OK:
+            e = capi.YtGpuError(code, err.message.decode(errors="replace"), err.cuda_error)
+            e.selected = count  # the needed rows_capacity when that was too small
+            raise e
+        return dict(bitmap=bitmap, bytemap=bytemap, rows=rows[:count] if rows is not None else None, count=count)
+
 
 class Column:
     """Host- or device-side description of IUnversionedColumnarRowBatch::TColumn (row_batch.h:49-191)."""
