@@ -374,12 +374,35 @@ public:
         const int whereIndex = query.WhereOp != EBinaryOp::None ? columnIndex(query.WhereColumn) : -1;
         if (query.Where && query.WhereOp != EBinaryOp::None)
             throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "a query has either Where or WhereColumn / WhereOp");
+        // with computed columns the WhereOp form runs as a one-node COMPARE program: the WHERE is then one filter pass that
+        // comes before the computed columns it does not read (its constant gets the column's type once that is known)
+        std::optional<TFilterExpression> where = query.Where;
+        const bool whereOpAsProgram = query.WhereOp != EBinaryOp::None &&
+            std::any_of(columns.begin(), columns.end(), [](const TFlatColumn& c) { return TMultiGroupQuery::IsComputedColumn(c.Position); });
+        if (whereOpAsProgram) {
+            where = TFilterExpression().Compare(query.WhereColumn, query.WhereOp, query.WhereConstant);
+            where->Nodes[0].Constant.Bits = query.WhereConstant.Data.Uint64;  // the built-in predicate's bits
+        }
         std::vector<int> filterIndex, filterIndex2;  // flattened columns of the expression's leaves
-        if (query.Where) {
-            for (const auto& node : query.Where->Nodes) {
+        if (where) {
+            for (const auto& node : where->Nodes) {
                 const bool leaf = node.Op != EFilterOp::And && node.Op != EFilterOp::Or && node.Op != EFilterOp::Not;
                 filterIndex.push_back(leaf ? columnIndex(node.Column) : -1);
                 filterIndex2.push_back(node.Op == EFilterOp::CompareColumns ? columnIndex(node.Column2) : -1);
+            }
+        }
+        // the input columns of every computed column that is named (leafIndex[j][k]: flattened column of node k, -1 for an op)
+        std::vector<std::vector<int>> leafIndex(query.Computed.size());
+        auto isComputed = [&](int i) { return i >= 0 && TMultiGroupQuery::IsComputedColumn(columns[i].Position); };
+        for (size_t i = 0; i < columns.size(); ++i) {
+            if (!isComputed((int)i)) continue;
+            const size_t j = (size_t)(-2 - columns[i].Position);
+            if (j >= query.Computed.size())
+                throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "no computed column " + std::to_string(j));
+            for (const auto& node : query.Computed[j].Nodes) {
+                if (node.Op == EExpressionOp::Column && TMultiGroupQuery::IsComputedColumn(node.Column))
+                    throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "a computed column reads input positions only");
+                leafIndex[j].push_back(node.Op == EExpressionOp::Column ? columnIndex(node.Column) : -1);
             }
         }
         std::vector<IUnversionedRowBatchPtr> keep;
@@ -387,6 +410,7 @@ public:
             if (batch->IsEmpty()) continue;
             const auto& rows = batch->MaterializeRows();
             for (auto& c : columns) {
+                if (TMultiGroupQuery::IsComputedColumn(c.Position)) continue;
                 const size_t base = c.Values.size();
                 c.Values.resize(base + rows.size());
                 c.Nulls.resize((base + rows.size() + 7) / 8, 0);
@@ -442,6 +466,56 @@ public:
                 v.mem = YTGPU_MEM_HOST;
                 return v;
             };
+            // a computed column: one ytgpu_evaluate_expression call over its input columns, rows outside `selection` NULL
+            auto evaluateComputed = [&](int i, const uint8_t* selection) {
+                const size_t j = (size_t)(-2 - columns[i].Position);
+                std::vector<ytgpu_column_view> inputs;
+                std::vector<int> slot(columns.size(), -1);
+                std::vector<ytgpu_expr_node> program;
+                for (size_t k = 0; k < query.Computed[j].Nodes.size(); ++k) {
+                    const TExpressionNode& node = query.Computed[j].Nodes[k];
+                    ytgpu_expr_node x{};
+                    x.op = (int32_t)node.Op;
+                    x.type = (uint8_t)node.Type;
+                    x.constant = node.Bits;
+                    if (const int leaf = leafIndex[j][k]; leaf >= 0) {
+                        if (slot[leaf] < 0) {
+                            slot[leaf] = (int)inputs.size();
+                            inputs.push_back(view(columns[leaf]));  // a string column is refused by the call (UNSUPPORTED)
+                        }
+                        x.column = slot[leaf];
+                    }
+                    program.push_back(x);
+                }
+                if (inputs.empty()) {  // constants only: a column without values gives the row count
+                    ytgpu_column_view rows{};
+                    rows.value_count = (int64_t)n;
+                    rows.value_type = YTGPU_TYPE_INT64;
+                    rows.bit_width = 64;
+                    rows.mem = YTGPU_MEM_HOST;
+                    inputs.push_back(rows);
+                }
+                TFlatColumn& c = columns[i];
+                c.Values.assign(n, 0);
+                c.Nulls.assign((n + 63) / 64 * 8, 0);
+                uint8_t type = 0;
+                uint64_t nullCount = 0;
+                ytgpu_error err{};
+                if (ytgpu_evaluate_expression(GetGpuContext(), inputs.data(), (uint32_t)inputs.size(), program.data(), (uint32_t)program.size(),
+                                              selection, c.Values.data(), c.Nulls.data(), &type, &nullCount, YTGPU_MEM_HOST, &err) != YTGPU_OK)
+                    ThrowFrom(err);
+                c.Type = (EValueType)type;
+                c.AnyNull = nullCount != 0;
+            };
+            // the computed columns the WHERE reads, over all rows
+            std::vector<uint8_t> evaluated(columns.size(), 0);
+            for (const auto* leaves : {&filterIndex, &filterIndex2})
+                for (int i : *leaves)
+                    if (isComputed(i) && !evaluated[i]) {
+                        evaluateComputed(i, nullptr);
+                        evaluated[i] = 1;
+                    }
+            if (whereOpAsProgram) where->Nodes[0].Constant.Type = columns[filterIndex[0]].Type;
             // scalar columns are value columns, string columns follow them as string columns of the call
             std::vector<int> argIndex(columns.size());
             std::vector<ytgpu_column_view> keyViews, valueViews;
@@ -463,7 +537,7 @@ public:
             }
             int predicateColumn = whereIndex;
             std::vector<uint8_t> selection;  // the WHERE expression's bitmap: one more BOOLEAN value column
-            if (query.Where) {
+            if (where) {
                 const int scalarCount = (int)valueViews.size();
                 auto callIndex = [&](int i) { return argIndex[i] >= 0 ? argIndex[i] : scalarCount + (-1 - argIndex[i]); };
                 std::vector<ytgpu_filter_node> program;
@@ -474,8 +548,8 @@ public:
                     constants += b;
                     return off;
                 };
-                for (size_t k = 0; k < query.Where->Nodes.size(); ++k) {
-                    const TFilterNode& node = query.Where->Nodes[k];
+                for (size_t k = 0; k < where->Nodes.size(); ++k) {
+                    const TFilterNode& node = where->Nodes[k];
                     ytgpu_filter_node f{(int32_t)node.Op, 0, -1, -1, 0, 0, 0};
                     if (filterIndex[k] < 0) {
                         program.push_back(f);
@@ -550,6 +624,12 @@ public:
                 predicateColumn = (int)valueViews.size();
                 valueViews.push_back(v);
             }
+            // the other computed columns, over the rows the WHERE selects
+            for (size_t i = 0; i < columns.size(); ++i)
+                if (isComputed((int)i) && !evaluated[i]) {
+                    evaluateComputed((int)i, where ? selection.data() : nullptr);
+                    valueViews[argIndex[i]] = view(columns[i]);
+                }
             for (auto& a : argIndex)
                 if (a < 0) a = (int)valueViews.size() + (-1 - a);
             for (int k : keyIndex) {
@@ -583,8 +663,8 @@ public:
                 for (size_t a = 0; a < na; ++a) { pv.push_back(values[a].data()); pvn.push_back(valueNull[a].data()); }
                 ytgpu_groupby_multi_result res{0, cap, pk.data(), pkn.data(), pv.data(), pvn.data(), nullptr, nullptr};
                 ytgpu_predicate pred{CmpOf(query.WhereOp), 0, query.WhereConstant.Data.Uint64};
-                if (query.Where) pred = ytgpu_predicate{YTGPU_CMP_EQ, 0, 1};
-                const int predArg = query.Where ? predicateColumn : (whereIndex >= 0 ? argIndex[whereIndex] : -1);
+                if (where) pred = ytgpu_predicate{YTGPU_CMP_EQ, 0, 1};
+                const int predArg = where ? predicateColumn : (whereIndex >= 0 ? argIndex[whereIndex] : -1);
                 ytgpu_error err{};
                 const int code = ytgpu_scan_filter_groupby_multi_strings(
                     GetGpuContext(), keyViews.data(), (uint32_t)nk, valueViews.data(), (uint32_t)valueViews.size(), aggregates.data(),
@@ -607,17 +687,90 @@ public:
                     }
                 };
                 auto stringsOf = [&](int index) { return columns[index].Type == EValueType::String ? &columns[index] : nullptr; };
-                owned.reserve(res.group_count);
-                for (uint64_t g = 0; g < res.group_count; ++g) {  // already in first-seen order
+                // the output row's positions: group items, then aggregates
+                struct TOutput {
+                    EValueType Type;
+                    const TFlatColumn* Strings;
+                    const uint64_t* Values;
+                    const uint8_t* Null;  // bytemap
+                };
+                std::vector<TOutput> outputs;
+                for (size_t k = 0; k < nk; ++k)
+                    outputs.push_back({columns[keyIndex[k]].Type, stringsOf(keyIndex[k]), keys[k].data(), keyNull[k].data()});
+                for (size_t a = 0; a < na; ++a) {
+                    const auto f = query.AggregateItems[a].Function;
+                    const EValueType type = f == EAggregateFunction::Count ? EValueType::Int64
+                        : f == EAggregateFunction::Avg ? EValueType::Double : columns[aggIndex[a]].Type;
+                    outputs.push_back({type, f == EAggregateFunction::Count ? nullptr : stringsOf(aggIndex[a]), values[a].data(), valueNull[a].data()});
+                }
+                const uint64_t groups = res.group_count;
+                // Select: a bare Column passes its position through; every other item is one ytgpu_evaluate_expression call over
+                // the result arrays (a string position is refused by the call as UNSUPPORTED)
+                std::vector<std::vector<uint64_t>> selectValues, selectNulls;  // selectNulls: null bitmaps
+                std::vector<TOutput> selected;
+                if (query.Select) {
+                    std::vector<std::vector<uint8_t>> bitmaps(outputs.size());
+                    std::vector<ytgpu_column_view> outViews;
+                    for (size_t p = 0; p < outputs.size(); ++p) {
+                        bitmaps[p].assign((groups + 63) / 64 * 8, 0);
+                        for (uint64_t g = 0; g < groups; ++g)
+                            if (outputs[p].Null[g]) bitmaps[p][g >> 3] |= (uint8_t)(1u << (g & 7));
+                        ytgpu_column_view v{};
+                        v.value_count = (int64_t)groups;
+                        v.value_type = (uint8_t)(outputs[p].Strings ? EValueType::String
+                                                 : outputs[p].Type == EValueType::Null ? EValueType::Int64 : outputs[p].Type);
+                        v.has_values = 1;
+                        v.bit_width = 64;
+                        v.values = outputs[p].Values;
+                        v.values_count = groups;
+                        v.null_bitmap = bitmaps[p].data();
+                        v.mem = YTGPU_MEM_HOST;
+                        outViews.push_back(v);
+                    }
+                    selectValues.resize(query.Select->size());
+                    selectNulls.resize(query.Select->size());
+                    for (size_t s = 0; s < query.Select->size(); ++s) {
+                        const auto& nodes = (*query.Select)[s].Nodes;
+                        if (nodes.size() == 1 && nodes[0].Op == EExpressionOp::Column) {
+                            if (nodes[0].Column < 0 || (size_t)nodes[0].Column >= outputs.size())
+                                throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "select item " + std::to_string(s) + ": no output position " +
+                                                                                      std::to_string(nodes[0].Column));
+                            selected.push_back(outputs[nodes[0].Column]);
+                            continue;
+                        }
+                        std::vector<ytgpu_expr_node> program;
+                        for (const auto& node : nodes) {
+                            ytgpu_expr_node x{};
+                            x.op = (int32_t)node.Op;
+                            x.column = node.Column;
+                            x.type = (uint8_t)node.Type;
+                            x.constant = node.Bits;
+                            program.push_back(x);
+                        }
+                        selectValues[s].assign(groups, 0);
+                        selectNulls[s].assign((groups + 63) / 64, 0);
+                        uint8_t type = 0;
+                        ytgpu_error serr{};
+                        if (ytgpu_evaluate_expression(GetGpuContext(), outViews.data(), (uint32_t)outViews.size(), program.data(),
+                                                      (uint32_t)program.size(), nullptr, selectValues[s].data(),
+                                                      reinterpret_cast<uint8_t*>(selectNulls[s].data()), &type, nullptr, YTGPU_MEM_HOST,
+                                                      &serr) != YTGPU_OK)
+                            ThrowFrom(serr);
+                        selected.push_back({(EValueType)type, nullptr, selectValues[s].data(), nullptr});
+                    }
+                }
+                owned.reserve(groups);
+                for (uint64_t g = 0; g < groups; ++g) {  // already in first-seen order
                     TUnversionedOwningRowBuilder b;
-                    int id = 0;
-                    for (size_t k = 0; k < nk; ++k, ++id)
-                        b.AddValue(make(stringsOf(keyIndex[k]), columns[keyIndex[k]].Type, keys[k][g], keyNull[k][g], id));
-                    for (size_t a = 0; a < na; ++a, ++id) {
-                        const auto f = query.AggregateItems[a].Function;
-                        const EValueType type = f == EAggregateFunction::Count ? EValueType::Int64
-                            : f == EAggregateFunction::Avg ? EValueType::Double : columns[aggIndex[a]].Type;
-                        b.AddValue(make(f == EAggregateFunction::Count ? nullptr : stringsOf(aggIndex[a]), type, values[a][g], valueNull[a][g], id));
+                    if (query.Select) {
+                        for (size_t s = 0; s < selected.size(); ++s) {
+                            const TOutput& o = selected[s];
+                            const bool null = o.Null ? o.Null[g] != 0 : ((selectNulls[s][g >> 6] >> (g & 63)) & 1) != 0;
+                            b.AddValue(make(o.Strings, o.Type, o.Values[g], null, (int)s));
+                        }
+                    } else {
+                        for (size_t p = 0; p < outputs.size(); ++p)
+                            b.AddValue(make(outputs[p].Strings, outputs[p].Type, outputs[p].Values[g], outputs[p].Null[g], (int)p));
                     }
                     owned.push_back(b.FinishRow());
                 }

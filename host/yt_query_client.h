@@ -156,6 +156,44 @@ struct TFilterExpression {
     TFilterExpression& Not() { Nodes.push_back({EFilterOp::Not, EBinaryOp::None, -1, -1, {}, {}}); return *this; }
 };
 
+//! An arithmetic, bitwise, cast or if_null expression, evaluated on the GPU into a computed column (ytgpu_evaluate_expression:
+//! the semantics — NULLs, wrap-around, division errors, casts — are in include/ytgpu.h).  Nodes are in postfix order; a
+//! Column leaf names a position (in the input rows for TMultiGroupQuery::Computed, in the output row for Select).  Binary
+//! operands have one type: there is no implicit widening, write Cast.
+enum class EExpressionOp {
+    Column = 1, Constant = 2, Add = 3, Sub = 4, Mul = 5, Div = 6, Mod = 7, Neg = 8, BitAnd = 9, BitOr = 10, BitXor = 11, BitNot = 12,
+    Cast = 13, IfNull = 14
+};
+struct TExpressionNode {
+    EExpressionOp Op = EExpressionOp::Column;
+    int Column = -1;                      // Column
+    EValueType Type = EValueType::Null;   // Constant: its type; Cast: the target type
+    uint64_t Bits = 0;                    // Constant: Int64 / Uint64 / Double bit pattern, Boolean 0 / 1
+};
+struct TExpression {
+    std::vector<TExpressionNode> Nodes;
+    TExpression& Column(int position) { Nodes.push_back({EExpressionOp::Column, position, EValueType::Null, 0}); return *this; }
+    TExpression& Constant(const TUnversionedValue& v) {
+        Nodes.push_back({EExpressionOp::Constant, -1, v.Type, v.Type == EValueType::Boolean ? (v.Data.Boolean ? 1u : 0u) : v.Data.Uint64});
+        return *this;
+    }
+    TExpression& Add() { return Op(EExpressionOp::Add); }
+    TExpression& Sub() { return Op(EExpressionOp::Sub); }
+    TExpression& Mul() { return Op(EExpressionOp::Mul); }
+    TExpression& Div() { return Op(EExpressionOp::Div); }
+    TExpression& Mod() { return Op(EExpressionOp::Mod); }
+    TExpression& Neg() { return Op(EExpressionOp::Neg); }
+    TExpression& BitAnd() { return Op(EExpressionOp::BitAnd); }
+    TExpression& BitOr() { return Op(EExpressionOp::BitOr); }
+    TExpression& BitXor() { return Op(EExpressionOp::BitXor); }
+    TExpression& BitNot() { return Op(EExpressionOp::BitNot); }
+    TExpression& Cast(EValueType type) { Nodes.push_back({EExpressionOp::Cast, -1, type, 0}); return *this; }
+    TExpression& IfNull() { return Op(EExpressionOp::IfNull); }
+
+private:
+    TExpression& Op(EExpressionOp op) { Nodes.push_back({op, -1, EValueType::Null, 0}); return *this; }
+};
+
 struct TMultiGroupQuery {
     std::vector<int> GroupColumns;               // positions of the group items in the input rows (1..8)
     std::vector<TAggregateItem> AggregateItems;
@@ -163,6 +201,15 @@ struct TMultiGroupQuery {
     EBinaryOp WhereOp = EBinaryOp::None;
     TUnversionedValue WhereConstant{};
     std::optional<TFilterExpression> Where;      // a general WHERE expression; not together with WhereOp
+    //! Computed columns: expressions over positions of the input rows.  Computed column j is named by the position
+    //! ComputedColumn(j) wherever an input position may stand: group items, aggregate Column / ByColumn, WhereColumn and the
+    //! leaves of Where.  Each one that is named is evaluated once.
+    std::vector<TExpression> Computed;
+    static constexpr int ComputedColumn(int j) { return -2 - j; }
+    static constexpr bool IsComputedColumn(int position) { return position <= -2; }
+    //! The output row: expressions over its positions (group items first, then aggregates), e.g. sum(b) + x.  Without it
+    //! the output row is the group items followed by the aggregates.
+    std::optional<std::vector<TExpression>> Select;
 };
 
 struct TQueryStatistics {
@@ -181,6 +228,13 @@ struct IEvaluator {
     //! most 2^30 per query fragment).  Every column holds one type of Int64 / Uint64 / Double / Boolean / String (or Null);
     //! a string group item goes through ytgpu_string_value_ids, and min / max / first / count / argmin / argmax take string
     //! arguments.  sum / avg of a string column and a string WHERE column throw YTGPU_ERR_UNSUPPORTED.
+    //! Computed columns are evaluated with ytgpu_evaluate_expression, nothing on the host, in QL's order: first those the
+    //! WHERE reads, over all rows; then the WHERE, once, as a filter pass (with computed columns the WhereOp form runs as a
+    //! one-node COMPARE program, which selects the same rows); then the other computed columns over the selected rows only,
+    //! so a division by zero in a row the WHERE drops does not throw.  Select items are evaluated the same way over the
+    //! result rows; a bare Column of a string result passes through, arithmetic on it throws YTGPU_ERR_UNSUPPORTED, as does
+    //! an expression over a string input column.  Errors of the calls (a division by zero, a mistyped expression:
+    //! YTGPU_ERR_INVALID_ARGUMENT) throw TErrorException.  A query without computed columns and Select runs as before.
     virtual TQueryStatistics Run(const TMultiGroupQuery& query, const ISchemalessMultiChunkReaderPtr& reader,
                                  const IUnversionedRowsetWriterPtr& writer) = 0;
 };

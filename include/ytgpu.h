@@ -663,6 +663,83 @@ int ytgpu_evaluate_filter(ytgpu_context* ctx, const ytgpu_column_view* columns, 
                           uint8_t* out_bitmap, uint8_t* out_bytemap, uint32_t* out_rows, uint64_t rows_capacity,
                           uint64_t* out_selected /* host */, int out_mem, ytgpu_error* err);
 
+/* ---- computed columns: arithmetic, bitwise, cast and if_null expressions ----
+ * The projections of YT QL's expression compiler (cg_fragment_compiler.cpp) that a GROUP BY key (`group by a % 2`), an
+ * aggregate argument (`sum(price * qty)`) or a WHERE leaf (`a + b > 10`) may hold.  An expression is a PROGRAM of nodes in
+ * POSTFIX order, evaluated row by row into a computed column.  The program is typed: the type of every node follows from the
+ * column types, the constants' types and the CAST targets, and is checked before the launch.
+ *   COLUMN(column)           the row's value of columns[column]: INT64, UINT64, DOUBLE or BOOLEAN, in any encoding the
+ *                            GROUP BY calls take (a BOOLEAN payload other than 0 is read as 1)
+ *   CONSTANT(type, constant) the bit pattern `constant` of type INT64, UINT64, DOUBLE or BOOLEAN (0 / 1)
+ *   ADD, SUB, MUL, DIV       two operands of one type INT64, UINT64 or DOUBLE; the result has that type
+ *   MOD                      two operands of one type INT64 or UINT64
+ *   NEG                      one operand INT64, UINT64 or DOUBLE
+ *   BIT_AND, BIT_OR, BIT_XOR two operands of one type INT64 or UINT64; BIT_NOT one
+ *   CAST(type)               one operand of any of the four types to INT64, UINT64 or DOUBLE
+ *   IF_NULL                  two operands of one type, any of the four
+ * There is no implicit widening (QL has none between int64 and uint64): binary operands of different types are an error,
+ * the caller inserts CAST.  Semantics:
+ *   NULL     a NULL operand makes the result NULL, except IF_NULL(a, b), which is a when a is not NULL and b otherwise.  NULL
+ *            is what the GROUP BY calls take as NULL: a null bit, an Arrow validity bit, a dictionary index of 0,
+ *            has_values = 0.
+ *   integers ADD, SUB, MUL and NEG wrap mod 2^64 (NEG of INT64_MIN is INT64_MIN).  DIV truncates toward zero and MOD has the
+ *            sign of the dividend, as C's / and %.  BIT_* act on the 64-bit pattern.
+ *   division an integer DIV or MOD by 0 fails the call with YTGPU_ERR_INVALID_ARGUMENT and the message "Division by zero";
+ *            INT64_MIN / -1 and INT64_MIN % -1 fail it with "Division INT_MIN by -1".  A row whose divisor or dividend is
+ *            NULL, and a row outside the selection, never fails.  After a failure the outputs' contents are unspecified.
+ *   doubles  IEEE-754 with round to nearest (x / 0 is +-inf, 0 / 0 is NaN); every operation is rounded on its own, never
+ *            contracted into an FMA.  NEG flips the sign bit.  The sign and payload of a NaN that ADD, SUB, MUL or DIV
+ *            produces are unspecified (the GPU returns a canonical NaN, not an operand's payload).
+ *   CAST     INT64 <-> UINT64 keeps the bits (two's complement); an integer to DOUBLE rounds to nearest; DOUBLE to an integer
+ *            truncates toward zero, and an out-of-range value follows PTX's saturating cvt.rzi: a value below / above the
+ *            range becomes the type's minimum / maximum.  NaN becomes 0 (tested for explicitly: on sm_90 the 64-bit
+ *            cvt.rzi.s64.f64 returns INT64_MIN for it).  The reference compiles this cast with
+ *            LLVM fptosi / fptoui, whose result for those inputs is poison, so this rule has no counterpart there.  BOOLEAN
+ *            becomes 0 / 1 or 0.0 / 1.0; a cast to the operand's own type is the identity.
+ * These rules were not checked against YT QL's own evaluator; in particular the two division-error messages and the
+ * INT64_MIN / -1 check are recalled from cg_fragment_compiler.cpp, not read there.
+ *
+ * selection (nullable, out_mem): a bitmap in the layout of ytgpu_evaluate_filter's out_bitmap.  A row whose bit is clear is
+ * not evaluated: its result is NULL and it raises no division error (QL evaluates projections after WHERE, so a division by
+ * zero in a row the WHERE drops must not fail the query).
+ * Outputs, in out_mem:
+ *   out_values      n 64-bit bit patterns in the result type; a NULL row holds 0.
+ *   out_null_bitmap 8 * ceil(n / 64) bytes; bit i (LSB first) set when row i is NULL, the bits past n zero.  So
+ *                   {value_type = *out_value_type, bit_width = 64, has_values = 1, values = out_values, values_count = n,
+ *                   value_count = n, null_bitmap = out_null_bitmap} is a column the GROUP BY, filter and decode calls take.
+ *   *out_value_type (host, nullable) the result type, written once the program is checked.
+ *   *out_null_count (host, nullable) the number of NULL rows, so a caller may drop the bitmap from the view when it is 0.
+ * Launches: one evaluation kernel and one read of the NULL count and the error word.  HOST inputs are copied to the device
+ * first.
+ * YTGPU_ERR_INVALID_ARGUMENT: a malformed program (stack underflow, other than one value left, a stack deeper than 16, more
+ * than 64 nodes, an unknown op or type, a column out of range), operand types an op does not take, a BOOLEAN constant other
+ * than 0 / 1, no columns (they give the row count), columns of different lengths, 2^32 rows or more, a division error
+ * above.  YTGPU_ERR_UNSUPPORTED: a column of
+ * another type (strings included). */
+typedef enum ytgpu_expr_op {
+    YTGPU_EXPR_COLUMN = 1, YTGPU_EXPR_CONSTANT = 2,
+    YTGPU_EXPR_ADD = 3, YTGPU_EXPR_SUB = 4, YTGPU_EXPR_MUL = 5, YTGPU_EXPR_DIV = 6, YTGPU_EXPR_MOD = 7, YTGPU_EXPR_NEG = 8,
+    YTGPU_EXPR_BIT_AND = 9, YTGPU_EXPR_BIT_OR = 10, YTGPU_EXPR_BIT_XOR = 11, YTGPU_EXPR_BIT_NOT = 12,
+    YTGPU_EXPR_CAST = 13, YTGPU_EXPR_IF_NULL = 14
+} ytgpu_expr_op;
+
+#define YTGPU_EXPR_MAX_NODES 64
+#define YTGPU_EXPR_MAX_DEPTH 16
+
+typedef struct ytgpu_expr_node {
+    int32_t op;          /* ytgpu_expr_op */
+    int32_t column;      /* COLUMN: index into columns */
+    uint8_t type;        /* CONSTANT: its value type; CAST: the target type (YTGPU_TYPE_*) */
+    uint8_t reserved[7];
+    uint64_t constant;   /* CONSTANT: the bit pattern in `type` */
+} ytgpu_expr_node;
+
+int ytgpu_evaluate_expression(ytgpu_context* ctx, const ytgpu_column_view* columns, uint32_t column_count,
+                              const ytgpu_expr_node* program /* host */, uint32_t node_count,
+                              const uint8_t* selection /* nullable, out_mem */, uint64_t* out_values,
+                              uint8_t* out_null_bitmap, uint8_t* out_value_type /* host, nullable */,
+                              uint64_t* out_null_count /* host, nullable */, int out_mem, ytgpu_error* err);
+
 /* ---- segmented SUM / COUNT over rows ALREADY SORTED by the group key (the aggregate stage after a sort) ----
  * Consecutive rows with equal keys form a group; no hash table.  Replaces the per-group accumulation of a GROUP BY
  * over a sorted stream / a sorted reduce (yt/yt/library/query/engine/cg_routines/registry.cpp:1838-1920 for the

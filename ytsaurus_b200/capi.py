@@ -113,7 +113,7 @@ EXPORTED_SYMBOLS = [
     "ytgpu_scatter_rows_to_peers", "ytgpu_shuffle_create", "ytgpu_shuffle_connect", "ytgpu_shuffle_sort",
     "ytgpu_shuffle_destroy", "ytgpu_reduce_sorted_fixed_rows", "ytgpu_context_set_option", "ytgpu_context_notify", "ytgpu_decode_horizontal_block", "ytgpu_encode_horizontal_block",
     "ytgpu_decode_column", "ytgpu_decode_string_offsets", "ytgpu_decode_string_pointers_and_lengths", "ytgpu_scan_filter_groupby", "ytgpu_scan_filter_groupby_multi",
-    "ytgpu_scan_filter_groupby_multi_strings", "ytgpu_evaluate_filter",
+    "ytgpu_scan_filter_groupby_multi_strings", "ytgpu_evaluate_filter", "ytgpu_evaluate_expression",
     "ytgpu_convert_integer_column", "ytgpu_encode_integer_column", "ytgpu_encode_double_column", "ytgpu_encode_boolean_column", "ytgpu_encode_string_column", "ytgpu_decode_string_segment", "ytgpu_string_value_ids", "ytgpu_extract_column",
     "ytgpu_block_agg_state_init", "ytgpu_block_combine_all",
     "ytgpu_build_bitmap_from_flags", "ytgpu_build_bytemap_from_flags", "ytgpu_count_flags", "ytgpu_build_dictionary_indexes",
@@ -164,6 +164,15 @@ FILTER_MAX_NODES, FILTER_MAX_DEPTH, FILTER_MAX_IN_ENTRIES, FILTER_MAX_STRING_CON
 class FilterNode(C.Structure):
     _fields_ = [("op", C.c_int32), ("cmp", C.c_int32), ("column", C.c_int32), ("column2", C.c_int32), ("constant", C.c_uint64),
                 ("length", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+(EXPR_COLUMN, EXPR_CONSTANT, EXPR_ADD, EXPR_SUB, EXPR_MUL, EXPR_DIV, EXPR_MOD, EXPR_NEG, EXPR_BIT_AND, EXPR_BIT_OR, EXPR_BIT_XOR,
+ EXPR_BIT_NOT, EXPR_CAST, EXPR_IF_NULL) = range(1, 15)
+EXPR_MAX_NODES, EXPR_MAX_DEPTH = 64, 16
+
+
+class ExprNode(C.Structure):
+    _fields_ = [("op", C.c_int32), ("column", C.c_int32), ("type", C.c_uint8), ("reserved", C.c_uint8 * 7), ("constant", C.c_uint64)]
 
 
 class GroupByMultiResult(C.Structure):
@@ -240,6 +249,8 @@ def load() -> C.CDLL:
     lib.ytgpu_evaluate_filter.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p,
                                           C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64,
                                           C.POINTER(C.c_uint64), C.c_int, C.POINTER(Error)]
+    lib.ytgpu_evaluate_expression.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.POINTER(C.c_uint8), C.POINTER(C.c_uint64), C.c_int, C.POINTER(Error)]
     lib.ytgpu_partition_rowset.argtypes = [C.c_void_p, C.POINTER(RowsetView), C.POINTER(PartitionSpec), C.c_void_p,
                                            C.c_void_p, C.c_int, C.POINTER(Error)]
     lib.ytgpu_partition_rowset_slabs.argtypes = [C.c_void_p, C.POINTER(RowsetView), C.POINTER(PartitionSpec), C.c_void_p, C.c_void_p,

@@ -133,6 +133,21 @@ __device__ __forceinline__ u64 decode_at(const ColumnDev& c, i64 i, bool* ch_nul
     return x;
 }
 
+// Value of row i of a column for interpreters that give each warp 32 consecutive rows (warp_row: the warp's first row) and
+// run the same node in every lane: lane 0 finds the run of the warp's first row of an RLE column, the other lanes walk on
+// from there.  A row that is not live reads nothing and is NULL.
+__device__ __forceinline__ u64 scalar_value(const ColumnDev& c, u64 i, u64 warp_row, bool live, bool* nul) {
+    u64 hint = kNoRleHint;
+    if (c.rle && c.has_values) {
+        u64 h = 0;
+        if ((threadIdx.x & 31) == 0) h = rle_pos(c.rle, c.rle_count, (u64)c.start + warp_row);
+        hint = __shfl_sync(0xffffffffu, h, 0);
+    }
+    *nul = true;
+    if (!live) return 0;
+    return decode_at(c, (i64)i, nul, hint);
+}
+
 // Fast path: plain 64-bit value vector (no dictionary / RLE / null bitmap); base and zig-zag still apply.
 __host__ __device__ __forceinline__ bool is_direct64(const ColumnDev& c) {
     return c.has_values && c.bit_width == 64 && !c.dict && !c.rle && !c.bitmap;

@@ -89,20 +89,6 @@ __device__ __forceinline__ const u8* const_heap(const FilterArgs& A, const u8* s
     return off + len <= A.staged_const ? s_const : A.consts;
 }
 
-// Scalar value of row i of a column; lane 0 finds the run of the warp's first row for an RLE column (uniform branch: every
-// lane evaluates the same node).
-__device__ __forceinline__ u64 scalar_value(const ColumnDev& c, u64 i, u64 warp_row, bool live, bool* nul) {
-    u64 hint = kNoRleHint;
-    if (c.rle && c.has_values) {
-        u64 h = 0;
-        if ((threadIdx.x & 31) == 0) h = rle_pos(c.rle, c.rle_count, (u64)c.start + warp_row);
-        hint = __shfl_sync(0xffffffffu, h, 0);
-    }
-    *nul = true;
-    if (!live) return 0;
-    return decode_at(c, (i64)i, nul, hint);
-}
-
 __global__ void __launch_bounds__(kFilterThreads) filter_kernel(const FilterArgs A) {
     extern __shared__ __align__(16) unsigned char smem[];
     NodeDev* s_nodes = reinterpret_cast<NodeDev*>(smem);

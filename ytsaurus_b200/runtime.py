@@ -848,6 +848,37 @@ class GpuContext:
             raise e
         return dict(bitmap=bitmap, bytemap=bytemap, rows=rows[:count] if rows is not None else None, count=count)
 
+    def evaluate_expression(self, columns, program, selection=None):
+        """Computed column (ytgpu_evaluate_expression) -> dict(values, null_bitmap, null_count, value_type, column).
+        columns: Column objects; program: postfix nodes, each a capi.ExprNode or a tuple (op, column, type, constant).
+        selection: nullable bitmap in ytgpu_evaluate_filter's layout (its "bitmap" output).  The outputs are in the inputs'
+        memory flavour: values n uint64 (int64 on the device), null_bitmap 8 * ceil(n / 64) bytes; `column` is a Column
+        over them (without the bitmap when no row is NULL), ready for scan_filter_groupby_multi / evaluate_filter."""
+        views = [c.view() for c in columns]
+        if not views:
+            raise ValueError("evaluate_expression needs at least one column")
+        mem, n = views[0].mem, int(views[0].value_count)
+        carr = (capi.ColumnView * len(views))(*views)
+        nodes = (capi.ExprNode * max(len(program), 1))()
+        for i, node in enumerate(program):
+            if isinstance(node, capi.ExprNode):
+                nodes[i] = node
+            else:
+                op, column, vtype, constant = (tuple(node) + (0,) * 4)[:4]
+                nodes[i].op, nodes[i].column, nodes[i].type = op, column, vtype
+                nodes[i].constant = int(constant) & 0xFFFFFFFFFFFFFFFF
+        words = (n + 63) // 64
+        values = self._out((n,), np.uint64, mem)
+        null_bitmap = self._out((words * 8,), np.uint8, mem)
+        vtype, nulls = C.c_uint8(0), C.c_uint64(0)
+        err = capi.Error()
+        capi.check(self.lib.ytgpu_evaluate_expression(self.handle, C.cast(carr, C.c_void_p), len(views), C.cast(nodes, C.c_void_p),
+                                                      len(program), _ptr_mem(selection)[0], _ptr_mem(values)[0],
+                                                      _ptr_mem(null_bitmap)[0], C.byref(vtype), C.byref(nulls), mem, C.byref(err)), err)
+        column = Column(int(vtype.value), values=values, value_count=n,
+                        null_bitmap=null_bitmap if nulls.value else None)
+        return dict(values=values, null_bitmap=null_bitmap, null_count=int(nulls.value), value_type=int(vtype.value), column=column)
+
 
 class Column:
     """Host- or device-side description of IUnversionedColumnarRowBatch::TColumn (row_batch.h:49-191)."""
