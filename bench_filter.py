@@ -15,9 +15,13 @@ steps; call time from CUDA events around the whole call):
   one_compare   ts >= a
   conjunction   ts >= a AND ts < b AND k IN (16 values) AND (d < x OR b)
   with_prefix   conjunction AND STARTS_WITH(url, "https://")
+  contains      CONTAINS(url, "site4")                           (QL is_substr("site4", url))
+  like          url LIKE 'https://www.site_.example.com/%q%'
 Each leg reports its algorithmic bytes per row — the bytes of the column data it reads plus 1/8 byte of bitmap written
 (the kernel evaluates every node for every row, so every referenced column is read) — and that traffic over the kernel
-time, against the HBM peak (MEASURED_PEAKS.json's when present, else the 3.35 TB/s data-sheet figure of the H100 SXM).
+time, against the HBM peak.  A CONTAINS / LIKE leg reads the start (8) and length (4) of every row and the value bytes the
+matcher consumes, which the bench counts exactly from the generated URLs: the matcher stops at a segment's earliest end
+and an anchored segment stops at its first mismatch (MEASURED_PEAKS.json's when present, else the 3.35 TB/s data-sheet figure of the H100 SXM).
 GROUP BY leg: two int64 keys (U[0, 1000) x U[0, 8)), SUM + MIN + MAX + AVG of an int64 column, through
 ytgpu_scan_filter_groupby_multi with `ts >= a` as its built-in predicate against the filter pass + the bitmap as a
 BOOLEAN column + the predicate {EQ, 1}; both results must be identical.
@@ -69,6 +73,52 @@ def hbm_peak():
     return DATASHEET_HBM_BPS, "H100 SXM data sheet"
 
 
+def _url_parts(heap, lengths):
+    """The generated URLs are "https://www.site<k>.example.com/" (k < 64) + lowercase letters, in 96-byte slots."""
+    import torch
+    rows = heap.view(-1, 96)
+    digit2 = (rows[:, 17] >= 48) & (rows[:, 17] <= 57)  # a two-digit site number
+    site4 = rows[:, 16] == ord("4")
+    one_digit = ~digit2
+    tail = rows[:, 30:]
+    valid = torch.arange(66, device=heap.device)[None, :] < (lengths.long() - 30)[:, None]
+    isq = (tail == ord("q")) & valid
+    has_q = isq.any(dim=1)
+    first_q = torch.where(has_q, isq.to(torch.uint8).argmax(dim=1), lengths.long() - 31)  # index of the last byte when no q
+    return site4, one_digit, has_q, first_q
+
+
+def url_bytes_read(heap, lengths, chunk=1 << 24):
+    """Mean value bytes the matcher consumes per row for CONTAINS(url, "site4") and the LIKE leg's pattern."""
+    n = len(lengths)
+    c_sum = l_sum = 0
+    for a in range(0, n, chunk):
+        b = min(n, a + chunk)
+        site4, one_digit, _, first_q = _url_parts(heap[a * 96:b * 96], lengths[a:b])
+        ln = lengths[a:b].long()
+        c_sum += int((ln.where(~site4, 17)).sum().item())  # "site4" ends at byte 17; no letter tail holds a digit
+        # the anchored first segment dies at byte 18 for a two-digit site; otherwise 30 bytes, then up to the first q
+        l_sum += int(torch_where(one_digit, 30 + first_q + 1, 18).sum().item())
+    return c_sum / n, l_sum / n
+
+
+def url_counts(heap, lengths, chunk=1 << 24):
+    """Rows the CONTAINS and LIKE legs select, from the generator's structure (a cross-check of the kernel's count)."""
+    n = len(lengths)
+    c = l_cnt = 0
+    for a in range(0, n, chunk):
+        b = min(n, a + chunk)
+        site4, one_digit, has_q, _ = _url_parts(heap[a * 96:b * 96], lengths[a:b])
+        c += int(site4.sum().item())
+        l_cnt += int((one_digit & has_q).sum().item())
+    return c, l_cnt
+
+
+def torch_where(cond, a, b):
+    import torch
+    return torch.where(cond, a, torch.as_tensor(b, device=cond.device))
+
+
 def median_ms(values):
     return round(statistics.median(values), 4)
 
@@ -115,16 +165,21 @@ def main():
             (cmp_, capi.CMP_LT, D, 0, x, 0), (cmp_, capi.CMP_EQ, B, 0, 1, 0), (or_,), (and_,)]
     prefix = conj + [(sw, 0, URL, 0, 0, 8), (and_,)]
     consts = b"https://"
+    needle, pattern = b"site4", b"https://www.site_.example.com/%q%"
     bitmap_write = 1 / 8
+    read_contains, read_like = url_bytes_read(heap, lengths)
     legs = {
-        "one_compare": (one, 8 + bitmap_write),
-        "conjunction": (conj, 8 + 4 + 8 + 1 / 8 + bitmap_write),
-        "with_prefix": (prefix, 8 + 4 + 8 + 1 / 8 + 8 + 4 + 8 + bitmap_write),  # + starts, lengths, the 8 prefix bytes
+        "one_compare": (one, consts, 8 + bitmap_write),
+        "conjunction": (conj, consts, 8 + 4 + 8 + 1 / 8 + bitmap_write),
+        "with_prefix": (prefix, consts, 8 + 4 + 8 + 1 / 8 + 8 + 4 + 8 + bitmap_write),  # + starts, lengths, the 8 prefix bytes
+        "contains": ([(capi.FILTER_CONTAINS, 0, URL, 0, 0, len(needle))], needle, 8 + 4 + read_contains + bitmap_write),
+        "like": ([(capi.FILTER_LIKE, 0, URL, -1, 0, len(pattern))], pattern, 8 + 4 + read_like + bitmap_write),
     }
+    line["url_mean_bytes"] = round(lengths.double().mean().item(), 4)
     ctx.enable_timers(True)
-    for leg_name, (prog, bytes_per_row) in legs.items():
-        def call(p=prog):
-            return ctx.evaluate_filter(cols, strings, p, in_list, consts, want_bytemap=False, want_rows=False)
+    for leg_name, (prog, leg_consts, bytes_per_row) in legs.items():
+        def call(p=prog, c=leg_consts):
+            return ctx.evaluate_filter(cols, strings, p, in_list, c, want_bytemap=False, want_rows=False)
         for _ in range(args.warmup):
             call()
         kernel, calls = [], []
@@ -145,6 +200,8 @@ def main():
     ctx.enable_timers(False)
     # parity of the one-comparison leg with torch
     line["one_compare"]["count_matches_torch"] = line["one_compare"]["selected"] == int((ts >= lo).sum().item())
+    line["contains"]["count_matches_torch"], line["like"]["count_matches_torch"] = [
+        line[k]["selected"] == c for k, c in zip(("contains", "like"), url_counts(heap, lengths))]
     del heap, starts, lengths, strings
 
     # GROUP BY: built-in predicate vs filter pass + bitmap column

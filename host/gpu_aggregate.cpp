@@ -588,9 +588,12 @@ public:
                             f.column2 = callIndex(filterIndex2[k]);
                             break;
                         case EFilterOp::StartsWith:
+                        case EFilterOp::Contains:
+                        case EFilterOp::Like:
                             typed(node.Constant);
                             f.constant = addString(node.Constant.Bytes);
                             f.length = (uint32_t)node.Constant.Bytes.size();
+                            if (node.Op == EFilterOp::Like) f.column2 = node.Escape;
                             break;
                         case EFilterOp::In:
                             f.constant = lists.size();

@@ -100,11 +100,14 @@ struct TAggregateItem {
     int Column = 0;     // position of the argument in the input rows (argmin / argmax: the returned column)
     int ByColumn = -1;  // argmin / argmax: the minimised / maximised column
 };
-//! A WHERE expression of AND / OR / NOT over comparisons, IN lists, NULL tests and prefix tests, evaluated on the GPU
+//! A WHERE expression of AND / OR / NOT over comparisons, IN lists, NULL tests, prefix and substring tests and LIKE
+//! patterns, evaluated on the GPU
 //! (ytgpu_evaluate_filter: the semantics, three-valued logic included, are in include/ytgpu.h).  Nodes are in postfix
 //! order; columns are positions in the input rows.  A constant has the column's type (a mistyped constant is
 //! INVALID_ARGUMENT); string constants and IN lists are owned by the expression.
-enum class EFilterOp { Compare = 1, CompareColumns = 2, In = 3, StartsWith = 4, IsNull = 5, IsNotNull = 6, And = 7, Or = 8, Not = 9 };
+enum class EFilterOp {
+    Compare = 1, CompareColumns = 2, In = 3, StartsWith = 4, IsNull = 5, IsNotNull = 6, And = 7, Or = 8, Not = 9, Contains = 10, Like = 11
+};
 struct TFilterConstant {
     EValueType Type = EValueType::Null;
     uint64_t Bits = 0;    // Int64 / Uint64 / Double bit pattern, Boolean 0 / 1
@@ -123,8 +126,9 @@ struct TFilterNode {
     EBinaryOp Cmp = EBinaryOp::None;       // Compare, CompareColumns
     int Column = -1;                       // leaves
     int Column2 = -1;                      // CompareColumns
-    TFilterConstant Constant;              // Compare; StartsWith: the prefix (a String)
+    TFilterConstant Constant;              // Compare; StartsWith / Contains / Like: the prefix, needle or pattern (a String)
     std::vector<TFilterConstant> List;     // In
+    int Escape = -1;                       // Like: the escape byte 0..255, -1 for none
 };
 struct TFilterExpression {
     std::vector<TFilterNode> Nodes;
@@ -147,6 +151,22 @@ struct TFilterExpression {
         c.Type = EValueType::String;
         c.Bytes = prefix;
         Nodes.push_back({EFilterOp::StartsWith, EBinaryOp::None, column, -1, c, {}});
+        return *this;
+    }
+    //! QL is_substr(needle, s) / ClickHouse position(s, needle) > 0.
+    TFilterExpression& Contains(int column, const std::string& needle) {
+        TFilterConstant c;
+        c.Type = EValueType::String;
+        c.Bytes = needle;
+        Nodes.push_back({EFilterOp::Contains, EBinaryOp::None, column, -1, c, {}});
+        return *this;
+    }
+    //! s LIKE pattern (% any bytes, _ one UTF-8 character, the escape byte quotes the next byte); NOT LIKE is Like(...).Not().
+    TFilterExpression& Like(int column, const std::string& pattern, std::optional<unsigned char> escape = std::nullopt) {
+        TFilterConstant c;
+        c.Type = EValueType::String;
+        c.Bytes = pattern;
+        Nodes.push_back({EFilterOp::Like, EBinaryOp::None, column, -1, c, {}, escape ? (int)*escape : -1});
         return *this;
     }
     TFilterExpression& IsNull(int column) { Nodes.push_back({EFilterOp::IsNull, EBinaryOp::None, column, -1, {}, {}}); return *this; }

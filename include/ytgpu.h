@@ -587,8 +587,8 @@ int ytgpu_scan_filter_groupby_multi_strings(ytgpu_context* ctx, const ytgpu_colu
 
 /* ---- WHERE expressions: a selection over several columns ----
  * The filter of YT QL's ScanOpHelper / FilterOpHelper (the WHERE clause compiled by the query evaluator) and of
- * ClickHouse's FilterTransform, for expressions built of comparisons, IN lists, NULL tests and prefix tests joined by
- * AND / OR / NOT.  A filter is a PROGRAM of nodes in POSTFIX order; a row is selected iff the program evaluates to TRUE
+ * ClickHouse's FilterTransform, for expressions built of comparisons, IN lists, NULL tests, prefix and substring tests and
+ * LIKE patterns joined by AND / OR / NOT.  A filter is a PROGRAM of nodes in POSTFIX order; a row is selected iff the program evaluates to TRUE
  * under three-valued (Kleene) logic:
  *   COMPARE(column, cmp, constant)        NULL if the value is NULL; otherwise the comparison of the built-in predicate:
  *                                         INT64 signed, UINT64 unsigned, DOUBLE by IEEE (a NaN operand makes every op false
@@ -602,6 +602,31 @@ int ytgpu_scan_filter_groupby_multi_strings(ytgpu_context* ctx, const ytgpu_colu
  *   STARTS_WITH(column, prefix)           string columns only (QL is_prefix, ClickHouse startsWith): NULL if the value is
  *                                         NULL, else whether its first len(prefix) bytes are the prefix.  An empty prefix
  *                                         matches every non-NULL value.
+ *   CONTAINS(column, needle)              string columns only (QL is_substr(needle, s), ClickHouse position(s, needle) > 0):
+ *                                         NULL if the value is NULL, else whether the needle occurs in the value as a
+ *                                         contiguous byte sequence.  An empty needle matches every non-NULL value.
+ *   LIKE(column, pattern, escape)         string columns only: NULL if the value is NULL, else whether the WHOLE value
+ *                                         matches the pattern.  NOT LIKE is LIKE followed by NOT.  Pattern bytes:
+ *                                           %  matches any byte sequence, including the empty one;
+ *                                           _  matches one character: one byte outside 0x80..0xBF, followed by any number
+ *                                              of bytes in 0x80..0xBF;
+ *                                           any other byte matches itself;
+ *                                           with an escape byte E (column2 = 0..255; -1: no escape), E followed by any
+ *                                           byte X matches X literally.  A pattern that ends in a lone E is an error.
+ *                                         A match exists iff some split of the value satisfies the pattern: as a regular
+ *                                         expression over bytes, fully matched, % is [\x00-\xff]*, _ is
+ *                                         [^\x80-\xbf][\x80-\xbf]* and every other byte is itself.  Newlines are ordinary
+ *                                         bytes and matching is case-sensitive.  When the value and the pattern are valid
+ *                                         UTF-8 this is exactly "_ = one code point, % = any code-point sequence", the rule
+ *                                         ClickHouse documents for LIKE.  YT QL's like compiles to an RE2 expression; how
+ *                                         that treats _ on multibyte input and whether % / _ cross a newline (RE2's dot_nl)
+ *                                         was not read in the reference, so those two rules are unverified against YT QL.
+ *                                         Work per row is bounded: the pattern is split at % into segments, each segment is
+ *                                         an NFA run bit-parallel (Shift-And) over ceil(positions / 64) 64-bit words, and
+ *                                         every middle segment takes its earliest end (the next % absorbs any gap).  Each
+ *                                         value byte is consumed by at most one segment scan, so a row costs at most
+ *                                         (value length) * ceil(positions / 64) + segments steps, whatever the pattern: no
+ *                                         backtracking.  CONTAINS(x) is compiled as the pattern %x% without wildcards.
  *   IS_NULL(column), IS_NOT_NULL(column)  never NULL.  NULL is what the group-by calls take as NULL: a dictionary index of
  *                                         0, a null bit or Arrow validity bit, has_values = 0; the null bytemap of a string
  *                                         column.
@@ -613,14 +638,22 @@ int ytgpu_scan_filter_groupby_multi_strings(ytgpu_context* ctx, const ytgpu_colu
  * Node fields by op:
  *   column     index into columns ++ string_columns (column_count + i is string_columns[i]), as ytgpu_aggregate::column
  *   cmp        ytgpu_cmp_op, LT .. NE (COMPARE, COMPARE_COLUMNS)
- *   column2    COMPARE_COLUMNS: the right-hand column
+ *   column2    COMPARE_COLUMNS: the right-hand column; LIKE: the escape byte 0..255, or -1 for none
  *   constant   COMPARE on a scalar column: the bit pattern in the column's type (length must be 0);
- *              COMPARE / STARTS_WITH on a string column: byte offset of the constant in string_constants, `length` bytes;
+ *              COMPARE / STARTS_WITH / CONTAINS / LIKE on a string column: byte offset of the constant (prefix, needle,
+ *              pattern) in string_constants, `length` bytes;
  *              IN: index of the first entry in list_values, `length` entries.  A scalar column's entries are bit patterns
  *              in its type; a string column's are (offset << 32) | length into string_constants.
  * Limits: 1 .. 64 nodes and a stack depth of at most 16; at most 65536 IN entries over all IN nodes of a call; at most
  * 1 MiB of string_constants; fewer than 2^32 rows, and every column (value_count) and string column (row_count) holds
  * the same number of rows.  Scalar columns are INT64, UINT64, DOUBLE or BOOLEAN.
+ * Pattern limits (CONTAINS and LIKE): at most YTGPU_FILTER_MAX_PATTERN_POSITIONS (256) positions per pattern, a position
+ * being one literal byte (an escaped byte included) or one _, so a pattern state is at most 4 words; a CONTAINS needle has
+ * one position per byte.  The patterns of a call compile to at most YTGPU_FILTER_MAX_PATTERN_BYTES (32 KiB), all staged
+ * in shared memory; a pattern with W = ceil(positions / 64) words (W = 1 when it has no position), S non-empty segments
+ * and C byte classes takes 272 + 8 * S + 8 * W * (C + 1) bytes, where C is the number of distinct literal bytes, plus one
+ * if some byte outside 0x80..0xBF is not among them, plus one if some byte in 0x80..0xBF is not among them.  A realistic
+ * 200-byte URL pattern of 40 distinct bytes takes about 2.6 KB.
  * Outputs, each nullable, in out_mem:
  *   out_bitmap   8 * ceil(n / 64) bytes; bit i (LSB first) = row i selected, the bits past n zero.  So
  *                {value_type = BOOLEAN, bit_width = 1, has_values = 1, values = out_bitmap, values_count = n, value_count = n}
@@ -631,25 +664,29 @@ int ytgpu_scan_filter_groupby_multi_strings(ytgpu_context* ctx, const ytgpu_colu
  * Launches: without out_rows one evaluation kernel and one read of the count and the error word; with out_rows four
  * more (an exclusive scan of the per-32-row counts and the row write).  HOST inputs are copied to the device first.
  * YTGPU_ERR_INVALID_ARGUMENT: a malformed program (stack underflow, other than one value left, an unknown op or cmp, a
- * column out of range), STARTS_WITH or a non-zero `length` on a scalar column, COMPARE_COLUMNS over different types, a
- * constant or list range outside its buffer, a limit above, rows_capacity below the selected count (the count is still in
+ * column out of range), STARTS_WITH, CONTAINS, LIKE or a non-zero `length` on a scalar column, COMPARE_COLUMNS over
+ * different types, a constant or list range outside its buffer, a LIKE escape outside -1..255, a LIKE pattern that ends in
+ * a lone escape byte, a limit above, rows_capacity below the selected count (the count is still in
  * *out_selected), a non-NULL string that leaves its heap (checked on the device for the string columns the program reads;
  * no byte outside the heap is read).  YTGPU_ERR_UNSUPPORTED: a scalar column of another type. */
 typedef enum ytgpu_filter_op {
     YTGPU_FILTER_COMPARE = 1, YTGPU_FILTER_COMPARE_COLUMNS = 2, YTGPU_FILTER_IN = 3, YTGPU_FILTER_STARTS_WITH = 4,
-    YTGPU_FILTER_IS_NULL = 5, YTGPU_FILTER_IS_NOT_NULL = 6, YTGPU_FILTER_AND = 7, YTGPU_FILTER_OR = 8, YTGPU_FILTER_NOT = 9
+    YTGPU_FILTER_IS_NULL = 5, YTGPU_FILTER_IS_NOT_NULL = 6, YTGPU_FILTER_AND = 7, YTGPU_FILTER_OR = 8, YTGPU_FILTER_NOT = 9,
+    YTGPU_FILTER_CONTAINS = 10, YTGPU_FILTER_LIKE = 11
 } ytgpu_filter_op;
 
 #define YTGPU_FILTER_MAX_NODES 64
 #define YTGPU_FILTER_MAX_DEPTH 16
 #define YTGPU_FILTER_MAX_IN_ENTRIES 65536
 #define YTGPU_FILTER_MAX_STRING_CONSTANT_BYTES (1u << 20)
+#define YTGPU_FILTER_MAX_PATTERN_POSITIONS 256
+#define YTGPU_FILTER_MAX_PATTERN_BYTES 32768
 
 typedef struct ytgpu_filter_node {
     int32_t op;         /* ytgpu_filter_op */
     int32_t cmp;        /* ytgpu_cmp_op: COMPARE, COMPARE_COLUMNS */
     int32_t column;     /* index into columns ++ string_columns */
-    int32_t column2;    /* COMPARE_COLUMNS */
+    int32_t column2;    /* COMPARE_COLUMNS: a column; LIKE: the escape byte or -1 */
     uint64_t constant;  /* see above */
     uint32_t length;    /* string constant: bytes; IN: number of entries */
     uint32_t reserved;

@@ -157,8 +157,9 @@ class StringColumn(C.Structure):
 
 
 (FILTER_COMPARE, FILTER_COMPARE_COLUMNS, FILTER_IN, FILTER_STARTS_WITH, FILTER_IS_NULL, FILTER_IS_NOT_NULL, FILTER_AND, FILTER_OR,
- FILTER_NOT) = range(1, 10)
+ FILTER_NOT, FILTER_CONTAINS, FILTER_LIKE) = range(1, 12)
 FILTER_MAX_NODES, FILTER_MAX_DEPTH, FILTER_MAX_IN_ENTRIES, FILTER_MAX_STRING_CONSTANT_BYTES = 64, 16, 65536, 1 << 20
+FILTER_MAX_PATTERN_POSITIONS, FILTER_MAX_PATTERN_BYTES = 256, 32768
 
 
 class FilterNode(C.Structure):

@@ -1,5 +1,6 @@
-// filter.cu — WHERE expressions over several columns: AND / OR / NOT of comparisons, IN lists, NULL tests and string
-// prefix tests, evaluated into a selection bitmap / bytemap / row list (ytgpu_evaluate_filter, semantics in ytgpu.h).
+// filter.cu — WHERE expressions over several columns: AND / OR / NOT of comparisons, IN lists, NULL tests, string
+// prefix and substring tests and LIKE patterns, evaluated into a selection bitmap / bytemap / row list
+// (ytgpu_evaluate_filter, semantics in ytgpu.h).
 //
 // One pass over the rows, separate from the aggregation: the result bitmap has the layout of a BOOLEAN column with
 // bit_width 1, so ytgpu_scan_filter_groupby_multi[_strings] aggregates the selected rows through its existing {EQ, 1}
@@ -11,7 +12,10 @@
 //     the lists and constants is read through __ldg;
 //   * the truth stack is two bits per entry (bit 0 TRUE, bit 1 FALSE, neither NULL) in one 32-bit register: 16 entries,
 //     Kleene AND / OR / NOT are two bit operations each, and nothing goes to local memory;
-//   * an RLE column finds its run from a hint that lane 0 finds once per 32 rows (rle_pos_from, as groupby_multi).
+//   * an RLE column finds its run from a hint that lane 0 finds once per 32 rows (rle_pos_from, as groupby_multi);
+//   * CONTAINS and LIKE run the bit-parallel matcher of strings.cuh over patterns compiled on the host and staged in
+//     shared memory after the constants.  The kernel is a template on "the program has pattern nodes", chosen by the host
+//     from the checked program, so programs without them run the same code as before.
 #include <algorithm>
 #include <cstring>
 #include <string>
@@ -55,6 +59,8 @@ struct FilterArgs {
     u32 list_count, staged_list;
     const u8* consts;
     u32 const_bytes, staged_const;
+    const u8* patterns;   // compiled CONTAINS / LIKE patterns (strings.cuh), all staged in shared memory
+    u32 pattern_bytes;
     u64 n;
     u32* bitmap;         // 2 * ceil(n / 64) words of 32 bits
     u8* bytemap;         // nullable
@@ -89,6 +95,10 @@ __device__ __forceinline__ const u8* const_heap(const FilterArgs& A, const u8* s
     return off + len <= A.staged_const ? s_const : A.consts;
 }
 
+// The shared-memory offset of the compiled patterns: after the staged constants, 16-byte aligned.
+__host__ __device__ __forceinline__ size_t pattern_smem_offset(size_t before) { return (before + 15) & ~(size_t)15; }
+
+template <bool kPatterns>
 __global__ void __launch_bounds__(kFilterThreads) filter_kernel(const FilterArgs A) {
     extern __shared__ __align__(16) unsigned char smem[];
     NodeDev* s_nodes = reinterpret_cast<NodeDev*>(smem);
@@ -96,6 +106,13 @@ __global__ void __launch_bounds__(kFilterThreads) filter_kernel(const FilterArgs
     StringDev* s_strings = reinterpret_cast<StringDev*>(s_scalars + A.scalar_count);
     u64* s_list = reinterpret_cast<u64*>(s_strings + A.string_count);
     u8* s_const = reinterpret_cast<u8*>(s_list + A.staged_list);
+    u8* s_pat = nullptr;
+    if constexpr (kPatterns) {
+        s_pat = smem + pattern_smem_offset((size_t)(s_const + A.staged_const - smem));
+        const uint4* src = reinterpret_cast<const uint4*>(A.patterns);
+        uint4* dst = reinterpret_cast<uint4*>(s_pat);
+        for (u32 k = threadIdx.x; k < A.pattern_bytes / 16; k += blockDim.x) dst[k] = src[k];
+    }
     {
         const u32* src = reinterpret_cast<const u32*>(A.nodes);
         u32* dst = reinterpret_cast<u32*>(s_nodes);
@@ -151,6 +168,8 @@ __global__ void __launch_bounds__(kFilterThreads) filter_kernel(const FilterArgs
                     c.length = nd.length;
                     c.data = nd.constant;
                     r = cmp_holds(nd.cmp, string_compare2(sc.heap, v, const_heap(A, s_const, nd.constant, nd.length), c)) ? kTrue : kFalse;
+                } else if (kPatterns && (nd.op == YTGPU_FILTER_CONTAINS || nd.op == YTGPU_FILTER_LIKE)) {
+                    r = pattern_match(s_pat + nd.constant, sc.heap + v.data, v.length) ? kTrue : kFalse;
                 } else if (nd.op == YTGPU_FILTER_STARTS_WITH) {
                     bool ok = v.length >= nd.length;
                     const u8* p = const_heap(A, s_const, nd.constant, nd.length) + nd.constant;
@@ -256,6 +275,7 @@ __global__ void __launch_bounds__(kFilterThreads) filter_rows_kernel(const u32* 
 struct Checked {
     std::vector<NodeDev> nodes;
     std::vector<u64> lists;   // sorted entries of every IN node, node by node
+    std::vector<u8> patterns; // compiled CONTAINS / LIKE patterns, node by node (strings.cuh)
     std::vector<int> scalar_of, string_of;  // caller column -> compact table slot (-1: not referenced)
     std::vector<u32> scalar_cols, string_cols;  // compact slot -> caller column
 };
@@ -299,7 +319,8 @@ Status check_program(const ytgpu_column_view* columns, u32 column_count, u32 str
         const ytgpu_filter_node& N = program[k];
         NodeDev d{};
         d.op = (u8)N.op;
-        const bool leaf = N.op >= YTGPU_FILTER_COMPARE && N.op <= YTGPU_FILTER_IS_NOT_NULL;
+        const bool leaf = (N.op >= YTGPU_FILTER_COMPARE && N.op <= YTGPU_FILTER_IS_NOT_NULL) || N.op == YTGPU_FILTER_CONTAINS ||
+                          N.op == YTGPU_FILTER_LIKE;
         if (!leaf && N.op != YTGPU_FILTER_AND && N.op != YTGPU_FILTER_OR && N.op != YTGPU_FILTER_NOT)
             return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: unknown op %d", k, N.op);
         if (!leaf) {
@@ -336,6 +357,22 @@ Status check_program(const ytgpu_column_view* columns, u32 column_count, u32 str
                 d.constant = N.constant;
                 d.length = N.length;
                 break;
+            case YTGPU_FILTER_CONTAINS:
+            case YTGPU_FILTER_LIKE: {
+                const bool like = N.op == YTGPU_FILTER_LIKE;
+                if (!str) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: %s on a scalar column", k, like ? "LIKE" : "CONTAINS");
+                if (!string_range_ok(N.constant, N.length))
+                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: %s outside string_constants", k, like ? "pattern" : "needle");
+                if (like && (N.column2 < -1 || N.column2 > 255))
+                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: LIKE escape %d outside -1 .. 255", k, N.column2);
+                d.constant = out->patterns.size();
+                if (const char* why = compile_pattern(consts + N.constant, N.length, like, like ? N.column2 : -1, &out->patterns))
+                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: %s", k, why);
+                if (out->patterns.size() > (size_t)YTGPU_FILTER_MAX_PATTERN_BYTES)
+                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "the patterns of a call compile to more than %d bytes",
+                                       YTGPU_FILTER_MAX_PATTERN_BYTES);
+                break;
+            }
             case YTGPU_FILTER_COMPARE_COLUMNS: {
                 if (N.column2 < 0 || (u64)N.column2 >= total)
                     return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: column2 %d out of range", k, N.column2);
@@ -429,18 +466,21 @@ Status evaluate_filter_impl(Context* ctx, const ytgpu_column_view* columns, u32 
         hs[k] = ss[k].dev;
     }
 
-    // one upload: nodes | scalar views | string views | sorted lists | string constants, then the outputs' scratch
+    // one upload: nodes | scalar views | string views | sorted lists | string constants | compiled patterns, then the
+    // outputs' scratch
     const size_t nodes_b = P.nodes.size() * sizeof(NodeDev), scal_b = hc.size() * sizeof(ColumnDev), str_b = hs.size() * sizeof(StringDev);
     const size_t list_b = P.lists.size() * 8, const_b = (size_t)const_bytes;
     auto up16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
     const size_t o_scal = up16(nodes_b), o_str = o_scal + up16(scal_b), o_list = o_str + up16(str_b), o_const = o_list + up16(list_b);
-    const size_t blob_b = o_const + up16(const_b);
+    const size_t o_pat = o_const + up16(const_b), pat_b = up16(P.patterns.size());  // staged in 16-byte units
+    const size_t blob_b = o_pat + pat_b;
     std::vector<u8> blob(blob_b, 0);
     if (nodes_b) memcpy(blob.data(), P.nodes.data(), nodes_b);
     if (scal_b) memcpy(blob.data() + o_scal, hc.data(), scal_b);
     if (str_b) memcpy(blob.data() + o_str, hs.data(), str_b);
     if (list_b) memcpy(blob.data() + o_list, P.lists.data(), list_b);
     if (const_b) memcpy(blob.data() + o_const, consts, const_b);
+    if (!P.patterns.empty()) memcpy(blob.data() + o_pat, P.patterns.data(), P.patterns.size());
     DevBuf<u8> dblob;
     YTGPU_TRY(dblob.allocate(ctx, blob_b));
     YTGPU_CUDA_TRY(cudaMemcpyAsync(dblob.p, blob.data(), blob_b, cudaMemcpyHostToDevice, ctx->stream));
@@ -478,6 +518,8 @@ Status evaluate_filter_impl(Context* ctx, const ytgpu_column_view* columns, u32 
     A.consts = dblob.p + o_const;
     A.const_bytes = (u32)const_bytes;
     A.staged_const = std::min<u32>(A.const_bytes, kStagedConstBytes);
+    A.patterns = dblob.p + o_pat;
+    A.pattern_bytes = (u32)pat_b;
     A.n = n;
     A.bitmap = dbitmap;
     A.bytemap = dbytemap;
@@ -485,13 +527,18 @@ Status evaluate_filter_impl(Context* ctx, const ytgpu_column_view* columns, u32 
     A.bytemap_vec = dbytemap && (reinterpret_cast<uintptr_t>(dbytemap) & 15) == 0;
     A.result = result.p;
     // shared memory in the kernel's order; every part is a multiple of 8 bytes (NodeDev 24, ColumnDev / StringDev 8-aligned)
-    const size_t smem = nodes_b + scal_b + str_b + (size_t)A.staged_list * 8 + A.staged_const;
+    const bool patterns = !P.patterns.empty();
+    size_t smem = nodes_b + scal_b + str_b + (size_t)A.staged_list * 8 + A.staged_const;
+    if (patterns) smem = pattern_smem_offset(smem) + pat_b;
     static_assert(sizeof(ColumnDev) % 8 == 0 && sizeof(StringDev) % 8 == 0, "shared-memory layout");
+    if (patterns)  // up to 32 KiB of patterns may take the stage past the 48 KB default
+        YTGPU_CUDA_TRY(cudaFuncSetAttribute(filter_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const u64 warps = words;
     const u32 blocks = (u32)std::max<u64>(1, std::min<u64>((warps * 32 + kFilterThreads - 1) / kFilterThreads, (u64)kNumSms * 8));
     {
         KernelTimer t(ctx, KC_DECODE);
-        filter_kernel<<<blocks, kFilterThreads, smem, ctx->stream>>>(A);
+        if (patterns) filter_kernel<true><<<blocks, kFilterThreads, smem, ctx->stream>>>(A);
+        else filter_kernel<false><<<blocks, kFilterThreads, smem, ctx->stream>>>(A);
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
     unsigned long long res[2] = {0, 0};  // the one host read: selected count and error bits

@@ -804,7 +804,7 @@ class GpuContext:
         """WHERE expression (ytgpu_evaluate_filter) -> dict(bitmap, bytemap, rows, count).
         columns: Column objects; string_columns: (heap, starts, lengths, nulls or None) per column, node column
         len(columns) + i naming string column i.  program: postfix nodes, each a capi.FilterNode or a tuple
-        (op, cmp, column, column2, constant, length).  list_values: IN entries (uint64 bit patterns; for a string column
+        (op, cmp, column, column2, constant, length); a LIKE node's column2 is its escape byte (-1: none).  list_values: IN entries (uint64 bit patterns; for a string column
         (offset << 32) | length into string_constants).  The outputs are in the inputs' memory flavour: bitmap
         8 * ceil(n / 64) bytes, bytemap n bytes, rows uint32 (int32 on the device) trimmed to the count; an output not
         wanted is None."""
