@@ -444,6 +444,82 @@ public:
             stats.RowsRead += (int64_t)rows.size();
         }
         const uint64_t n = (uint64_t)stats.RowsRead;
+        // The result type of computed column j, from its program and its inputs' types, by the typing rules of
+        // check_expression (csrc/expression.cu): the value / string split below needs it before the column is evaluated.
+        // An input column without a non-NULL value has no type: it is a STRING where the program reads it as one (an
+        // operand of CONCAT, LOWER, UPPER or of IF_NULL with a STRING; *stringLeaves marks it, and it is passed as an
+        // all-NULL string column), INT64 everywhere else, as view() passes it.  A malformed program types as INT64 and is
+        // refused by the call.
+        auto typeComputed = [&](size_t j, std::vector<uint8_t>* stringLeaves) {
+            struct TEntry {
+                EValueType Type;
+                std::vector<int> NullLeaves;  // untyped input columns the entry may be
+            };
+            auto asString = [&](TEntry& e) {
+                for (int leaf : e.NullLeaves) (*stringLeaves)[leaf] = 1;
+                e = {EValueType::String, {}};
+            };
+            auto asNumber = [](TEntry& e) {
+                if (e.Type == EValueType::Null) e.Type = EValueType::Int64;
+                e.NullLeaves.clear();
+            };
+            std::vector<TEntry> st;
+            for (size_t k = 0; k < query.Computed[j].Nodes.size(); ++k) {
+                const TExpressionNode& node = query.Computed[j].Nodes[k];
+                const size_t need = node.Op == EExpressionOp::Column || node.Op == EExpressionOp::Constant ? 0
+                                  : node.Op == EExpressionOp::FarmHash ? (size_t)std::max(node.Column, 1)
+                                  : (node.Op == EExpressionOp::Neg || node.Op == EExpressionOp::BitNot || node.Op == EExpressionOp::Cast ||
+                                     node.Op == EExpressionOp::Lower || node.Op == EExpressionOp::Upper) ? 1 : 2;
+                if (st.size() < need) return EValueType::Int64;
+                switch (node.Op) {
+                    case EExpressionOp::Column: {
+                        const int leaf = leafIndex[j][k];
+                        const EValueType t = columns[leaf].Type;
+                        st.push_back(t == EValueType::Null ? TEntry{EValueType::Null, {leaf}} : TEntry{t, {}});
+                        break;
+                    }
+                    case EExpressionOp::Constant: st.push_back({node.Type, {}}); break;
+                    case EExpressionOp::Lower: case EExpressionOp::Upper:
+                        if (st.back().Type == EValueType::Null) asString(st.back());
+                        break;
+                    case EExpressionOp::Neg: case EExpressionOp::BitNot:
+                        asNumber(st.back());
+                        break;
+                    case EExpressionOp::Cast:
+                        asNumber(st.back());
+                        st.back().Type = node.Type;
+                        break;
+                    case EExpressionOp::FarmHash:  // a NULL hashes alike whichever type it is read as
+                        st.resize(st.size() - need);
+                        st.push_back({EValueType::Uint64, {}});
+                        break;
+                    default: {  // binary ops, IfNull, Concat: operands of one type
+                        TEntry b = std::move(st.back());
+                        st.pop_back();
+                        TEntry& a = st.back();
+                        const bool str = node.Op == EExpressionOp::Concat ||
+                                         (node.Op == EExpressionOp::IfNull && (a.Type == EValueType::String || b.Type == EValueType::String));
+                        if (str) {
+                            if (a.Type == EValueType::Null) asString(a);
+                            if (b.Type == EValueType::Null) asString(b);
+                        } else if (node.Op == EExpressionOp::IfNull && a.Type == EValueType::Null && b.Type == EValueType::Null) {
+                            a.NullLeaves.insert(a.NullLeaves.end(), b.NullLeaves.begin(), b.NullLeaves.end());
+                        } else {
+                            if (a.Type == EValueType::Null) a.Type = b.Type;
+                            asNumber(a);
+                        }
+                        break;
+                    }
+                }
+            }
+            if (st.size() != 1) return EValueType::Int64;
+            return st[0].Type == EValueType::Null ? EValueType::Int64 : st[0].Type;
+        };
+        for (size_t i = 0; i < columns.size(); ++i) {
+            if (!isComputed((int)i)) continue;
+            std::vector<uint8_t> stringLeaves(columns.size(), 0);
+            columns[i].Type = typeComputed((size_t)(-2 - columns[i].Position), &stringLeaves);
+        }
         if (whereIndex >= 0 && columns[whereIndex].Type == EValueType::String)
             throw TErrorException(YTGPU_ERR_UNSUPPORTED, "the WHERE column (position " + std::to_string(query.WhereColumn) +
                                                              ") holds strings: string predicates are not on the GPU path");
@@ -466,28 +542,52 @@ public:
                 v.mem = YTGPU_MEM_HOST;
                 return v;
             };
-            // a computed column: one ytgpu_evaluate_expression call over its input columns, rows outside `selection` NULL
+            auto stringView = [&](const TFlatColumn& c) {
+                return ytgpu_string_column{reinterpret_cast<const uint8_t*>(c.Heap.data()), c.Heap.size(), c.Starts.data(), c.Lengths.data(),
+                                           c.NullBytes.data(), n, YTGPU_MEM_HOST, 0};
+            };
+            // a computed column: one ytgpu_evaluate_expression_strings call over its input columns (string inputs as string
+            // columns), rows outside `selection` NULL; a string result takes a second call once its heap is sized
             auto evaluateComputed = [&](int i, const uint8_t* selection) {
                 const size_t j = (size_t)(-2 - columns[i].Position);
                 std::vector<ytgpu_column_view> inputs;
-                std::vector<int> slot(columns.size(), -1);
+                std::vector<ytgpu_string_column> stringInputs;
+                std::string constants;
+                std::vector<int> slot(columns.size(), -1);  // scalar: slot; string: -1 - string slot
+                std::vector<int> leafOf;
                 std::vector<ytgpu_expr_node> program;
+                std::vector<uint8_t> stringLeaves(columns.size(), 0);  // untyped input columns read as strings
+                typeComputed(j, &stringLeaves);
                 for (size_t k = 0; k < query.Computed[j].Nodes.size(); ++k) {
                     const TExpressionNode& node = query.Computed[j].Nodes[k];
                     ytgpu_expr_node x{};
                     x.op = (int32_t)node.Op;
                     x.type = (uint8_t)node.Type;
                     x.constant = node.Bits;
-                    if (const int leaf = leafIndex[j][k]; leaf >= 0) {
-                        if (slot[leaf] < 0) {
-                            slot[leaf] = (int)inputs.size();
-                            inputs.push_back(view(columns[leaf]));  // a string column is refused by the call (UNSUPPORTED)
-                        }
-                        x.column = slot[leaf];
+                    if (node.Op == EExpressionOp::FarmHash) x.column = node.Column;
+                    if (node.Op == EExpressionOp::Constant && node.Type == EValueType::String) {
+                        x.constant = ((uint64_t)constants.size() << 32) | node.Bytes.size();
+                        constants += node.Bytes;
                     }
+                    const int leaf = leafIndex[j][k];
+                    if (leaf >= 0 && slot[leaf] == -1) {
+                        if (columns[leaf].Type == EValueType::String || stringLeaves[leaf]) {  // all-NULL: an empty heap
+                            columns[leaf].Starts.resize(n, 0);
+                            columns[leaf].Lengths.resize(n, 0);
+                            slot[leaf] = -2 - (int)stringInputs.size();
+                            stringInputs.push_back(stringView(columns[leaf]));
+                        } else {
+                            slot[leaf] = (int)inputs.size();
+                            inputs.push_back(view(columns[leaf]));
+                        }
+                    }
+                    leafOf.push_back(leaf);
                     program.push_back(x);
                 }
-                if (inputs.empty()) {  // constants only: a column without values gives the row count
+                for (size_t k = 0; k < program.size(); ++k)  // string inputs follow the scalar ones
+                    if (const int leaf = leafOf[k]; leaf >= 0)
+                        program[k].column = slot[leaf] >= 0 ? slot[leaf] : (int)inputs.size() + (-2 - slot[leaf]);
+                if (inputs.empty() && stringInputs.empty()) {  // constants only: a column without values gives the row count
                     ytgpu_column_view rows{};
                     rows.value_count = (int64_t)n;
                     rows.value_type = YTGPU_TYPE_INT64;
@@ -499,13 +599,29 @@ public:
                 c.Values.assign(n, 0);
                 c.Nulls.assign((n + 63) / 64 * 8, 0);
                 uint8_t type = 0;
-                uint64_t nullCount = 0;
+                uint64_t nullCount = 0, heapBytes = 0;
                 ytgpu_error err{};
-                if (ytgpu_evaluate_expression(GetGpuContext(), inputs.data(), (uint32_t)inputs.size(), program.data(), (uint32_t)program.size(),
-                                              selection, c.Values.data(), c.Nulls.data(), &type, &nullCount, YTGPU_MEM_HOST, &err) != YTGPU_OK)
-                    ThrowFrom(err);
+                auto call = [&](bool fill) {
+                    if (ytgpu_evaluate_expression_strings(
+                            GetGpuContext(), inputs.data(), (uint32_t)inputs.size(), stringInputs.data(), (uint32_t)stringInputs.size(),
+                            reinterpret_cast<const uint8_t*>(constants.data()), constants.size(), program.data(), (uint32_t)program.size(),
+                            selection, c.Values.data(), c.Nulls.data(), fill ? reinterpret_cast<uint8_t*>(c.Heap.data()) : nullptr,
+                            c.Heap.size(), c.Starts.data(), c.Lengths.data(), c.NullBytes.data(), &heapBytes, &type, &nullCount,
+                            YTGPU_MEM_HOST, &err) != YTGPU_OK)
+                        ThrowFrom(err);
+                };
+                call(false);  // a numeric result is complete; a string result has its heap size
                 c.Type = (EValueType)type;
                 c.AnyNull = nullCount != 0;
+                if (c.Type == EValueType::String) {
+                    c.Heap.assign(heapBytes, '\0');
+                    c.Starts.assign(n, 0);
+                    c.Lengths.assign(n, 0);
+                    c.NullBytes.assign(n, 0);
+                    call(true);
+                    for (uint64_t r = 0; r < n; ++r)  // a string GROUP BY key's NULLs are the ids' null bitmap (view())
+                        if (c.NullBytes[r]) c.Nulls[r >> 3] |= (uint8_t)(1u << (r & 7));
+                }
             };
             // the computed columns the WHERE reads, over all rows
             std::vector<uint8_t> evaluated(columns.size(), 0);
@@ -630,8 +746,13 @@ public:
             // the other computed columns, over the rows the WHERE selects
             for (size_t i = 0; i < columns.size(); ++i)
                 if (isComputed((int)i) && !evaluated[i]) {
+                    const EValueType planned = columns[i].Type;
                     evaluateComputed((int)i, where ? selection.data() : nullptr);
-                    valueViews[argIndex[i]] = view(columns[i]);
+                    if ((columns[i].Type == EValueType::String) != (planned == EValueType::String))
+                        throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "computed column " + std::to_string(-2 - columns[i].Position) +
+                                                                              ": result type differs from its inputs' typing");
+                    if (argIndex[i] >= 0) valueViews[argIndex[i]] = view(columns[i]);
+                    else stringViews[-1 - argIndex[i]] = stringView(columns[i]);
                 }
             for (auto& a : argIndex)
                 if (a < 0) a = (int)valueViews.size() + (-1 - a);
@@ -743,6 +864,8 @@ public:
                         }
                         std::vector<ytgpu_expr_node> program;
                         for (const auto& node : nodes) {
+                            if ((int)node.Op > (int)EExpressionOp::IfNull)
+                                throw TErrorException(YTGPU_ERR_UNSUPPORTED, "select item " + std::to_string(s) + ": string functions in the select list");
                             ytgpu_expr_node x{};
                             x.op = (int32_t)node.Op;
                             x.column = node.Column;

@@ -176,24 +176,30 @@ struct TFilterExpression {
     TFilterExpression& Not() { Nodes.push_back({EFilterOp::Not, EBinaryOp::None, -1, -1, {}, {}}); return *this; }
 };
 
-//! An arithmetic, bitwise, cast or if_null expression, evaluated on the GPU into a computed column (ytgpu_evaluate_expression:
-//! the semantics — NULLs, wrap-around, division errors, casts — are in include/ytgpu.h).  Nodes are in postfix order; a
-//! Column leaf names a position (in the input rows for TMultiGroupQuery::Computed, in the output row for Select).  Binary
-//! operands have one type: there is no implicit widening, write Cast.
+//! An arithmetic, bitwise, cast, if_null, concat, lower, upper or farm_hash expression, evaluated on the GPU into a computed
+//! column (ytgpu_evaluate_expression_strings: the semantics — NULLs, wrap-around, division errors, casts, ASCII case
+//! mapping, the fingerprint — are in include/ytgpu.h).  Nodes are in postfix order; a Column leaf names a position (in the
+//! input rows for TMultiGroupQuery::Computed, in the output row for Select).  Binary operands have one type: there is no
+//! implicit widening, write Cast.  Select takes no string ops.
 enum class EExpressionOp {
     Column = 1, Constant = 2, Add = 3, Sub = 4, Mul = 5, Div = 6, Mod = 7, Neg = 8, BitAnd = 9, BitOr = 10, BitXor = 11, BitNot = 12,
-    Cast = 13, IfNull = 14
+    Cast = 13, IfNull = 14, Concat = 15, Lower = 16, Upper = 17, FarmHash = 18
 };
 struct TExpressionNode {
     EExpressionOp Op = EExpressionOp::Column;
-    int Column = -1;                      // Column
+    int Column = -1;                      // Column; FarmHash: the operand count
     EValueType Type = EValueType::Null;   // Constant: its type; Cast: the target type
     uint64_t Bits = 0;                    // Constant: Int64 / Uint64 / Double bit pattern, Boolean 0 / 1
+    std::string Bytes = {};               // Constant: a String's bytes
 };
 struct TExpression {
     std::vector<TExpressionNode> Nodes;
     TExpression& Column(int position) { Nodes.push_back({EExpressionOp::Column, position, EValueType::Null, 0}); return *this; }
     TExpression& Constant(const TUnversionedValue& v) {
+        if (v.Type == EValueType::String) {
+            Nodes.push_back({EExpressionOp::Constant, -1, v.Type, 0, std::string(v.Data.String, v.Length)});
+            return *this;
+        }
         Nodes.push_back({EExpressionOp::Constant, -1, v.Type, v.Type == EValueType::Boolean ? (v.Data.Boolean ? 1u : 0u) : v.Data.Uint64});
         return *this;
     }
@@ -209,6 +215,12 @@ struct TExpression {
     TExpression& BitNot() { return Op(EExpressionOp::BitNot); }
     TExpression& Cast(EValueType type) { Nodes.push_back({EExpressionOp::Cast, -1, type, 0}); return *this; }
     TExpression& IfNull() { return Op(EExpressionOp::IfNull); }
+    //! concat(a, b) of two strings; lower / upper of a string (ASCII only: a byte >= 0x80 throws YTGPU_ERR_UNSUPPORTED).
+    TExpression& Concat() { return Op(EExpressionOp::Concat); }
+    TExpression& Lower() { return Op(EExpressionOp::Lower); }
+    TExpression& Upper() { return Op(EExpressionOp::Upper); }
+    //! farm_hash of the last `count` (1..16) values, of any type: a Uint64, never NULL.
+    TExpression& FarmHash(int count) { Nodes.push_back({EExpressionOp::FarmHash, count, EValueType::Null, 0}); return *this; }
 
 private:
     TExpression& Op(EExpressionOp op) { Nodes.push_back({op, -1, EValueType::Null, 0}); return *this; }
@@ -248,12 +260,14 @@ struct IEvaluator {
     //! most 2^30 per query fragment).  Every column holds one type of Int64 / Uint64 / Double / Boolean / String (or Null);
     //! a string group item goes through ytgpu_string_value_ids, and min / max / first / count / argmin / argmax take string
     //! arguments.  sum / avg of a string column and a string WHERE column throw YTGPU_ERR_UNSUPPORTED.
-    //! Computed columns are evaluated with ytgpu_evaluate_expression, nothing on the host, in QL's order: first those the
+    //! Computed columns are evaluated with ytgpu_evaluate_expression_strings, nothing on the host, in QL's order: first those the
     //! WHERE reads, over all rows; then the WHERE, once, as a filter pass (with computed columns the WhereOp form runs as a
     //! one-node COMPARE program, which selects the same rows); then the other computed columns over the selected rows only,
     //! so a division by zero in a row the WHERE drops does not throw.  Select items are evaluated the same way over the
     //! result rows; a bare Column of a string result passes through, arithmetic on it throws YTGPU_ERR_UNSUPPORTED, as does
-    //! an expression over a string input column.  Errors of the calls (a division by zero, a mistyped expression:
+    //! a numeric op over a string input column.  A computed column may yield a string (concat, lower, upper, if_null): it is
+    //! a string column to every consumer (group item, string aggregate argument, WHERE leaf); lower / upper of a non-ASCII
+    //! value throws YTGPU_ERR_UNSUPPORTED.  Errors of the calls (a division by zero, a mistyped expression:
     //! YTGPU_ERR_INVALID_ARGUMENT) throw TErrorException.  A query without computed columns and Select runs as before.
     virtual TQueryStatistics Run(const TMultiGroupQuery& query, const ISchemalessMultiChunkReaderPtr& reader,
                                  const IUnversionedRowsetWriterPtr& writer) = 0;

@@ -757,18 +757,23 @@ typedef enum ytgpu_expr_op {
     YTGPU_EXPR_COLUMN = 1, YTGPU_EXPR_CONSTANT = 2,
     YTGPU_EXPR_ADD = 3, YTGPU_EXPR_SUB = 4, YTGPU_EXPR_MUL = 5, YTGPU_EXPR_DIV = 6, YTGPU_EXPR_MOD = 7, YTGPU_EXPR_NEG = 8,
     YTGPU_EXPR_BIT_AND = 9, YTGPU_EXPR_BIT_OR = 10, YTGPU_EXPR_BIT_XOR = 11, YTGPU_EXPR_BIT_NOT = 12,
-    YTGPU_EXPR_CAST = 13, YTGPU_EXPR_IF_NULL = 14
+    YTGPU_EXPR_CAST = 13, YTGPU_EXPR_IF_NULL = 14,
+    /* ytgpu_evaluate_expression_strings only */
+    YTGPU_EXPR_CONCAT = 15, YTGPU_EXPR_LOWER = 16, YTGPU_EXPR_UPPER = 17, YTGPU_EXPR_FARM_HASH = 18
 } ytgpu_expr_op;
 
 #define YTGPU_EXPR_MAX_NODES 64
 #define YTGPU_EXPR_MAX_DEPTH 16
+#define YTGPU_EXPR_MAX_PIECES 16
+#define YTGPU_EXPR_MAX_HASH_OPERANDS 16
+#define YTGPU_EXPR_MAX_STRING_CONSTANT_BYTES (1u << 20)
 
 typedef struct ytgpu_expr_node {
     int32_t op;          /* ytgpu_expr_op */
-    int32_t column;      /* COLUMN: index into columns */
+    int32_t column;      /* COLUMN: index into columns (++ string_columns); FARM_HASH: its operand count */
     uint8_t type;        /* CONSTANT: its value type; CAST: the target type (YTGPU_TYPE_*) */
     uint8_t reserved[7];
-    uint64_t constant;   /* CONSTANT: the bit pattern in `type` */
+    uint64_t constant;   /* CONSTANT: the bit pattern in `type`; a STRING one: (offset << 32) | length into string_constants */
 } ytgpu_expr_node;
 
 int ytgpu_evaluate_expression(ytgpu_context* ctx, const ytgpu_column_view* columns, uint32_t column_count,
@@ -776,6 +781,74 @@ int ytgpu_evaluate_expression(ytgpu_context* ctx, const ytgpu_column_view* colum
                               const uint8_t* selection /* nullable, out_mem */, uint64_t* out_values,
                               uint8_t* out_null_bitmap, uint8_t* out_value_type /* host, nullable */,
                               uint64_t* out_null_count /* host, nullable */, int out_mem, ytgpu_error* err);
+
+/* ---- computed string columns: concat, lower, upper, if_null and farm_hash ----
+ * ytgpu_evaluate_expression with string leaves and string results: `group by lower(host)`, `group by concat(region, '/',
+ * city)`, `group by if_null(campaign, 'none')`, `group by farm_hash(user_id) % 64`, `where farm_hash(k) % 100 < 5`.  The
+ * ops are QL's concat / lower / upper / if_null / farm_hash UDFs, recalled, not read.  With string_count = 0 and a program
+ * of the ops above (COLUMN .. IF_NULL) this call is exactly ytgpu_evaluate_expression; the string ops and string leaves
+ * are taken by this entry point only (ytgpu_evaluate_expression keeps refusing them).
+ *   COLUMN(column)           column indexes columns ++ string_columns: column_count + i is string_columns[i], a STRING
+ *   CONSTANT(STRING)         `constant` = (offset << 32) | length: the bytes string_constants[offset, offset + length)
+ *   CONCAT                   two STRING operands -> STRING, the first one's bytes then the second's
+ *   LOWER, UPPER             one STRING -> STRING: ASCII A-Z -> a-z (LOWER) or a-z -> A-Z (UPPER), every other byte kept.
+ *                            QL's lower / upper are recalled to map UTF-8 with Unicode case tables, which this library does
+ *                            not have; on pure-ASCII values any such mapping agrees with this one.  So an operand with a byte
+ *                            >= 0x80 in a row that is evaluated (selected and non-NULL) fails the call with
+ *                            YTGPU_ERR_UNSUPPORTED rather than yield a different string; a caller takes its CPU path then.
+ *   IF_NULL                  also two STRING operands -> STRING
+ *   FARM_HASH(k)             k = `column` in 1 .. YTGPU_EXPR_MAX_HASH_OPERANDS (16) operands of any type, STRING included ->
+ *                            UINT64, never NULL: GetFarmFingerprint over the k values in order (the first pushed first),
+ *                            bit-identical to ytgpu_farm_fingerprint_rowset over a row of those k values: each value's
+ *                            fingerprint (a string's FarmHash Fingerprint64 of its bytes, a number's Fingerprint(uint64) of
+ *                            its bits, BOOLEAN as 0 / 1, NULL as Fingerprint(0)) folded from 0xdeadc0de with
+ *                            Fingerprint(uint128), then xor k.  That QL's farm_hash(a, b, ...) is GetFarmFingerprint of its
+ *                            arguments is recalled from its UDF, not read.  A STRING operand must be a leaf, a constant or
+ *                            IF_NULL of those; a CONCAT, LOWER or UPPER result under FARM_HASH is YTGPU_ERR_UNSUPPORTED.
+ * NULL: a NULL operand makes CONCAT, LOWER and UPPER NULL; IF_NULL and FARM_HASH as above.  The numeric ops are those of
+ * ytgpu_evaluate_expression, and they do not take strings (YTGPU_ERR_UNSUPPORTED).  There are no comparisons, no substr.
+ * Limits: those of ytgpu_evaluate_expression; at most YTGPU_EXPR_MAX_PIECES (16) string pieces on the stack at any node,
+ * where a leaf or constant is one piece, CONCAT adds its operands' pieces and IF_NULL takes the larger count (so a program
+ * concatenates at most 16 values); at most 1 MiB of string_constants; a result value of at most 2^32 - 1 bytes.
+ * selection: as ytgpu_evaluate_expression; an unselected row is NULL and not evaluated, so a non-ASCII value or a value
+ * outside its heap there does not fail the call.
+ * Outputs, in out_mem:
+ *   a numeric result  out_values / out_null_bitmap as ytgpu_evaluate_expression; the string outputs are not touched.
+ *   a STRING result   out_values / out_null_bitmap are not touched, and
+ *     *out_heap_bytes (host)  the bytes of all result values, always written once the program is checked and evaluated;
+ *     out_heap                the values back to back in row order (out_heap_capacity bytes).  NULL: a size query that
+ *                             writes *out_heap_bytes only, so a caller sizes the heap and calls again;
+ *     out_starts (u64), out_lengths (u32), out_null_bytemap (u8), n entries each: value i is the out_lengths[i] bytes at
+ *                             out_heap + out_starts[i]; a NULL row has length 0 and null byte 1.  So {out_heap,
+ *                             *out_heap_bytes, out_starts, out_lengths, out_null_bytemap, n, out_mem} is the
+ *                             ytgpu_string_column that ytgpu_evaluate_filter, ytgpu_string_value_ids and
+ *                             ytgpu_scan_filter_groupby_multi_strings take.
+ *   *out_value_type, *out_null_count as ytgpu_evaluate_expression.
+ *   A first call with out_heap, out_values and out_null_bitmap all NULL is a type and size query: a numeric result is
+ *   checked and typed but not evaluated (no launch), a STRING one is sized as above.  A caller that does not know the
+ *   result type makes it, then allocates only the outputs that type needs; for a STRING result the second call runs the
+ *   size pass again.
+ * Launches: a numeric result: one evaluation kernel and one host read, as ytgpu_evaluate_expression (none for a type
+ * query).  A STRING result: a
+ * size pass and a three-kernel scan of the lengths, then one host read (NULL count, error bits, heap size); with out_heap
+ * a fill pass follows (five launches).  HOST inputs are copied to the device first.
+ * YTGPU_ERR_INVALID_ARGUMENT: everything ytgpu_evaluate_expression refuses; a new op over a type it does not take, FARM_HASH
+ * with k outside 1 .. 16, more than 16 pieces, a string constant outside string_constants or more than 1 MiB of them, a
+ * string column of another length, null starts / lengths, a null heap with heap_bytes > 0 or a mem that is neither DEVICE
+ * nor HOST, a non-NULL value whose [start, start + length) leaves its heap (checked on the device for the string columns
+ * the program reads; no byte outside the heap is read), a result value longer than 2^32 - 1 bytes, out_heap_capacity
+ * below the heap size (which is still written), a null out_heap_bytes with a STRING result.  YTGPU_ERR_UNSUPPORTED: a
+ * numeric op over a STRING, a non-ASCII LOWER / UPPER operand, a CONCAT / LOWER / UPPER result under FARM_HASH.  After a
+ * failure the outputs' contents are unspecified. */
+int ytgpu_evaluate_expression_strings(ytgpu_context* ctx, const ytgpu_column_view* columns, uint32_t column_count,
+                                      const ytgpu_string_column* string_columns, uint32_t string_count,
+                                      const uint8_t* string_constants /* host */, uint64_t string_constant_bytes,
+                                      const ytgpu_expr_node* program /* host */, uint32_t node_count,
+                                      const uint8_t* selection /* nullable, out_mem */, uint64_t* out_values,
+                                      uint8_t* out_null_bitmap, uint8_t* out_heap, uint64_t out_heap_capacity,
+                                      uint64_t* out_starts, uint32_t* out_lengths, uint8_t* out_null_bytemap,
+                                      uint64_t* out_heap_bytes /* host */, uint8_t* out_value_type /* host, nullable */,
+                                      uint64_t* out_null_count /* host, nullable */, int out_mem, ytgpu_error* err);
 
 /* ---- segmented SUM / COUNT over rows ALREADY SORTED by the group key (the aggregate stage after a sort) ----
  * Consecutive rows with equal keys form a group; no hash table.  Replaces the per-group accumulation of a GROUP BY

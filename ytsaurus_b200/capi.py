@@ -114,6 +114,7 @@ EXPORTED_SYMBOLS = [
     "ytgpu_shuffle_destroy", "ytgpu_reduce_sorted_fixed_rows", "ytgpu_context_set_option", "ytgpu_context_notify", "ytgpu_decode_horizontal_block", "ytgpu_encode_horizontal_block",
     "ytgpu_decode_column", "ytgpu_decode_string_offsets", "ytgpu_decode_string_pointers_and_lengths", "ytgpu_scan_filter_groupby", "ytgpu_scan_filter_groupby_multi",
     "ytgpu_scan_filter_groupby_multi_strings", "ytgpu_evaluate_filter", "ytgpu_evaluate_expression",
+    "ytgpu_evaluate_expression_strings",
     "ytgpu_convert_integer_column", "ytgpu_encode_integer_column", "ytgpu_encode_double_column", "ytgpu_encode_boolean_column", "ytgpu_encode_string_column", "ytgpu_decode_string_segment", "ytgpu_string_value_ids", "ytgpu_extract_column",
     "ytgpu_block_agg_state_init", "ytgpu_block_combine_all",
     "ytgpu_build_bitmap_from_flags", "ytgpu_build_bytemap_from_flags", "ytgpu_count_flags", "ytgpu_build_dictionary_indexes",
@@ -168,8 +169,9 @@ class FilterNode(C.Structure):
 
 
 (EXPR_COLUMN, EXPR_CONSTANT, EXPR_ADD, EXPR_SUB, EXPR_MUL, EXPR_DIV, EXPR_MOD, EXPR_NEG, EXPR_BIT_AND, EXPR_BIT_OR, EXPR_BIT_XOR,
- EXPR_BIT_NOT, EXPR_CAST, EXPR_IF_NULL) = range(1, 15)
+ EXPR_BIT_NOT, EXPR_CAST, EXPR_IF_NULL, EXPR_CONCAT, EXPR_LOWER, EXPR_UPPER, EXPR_FARM_HASH) = range(1, 19)
 EXPR_MAX_NODES, EXPR_MAX_DEPTH = 64, 16
+EXPR_MAX_PIECES, EXPR_MAX_HASH_OPERANDS, EXPR_MAX_STRING_CONSTANT_BYTES = 16, 16, 1 << 20
 
 
 class ExprNode(C.Structure):
@@ -252,6 +254,10 @@ def load() -> C.CDLL:
                                           C.POINTER(C.c_uint64), C.c_int, C.POINTER(Error)]
     lib.ytgpu_evaluate_expression.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p,
                                               C.c_void_p, C.POINTER(C.c_uint8), C.POINTER(C.c_uint64), C.c_int, C.POINTER(Error)]
+    lib.ytgpu_evaluate_expression_strings.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64,
+                                                      C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64,
+                                                      C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint8),
+                                                      C.POINTER(C.c_uint64), C.c_int, C.POINTER(Error)]
     lib.ytgpu_partition_rowset.argtypes = [C.c_void_p, C.POINTER(RowsetView), C.POINTER(PartitionSpec), C.c_void_p,
                                            C.c_void_p, C.c_int, C.POINTER(Error)]
     lib.ytgpu_partition_rowset_slabs.argtypes = [C.c_void_p, C.POINTER(RowsetView), C.POINTER(PartitionSpec), C.c_void_p, C.c_void_p,

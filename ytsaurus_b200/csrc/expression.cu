@@ -13,28 +13,51 @@
 //     a bit stack in one register.  The depth at every node is the same in all lanes, so nothing goes to local memory;
 //   * a 32-row group without a selected row skips the program;
 //   * the NULL count and the division-error bits are reduced per warp, one atomic each.
+//
+// String expressions (ytgpu_evaluate_expression_strings) run the instantiation expression_kernel<true>.  A STRING stack
+// entry is a list of pieces (pointer, length, case map): a leaf makes one piece, CONCAT appends the lists, LOWER / UPPER
+// set the case map of every piece (on ASCII lower(upper(x)) = lower(x), so the outermost wins) and IF_NULL keeps one of
+// them.  The pieces form a second stack in shared memory, [piece][threadIdx.x] (pointer u64, length u32); the value
+// stack holds a string entry's piece count, 0 when it is NULL, and the case maps are 2 bits per piece in one register.
+// So no piece is ever moved: CONCAT's operands are adjacent already and IF_NULL's NULL first operand has no pieces.  The
+// piece count is bounded at check time (YTGPU_EXPR_MAX_PIECES).  A STRING result takes two passes of the same program:
+//   1. kModeSize writes each row's length, NULL byte and (as the scan input) its length into starts, and checks the
+//      bytes under LOWER / UPPER are ASCII;
+//   2. an exclusive scan (scan.cuh) turns the lengths into starts, its total is the heap size;
+//   3. kModeFill evaluates the program again and copies the pieces with their case maps, row-centric as
+//      string_to_ch.cu's copy: a warp whose 32 values are short assembles them in shared memory and writes the stretch
+//      with 16-byte stores; a long value is copied by the whole warp, 4 bytes per lane when aligned.
+// FARM_HASH hashes its operands with farmhash.cuh's value and row combiners; a string operand is one piece.
 #include <algorithm>
 #include <cstring>
 #include <vector>
 
 #include "columnar.cuh"
 #include "context.cuh"
+#include "farmhash.cuh"
+#include "scan.cuh"
+#include "strings.cuh"
 
 using namespace ytgpu;
 
 namespace {
 
 constexpr int kExprThreads = 256;
-constexpr u32 kErrDivZero = 1, kErrIntMinByMinusOne = 2;
+constexpr u32 kErrDivZero = 1, kErrIntMinByMinusOne = 2, kErrOutOfHeap = 4, kErrNonAscii = 8, kErrTooLong = 16;
+constexpr u32 kModeValues = 0, kModeSize = 1, kModeFill = 2;  // a 64-bit result; a STRING result's two passes
+constexpr u32 kCaseLower = 1, kCaseUpper = 2;
+constexpr u32 kShortValue = 48;                                        // longer values are copied by the whole warp
+constexpr u32 kStageBytes = 32 * kShortValue + 16;                     // a warp's short values and the 16-byte skew
 
 struct ExprNodeDev {
     u8 op;
     u8 type;  // the node's result type
     u8 from;  // CAST: the operand's type
     u8 pad;
-    u16 col;  // COLUMN: compact column table (referenced columns only)
+    u16 col;  // COLUMN: compact column table (referenced columns only; a STRING leaf: the compact string table);
+              // FARM_HASH: its operand count
     u16 pad2;
-    u64 constant;
+    u64 constant;  // CONSTANT: the bit pattern, a STRING one (offset << 32) | length; FARM_HASH: bit j = operand j is a STRING
 };
 static_assert(sizeof(ExprNodeDev) == 16, "ExprNodeDev layout");
 
@@ -47,7 +70,18 @@ struct ExprArgs {
     u64 n;
     u64* values;
     u32* nulls;                   // 2 * ceil(n / 64) words of 32 bits
-    unsigned long long* result;   // [0] NULL rows, [1] error bits
+    unsigned long long* result;   // [0] NULL rows, [1] error bits, [2] (STRING result) heap bytes
+    // expression_kernel<true> only
+    const StringDev* strings;
+    u32 string_count;
+    u32 mode;
+    u32 max_depth;                // stack entries below the top: max_depth - 1
+    u32 max_pieces;
+    const u8* consts;             // the string constants
+    u64* starts;                  // kModeSize: the lengths (the scan's input); kModeFill: the starts
+    u32* lengths;
+    u8* null_bytes;
+    u8* heap;
 };
 
 __device__ __forceinline__ double as_double(u64 x) { return __longlong_as_double((long long)x); }
@@ -100,11 +134,59 @@ __device__ __forceinline__ u64 unary_op(u32 op, u32 type, u32 from, u64 a) {
     return a;  // INT64 <-> UINT64, BOOLEAN -> integer
 }
 
+// A byte under a case map; ASCII letters only (a mapped piece holds ASCII bytes, checked in kModeSize).
+__device__ __forceinline__ u32 case_byte(u32 b, u32 cm) {
+    if (cm == kCaseLower) return b - 'A' < 26u ? b + 32 : b;
+    if (cm == kCaseUpper) return b - 'a' < 26u ? b - 32 : b;
+    return b;
+}
+
+// Four ASCII bytes at once: bit 7 of a byte of (w + 0x3f..) is set iff the byte is >= 'A', of (w + 0x25..) iff > 'Z'; no
+// carry crosses a byte while every byte is below 0x80.
+__device__ __forceinline__ u32 case_word(u32 w, u32 cm) {
+    if (cm == kCaseLower) return w ^ ((((w + 0x3f3f3f3fu) & ~(w + 0x25252525u)) & 0x80808080u) >> 2);
+    if (cm == kCaseUpper) return w ^ ((((w + 0x1f1f1f1fu) & ~(w + 0x05050505u)) & 0x80808080u) >> 2);
+    return w;
+}
+
+__device__ __forceinline__ bool ascii_only(const u8* p, u32 len) {
+    const u32 head = min(len, (u32)((8 - (reinterpret_cast<uintptr_t>(p) & 7)) & 7));
+    u32 acc = 0, j = 0;
+    for (; j < head; ++j) acc |= __ldg(p + j);
+    for (; j + 8 <= len; j += 8)
+        if (__ldg(reinterpret_cast<const unsigned long long*>(p + j)) & 0x8080808080808080ull) return false;
+    for (; j < len; ++j) acc |= __ldg(p + j);
+    return (acc & 0x80) == 0;
+}
+
+// The whole warp copies len bytes: bytes up to the destination's 4-byte boundary, then 4 bytes per lane when the source
+// is aligned there too (else 1), then the tail — string_to_ch.cu's long-value copy, with the case map applied.
+__device__ __forceinline__ void warp_copy(u8* dst, const u8* src, u64 len, u32 cm, u32 lane) {
+    const u32 head = (u32)min(len, (u64)((4 - (reinterpret_cast<uintptr_t>(dst) & 3)) & 3));
+    for (u32 j = lane; j < head; j += 32) dst[j] = (u8)case_byte(__ldg(src + j), cm);
+    const u64 body = (len - head) & ~3ull;
+    if (((reinterpret_cast<uintptr_t>(src) + head) & 3) == 0) {
+        const u32* s4 = reinterpret_cast<const u32*>(src + head);
+        u32* d4 = reinterpret_cast<u32*>(dst + head);
+        for (u64 w = lane; w < body / 4; w += 32) d4[w] = case_word(__ldg(s4 + w), cm);
+    } else {
+        for (u64 j = lane; j < body; j += 32) dst[head + j] = (u8)case_byte(__ldg(src + head + j), cm);
+    }
+    for (u64 j = head + body + lane; j < len; j += 32) dst[j] = (u8)case_byte(__ldg(src + j), cm);
+}
+
+template <bool kStrings>
 __global__ void __launch_bounds__(kExprThreads) expression_kernel(const ExprArgs A) {
     extern __shared__ __align__(16) unsigned char smem[];
     ExprNodeDev* s_nodes = reinterpret_cast<ExprNodeDev*>(smem);
     ColumnDev* s_cols = reinterpret_cast<ColumnDev*>(s_nodes + A.node_count);
-    u64* s_stack = reinterpret_cast<u64*>(s_cols + A.column_count) + threadIdx.x;  // entry d of this thread: [d * kExprThreads]
+    StringDev* s_strs = reinterpret_cast<StringDev*>(s_cols + A.column_count);
+    u64* s_stack = reinterpret_cast<u64*>(s_strs + (kStrings ? A.string_count : 0)) + threadIdx.x;  // entry d: [d * kExprThreads]
+    // expression_kernel<true>: the piece stack [p * kExprThreads], then a short-value stage per warp
+    u64* s_pptr = s_stack + (kStrings ? (size_t)(A.max_depth - 1) * kExprThreads : 0);
+    u32* s_plen = reinterpret_cast<u32*>(s_pptr - threadIdx.x + (size_t)A.max_pieces * kExprThreads) + threadIdx.x;
+    u8* s_stage = reinterpret_cast<u8*>((reinterpret_cast<uintptr_t>(s_plen - threadIdx.x + (size_t)A.max_pieces * kExprThreads) + 15) & ~(uintptr_t)15) +
+                  (threadIdx.x >> 5) * kStageBytes;
     {
         const u32* src = reinterpret_cast<const u32*>(A.nodes);
         u32* dst = reinterpret_cast<u32*>(s_nodes);
@@ -112,6 +194,11 @@ __global__ void __launch_bounds__(kExprThreads) expression_kernel(const ExprArgs
         src = reinterpret_cast<const u32*>(A.columns);
         dst = reinterpret_cast<u32*>(s_cols);
         for (u32 k = threadIdx.x; k < A.column_count * (u32)(sizeof(ColumnDev) / 4); k += blockDim.x) dst[k] = src[k];
+        if constexpr (kStrings) {
+            src = reinterpret_cast<const u32*>(A.strings);
+            dst = reinterpret_cast<u32*>(s_strs);
+            for (u32 k = threadIdx.x; k < A.string_count * (u32)(sizeof(StringDev) / 4); k += blockDim.x) dst[k] = src[k];
+        }
     }
     __syncthreads();
 
@@ -127,6 +214,8 @@ __global__ void __launch_bounds__(kExprThreads) expression_kernel(const ExprArgs
         const bool live = i < A.n && ((sel >> lane) & 1);
         u64 top = 0;
         u32 nul_stack = 1;  // bit d: entry d from the top is NULL
+        u32 np = 0;         // pieces on the piece stack
+        u32 cases = 0;      // 2 bits per piece: its case map
         if (sel != 0) {
             u32 depth = 0;  // entries below the top, in s_stack
 #pragma unroll 1
@@ -135,7 +224,27 @@ __global__ void __launch_bounds__(kExprThreads) expression_kernel(const ExprArgs
                 if (nd.op == YTGPU_EXPR_COLUMN || nd.op == YTGPU_EXPR_CONSTANT) {
                     bool nul = !live;
                     u64 v = nd.constant;
-                    if (nd.op == YTGPU_EXPR_COLUMN) {
+                    if (kStrings && nd.type == YTGPU_TYPE_STRING) {
+                        const u8* p = A.consts + (nd.constant >> 32);
+                        u32 len = (u32)nd.constant;
+                        if (nd.op == YTGPU_EXPR_COLUMN && !nul) {
+                            const StringDev& sc = s_strs[nd.col];
+                            ytgpu_value sv;
+                            u32 bad = 0;
+                            nul = !string_at(sc, i, &sv, &bad);
+                            if (bad) err |= kErrOutOfHeap;
+                            p = sc.heap + sv.data;
+                            len = sv.length;
+                        }
+                        v = 0;
+                        if (!nul) {  // one piece
+                            s_pptr[np * kExprThreads] = reinterpret_cast<u64>(p);
+                            s_plen[np * kExprThreads] = len;
+                            cases &= ~(3u << (2 * np));
+                            ++np;
+                            v = 1;
+                        }
+                    } else if (nd.op == YTGPU_EXPR_COLUMN) {
                         const ColumnDev& c = s_cols[nd.col];
                         v = scalar_value(c, i, row0, live, &nul);
                         if (c.value_type == YTGPU_TYPE_BOOLEAN) v = v != 0;
@@ -145,6 +254,40 @@ __global__ void __launch_bounds__(kExprThreads) expression_kernel(const ExprArgs
                     nul_stack = (nul_stack << 1) | (nul ? 1u : 0u);
                 } else if (nd.op == YTGPU_EXPR_NEG || nd.op == YTGPU_EXPR_BIT_NOT || nd.op == YTGPU_EXPR_CAST) {
                     if (!(nul_stack & 1)) top = unary_op(nd.op, nd.type, nd.from, top);
+                } else if (kStrings && (nd.op == YTGPU_EXPR_LOWER || nd.op == YTGPU_EXPR_UPPER)) {
+                    if (!(nul_stack & 1)) {
+                        const u32 first = np - (u32)top;
+                        if (A.mode == kModeSize)
+                            for (u32 p = first; p < np; ++p)
+                                if (!ascii_only(reinterpret_cast<const u8*>(s_pptr[p * kExprThreads]), s_plen[p * kExprThreads]))
+                                    err |= kErrNonAscii;
+                        const u32 mask = (u32)(((1ull << (2 * np)) - 1) & ~((1ull << (2 * first)) - 1));
+                        cases = (cases & ~mask) | ((nd.op == YTGPU_EXPR_LOWER ? 0x55555555u : 0xaaaaaaaau) & mask);
+                    }
+                } else if (kStrings && nd.op == YTGPU_EXPR_FARM_HASH) {
+                    // GetFarmFingerprint over the operands, deepest first; a NULL operand (a numeric one holds 0) hashes as
+                    // fingerprint_u64(0), a string one is a single piece
+                    const u32 count = nd.col, strs = (u32)nd.constant, below = depth - (count - 1);
+                    u32 sp = 0;
+                    for (u32 j = 0; j < count; ++j)
+                        if ((strs >> j) & 1) sp += (u32)(j + 1 == count ? top : s_stack[(below + j) * kExprThreads]);
+                    u32 p = np - sp;
+                    u64 h = 0xdeadc0deULL;
+                    for (u32 j = 0; j < count; ++j) {
+                        const u64 v = j + 1 == count ? top : s_stack[(below + j) * kExprThreads];
+                        u64 f;
+                        if (((strs >> j) & 1) && v) {
+                            f = fh::fingerprint_bytes(reinterpret_cast<const u8*>(s_pptr[p * kExprThreads]), s_plen[p * kExprThreads]);
+                            ++p;
+                        } else {
+                            f = fh::fingerprint_u64((strs >> j) & 1 ? 0 : v);
+                        }
+                        h = fh::fingerprint_u128(h, f);
+                    }
+                    np -= sp;
+                    depth = below;
+                    top = h ^ (u64)count;
+                    nul_stack = (nul_stack >> count) << 1;
                 } else {
                     const u64 a = s_stack[--depth * kExprThreads], b = top;
                     const u32 nb = nul_stack & 1, na = (nul_stack >> 1) & 1;
@@ -152,6 +295,11 @@ __global__ void __launch_bounds__(kExprThreads) expression_kernel(const ExprArgs
                     if (nd.op == YTGPU_EXPR_IF_NULL) {
                         top = na ? b : a;
                         nr = na & nb;
+                        if (kStrings && nd.type == YTGPU_TYPE_STRING && !na) np -= (u32)b;  // a NULL first operand has no pieces
+                    } else if (kStrings && nd.op == YTGPU_EXPR_CONCAT) {
+                        nr = na | nb;
+                        np -= nr ? (u32)(a + b) : 0;
+                        top = nr ? 0 : a + b;
                     } else {
                         nr = na | nb;
                         top = nr ? 0 : binary_op(nd.op, nd.type, a, b, &err);
@@ -161,11 +309,92 @@ __global__ void __launch_bounds__(kExprThreads) expression_kernel(const ExprArgs
             }
         }
         const bool nul = !live || (nul_stack & 1);
-        const u32 m = __ballot_sync(0xffffffffu, nul && i < A.n);
-        if (i < A.n) A.values[i] = nul ? 0 : top;
-        if (lane == 0) {
-            A.nulls[w] = m;
-            null_rows += (u64)__popc(m);
+        if (!kStrings || A.mode == kModeValues) {
+            const u32 m = __ballot_sync(0xffffffffu, nul && i < A.n);
+            if (i < A.n) A.values[i] = nul ? 0 : top;
+            if (lane == 0) {
+                A.nulls[w] = m;
+                null_rows += (u64)__popc(m);
+            }
+            continue;
+        }
+        if constexpr (kStrings) {
+            u64 len = 0;
+            if (!nul)
+                for (u32 p = 0; p < np; ++p) len += s_plen[p * kExprThreads];
+            if (A.mode == kModeSize) {
+                if (len > 0xffffffffull) {
+                    err |= kErrTooLong;
+                    len = 0;
+                }
+                const u32 m = __ballot_sync(0xffffffffu, nul && i < A.n);
+                if (i < A.n) {
+                    A.starts[i] = len;
+                    A.lengths[i] = (u32)len;
+                    A.null_bytes[i] = nul ? 1 : 0;
+                }
+                if (lane == 0) null_rows += (u64)__popc(m);
+                continue;
+            }
+            // kModeFill
+            if (row0 >= A.n) continue;  // a group past the last row (the bitmap's last word); warp-uniform
+            const u64 pos = i < A.n ? A.starts[i] : 0;
+            const bool is_long = len > kShortValue;
+            u32 todo = __ballot_sync(0xffffffffu, is_long);
+            if (todo == 0) {
+                // every value of the group is short: the group's output [p0, p1) is one stretch, assembled in the warp's stage
+                // from its 16-byte boundary below heap + p0 and written out with 16-byte stores
+                const u64 p0 = __shfl_sync(0xffffffffu, pos, 0);
+                u64 p1 = i < A.n ? pos + len : p0;
+#pragma unroll
+                for (int d = 16; d > 0; d >>= 1) p1 = max(p1, __shfl_xor_sync(0xffffffffu, p1, d));
+                const u32 skew = (u32)(reinterpret_cast<uintptr_t>(A.heap + p0) & 15);
+                u8* dst = s_stage + skew + (u32)(pos - p0);
+                if (len)
+                    for (u32 p = 0; p < np; ++p) {
+                        const u8* src = reinterpret_cast<const u8*>(s_pptr[p * kExprThreads]);
+                        const u32 l = s_plen[p * kExprThreads], cm = (cases >> (2 * p)) & 3;
+                        for (u32 j = 0; j < l; ++j) dst[j] = (u8)case_byte(__ldg(src + j), cm);
+                        dst += l;
+                    }
+                __syncwarp();
+                const u32 begin = skew, end = skew + (u32)(p1 - p0);
+                u8* gbase = A.heap + p0 - skew;  // 16-byte aligned
+                for (u32 q = lane; q * 16 < end; q += 32) {
+                    const u32 lo = q * 16, hi = lo + 16;
+                    if (lo >= begin && hi <= end) {
+                        reinterpret_cast<uint4*>(gbase)[q] = reinterpret_cast<const uint4*>(s_stage)[q];
+                    } else {
+                        for (u32 b = max(lo, begin); b < min(hi, end); ++b) gbase[b] = s_stage[b];
+                    }
+                }
+                __syncwarp();  // the stage is reused by the next group
+                continue;
+            }
+            if (!is_long && len) {
+                u8* dst = A.heap + pos;
+                for (u32 p = 0; p < np; ++p) {
+                    const u8* src = reinterpret_cast<const u8*>(s_pptr[p * kExprThreads]);
+                    const u32 l = s_plen[p * kExprThreads], cm = (cases >> (2 * p)) & 3;
+                    for (u32 j = 0; j < l; ++j) dst[j] = (u8)case_byte(__ldg(src + j), cm);
+                    dst += l;
+                }
+            }
+            __syncwarp();  // the owners' piece stacks, written while the program ran, are read by the whole warp
+            while (todo) {  // long values, one at a time by the whole warp, piece by piece from the owner's piece stack
+                const int l = __ffs(todo) - 1;
+                todo &= todo - 1;
+                const u32 owner = (threadIdx.x & ~31u) + (u32)l;
+                const u32 lnp = __shfl_sync(0xffffffffu, np, l), lcases = __shfl_sync(0xffffffffu, cases, l);
+                u8* dst = A.heap + __shfl_sync(0xffffffffu, pos, l);
+                for (u32 p = 0; p < lnp; ++p) {
+                    const u8* src = reinterpret_cast<const u8*>(s_pptr[p * kExprThreads - threadIdx.x + owner]);
+                    const u32 pl = s_plen[p * kExprThreads - threadIdx.x + owner];
+                    warp_copy(dst, src, pl, (lcases >> (2 * p)) & 3, lane);
+                    dst += pl;
+                }
+            }
+            __syncwarp();  // ... and are overwritten by the next group's program
         }
     }
     err = __reduce_or_sync(0xffffffffu, err);
@@ -178,8 +407,11 @@ __global__ void __launch_bounds__(kExprThreads) expression_kernel(const ExprArgs
 // ---- host ----
 struct CheckedExpr {
     std::vector<ExprNodeDev> nodes;
-    std::vector<u32> cols;  // compact slot -> caller column
+    std::vector<u32> cols;     // compact slot -> caller column
+    std::vector<u32> strings;  // compact string slot -> caller string column
     u32 max_depth = 0;
+    u32 max_pieces = 0;
+    bool strings_kernel = false;  // a STRING node or FARM_HASH: expression_kernel<true>
     u8 type = 0;  // the result type
 };
 
@@ -189,21 +421,42 @@ bool is_expr_type(u32 t) {
 bool is_number_type(u32 t) { return t == YTGPU_TYPE_INT64 || t == YTGPU_TYPE_UINT64 || t == YTGPU_TYPE_DOUBLE; }
 bool is_integer_type(u32 t) { return t == YTGPU_TYPE_INT64 || t == YTGPU_TYPE_UINT64; }
 
-Status check_expression(const ytgpu_column_view* columns, u32 column_count, const ytgpu_expr_node* program, u32 node_count,
-                        CheckedExpr* out) {
+// `strings`: the program comes through ytgpu_evaluate_expression_strings, which takes string leaves and the string ops.
+Status check_expression(const ytgpu_column_view* columns, u32 column_count, bool strings, u32 string_count, u64 const_bytes,
+                        const ytgpu_expr_node* program, u32 node_count, CheckedExpr* out) {
     if (node_count == 0 || node_count > (u32)YTGPU_EXPR_MAX_NODES)
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "an expression program has 1 .. %d nodes", YTGPU_EXPR_MAX_NODES);
     if (!program) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null program");
-    std::vector<int> slot_of(column_count, -1);
-    std::vector<u8> types;  // the type stack
+    std::vector<int> slot_of(column_count, -1), string_slot_of(string_count, -1);
+    struct Entry {
+        u8 type;
+        u8 plain;     // STRING: one piece without a case map at most (a leaf, a constant or IF_NULL of those)
+        u32 pieces;   // STRING: the most pieces it may have
+    };
+    std::vector<Entry> stack;
+    u32 pieces = 0;  // on the whole stack
     for (u32 k = 0; k < node_count; ++k) {
         const ytgpu_expr_node& N = program[k];
         ExprNodeDev d{};
         d.op = (u8)N.op;
+        const bool string_op = N.op == YTGPU_EXPR_CONCAT || N.op == YTGPU_EXPR_LOWER || N.op == YTGPU_EXPR_UPPER || N.op == YTGPU_EXPR_FARM_HASH;
+        if (string_op && !strings) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: unknown op %d", k, N.op);
         switch (N.op) {
             case YTGPU_EXPR_COLUMN: {
-                if (N.column < 0 || (u32)N.column >= column_count)
+                if (N.column < 0 || (u64)N.column >= (u64)column_count + (strings ? string_count : 0))
                     return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: column %d out of range", k, N.column);
+                if ((u32)N.column >= column_count) {  // string_columns[column - column_count]
+                    const u32 s = (u32)N.column - column_count;
+                    if (string_slot_of[s] < 0) {
+                        string_slot_of[s] = (int)out->strings.size();
+                        out->strings.push_back(s);
+                    }
+                    d.col = (u16)string_slot_of[s];
+                    d.type = YTGPU_TYPE_STRING;
+                    stack.push_back({YTGPU_TYPE_STRING, 1, 1});
+                    ++pieces;
+                    break;
+                }
                 const u8 t = columns[N.column].value_type;
                 if (!is_expr_type(t))
                     return make_status(YTGPU_ERR_UNSUPPORTED, "node %u: column %d has value type 0x%x (INT64, UINT64, DOUBLE or BOOLEAN)", k,
@@ -214,22 +467,33 @@ Status check_expression(const ytgpu_column_view* columns, u32 column_count, cons
                 }
                 d.col = (u16)slot_of[N.column];
                 d.type = t;
-                types.push_back(t);
+                stack.push_back({t, 0, 0});
                 break;
             }
             case YTGPU_EXPR_CONSTANT:
+                if (strings && N.type == YTGPU_TYPE_STRING) {
+                    const u64 off = N.constant >> 32, len = N.constant & 0xffffffffull;
+                    if (off + len > const_bytes)
+                        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: string constant outside string_constants", k);
+                    d.type = N.type;
+                    d.constant = N.constant;
+                    stack.push_back({YTGPU_TYPE_STRING, 1, 1});
+                    ++pieces;
+                    break;
+                }
                 if (!is_expr_type(N.type)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: unknown constant type 0x%x", k, N.type);
                 if (N.type == YTGPU_TYPE_BOOLEAN && N.constant > 1)
                     return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: a BOOLEAN constant is 0 or 1", k);
                 d.type = N.type;
                 d.constant = N.constant;
-                types.push_back(N.type);
+                stack.push_back({N.type, 0, 0});
                 break;
             case YTGPU_EXPR_NEG:
             case YTGPU_EXPR_BIT_NOT:
             case YTGPU_EXPR_CAST: {
-                if (types.empty()) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: stack underflow", k);
-                const u8 t = types.back();
+                if (stack.empty()) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: stack underflow", k);
+                const u8 t = stack.back().type;
+                if (t == YTGPU_TYPE_STRING) return make_status(YTGPU_ERR_UNSUPPORTED, "node %u: op %d does not take strings", k, N.op);
                 if (N.op == YTGPU_EXPR_CAST) {
                     if (!is_number_type(N.type))
                         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: CAST to type 0x%x (INT64, UINT64 or DOUBLE)", k, N.type);
@@ -240,7 +504,37 @@ Status check_expression(const ytgpu_column_view* columns, u32 column_count, cons
                         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: op %d does not take type 0x%x", k, N.op, t);
                     d.type = t;
                 }
-                types.back() = d.type;
+                stack.back().type = d.type;
+                break;
+            }
+            case YTGPU_EXPR_LOWER:
+            case YTGPU_EXPR_UPPER:
+                if (stack.empty()) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: stack underflow", k);
+                if (stack.back().type != YTGPU_TYPE_STRING)
+                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: op %d takes a STRING, not type 0x%x", k, N.op, stack.back().type);
+                d.type = YTGPU_TYPE_STRING;
+                stack.back().plain = 0;
+                break;
+            case YTGPU_EXPR_FARM_HASH: {
+                if (N.column < 1 || N.column > YTGPU_EXPR_MAX_HASH_OPERANDS)
+                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: FARM_HASH of %d operands (1 .. %d)", k, N.column,
+                                       YTGPU_EXPR_MAX_HASH_OPERANDS);
+                const u32 count = (u32)N.column;
+                if (stack.size() < count) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: stack underflow", k);
+                u64 strs = 0;
+                for (u32 j = 0; j < count; ++j) {
+                    const Entry& e = stack[stack.size() - count + j];
+                    if (e.type != YTGPU_TYPE_STRING) continue;
+                    if (!e.plain)
+                        return make_status(YTGPU_ERR_UNSUPPORTED, "node %u: FARM_HASH of a CONCAT, LOWER or UPPER result", k);
+                    strs |= 1ull << j;
+                    pieces -= e.pieces;
+                }
+                stack.resize(stack.size() - count);
+                d.col = (u16)count;
+                d.constant = strs;
+                d.type = YTGPU_TYPE_UINT64;
+                stack.push_back({YTGPU_TYPE_UINT64, 0, 0});
                 break;
             }
             case YTGPU_EXPR_ADD:
@@ -251,49 +545,100 @@ Status check_expression(const ytgpu_column_view* columns, u32 column_count, cons
             case YTGPU_EXPR_BIT_AND:
             case YTGPU_EXPR_BIT_OR:
             case YTGPU_EXPR_BIT_XOR:
-            case YTGPU_EXPR_IF_NULL: {
-                if (types.size() < 2) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: stack underflow", k);
-                const u8 b = types.back();
-                types.pop_back();
-                const u8 a = types.back();
+            case YTGPU_EXPR_IF_NULL:
+            case YTGPU_EXPR_CONCAT: {
+                if (stack.size() < 2) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: stack underflow", k);
+                const Entry eb = stack.back();
+                stack.pop_back();
+                const Entry ea = stack.back();
+                const u8 a = ea.type, b = eb.type;
+                if (N.op == YTGPU_EXPR_CONCAT) {
+                    if (a != YTGPU_TYPE_STRING || b != YTGPU_TYPE_STRING)
+                        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: CONCAT of types 0x%x and 0x%x (two STRINGs)", k, a, b);
+                    stack.back() = {YTGPU_TYPE_STRING, 0, ea.pieces + eb.pieces};
+                    d.type = YTGPU_TYPE_STRING;
+                    break;
+                }
+                if (N.op != YTGPU_EXPR_IF_NULL && (a == YTGPU_TYPE_STRING || b == YTGPU_TYPE_STRING))
+                    return make_status(YTGPU_ERR_UNSUPPORTED, "node %u: op %d does not take strings", k, N.op);
                 if (a != b) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: operands of types 0x%x and 0x%x (CAST one of them)", k, a, b);
                 const bool ok = N.op == YTGPU_EXPR_IF_NULL ? true
                               : (N.op <= YTGPU_EXPR_DIV ? is_number_type(a) : is_integer_type(a));
                 if (!ok) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: op %d does not take type 0x%x", k, N.op, a);
                 d.type = a;
+                if (a == YTGPU_TYPE_STRING) {  // IF_NULL keeps one operand's pieces
+                    stack.back() = {YTGPU_TYPE_STRING, (u8)(ea.plain & eb.plain), std::max(ea.pieces, eb.pieces)};
+                    pieces -= std::min(ea.pieces, eb.pieces);
+                }
                 break;
             }
             default:
                 return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: unknown op %d", k, N.op);
         }
-        if (types.size() > (size_t)YTGPU_EXPR_MAX_DEPTH)
+        if (stack.size() > (size_t)YTGPU_EXPR_MAX_DEPTH)
             return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: stack deeper than %d", k, YTGPU_EXPR_MAX_DEPTH);
-        out->max_depth = std::max(out->max_depth, (u32)types.size());
+        if (pieces > (u32)YTGPU_EXPR_MAX_PIECES)
+            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: more than %d string pieces on the stack", k, YTGPU_EXPR_MAX_PIECES);
+        out->max_depth = std::max(out->max_depth, (u32)stack.size());
+        out->max_pieces = std::max(out->max_pieces, pieces);
+        out->strings_kernel |= d.type == YTGPU_TYPE_STRING || N.op == YTGPU_EXPR_FARM_HASH;
         out->nodes.push_back(d);
     }
-    if (types.size() != 1)
-        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "the program leaves %d values on the stack, not 1", (int)types.size());
-    out->type = types[0];
+    if (stack.size() != 1)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "the program leaves %d values on the stack, not 1", (int)stack.size());
+    out->type = stack[0].type;
     return Status{};
 }
 
-Status evaluate_expression_impl(Context* ctx, const ytgpu_column_view* columns, u32 column_count, const ytgpu_expr_node* program,
-                                u32 node_count, const u8* selection, u64* out_values, u8* out_null_bitmap, u8* out_value_type,
-                                u64* out_null_count, int out_mem) {
-    if (column_count && !columns) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null columns");
-    if (column_count == 0) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "no columns");
+// The outputs of a STRING result (ytgpu_evaluate_expression_strings).
+struct StringResult {
+    u8* heap;
+    u64 capacity;
+    u64* starts;
+    u32* lengths;
+    u8* null_bytemap;
+    u64* heap_bytes;
+};
+
+Status evaluate_expression_impl(Context* ctx, const ytgpu_column_view* columns, u32 column_count, const ytgpu_string_column* string_columns,
+                                u32 string_count, const u8* consts, u64 const_bytes, const StringResult* sr,
+                                const ytgpu_expr_node* program, u32 node_count, const u8* selection, u64* out_values, u8* out_null_bitmap,
+                                u8* out_value_type, u64* out_null_count, int out_mem) {
+    const bool strings = sr != nullptr;  // the string entry point
+    if ((column_count && !columns) || (string_count && !string_columns)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null columns");
+    if (column_count + (u64)string_count == 0) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "no columns");
     if (out_mem != YTGPU_MEM_DEVICE && out_mem != YTGPU_MEM_HOST)
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "out_mem must be YTGPU_MEM_DEVICE or YTGPU_MEM_HOST");
-    const u64 n = (u64)columns[0].value_count;
+    const u64 n = column_count ? (u64)columns[0].value_count : string_columns[0].row_count;
     for (u32 c = 0; c < column_count; ++c)
         if (columns[c].value_count < 0 || (u64)columns[c].value_count != n)
             return make_status(YTGPU_ERR_INVALID_ARGUMENT, "column %u differs in length", c);
+    for (u32 s = 0; s < string_count; ++s) {
+        const ytgpu_string_column& S = string_columns[s];
+        if (S.row_count != n) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "string column %u differs in length", s);
+        if ((S.heap_bytes && !S.heap) || (n && (!S.starts || !S.lengths)))
+            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "string column %u: null heap, starts or lengths", s);
+        if (S.mem != YTGPU_MEM_DEVICE && S.mem != YTGPU_MEM_HOST)
+            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "string column %u: mem must be YTGPU_MEM_DEVICE or YTGPU_MEM_HOST", s);
+    }
+    if (const_bytes > YTGPU_EXPR_MAX_STRING_CONSTANT_BYTES)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "more than %u bytes of string_constants", (unsigned)YTGPU_EXPR_MAX_STRING_CONSTANT_BYTES);
+    if (const_bytes && !consts) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null string_constants");
     if (n >= (1ull << 32)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "fewer than 2^32 rows per call");
     CheckedExpr P;
-    YTGPU_TRY(check_expression(columns, column_count, program, node_count, &P));
+    YTGPU_TRY(check_expression(columns, column_count, strings, string_count, const_bytes, program, node_count, &P));
     if (out_value_type) *out_value_type = P.type;
     if (out_null_count) *out_null_count = 0;
-    if (n && (!out_values || !out_null_bitmap)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null out_values or out_null_bitmap");
+    const bool string_result = P.type == YTGPU_TYPE_STRING;
+    if (string_result) {
+        if (!sr->heap_bytes) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null out_heap_bytes");
+        *sr->heap_bytes = 0;
+        if (n && sr->heap && (!sr->starts || !sr->lengths || !sr->null_bytemap))
+            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null out_starts, out_lengths or out_null_bytemap");
+    } else if (n && (!out_values || !out_null_bitmap)) {
+        if (strings && !sr->heap && !out_values && !out_null_bitmap) return Status{};  // a type query: nothing is evaluated
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null out_values or out_null_bitmap");
+    }
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
     if (n == 0) return Status{};
 
@@ -303,36 +648,62 @@ Status evaluate_expression_impl(Context* ctx, const ytgpu_column_view* columns, 
         YTGPU_TRY(stage_column(ctx, &columns[P.cols[k]], &sc[k]));
         hc[k] = sc[k].dev;
     }
-    // one upload: nodes | column views
-    const size_t nodes_b = P.nodes.size() * sizeof(ExprNodeDev), cols_b = hc.size() * sizeof(ColumnDev);
-    std::vector<u8> blob(nodes_b + cols_b);
+    std::vector<StagedStrings> ss(P.strings.size());
+    std::vector<StringDev> hs(P.strings.size());
+    for (size_t k = 0; k < ss.size(); ++k) {
+        YTGPU_TRY(stage_strings(ctx, string_columns[P.strings[k]], &ss[k]));
+        hs[k] = ss[k].dev;
+    }
+    // one upload: nodes | column views | string views | string constants
+    const size_t nodes_b = P.nodes.size() * sizeof(ExprNodeDev), cols_b = hc.size() * sizeof(ColumnDev), strs_b = hs.size() * sizeof(StringDev);
+    std::vector<u8> blob(nodes_b + cols_b + strs_b + const_bytes);
     memcpy(blob.data(), P.nodes.data(), nodes_b);
     if (cols_b) memcpy(blob.data() + nodes_b, hc.data(), cols_b);
+    if (strs_b) memcpy(blob.data() + nodes_b + cols_b, hs.data(), strs_b);
+    if (const_bytes) memcpy(blob.data() + nodes_b + cols_b + strs_b, consts, const_bytes);
     DevBuf<u8> dblob;
     YTGPU_TRY(dblob.allocate(ctx, blob.size()));
     YTGPU_CUDA_TRY(cudaMemcpyAsync(dblob.p, blob.data(), blob.size(), cudaMemcpyHostToDevice, ctx->stream));
 
     const u64 words = (n + 63) / 64 * 2;  // 32-bit bitmap words
     const bool host = out_mem == YTGPU_MEM_HOST;
-    DevBuf<u64> tvalues;
-    DevBuf<u32> tnulls, tselection;
+    DevBuf<u64> tvalues, tstarts, scan_sums;
+    DevBuf<u32> tnulls, tselection, tlengths;
+    DevBuf<u8> tnull_bytes, theap;
     DevBuf<unsigned long long> result;
     u64* dvalues = out_values;
     u32* dnulls = reinterpret_cast<u32*>(out_null_bitmap);
     const u32* dselection = reinterpret_cast<const u32*>(selection);
-    if (host) {
+    if (host && selection) {
+        YTGPU_TRY(tselection.allocate(ctx, words));
+        YTGPU_TRY(copy_in(ctx, tselection.p, selection, words * 4, YTGPU_MEM_HOST));
+        dselection = tselection.p;
+    }
+    u64* dstarts = nullptr;
+    u32* dlengths = nullptr;
+    u8* dnull_bytes = nullptr;
+    if (string_result) {  // the size pass writes the caller's DEVICE outputs only when they are filled too
+        const bool direct = !host && sr->heap;
+        dstarts = direct ? sr->starts : nullptr;
+        dlengths = direct ? sr->lengths : nullptr;
+        dnull_bytes = direct ? sr->null_bytemap : nullptr;
+        if (!direct) {
+            YTGPU_TRY(tstarts.allocate(ctx, n));
+            YTGPU_TRY(tlengths.allocate(ctx, n));
+            YTGPU_TRY(tnull_bytes.allocate(ctx, n));
+            dstarts = tstarts.p;
+            dlengths = tlengths.p;
+            dnull_bytes = tnull_bytes.p;
+        }
+        YTGPU_TRY(scan_sums.allocate(ctx, scan_block_count(n)));
+    } else if (host) {
         YTGPU_TRY(tvalues.allocate(ctx, n));
         YTGPU_TRY(tnulls.allocate(ctx, words));
         dvalues = tvalues.p;
         dnulls = tnulls.p;
-        if (selection) {
-            YTGPU_TRY(tselection.allocate(ctx, words));
-            YTGPU_TRY(copy_in(ctx, tselection.p, selection, words * 4, YTGPU_MEM_HOST));
-            dselection = tselection.p;
-        }
     }
-    YTGPU_TRY(result.allocate(ctx, 2));
-    YTGPU_CUDA_TRY(cudaMemsetAsync(result.p, 0, 16, ctx->stream));
+    YTGPU_TRY(result.allocate(ctx, 3));
+    YTGPU_CUDA_TRY(cudaMemsetAsync(result.p, 0, 24, ctx->stream));
 
     ExprArgs A{};
     A.nodes = reinterpret_cast<const ExprNodeDev*>(dblob.p);
@@ -344,25 +715,79 @@ Status evaluate_expression_impl(Context* ctx, const ytgpu_column_view* columns, 
     A.values = dvalues;
     A.nulls = dnulls;
     A.result = result.p;
-    // shared memory in the kernel's order: nodes (16 B each), column views (8-byte multiple), the stack below the top
-    static_assert(sizeof(ColumnDev) % 8 == 0, "shared-memory layout");
-    const size_t smem = nodes_b + cols_b + (size_t)(P.max_depth - 1) * kExprThreads * sizeof(u64);
+    A.strings = reinterpret_cast<const StringDev*>(dblob.p + nodes_b + cols_b);
+    A.string_count = (u32)hs.size();
+    A.mode = string_result ? kModeSize : kModeValues;
+    A.max_depth = P.max_depth;
+    A.max_pieces = P.max_pieces;
+    A.consts = dblob.p + nodes_b + cols_b + strs_b;
+    A.starts = dstarts;
+    A.lengths = dlengths;
+    A.null_bytes = dnull_bytes;
+    // shared memory in the kernel's order: nodes (16 B each), column views, string views (8-byte multiples), the stack
+    // below the top; expression_kernel<true>: the piece stack and, 16-byte aligned, a short-value stage per warp
+    static_assert(sizeof(ColumnDev) % 8 == 0 && sizeof(StringDev) % 8 == 0, "shared-memory layout");
+    const size_t stack_b = (size_t)(P.max_depth - 1) * kExprThreads * sizeof(u64);
     const u32 blocks = (u32)std::max<u64>(1, std::min<u64>((words * 32 + kExprThreads - 1) / kExprThreads, (u64)kNumSms * 8));
-    {
+    if (!P.strings_kernel) {
+        const size_t smem = nodes_b + cols_b + stack_b;
         KernelTimer t(ctx, KC_DECODE);
-        expression_kernel<<<blocks, kExprThreads, smem, ctx->stream>>>(A);
+        expression_kernel<false><<<blocks, kExprThreads, smem, ctx->stream>>>(A);
+        YTGPU_CUDA_TRY(cudaGetLastError());
+    } else {
+        const size_t smem = nodes_b + cols_b + strs_b + stack_b + (size_t)P.max_pieces * kExprThreads * 12 + 16 +
+                            (size_t)(kExprThreads / 32) * kStageBytes;
+        // up to 16 pieces and a 16-deep stack take the stage past the 48 KB default
+        YTGPU_CUDA_TRY(cudaFuncSetAttribute(expression_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        KernelTimer t(ctx, KC_DECODE, string_result ? 4 : 1);
+        expression_kernel<true><<<blocks, kExprThreads, smem, ctx->stream>>>(A);
+        if (string_result)  // starts = exclusive scan of the lengths, the total into result[2]
+            exclusive_scan_u64(ctx->stream, dstarts, n, scan_sums.p, reinterpret_cast<u64*>(result.p + 2));
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
-    unsigned long long res[2] = {0, 0};  // the one host read: NULL count and error bits
-    YTGPU_CUDA_TRY(cudaMemcpyAsync(res, result.p, 16, cudaMemcpyDeviceToHost, ctx->stream));
-    if (host) {
+    unsigned long long res[3] = {0, 0, 0};  // the one host read: NULL count, error bits and the heap size
+    YTGPU_CUDA_TRY(cudaMemcpyAsync(res, result.p, string_result ? 24 : 16, cudaMemcpyDeviceToHost, ctx->stream));
+    if (host && !string_result) {
         YTGPU_TRY(copy_out(ctx, out_values, dvalues, n * 8, YTGPU_MEM_HOST));
         YTGPU_TRY(copy_out(ctx, out_null_bitmap, dnulls, words * 4, YTGPU_MEM_HOST));
     }
     YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    if (res[1] & kErrOutOfHeap) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "a string value of an expression column leaves its heap");
+    if (res[1] & kErrNonAscii)
+        return make_status(YTGPU_ERR_UNSUPPORTED, "lower / upper of a value with a byte >= 0x80: Unicode case mapping is not on the GPU path");
+    if (res[1] & kErrTooLong) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "a string result is longer than 2^32 - 1 bytes");
     if (res[1] & kErrDivZero) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "Division by zero");
     if (res[1] & kErrIntMinByMinusOne) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "Division INT_MIN by -1");
     if (out_null_count) *out_null_count = res[0];
+    if (!string_result) return Status{};
+
+    const u64 total = res[2];
+    *sr->heap_bytes = total;
+    if (!sr->heap) return Status{};
+    if (sr->capacity < total)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "out_heap holds %llu bytes, %llu are needed", (unsigned long long)sr->capacity,
+                           (unsigned long long)total);
+    u8* dheap = sr->heap;
+    if (host) {
+        YTGPU_TRY(theap.allocate(ctx, total));
+        dheap = theap.p;
+    }
+    A.mode = kModeFill;
+    A.heap = dheap;
+    {
+        const size_t smem = nodes_b + cols_b + strs_b + stack_b + (size_t)P.max_pieces * kExprThreads * 12 + 16 +
+                            (size_t)(kExprThreads / 32) * kStageBytes;
+        KernelTimer t(ctx, KC_GATHER);
+        expression_kernel<true><<<blocks, kExprThreads, smem, ctx->stream>>>(A);
+        YTGPU_CUDA_TRY(cudaGetLastError());
+    }
+    if (host) {
+        YTGPU_TRY(copy_out(ctx, sr->heap, dheap, total, YTGPU_MEM_HOST));
+        YTGPU_TRY(copy_out(ctx, sr->starts, dstarts, n * 8, YTGPU_MEM_HOST));
+        YTGPU_TRY(copy_out(ctx, sr->lengths, dlengths, n * 4, YTGPU_MEM_HOST));
+        YTGPU_TRY(copy_out(ctx, sr->null_bytemap, dnull_bytes, n, YTGPU_MEM_HOST));
+        YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    }
     return Status{};
 }
 
@@ -376,7 +801,22 @@ int ytgpu_evaluate_expression(ytgpu_context* h, const ytgpu_column_view* columns
                               ytgpu_error* err) {
     if (!h) return fill_error(err, make_status(YTGPU_ERR_INVALID_ARGUMENT, "null context"));
     CtxLock lock(h);
-    return fill_error(err, evaluate_expression_impl(as_context(h), columns, column_count, program, node_count, selection, out_values,
+    return fill_error(err, evaluate_expression_impl(as_context(h), columns, column_count, nullptr, 0, nullptr, 0, nullptr, program, node_count,
+                                                    selection, out_values, out_null_bitmap, out_value_type, out_null_count, out_mem));
+}
+
+int ytgpu_evaluate_expression_strings(ytgpu_context* h, const ytgpu_column_view* columns, uint32_t column_count,
+                                      const ytgpu_string_column* string_columns, uint32_t string_count,
+                                      const uint8_t* string_constants, uint64_t string_constant_bytes, const ytgpu_expr_node* program,
+                                      uint32_t node_count, const uint8_t* selection, uint64_t* out_values, uint8_t* out_null_bitmap,
+                                      uint8_t* out_heap, uint64_t out_heap_capacity, uint64_t* out_starts, uint32_t* out_lengths,
+                                      uint8_t* out_null_bytemap, uint64_t* out_heap_bytes, uint8_t* out_value_type,
+                                      uint64_t* out_null_count, int out_mem, ytgpu_error* err) {
+    if (!h) return fill_error(err, make_status(YTGPU_ERR_INVALID_ARGUMENT, "null context"));
+    CtxLock lock(h);
+    const StringResult sr{out_heap, out_heap_capacity, out_starts, out_lengths, out_null_bytemap, out_heap_bytes};
+    return fill_error(err, evaluate_expression_impl(as_context(h), columns, column_count, string_columns, string_count, string_constants,
+                                                    string_constant_bytes, &sr, program, node_count, selection, out_values,
                                                     out_null_bitmap, out_value_type, out_null_count, out_mem));
 }
 

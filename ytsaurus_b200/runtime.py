@@ -848,17 +848,29 @@ class GpuContext:
             raise e
         return dict(bitmap=bitmap, bytemap=bytemap, rows=rows[:count] if rows is not None else None, count=count)
 
-    def evaluate_expression(self, columns, program, selection=None):
+    def evaluate_expression(self, columns, program, selection=None, string_columns=(), string_constants=b""):
         """Computed column (ytgpu_evaluate_expression) -> dict(values, null_bitmap, null_count, value_type, column).
         columns: Column objects; program: postfix nodes, each a capi.ExprNode or a tuple (op, column, type, constant).
         selection: nullable bitmap in ytgpu_evaluate_filter's layout (its "bitmap" output).  The outputs are in the inputs'
         memory flavour: values n uint64 (int64 on the device), null_bitmap 8 * ceil(n / 64) bytes; `column` is a Column
-        over them (without the bitmap when no row is NULL), ready for scan_filter_groupby_multi / evaluate_filter."""
+        over them (without the bitmap when no row is NULL), ready for scan_filter_groupby_multi / evaluate_filter.
+        string_columns: (heap, starts, lengths, nulls or None) per column, node column len(columns) + i naming string column
+        i; a STRING constant is (offset << 32) | length into string_constants.  With either, or a string op in the program,
+        the call is ytgpu_evaluate_expression_strings, made twice: a type and size query, then the call that fills the outputs
+        of that type, so a STRING result runs its size pass twice (a caller that knows the heap size calls the library once).
+        A STRING result comes back as heap / starts / lengths / null_bytemap (values, null_bitmap and column None), ready
+        for evaluate_filter's string_columns and string_value_ids."""
         views = [c.view() for c in columns]
-        if not views:
+        sarr = (capi.StringColumn * max(len(string_columns), 1))()
+        for i, column in enumerate(string_columns):
+            sarr[i] = _string_column(*column)
+        if views:
+            mem, n = views[0].mem, int(views[0].value_count)
+        elif string_columns:
+            mem, n = sarr[0].mem, int(sarr[0].row_count)
+        else:
             raise ValueError("evaluate_expression needs at least one column")
-        mem, n = views[0].mem, int(views[0].value_count)
-        carr = (capi.ColumnView * len(views))(*views)
+        carr = (capi.ColumnView * max(len(views), 1))(*views)
         nodes = (capi.ExprNode * max(len(program), 1))()
         for i, node in enumerate(program):
             if isinstance(node, capi.ExprNode):
@@ -868,16 +880,48 @@ class GpuContext:
                 nodes[i].op, nodes[i].column, nodes[i].type = op, column, vtype
                 nodes[i].constant = int(constant) & 0xFFFFFFFFFFFFFFFF
         words = (n + 63) // 64
-        values = self._out((n,), np.uint64, mem)
-        null_bitmap = self._out((words * 8,), np.uint8, mem)
         vtype, nulls = C.c_uint8(0), C.c_uint64(0)
         err = capi.Error()
-        capi.check(self.lib.ytgpu_evaluate_expression(self.handle, C.cast(carr, C.c_void_p), len(views), C.cast(nodes, C.c_void_p),
-                                                      len(program), _ptr_mem(selection)[0], _ptr_mem(values)[0],
-                                                      _ptr_mem(null_bitmap)[0], C.byref(vtype), C.byref(nulls), mem, C.byref(err)), err)
-        column = Column(int(vtype.value), values=values, value_count=n,
-                        null_bitmap=null_bitmap if nulls.value else None)
-        return dict(values=values, null_bitmap=null_bitmap, null_count=int(nulls.value), value_type=int(vtype.value), column=column)
+        strings = bool(string_columns) or len(string_constants) > 0 or any(nodes[i].op > capi.EXPR_IF_NULL for i in range(len(program)))
+        if not strings:
+            values = self._out((n,), np.uint64, mem)
+            null_bitmap = self._out((words * 8,), np.uint8, mem)
+            capi.check(self.lib.ytgpu_evaluate_expression(self.handle, C.cast(carr, C.c_void_p), len(views), C.cast(nodes, C.c_void_p),
+                                                          len(program), _ptr_mem(selection)[0], _ptr_mem(values)[0],
+                                                          _ptr_mem(null_bitmap)[0], C.byref(vtype), C.byref(nulls), mem, C.byref(err)), err)
+            column = Column(int(vtype.value), values=values, value_count=n,
+                            null_bitmap=null_bitmap if nulls.value else None)
+            return dict(values=values, null_bitmap=null_bitmap, null_count=int(nulls.value), value_type=int(vtype.value), column=column)
+        sc = np.frombuffer(bytes(string_constants), dtype=np.uint8) if len(string_constants) else np.zeros(0, np.uint8)
+        heap_bytes = C.c_uint64(0)
+
+        def call(values=None, null_bitmap=None, heap=None, capacity=0, starts=None, lengths=None, null_bytemap=None):
+            capi.check(self.lib.ytgpu_evaluate_expression_strings(
+                self.handle, C.cast(carr, C.c_void_p), len(views), C.cast(sarr, C.c_void_p), len(string_columns),
+                sc.ctypes.data if sc.size else None, sc.size, C.cast(nodes, C.c_void_p), len(program), _ptr_mem(selection)[0],
+                _ptr_mem(values)[0], _ptr_mem(null_bitmap)[0], _ptr_mem(heap)[0], capacity, _ptr_mem(starts)[0],
+                _ptr_mem(lengths)[0], _ptr_mem(null_bytemap)[0], C.byref(heap_bytes), C.byref(vtype), C.byref(nulls), mem,
+                C.byref(err)), err)
+        # a type and size query first (no launch for a numeric result, the size pass and scan for a STRING one), then the
+        # call that fills the outputs of that type: a STRING result pays the size pass twice
+        call()
+        if int(vtype.value) != int(EValueType.String):
+            values = self._out((n,), np.uint64, mem)
+            null_bitmap = self._out((words * 8,), np.uint8, mem)
+            if n:
+                call(values, null_bitmap)
+            column = Column(int(vtype.value), values=values, value_count=n,
+                            null_bitmap=null_bitmap if nulls.value else None)
+            return dict(values=values, null_bitmap=null_bitmap, null_count=int(nulls.value), value_type=int(vtype.value), column=column)
+        size = int(heap_bytes.value)
+        heap = self._out((max(size, 1),), np.uint8, mem)
+        starts = self._out((n,), np.uint64, mem)
+        lengths = self._out((n,), np.uint32, mem)
+        null_bytemap = self._out((n,), np.uint8, mem)
+        if n:
+            call(heap=heap, capacity=size, starts=starts, lengths=lengths, null_bytemap=null_bytemap)
+        return dict(values=None, null_bitmap=None, null_count=int(nulls.value), value_type=int(vtype.value), column=None,
+                    heap=heap[:size], starts=starts, lengths=lengths, null_bytemap=null_bytemap)
 
 
 class Column:
