@@ -12,6 +12,9 @@ from CUDA events around the whole call):
   mul_double    price * qty
   cast_div      int64(d * 100.0) / 7
   chain_16      a 16-node chain over a and b: ((((a + b) * 3 - a) ^ 5) + b) & c | a, negated
+  guarded_div   if(b = 0, 0, a / b)            (a division whose zero divisors the IF guards; b has zeros here)
+  if_bucket     if(a < 0, 0, if(a < 5 * 10^8, 1, 2))   (a two-level if)
+  and_signs     (a > 0) AND (b < 0)            (a BOOLEAN result)
 Each leg reports its algorithmic bytes per row — 8 per referenced column read, plus 8 bytes of value and 1/8 byte of null
 bitmap written — and that traffic over the kernel time, against the HBM peak (MEASURED_PEAKS.json's when present, else
 the 3.35 TB/s data-sheet figure of the H100 SXM).
@@ -61,13 +64,15 @@ def main():
 
     a = torch.randint(-10**9, 10**9, (n,), device="cuda", generator=g)
     b = torch.randint(-10**9, 10**9, (n,), device="cuda", generator=g)
+    bz = torch.where(b % 16 == 0, torch.zeros_like(b), b)  # b with zero divisors in 1/16 of the rows
     price = torch.rand(n, device="cuda", generator=g, dtype=torch.float64) * 100
     qty = torch.rand(n, device="cuda", generator=g, dtype=torch.float64) * 10
     d = torch.randn(n, device="cuda", generator=g, dtype=torch.float64)
     cols = [Column(T.Int64, values=a), Column(T.Int64, values=b), Column(T.Double, values=price.view(torch.int64)),
-            Column(T.Double, values=qty.view(torch.int64)), Column(T.Double, values=d.view(torch.int64))]
-    A, B, PRICE, QTY, D = range(5)
+            Column(T.Double, values=qty.view(torch.int64)), Column(T.Double, values=d.view(torch.int64)), Column(T.Int64, values=bz)]
+    A, B, PRICE, QTY, D, BZ = range(6)
     col, const, cast = capi.EXPR_COLUMN, capi.EXPR_CONSTANT, capi.EXPR_CAST
+    cmp, iff = capi.EXPR_COMPARE, capi.EXPR_IF
     i64, f64 = int(T.Int64), int(T.Double)
 
     def dbl(x):
@@ -84,6 +89,12 @@ def main():
         "cast_div": ([(col, D), (const, 0, f64, dbl(100.0)), (capi.EXPR_MUL,), (cast, 0, i64), (const, 0, i64, 7), (capi.EXPR_DIV,)],
                      8 + written),
         "chain_16": (chain, 16 + written),
+        "guarded_div": ([(col, BZ), (const, 0, i64, 0), (cmp, capi.CMP_EQ), (const, 0, i64, 0), (col, A), (col, BZ), (capi.EXPR_DIV,),
+                         (iff,)], 16 + written),
+        "if_bucket": ([(col, A), (const, 0, i64, 0), (cmp, capi.CMP_LT), (const, 0, i64, 0), (col, A), (const, 0, i64, 5 * 10**8),
+                       (cmp, capi.CMP_LT), (const, 0, i64, 1), (const, 0, i64, 2), (iff,), (iff,)], 8 + written),
+        "and_signs": ([(col, A), (const, 0, i64, 0), (cmp, capi.CMP_GT), (col, B), (const, 0, i64, 0), (cmp, capi.CMP_LT), (capi.EXPR_AND,)],
+                      16 + written),
     }
     ctx.enable_timers(True)
     results = {}
@@ -112,7 +123,13 @@ def main():
     # parity of two legs with torch
     line["add"]["matches_torch"] = bool(torch.equal(results["add"]["values"], a + b))
     line["mod_1000"]["matches_torch"] = bool(torch.equal(results["mod_1000"]["values"], torch.fmod(a, 1000)))
-    del results, price, qty, d
+    safe = torch.where(bz == 0, torch.ones_like(bz), bz)
+    line["guarded_div"]["matches_torch"] = bool(torch.equal(results["guarded_div"]["values"],
+                                                            torch.where(bz == 0, torch.zeros_like(a), torch.div(a, safe, rounding_mode="trunc"))))
+    line["if_bucket"]["matches_torch"] = bool(torch.equal(results["if_bucket"]["values"],
+                                                          torch.where(a < 0, 0, torch.where(a < 5 * 10**8, 1, 2))))
+    line["and_signs"]["matches_torch"] = bool(torch.equal(results["and_signs"]["values"], ((a > 0) & (b < 0)).to(torch.int64)))
+    del results, price, qty, d, bz, safe
 
     # GROUP BY over (a % 1000, k): the computed key against the same key precomputed
     k = torch.randint(0, 8, (n,), device="cuda", generator=g)

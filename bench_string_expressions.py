@@ -13,9 +13,12 @@ call with a heap sized beforehand, so a size pass, a three-kernel scan and a fil
   if_null_url           if_null(url, '') with 5 % of the rows NULL
   farm_hash_url         farm_hash(url)
   farm_hash_a_url_mod   farm_hash(a, url) % 64
+  if_a_url_other        if(a > 0, url, 'other')          (a STRING IF: about half the rows keep url's piece)
+  url_lt_site5          url < 'https://www.site5'        (a STRING COMPARE, BOOLEAN result)
 Algorithmic bytes per row: a string input reads its 8-byte start, 4-byte length and its bytes (+1 null byte when it has
 NULLs), a numeric one 8 bytes; a STRING result writes its bytes, an 8-byte start, a 4-byte length and a null byte, a
-numeric one 8 bytes and 1/8 byte of null bitmap.  That traffic over the kernel time is set against the HBM peak
+numeric one 8 bytes and 1/8 byte of null bitmap; a COMPARE against a constant of c bytes reads at most c + 1 bytes of a
+value.  That traffic over the kernel time is set against the HBM peak
 (MEASURED_PEAKS.json's when present, else the 3.35 TB/s data-sheet figure of the H100 SXM).
 GROUP BY leg: COUNT and SUM of a grouped by lower(host), once computed (lower as one call into outputs allocated once, as
 the string legs, then string_value_ids and the GROUP BY) and once over the host names lowered beforehand; both results must
@@ -78,8 +81,8 @@ def main():
     url = _string_column(heap, starts, lengths)
     url_nulls = _string_column(heap, starts, lengths, nulls)
     acol = Column(T.Int64, values=a)
-    col, const, STR, U64 = capi.EXPR_COLUMN, capi.EXPR_CONSTANT, int(T.String), int(T.Uint64)
-    consts = np.frombuffer(b"/x", np.uint8).copy()
+    col, const, STR, U64, I64 = capi.EXPR_COLUMN, capi.EXPR_CONSTANT, int(T.String), int(T.Uint64), int(T.Int64)
+    consts = np.frombuffer(b"/xotherhttps://www.site5", np.uint8).copy()  # "/x" at 0, "other" at 2, the URL bound at 7
 
     out_heap = torch.empty(int(heap.numel()) + 2 * n, dtype=torch.uint8, device="cuda")
     out_starts = torch.empty(n, dtype=torch.int64, device="cuda")
@@ -115,6 +118,10 @@ def main():
         "farm_hash_url": ([(col, 0), (capi.EXPR_FARM_HASH, 1)], [url], (), string_in + numeric_out),
         "farm_hash_a_url_mod": ([(col, 0), (col, 1), (capi.EXPR_FARM_HASH, 2), (const, 0, U64, 64), (capi.EXPR_MOD,)], [url], [acol],
                                 8 + string_in + numeric_out),
+        "if_a_url_other": ([(col, 0), (const, 0, I64, 0), (capi.EXPR_COMPARE, capi.CMP_GT), (col, 1), (const, 0, STR, (2 << 32) | 5),
+                            (capi.EXPR_IF,)], [url], [acol], 8 + 12 + 0.5 * mean_len + (0.5 * mean_len + 0.5 * 5 + 13)),
+        "url_lt_site5": ([(col, 0), (const, 0, STR, (7 << 32) | 17), (capi.EXPR_COMPARE, capi.CMP_LT)], [url], (),
+                         12 + 18 + numeric_out),
     }
     ctx.enable_timers(True)
     for leg_name, (prog, scols, numeric, bytes_per_row) in legs.items():

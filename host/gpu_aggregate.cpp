@@ -447,18 +447,21 @@ public:
         // The result type of computed column j, from its program and its inputs' types, by the typing rules of
         // check_expression (csrc/expression.cu): the value / string split below needs it before the column is evaluated.
         // An input column without a non-NULL value has no type: it is a STRING where the program reads it as one (an
-        // operand of CONCAT, LOWER, UPPER or of IF_NULL with a STRING; *stringLeaves marks it, and it is passed as an
-        // all-NULL string column), INT64 everywhere else, as view() passes it.  A malformed program types as INT64 and is
-        // refused by the call.
-        auto typeComputed = [&](size_t j, std::vector<uint8_t>* stringLeaves) {
+        // operand of CONCAT, LOWER, UPPER, of IF_NULL or COMPARE with a STRING, or an IF branch beside one; it is passed as
+        // an all-NULL string column), a BOOLEAN under AND / OR / NOT or as IF's condition, the other operand's type in a
+        // COMPARE or beside an IF branch, INT64 everywhere else, as view() passes it.  (*leafTypes)[leaf] records the type
+        // it is read as (Null: INT64).  A malformed program types as INT64 and is refused by the call.
+        auto typeComputed = [&](size_t j, std::vector<EValueType>* leafTypes) {
             struct TEntry {
                 EValueType Type;
                 std::vector<int> NullLeaves;  // untyped input columns the entry may be
             };
-            auto asString = [&](TEntry& e) {
-                for (int leaf : e.NullLeaves) (*stringLeaves)[leaf] = 1;
-                e = {EValueType::String, {}};
+            auto asType = [&](TEntry& e, EValueType type) {
+                if (e.Type != EValueType::Null || type == EValueType::Null) return;
+                for (int leaf : e.NullLeaves) (*leafTypes)[leaf] = type;
+                e = {type, {}};
             };
+            auto asString = [&](TEntry& e) { asType(e, EValueType::String); };
             auto asNumber = [](TEntry& e) {
                 if (e.Type == EValueType::Null) e.Type = EValueType::Int64;
                 e.NullLeaves.clear();
@@ -468,8 +471,10 @@ public:
                 const TExpressionNode& node = query.Computed[j].Nodes[k];
                 const size_t need = node.Op == EExpressionOp::Column || node.Op == EExpressionOp::Constant ? 0
                                   : node.Op == EExpressionOp::FarmHash ? (size_t)std::max(node.Column, 1)
+                                  : node.Op == EExpressionOp::If ? 3
                                   : (node.Op == EExpressionOp::Neg || node.Op == EExpressionOp::BitNot || node.Op == EExpressionOp::Cast ||
-                                     node.Op == EExpressionOp::Lower || node.Op == EExpressionOp::Upper) ? 1 : 2;
+                                     node.Op == EExpressionOp::Lower || node.Op == EExpressionOp::Upper || node.Op == EExpressionOp::Not ||
+                                     node.Op == EExpressionOp::IsNull || node.Op == EExpressionOp::IsNotNull) ? 1 : 2;
                 if (st.size() < need) return EValueType::Int64;
                 switch (node.Op) {
                     case EExpressionOp::Column: {
@@ -493,6 +498,38 @@ public:
                         st.resize(st.size() - need);
                         st.push_back({EValueType::Uint64, {}});
                         break;
+                    case EExpressionOp::Not:
+                        asType(st.back(), EValueType::Boolean);
+                        break;
+                    case EExpressionOp::IsNull: case EExpressionOp::IsNotNull:  // NULL whichever type it is read as
+                        st.back() = {EValueType::Boolean, {}};
+                        break;
+                    case EExpressionOp::Compare: case EExpressionOp::And: case EExpressionOp::Or: {
+                        TEntry b = std::move(st.back());
+                        st.pop_back();
+                        TEntry& a = st.back();
+                        if (node.Op != EExpressionOp::Compare) {
+                            asType(a, EValueType::Boolean);
+                            asType(b, EValueType::Boolean);
+                        } else {
+                            asType(a, b.Type);
+                            asType(b, a.Type);
+                        }
+                        a = {EValueType::Boolean, {}};
+                        break;
+                    }
+                    case EExpressionOp::If: {
+                        TEntry b = std::move(st.back());
+                        st.pop_back();
+                        TEntry a = std::move(st.back());
+                        st.pop_back();
+                        asType(st.back(), EValueType::Boolean);
+                        asType(a, b.Type);
+                        asType(b, a.Type);
+                        a.NullLeaves.insert(a.NullLeaves.end(), b.NullLeaves.begin(), b.NullLeaves.end());  // both untyped
+                        st.back() = std::move(a);
+                        break;
+                    }
                     default: {  // binary ops, IfNull, Concat: operands of one type
                         TEntry b = std::move(st.back());
                         st.pop_back();
@@ -517,8 +554,8 @@ public:
         };
         for (size_t i = 0; i < columns.size(); ++i) {
             if (!isComputed((int)i)) continue;
-            std::vector<uint8_t> stringLeaves(columns.size(), 0);
-            columns[i].Type = typeComputed((size_t)(-2 - columns[i].Position), &stringLeaves);
+            std::vector<EValueType> leafTypes(columns.size(), EValueType::Null);
+            columns[i].Type = typeComputed((size_t)(-2 - columns[i].Position), &leafTypes);
         }
         if (whereIndex >= 0 && columns[whereIndex].Type == EValueType::String)
             throw TErrorException(YTGPU_ERR_UNSUPPORTED, "the WHERE column (position " + std::to_string(query.WhereColumn) +
@@ -529,6 +566,56 @@ public:
                 throw TErrorException(YTGPU_ERR_UNSUPPORTED, "sum / avg of a string column");
         }
         std::vector<TUnversionedOwningRow> owned;
+        // a program over output positions; the string functions are not taken there
+        auto outputProgram = [&](const TExpression& e, const std::string& what) {
+            std::vector<ytgpu_expr_node> program;
+            for (const auto& node : e.Nodes) {
+                if (node.Op == EExpressionOp::Concat || node.Op == EExpressionOp::Lower || node.Op == EExpressionOp::Upper ||
+                    node.Op == EExpressionOp::FarmHash)
+                    throw TErrorException(YTGPU_ERR_UNSUPPORTED, what + ": string functions over the output row");
+                ytgpu_expr_node x{};
+                x.op = (int32_t)node.Op;
+                x.column = node.Column;
+                x.type = (uint8_t)node.Type;
+                x.constant = node.Bits;
+                program.push_back(x);
+            }
+            return program;
+        };
+        // Having over the output row's views (`groups` rows each) -> its TRUE rows as a selection bitmap in the layout of
+        // ytgpu_evaluate_filter's out_bitmap (ceil(groups / 64) words).  With no groups the call only checks the program:
+        // a Having that is not a Boolean, or reads a string position, is refused whatever the data.
+        auto evaluateHaving = [&](const std::vector<ytgpu_column_view>& views, uint64_t groups) {
+            const auto program = outputProgram(*query.Having, "having");
+            std::vector<uint64_t> values(groups), nulls((groups + 63) / 64), kept((groups + 63) / 64, 0);
+            uint8_t type = 0;
+            ytgpu_error herr{};
+            if (ytgpu_evaluate_expression(GetGpuContext(), views.data(), (uint32_t)views.size(), program.data(), (uint32_t)program.size(),
+                                          nullptr, values.data(), reinterpret_cast<uint8_t*>(nulls.data()), &type, nullptr, YTGPU_MEM_HOST,
+                                          &herr) != YTGPU_OK)
+                ThrowFrom(herr);
+            if (type != (uint8_t)EValueType::Boolean)
+                throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "having: the expression is not a Boolean");
+            for (uint64_t g = 0; g < groups; ++g)
+                if (values[g] == 1 && !((nulls[g >> 6] >> (g & 63)) & 1)) kept[g >> 6] |= 1ull << (g & 63);
+            return kept;
+        };
+        if (n == 0 && query.Having) {  // no rows, no groups: the output row's types from the columns' (NULL: INT64)
+            std::vector<ytgpu_column_view> views;
+            auto add = [&](EValueType type) {
+                ytgpu_column_view v{};
+                v.value_type = (uint8_t)(type == EValueType::Null ? EValueType::Int64 : type);
+                v.bit_width = 64;
+                v.mem = YTGPU_MEM_HOST;
+                views.push_back(v);
+            };
+            for (int k : keyIndex) add(columns[k].Type);
+            for (size_t a = 0; a < query.AggregateItems.size(); ++a) {
+                const auto f = query.AggregateItems[a].Function;
+                add(f == EAggregateFunction::Count ? EValueType::Int64 : f == EAggregateFunction::Avg ? EValueType::Double : columns[aggIndex[a]].Type);
+            }
+            evaluateHaving(views, 0);
+        }
         if (n > 0) {
             auto view = [&](const TFlatColumn& c) {
                 ytgpu_column_view v{};
@@ -556,22 +643,22 @@ public:
                 std::vector<int> slot(columns.size(), -1);  // scalar: slot; string: -1 - string slot
                 std::vector<int> leafOf;
                 std::vector<ytgpu_expr_node> program;
-                std::vector<uint8_t> stringLeaves(columns.size(), 0);  // untyped input columns read as strings
-                typeComputed(j, &stringLeaves);
+                std::vector<EValueType> leafTypes(columns.size(), EValueType::Null);  // the types untyped input columns are read as
+                typeComputed(j, &leafTypes);
                 for (size_t k = 0; k < query.Computed[j].Nodes.size(); ++k) {
                     const TExpressionNode& node = query.Computed[j].Nodes[k];
                     ytgpu_expr_node x{};
                     x.op = (int32_t)node.Op;
                     x.type = (uint8_t)node.Type;
                     x.constant = node.Bits;
-                    if (node.Op == EExpressionOp::FarmHash) x.column = node.Column;
+                    if (node.Op == EExpressionOp::FarmHash || node.Op == EExpressionOp::Compare) x.column = node.Column;
                     if (node.Op == EExpressionOp::Constant && node.Type == EValueType::String) {
                         x.constant = ((uint64_t)constants.size() << 32) | node.Bytes.size();
                         constants += node.Bytes;
                     }
                     const int leaf = leafIndex[j][k];
                     if (leaf >= 0 && slot[leaf] == -1) {
-                        if (columns[leaf].Type == EValueType::String || stringLeaves[leaf]) {  // all-NULL: an empty heap
+                        if (columns[leaf].Type == EValueType::String || leafTypes[leaf] == EValueType::String) {  // all-NULL: an empty heap
                             columns[leaf].Starts.resize(n, 0);
                             columns[leaf].Lengths.resize(n, 0);
                             slot[leaf] = -2 - (int)stringInputs.size();
@@ -579,6 +666,8 @@ public:
                         } else {
                             slot[leaf] = (int)inputs.size();
                             inputs.push_back(view(columns[leaf]));
+                            if (columns[leaf].Type == EValueType::Null && leafTypes[leaf] != EValueType::Null)
+                                inputs.back().value_type = (uint8_t)leafTypes[leaf];  // all-NULL, read as the program reads it
                         }
                     }
                     leafOf.push_back(leaf);
@@ -828,13 +917,14 @@ public:
                     outputs.push_back({type, f == EAggregateFunction::Count ? nullptr : stringsOf(aggIndex[a]), values[a].data(), valueNull[a].data()});
                 }
                 const uint64_t groups = res.group_count;
-                // Select: a bare Column passes its position through; every other item is one ytgpu_evaluate_expression call over
-                // the result arrays (a string position is refused by the call as UNSUPPORTED)
+                // Select: a bare Column passes its position through; every other item, and Having, is one
+                // ytgpu_evaluate_expression call over the result arrays (a string position is refused by the call as UNSUPPORTED)
                 std::vector<std::vector<uint64_t>> selectValues, selectNulls;  // selectNulls: null bitmaps
                 std::vector<TOutput> selected;
-                if (query.Select) {
-                    std::vector<std::vector<uint8_t>> bitmaps(outputs.size());
-                    std::vector<ytgpu_column_view> outViews;
+                std::vector<uint64_t> having;  // Having: bit g set where group g is written
+                std::vector<std::vector<uint8_t>> bitmaps(outputs.size());
+                std::vector<ytgpu_column_view> outViews;
+                if (query.Select || query.Having) {
                     for (size_t p = 0; p < outputs.size(); ++p) {
                         bitmaps[p].assign((groups + 63) / 64 * 8, 0);
                         for (uint64_t g = 0; g < groups; ++g)
@@ -851,6 +941,12 @@ public:
                         v.mem = YTGPU_MEM_HOST;
                         outViews.push_back(v);
                     }
+                }
+                if (query.Having) having = evaluateHaving(outViews, groups);
+                // Select is evaluated over the groups Having keeps only, as QL projects after HAVING: a division by zero in a
+                // dropped group does not throw
+                const uint8_t* selectSelection = query.Having ? reinterpret_cast<const uint8_t*>(having.data()) : nullptr;
+                if (query.Select) {
                     selectValues.resize(query.Select->size());
                     selectNulls.resize(query.Select->size());
                     for (size_t s = 0; s < query.Select->size(); ++s) {
@@ -862,23 +958,13 @@ public:
                             selected.push_back(outputs[nodes[0].Column]);
                             continue;
                         }
-                        std::vector<ytgpu_expr_node> program;
-                        for (const auto& node : nodes) {
-                            if ((int)node.Op > (int)EExpressionOp::IfNull)
-                                throw TErrorException(YTGPU_ERR_UNSUPPORTED, "select item " + std::to_string(s) + ": string functions in the select list");
-                            ytgpu_expr_node x{};
-                            x.op = (int32_t)node.Op;
-                            x.column = node.Column;
-                            x.type = (uint8_t)node.Type;
-                            x.constant = node.Bits;
-                            program.push_back(x);
-                        }
+                        const auto program = outputProgram((*query.Select)[s], "select item " + std::to_string(s));
                         selectValues[s].assign(groups, 0);
                         selectNulls[s].assign((groups + 63) / 64, 0);
                         uint8_t type = 0;
                         ytgpu_error serr{};
                         if (ytgpu_evaluate_expression(GetGpuContext(), outViews.data(), (uint32_t)outViews.size(), program.data(),
-                                                      (uint32_t)program.size(), nullptr, selectValues[s].data(),
+                                                      (uint32_t)program.size(), selectSelection, selectValues[s].data(),
                                                       reinterpret_cast<uint8_t*>(selectNulls[s].data()), &type, nullptr, YTGPU_MEM_HOST,
                                                       &serr) != YTGPU_OK)
                             ThrowFrom(serr);
@@ -887,6 +973,7 @@ public:
                 }
                 owned.reserve(groups);
                 for (uint64_t g = 0; g < groups; ++g) {  // already in first-seen order
+                    if (query.Having && !((having[g >> 6] >> (g & 63)) & 1)) continue;
                     TUnversionedOwningRowBuilder b;
                     if (query.Select) {
                         for (size_t s = 0; s < selected.size(); ++s) {

@@ -176,18 +176,20 @@ struct TFilterExpression {
     TFilterExpression& Not() { Nodes.push_back({EFilterOp::Not, EBinaryOp::None, -1, -1, {}, {}}); return *this; }
 };
 
-//! An arithmetic, bitwise, cast, if_null, concat, lower, upper or farm_hash expression, evaluated on the GPU into a computed
-//! column (ytgpu_evaluate_expression_strings: the semantics — NULLs, wrap-around, division errors, casts, ASCII case
-//! mapping, the fingerprint — are in include/ytgpu.h).  Nodes are in postfix order; a Column leaf names a position (in the
+//! An arithmetic, bitwise, cast, if_null, concat, lower, upper, farm_hash or conditional (comparison, and / or / not,
+//! is_null, if) expression, evaluated on the GPU into a computed column (ytgpu_evaluate_expression_strings: the semantics —
+//! NULLs, wrap-around, division errors and the branches they follow, casts, ASCII case mapping, the fingerprint — are in
+//! include/ytgpu.h).  Nodes are in postfix order; a Column leaf names a position (in the
 //! input rows for TMultiGroupQuery::Computed, in the output row for Select).  Binary operands have one type: there is no
 //! implicit widening, write Cast.  Select takes no string ops.
 enum class EExpressionOp {
     Column = 1, Constant = 2, Add = 3, Sub = 4, Mul = 5, Div = 6, Mod = 7, Neg = 8, BitAnd = 9, BitOr = 10, BitXor = 11, BitNot = 12,
-    Cast = 13, IfNull = 14, Concat = 15, Lower = 16, Upper = 17, FarmHash = 18
+    Cast = 13, IfNull = 14, Concat = 15, Lower = 16, Upper = 17, FarmHash = 18,
+    Compare = 19, And = 20, Or = 21, Not = 22, IsNull = 23, IsNotNull = 24, If = 25
 };
 struct TExpressionNode {
     EExpressionOp Op = EExpressionOp::Column;
-    int Column = -1;                      // Column; FarmHash: the operand count
+    int Column = -1;                      // Column; FarmHash: the operand count; Compare: the EBinaryOp
     EValueType Type = EValueType::Null;   // Constant: its type; Cast: the target type
     uint64_t Bits = 0;                    // Constant: Int64 / Uint64 / Double bit pattern, Boolean 0 / 1
     std::string Bytes = {};               // Constant: a String's bytes
@@ -221,6 +223,18 @@ struct TExpression {
     TExpression& Upper() { return Op(EExpressionOp::Upper); }
     //! farm_hash of the last `count` (1..16) values, of any type: a Uint64, never NULL.
     TExpression& FarmHash(int count) { Nodes.push_back({EExpressionOp::FarmHash, count, EValueType::Null, 0}); return *this; }
+    //! a <cmp> b over two values of one type (strings included): a Boolean, NULL if either is NULL.  EBinaryOp Less .. NotEqual
+    //! are ytgpu_cmp_op LT .. NE.
+    TExpression& Compare(EBinaryOp cmp) { Nodes.push_back({EExpressionOp::Compare, (int)cmp, EValueType::Null, 0}); return *this; }
+    //! Kleene and / or / not over Booleans; is_null / is_not_null of any value (never NULL).
+    TExpression& And() { return Op(EExpressionOp::And); }
+    TExpression& Or() { return Op(EExpressionOp::Or); }
+    TExpression& Not() { return Op(EExpressionOp::Not); }
+    TExpression& IsNull() { return Op(EExpressionOp::IsNull); }
+    TExpression& IsNotNull() { return Op(EExpressionOp::IsNotNull); }
+    //! if(c, a, b) over the last three values: a where c is true, b where it is false, NULL where c is NULL.  A division or
+    //! case-mapping error in the branch not taken does not throw.
+    TExpression& If() { return Op(EExpressionOp::If); }
 
 private:
     TExpression& Op(EExpressionOp op) { Nodes.push_back({op, -1, EValueType::Null, 0}); return *this; }
@@ -242,6 +256,11 @@ struct TMultiGroupQuery {
     //! The output row: expressions over its positions (group items first, then aggregates), e.g. sum(b) + x.  Without it
     //! the output row is the group items followed by the aggregates.
     std::optional<std::vector<TExpression>> Select;
+    //! HAVING: a Boolean expression over the output row's positions, as Select's (e.g. sum(x) > 100).  Only the groups where
+    //! it is true are written, and RowsWritten counts them.  Select is evaluated over those groups only (its selection), so a
+    //! division by zero in a dropped group does not throw.  The program is checked whatever the data: a Having that is not
+    //! a Boolean throws on an empty input too.  Without it every group is written.
+    std::optional<TExpression> Having;
 };
 
 struct TQueryStatistics {
@@ -263,8 +282,8 @@ struct IEvaluator {
     //! Computed columns are evaluated with ytgpu_evaluate_expression_strings, nothing on the host, in QL's order: first those the
     //! WHERE reads, over all rows; then the WHERE, once, as a filter pass (with computed columns the WhereOp form runs as a
     //! one-node COMPARE program, which selects the same rows); then the other computed columns over the selected rows only,
-    //! so a division by zero in a row the WHERE drops does not throw.  Select items are evaluated the same way over the
-    //! result rows; a bare Column of a string result passes through, arithmetic on it throws YTGPU_ERR_UNSUPPORTED, as does
+    //! so a division by zero in a row the WHERE drops does not throw.  Select items and Having are evaluated the same way over
+    //! the result rows; a bare Column of a string result passes through, arithmetic on it throws YTGPU_ERR_UNSUPPORTED, as does
     //! a numeric op over a string input column.  A computed column may yield a string (concat, lower, upper, if_null): it is
     //! a string column to every consumer (group item, string aggregate argument, WHERE leaf); lower / upper of a non-ASCII
     //! value throws YTGPU_ERR_UNSUPPORTED.  Errors of the calls (a division by zero, a mistyped expression:

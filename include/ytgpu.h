@@ -700,7 +700,7 @@ int ytgpu_evaluate_filter(ytgpu_context* ctx, const ytgpu_column_view* columns, 
                           uint8_t* out_bitmap, uint8_t* out_bytemap, uint32_t* out_rows, uint64_t rows_capacity,
                           uint64_t* out_selected /* host */, int out_mem, ytgpu_error* err);
 
-/* ---- computed columns: arithmetic, bitwise, cast and if_null expressions ----
+/* ---- computed columns: arithmetic, bitwise, cast, if_null and conditional expressions ----
  * The projections of YT QL's expression compiler (cg_fragment_compiler.cpp) that a GROUP BY key (`group by a % 2`), an
  * aggregate argument (`sum(price * qty)`) or a WHERE leaf (`a + b > 10`) may hold.  An expression is a PROGRAM of nodes in
  * POSTFIX order, evaluated row by row into a computed column.  The program is typed: the type of every node follows from the
@@ -736,6 +736,31 @@ int ytgpu_evaluate_filter(ytgpu_context* ctx, const ytgpu_column_view* columns, 
  * These rules were not checked against YT QL's own evaluator; in particular the two division-error messages and the
  * INT64_MIN / -1 check are recalled from cg_fragment_compiler.cpp, not read there.
  *
+ * Conditional expressions (`sum(if(status = 200, 1, 0))`, `sum(if(b = 0, 0, a / b))`, `group by if(latency > 1000, 'slow',
+ * 'fast')`, `group by lower(host) = 'example.com'`), taken by both entry points; STRING operands by
+ * ytgpu_evaluate_expression_strings only:
+ *   COMPARE(cmp)             two operands of one type, any of the four or STRING, -> BOOLEAN; `column` holds the
+ *                            ytgpu_cmp_op LT .. NE.  No implicit widening: the caller casts.  The comparison is the filter's
+ *                            COMPARE rule: INT64 signed, UINT64 unsigned, DOUBLE by IEEE (a NaN operand makes every op false
+ *                            except NE; -0.0 == +0.0), BOOLEAN 0 < 1, STRING as unsigned bytes, then the shorter value
+ *                            first.  NULL if either operand is NULL (the filter's SQL rule).  A STRING operand may be any
+ *                            string result (lower(x), concat(a, b), ...): the bytes are compared as they would be written.
+ *   AND, OR                  two BOOLEANs -> BOOLEAN, Kleene logic as the filter: F AND x = F, T OR x = T, otherwise a NULL
+ *                            operand makes the result NULL.
+ *   NOT                      one BOOLEAN -> BOOLEAN; NOT NULL is NULL.
+ *   IS_NULL, IS_NOT_NULL     one operand of any type, STRING included -> BOOLEAN, never NULL.
+ *   IF                       postfix `c a b IF`: c a BOOLEAN, a and b of one type (STRING included) -> that type: a where c
+ *                            is TRUE, b where it is FALSE, NULL where c is NULL.  That a NULL condition gives NULL is
+ *                            recalled from QL's TIfFunctionCodegen (builtin_function_profiler.cpp), not read there.
+ * Errors follow the data.  Each stack entry carries the errors its value met (a division error; in
+ * ytgpu_evaluate_expression_strings also a non-ASCII LOWER / UPPER operand); every op passes on the union of its operands'
+ * errors, and only the errors of the program's result fail the call.  The exceptions: IF keeps c's errors and those of the
+ * branch it takes (c's alone when c is NULL); AND whose left operand is FALSE and OR whose left operand is TRUE drop the
+ * right operand's errors.  So `if(b = 0, 0, a / b)` never fails, `if(b = 0, a / b, 0)` fails where b = 0, `FALSE AND (a /
+ * 0 > 1)` never fails and `NULL AND (a / 0 > 1)` does.  A program without IF, AND or OR fails on exactly the rows where
+ * any of its divisions (or case maps) fails, as it always has.  A string value outside its heap is an input error and
+ * fails the call wherever it is read.
+ *
  * selection (nullable, out_mem): a bitmap in the layout of ytgpu_evaluate_filter's out_bitmap.  A row whose bit is clear is
  * not evaluated: its result is NULL and it raises no division error (QL evaluates projections after WHERE, so a division by
  * zero in a row the WHERE drops must not fail the query).
@@ -759,7 +784,10 @@ typedef enum ytgpu_expr_op {
     YTGPU_EXPR_BIT_AND = 9, YTGPU_EXPR_BIT_OR = 10, YTGPU_EXPR_BIT_XOR = 11, YTGPU_EXPR_BIT_NOT = 12,
     YTGPU_EXPR_CAST = 13, YTGPU_EXPR_IF_NULL = 14,
     /* ytgpu_evaluate_expression_strings only */
-    YTGPU_EXPR_CONCAT = 15, YTGPU_EXPR_LOWER = 16, YTGPU_EXPR_UPPER = 17, YTGPU_EXPR_FARM_HASH = 18
+    YTGPU_EXPR_CONCAT = 15, YTGPU_EXPR_LOWER = 16, YTGPU_EXPR_UPPER = 17, YTGPU_EXPR_FARM_HASH = 18,
+    /* conditional expressions, both entry points (see below) */
+    YTGPU_EXPR_COMPARE = 19, YTGPU_EXPR_AND = 20, YTGPU_EXPR_OR = 21, YTGPU_EXPR_NOT = 22, YTGPU_EXPR_IS_NULL = 23,
+    YTGPU_EXPR_IS_NOT_NULL = 24, YTGPU_EXPR_IF = 25
 } ytgpu_expr_op;
 
 #define YTGPU_EXPR_MAX_NODES 64
@@ -770,7 +798,8 @@ typedef enum ytgpu_expr_op {
 
 typedef struct ytgpu_expr_node {
     int32_t op;          /* ytgpu_expr_op */
-    int32_t column;      /* COLUMN: index into columns (++ string_columns); FARM_HASH: its operand count */
+    int32_t column;      /* COLUMN: index into columns (++ string_columns); FARM_HASH: its operand count;
+                            COMPARE: the ytgpu_cmp_op */
     uint8_t type;        /* CONSTANT: its value type; CAST: the target type (YTGPU_TYPE_*) */
     uint8_t reserved[7];
     uint64_t constant;   /* CONSTANT: the bit pattern in `type`; a STRING one: (offset << 32) | length into string_constants */
@@ -806,10 +835,12 @@ int ytgpu_evaluate_expression(ytgpu_context* ctx, const ytgpu_column_view* colum
  *                            arguments is recalled from its UDF, not read.  A STRING operand must be a leaf, a constant or
  *                            IF_NULL of those; a CONCAT, LOWER or UPPER result under FARM_HASH is YTGPU_ERR_UNSUPPORTED.
  * NULL: a NULL operand makes CONCAT, LOWER and UPPER NULL; IF_NULL and FARM_HASH as above.  The numeric ops are those of
- * ytgpu_evaluate_expression, and they do not take strings (YTGPU_ERR_UNSUPPORTED).  There are no comparisons, no substr.
+ * ytgpu_evaluate_expression, and they do not take strings (YTGPU_ERR_UNSUPPORTED).  The conditional ops above take
+ * STRING operands here.  There is no substr.
  * Limits: those of ytgpu_evaluate_expression; at most YTGPU_EXPR_MAX_PIECES (16) string pieces on the stack at any node,
- * where a leaf or constant is one piece, CONCAT adds its operands' pieces and IF_NULL takes the larger count (so a program
- * concatenates at most 16 values); at most 1 MiB of string_constants; a result value of at most 2^32 - 1 bytes.
+ * where a leaf or constant is one piece, CONCAT adds its operands' pieces, IF_NULL and IF take the larger count and
+ * COMPARE, IS_NULL and IS_NOT_NULL leave none (so a program concatenates at most 16 values); at most 1 MiB of
+ * string_constants; a result value of at most 2^32 - 1 bytes.
  * selection: as ytgpu_evaluate_expression; an unselected row is NULL and not evaluated, so a non-ASCII value or a value
  * outside its heap there does not fail the call.
  * Outputs, in out_mem:

@@ -170,6 +170,8 @@ class FilterNode(C.Structure):
 
 (EXPR_COLUMN, EXPR_CONSTANT, EXPR_ADD, EXPR_SUB, EXPR_MUL, EXPR_DIV, EXPR_MOD, EXPR_NEG, EXPR_BIT_AND, EXPR_BIT_OR, EXPR_BIT_XOR,
  EXPR_BIT_NOT, EXPR_CAST, EXPR_IF_NULL, EXPR_CONCAT, EXPR_LOWER, EXPR_UPPER, EXPR_FARM_HASH) = range(1, 19)
+(EXPR_COMPARE, EXPR_AND, EXPR_OR, EXPR_NOT, EXPR_IS_NULL, EXPR_IS_NOT_NULL, EXPR_IF) = range(19, 26)
+EXPR_STRING_OPS = (EXPR_CONCAT, EXPR_LOWER, EXPR_UPPER, EXPR_FARM_HASH)  # ytgpu_evaluate_expression_strings only
 EXPR_MAX_NODES, EXPR_MAX_DEPTH = 64, 16
 EXPR_MAX_PIECES, EXPR_MAX_HASH_OPERANDS, EXPR_MAX_STRING_CONSTANT_BYTES = 16, 16, 1 << 20
 

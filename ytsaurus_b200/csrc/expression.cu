@@ -14,7 +14,7 @@
 //   * a 32-row group without a selected row skips the program;
 //   * the NULL count and the division-error bits are reduced per warp, one atomic each.
 //
-// String expressions (ytgpu_evaluate_expression_strings) run the instantiation expression_kernel<true>.  A STRING stack
+// String expressions (ytgpu_evaluate_expression_strings) run the instantiation expression_kernel<true, true>.  A STRING stack
 // entry is a list of pieces (pointer, length, case map): a leaf makes one piece, CONCAT appends the lists, LOWER / UPPER
 // set the case map of every piece (on ASCII lower(upper(x)) = lower(x), so the outermost wins) and IF_NULL keeps one of
 // them.  The pieces form a second stack in shared memory, [piece][threadIdx.x] (pointer u64, length u32); the value
@@ -28,8 +28,16 @@
 //      string_to_ch.cu's copy: a warp whose 32 values are short assembles them in shared memory and writes the stretch
 //      with 16-byte stores; a long value is copied by the whole warp, 4 bytes per lane when aligned.
 // FARM_HASH hashes its operands with farmhash.cuh's value and row combiners; a string operand is one piece.
+//
+// Conditional ops (COMPARE, AND, OR, NOT, IS_NULL, IS_NOT_NULL, IF) run in both instantiations.  A BOOLEAN entry holds 0 / 1
+// (0 when NULL), so Kleene AND / OR are a & b / a | b plus a NULL rule.  A STRING COMPARE walks both piece lists byte by
+// byte under their case maps and drops both; a STRING IF keeps a's pieces, or moves b's (at most 16) down over them.
+// Errors follow the data: each entry carries its error kinds in a bit stack in registers (kEW bits per entry), every op
+// ORs its operands' bits, IF takes the condition's and the taken branch's, FALSE AND x / TRUE OR x drop x's, and only the
+// result's bits reach the error word.  So a program without IF / AND / OR fails on the rows it always failed on.
 #include <algorithm>
 #include <cstring>
+#include <type_traits>
 #include <vector>
 
 #include "columnar.cuh"
@@ -43,7 +51,12 @@ using namespace ytgpu;
 namespace {
 
 constexpr int kExprThreads = 256;
-constexpr u32 kErrDivZero = 1, kErrIntMinByMinusOne = 2, kErrOutOfHeap = 4, kErrNonAscii = 8, kErrTooLong = 16;
+// Errors that follow the data: a bit stack per kind beside the NULL stack, 2 bits per entry in expression_kernel<false, true>,
+// 3 in expression_kernel<true, true>; only the result's bits fail the call.  expression_kernel<false, false> runs programs
+// without conditional ops, where every error reaches the result, so it raises them at once.  The other two are input
+// checks, raised at once.
+constexpr u32 kErrDivZero = 1, kErrIntMinByMinusOne = 2, kErrNonAscii = 4;
+constexpr u32 kErrOutOfHeap = 8, kErrTooLong = 16;
 constexpr u32 kModeValues = 0, kModeSize = 1, kModeFill = 2;  // a 64-bit result; a STRING result's two passes
 constexpr u32 kCaseLower = 1, kCaseUpper = 2;
 constexpr u32 kShortValue = 48;                                        // longer values are copied by the whole warp
@@ -52,10 +65,10 @@ constexpr u32 kStageBytes = 32 * kShortValue + 16;                     // a warp
 struct ExprNodeDev {
     u8 op;
     u8 type;  // the node's result type
-    u8 from;  // CAST: the operand's type
+    u8 from;  // CAST, COMPARE, IS_NULL, IS_NOT_NULL: the operand's type
     u8 pad;
     u16 col;  // COLUMN: compact column table (referenced columns only; a STRING leaf: the compact string table);
-              // FARM_HASH: its operand count
+              // FARM_HASH: its operand count; COMPARE: the ytgpu_cmp_op
     u16 pad2;
     u64 constant;  // CONSTANT: the bit pattern, a STRING one (offset << 32) | length; FARM_HASH: bit j = operand j is a STRING
 };
@@ -71,7 +84,7 @@ struct ExprArgs {
     u64* values;
     u32* nulls;                   // 2 * ceil(n / 64) words of 32 bits
     unsigned long long* result;   // [0] NULL rows, [1] error bits, [2] (STRING result) heap bytes
-    // expression_kernel<true> only
+    // expression_kernel<true, true> only
     const StringDev* strings;
     u32 string_count;
     u32 mode;
@@ -175,14 +188,59 @@ __device__ __forceinline__ void warp_copy(u8* dst, const u8* src, u64 len, u32 c
     for (u64 j = head + body + lane; j < len; j += 32) dst[j] = (u8)case_byte(__ldg(src + j), cm);
 }
 
-template <bool kStrings>
+// A STRING COMPARE: the pieces [a, a + na) against [b, b + nb) of this thread's piece stack (pptr / plen: its entry 0,
+// stride kExprThreads), byte by byte under their case maps: unsigned bytes, then the shorter value first.
+__device__ __forceinline__ int pieces_compare(const u64* pptr, const u32* plen, u32 cases, u32 a, u32 na, u32 b, u32 nb) {
+    const u32 ea = a + na, eb = b + nb;
+    const u8 *pa = nullptr, *pb = nullptr;
+    u32 la = 0, lb = 0, ca = 0, cb = 0;  // bytes left in the current pieces, their case maps
+    for (;;) {
+        while (la == 0 && a < ea) {
+            pa = reinterpret_cast<const u8*>(pptr[a * kExprThreads]);
+            la = plen[a * kExprThreads];
+            ca = (cases >> (2 * a)) & 3;
+            ++a;
+        }
+        while (lb == 0 && b < eb) {
+            pb = reinterpret_cast<const u8*>(pptr[b * kExprThreads]);
+            lb = plen[b * kExprThreads];
+            cb = (cases >> (2 * b)) & 3;
+            ++b;
+        }
+        if (la == 0 || lb == 0) return (la != 0) - (lb != 0);
+        const u32 x = case_byte(__ldg(pa), ca), y = case_byte(__ldg(pb), cb);
+        if (x != y) return x < y ? -1 : 1;
+        ++pa, ++pb, --la, --lb;
+    }
+}
+
+__device__ __forceinline__ bool cmp_holds(u32 cmp, int c) {
+    switch (cmp) {
+        case YTGPU_CMP_LT: return c < 0;
+        case YTGPU_CMP_LE: return c <= 0;
+        case YTGPU_CMP_GT: return c > 0;
+        case YTGPU_CMP_GE: return c >= 0;
+        case YTGPU_CMP_EQ: return c == 0;
+        default: return c != 0;
+    }
+}
+
+// kCond: the program may hold COMPARE, AND, OR, NOT, IS_NULL, IS_NOT_NULL or IF.  Without them the scalar instantiation
+// keeps the dispatch and the error handling of a program of arithmetic only (the conditional ops cost the old programs
+// 6-14 % in bench_expressions.py when compiled in); the string one always takes them.
+template <bool kStrings, bool kCond>
 __global__ void __launch_bounds__(kExprThreads) expression_kernel(const ExprArgs A) {
+    static_assert(kCond || !kStrings, "expression_kernel<true, false> is not instantiated");
+    // the error bit stacks: kEW bits per entry, entry d from the top at bit kEW * d (a 16-deep stack fills 32 / 48 bits)
+    using ErrStack = typename std::conditional<kStrings, u64, u32>::type;
+    constexpr u32 kEW = kStrings ? 3 : 2;
+    constexpr ErrStack kEM = (ErrStack)((1u << kEW) - 1);
     extern __shared__ __align__(16) unsigned char smem[];
     ExprNodeDev* s_nodes = reinterpret_cast<ExprNodeDev*>(smem);
     ColumnDev* s_cols = reinterpret_cast<ColumnDev*>(s_nodes + A.node_count);
     StringDev* s_strs = reinterpret_cast<StringDev*>(s_cols + A.column_count);
     u64* s_stack = reinterpret_cast<u64*>(s_strs + (kStrings ? A.string_count : 0)) + threadIdx.x;  // entry d: [d * kExprThreads]
-    // expression_kernel<true>: the piece stack [p * kExprThreads], then a short-value stage per warp
+    // expression_kernel<true, true>: the piece stack [p * kExprThreads], then a short-value stage per warp
     u64* s_pptr = s_stack + (kStrings ? (size_t)(A.max_depth - 1) * kExprThreads : 0);
     u32* s_plen = reinterpret_cast<u32*>(s_pptr - threadIdx.x + (size_t)A.max_pieces * kExprThreads) + threadIdx.x;
     u8* s_stage = reinterpret_cast<u8*>((reinterpret_cast<uintptr_t>(s_plen - threadIdx.x + (size_t)A.max_pieces * kExprThreads) + 15) & ~(uintptr_t)15) +
@@ -216,6 +274,7 @@ __global__ void __launch_bounds__(kExprThreads) expression_kernel(const ExprArgs
         u32 nul_stack = 1;  // bit d: entry d from the top is NULL
         u32 np = 0;         // pieces on the piece stack
         u32 cases = 0;      // 2 bits per piece: its case map
+        ErrStack es = 0;    // the entries' error bits
         if (sel != 0) {
             u32 depth = 0;  // entries below the top, in s_stack
 #pragma unroll 1
@@ -252,15 +311,22 @@ __global__ void __launch_bounds__(kExprThreads) expression_kernel(const ExprArgs
                     if (k) s_stack[depth++ * kExprThreads] = top;
                     top = nul ? 0 : v;
                     nul_stack = (nul_stack << 1) | (nul ? 1u : 0u);
+                    if (kCond) es <<= kEW;
                 } else if (nd.op == YTGPU_EXPR_NEG || nd.op == YTGPU_EXPR_BIT_NOT || nd.op == YTGPU_EXPR_CAST) {
                     if (!(nul_stack & 1)) top = unary_op(nd.op, nd.type, nd.from, top);
+                } else if (kCond && nd.op == YTGPU_EXPR_NOT) {
+                    top ^= (nul_stack & 1) ^ 1;  // a NULL entry holds 0 and stays NULL
+                } else if (kCond && (nd.op == YTGPU_EXPR_IS_NULL || nd.op == YTGPU_EXPR_IS_NOT_NULL)) {
+                    if (kStrings && nd.from == YTGPU_TYPE_STRING) np -= (u32)top;  // a NULL string has no pieces
+                    top = (nul_stack & 1) ^ (nd.op == YTGPU_EXPR_IS_NULL ? 0u : 1u);
+                    nul_stack &= ~1u;
                 } else if (kStrings && (nd.op == YTGPU_EXPR_LOWER || nd.op == YTGPU_EXPR_UPPER)) {
                     if (!(nul_stack & 1)) {
                         const u32 first = np - (u32)top;
-                        if (A.mode == kModeSize)
+                        if (A.mode != kModeFill)  // the fill pass runs only once the size pass found no error
                             for (u32 p = first; p < np; ++p)
                                 if (!ascii_only(reinterpret_cast<const u8*>(s_pptr[p * kExprThreads]), s_plen[p * kExprThreads]))
-                                    err |= kErrNonAscii;
+                                    es |= kErrNonAscii;
                         const u32 mask = (u32)(((1ull << (2 * np)) - 1) & ~((1ull << (2 * first)) - 1));
                         cases = (cases & ~mask) | ((nd.op == YTGPU_EXPR_LOWER ? 0x55555555u : 0xaaaaaaaau) & mask);
                     }
@@ -288,9 +354,40 @@ __global__ void __launch_bounds__(kExprThreads) expression_kernel(const ExprArgs
                     depth = below;
                     top = h ^ (u64)count;
                     nul_stack = (nul_stack >> count) << 1;
+                    ErrStack er = 0;
+                    for (u32 j = 0; j < count; ++j) er |= (es >> (kEW * j)) & kEM;
+                    es = ((es >> (kEW * count)) << kEW) | er;
+                } else if (kCond && nd.op == YTGPU_EXPR_IF) {
+                    // c a b IF: the value, NULL flag and error bits of the branch c takes; a NULL c takes neither
+                    const u64 b = top, a = s_stack[(depth - 1) * kExprThreads], c = s_stack[(depth - 2) * kExprThreads];
+                    depth -= 2;
+                    const u32 nb = nul_stack & 1, na = (nul_stack >> 1) & 1, nc = (nul_stack >> 2) & 1;
+                    if (kStrings && nd.type == YTGPU_TYPE_STRING) {  // a's pieces, then b's, on top of the piece stack
+                        const u32 first = np - (u32)(a + b);
+                        if (nc) {
+                            np = first;
+                        } else if (c) {
+                            np -= (u32)b;
+                        } else {  // b's pieces move down over a's, at most YTGPU_EXPR_MAX_PIECES of them
+                            for (u32 p = 0; p < (u32)b; ++p) {
+                                s_pptr[(first + p) * kExprThreads] = s_pptr[(first + (u32)a + p) * kExprThreads];
+                                s_plen[(first + p) * kExprThreads] = s_plen[(first + (u32)a + p) * kExprThreads];
+                            }
+                            const u64 bc = ((u64)cases >> (2 * (first + (u32)a))) & ((1ull << (2 * (u32)b)) - 1);
+                            cases = (u32)(((u64)cases & ((1ull << (2 * first)) - 1)) | (bc << (2 * first)));
+                            np = first + (u32)b;
+                        }
+                    }
+                    top = c ? a : b;  // a NULL c holds 0: b, which nc makes NULL below
+                    const u32 nr = nc | (c ? na : nb);
+                    top = nr ? 0 : top;
+                    nul_stack = ((nul_stack >> 3) << 1) | nr;
+                    const ErrStack er = ((es >> (2 * kEW)) & kEM) | (nc ? 0 : (es >> (c ? kEW : 0)) & kEM);
+                    es = ((es >> (3 * kEW)) << kEW) | er;
                 } else {
                     const u64 a = s_stack[--depth * kExprThreads], b = top;
                     const u32 nb = nul_stack & 1, na = (nul_stack >> 1) & 1;
+                    ErrStack er = (es | (es >> kEW)) & kEM;  // both operands' bits
                     u32 nr;
                     if (nd.op == YTGPU_EXPR_IF_NULL) {
                         top = na ? b : a;
@@ -300,14 +397,37 @@ __global__ void __launch_bounds__(kExprThreads) expression_kernel(const ExprArgs
                         nr = na | nb;
                         np -= nr ? (u32)(a + b) : 0;
                         top = nr ? 0 : a + b;
+                    } else if (kCond && nd.op == YTGPU_EXPR_COMPARE) {
+                        nr = na | nb;
+                        bool r;
+                        if (kStrings && nd.from == YTGPU_TYPE_STRING) {  // both operands' pieces are dropped
+                            np -= (u32)(a + b);
+                            r = !nr && cmp_holds(nd.col, pieces_compare(s_pptr, s_plen, cases, np, (u32)a, np + (u32)a, (u32)b));
+                        } else {
+                            r = !nr && passes(nd.col, nd.from, a, b);
+                        }
+                        top = r ? 1 : 0;
+                    } else if (kCond && (nd.op == YTGPU_EXPR_AND || nd.op == YTGPU_EXPR_OR)) {
+                        // Kleene over 0 / 1 entries (a NULL one holds 0): F AND x = F, T OR x = T, else NULL with a NULL
+                        // operand.  A deciding left operand drops the right one's error bits.
+                        const bool is_and = nd.op == YTGPU_EXPR_AND;
+                        const bool left_decides = is_and ? (!na && !a) : (a != 0);
+                        const bool decided = left_decides || (is_and ? (!nb && !b) : (b != 0));
+                        top = is_and ? (a & b) : (a | b);
+                        nr = !decided && (na | nb);
+                        if (left_decides) er = (es >> kEW) & kEM;
                     } else {
                         nr = na | nb;
-                        top = nr ? 0 : binary_op(nd.op, nd.type, a, b, &err);
+                        u32 e = 0;
+                        top = nr ? 0 : binary_op(nd.op, nd.type, a, b, kCond ? &e : &err);
+                        if (kCond) er |= e;
                     }
                     nul_stack = ((nul_stack >> 2) << 1) | nr;
+                    if (kCond) es = ((es >> (2 * kEW)) << kEW) | er;
                 }
             }
         }
+        if (kCond) err |= (u32)(es & kEM);  // the result's error bits
         const bool nul = !live || (nul_stack & 1);
         if (!kStrings || A.mode == kModeValues) {
             const u32 m = __ballot_sync(0xffffffffu, nul && i < A.n);
@@ -411,7 +531,8 @@ struct CheckedExpr {
     std::vector<u32> strings;  // compact string slot -> caller string column
     u32 max_depth = 0;
     u32 max_pieces = 0;
-    bool strings_kernel = false;  // a STRING node or FARM_HASH: expression_kernel<true>
+    bool strings_kernel = false;  // a STRING node or FARM_HASH: expression_kernel<true, true>
+    bool conditional = false;     // a conditional op: expression_kernel<false, true> for a scalar program
     u8 type = 0;  // the result type
 };
 
@@ -537,6 +658,57 @@ Status check_expression(const ytgpu_column_view* columns, u32 column_count, bool
                 stack.push_back({YTGPU_TYPE_UINT64, 0, 0});
                 break;
             }
+            case YTGPU_EXPR_NOT:
+            case YTGPU_EXPR_IS_NULL:
+            case YTGPU_EXPR_IS_NOT_NULL: {
+                if (stack.empty()) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: stack underflow", k);
+                const Entry e = stack.back();
+                if (N.op == YTGPU_EXPR_NOT && e.type != YTGPU_TYPE_BOOLEAN)
+                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: NOT takes a BOOLEAN, not type 0x%x", k, e.type);
+                pieces -= e.pieces;
+                d.from = e.type;
+                d.type = YTGPU_TYPE_BOOLEAN;
+                stack.back() = {YTGPU_TYPE_BOOLEAN, 0, 0};
+                break;
+            }
+            case YTGPU_EXPR_IF: {
+                if (stack.size() < 3) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: stack underflow", k);
+                const Entry eb = stack.back();
+                stack.pop_back();
+                const Entry ea = stack.back();
+                stack.pop_back();
+                if (stack.back().type != YTGPU_TYPE_BOOLEAN)
+                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: IF's condition has type 0x%x, not BOOLEAN", k, stack.back().type);
+                if (ea.type != eb.type)
+                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: IF branches of types 0x%x and 0x%x (CAST one of them)", k, ea.type,
+                                       eb.type);
+                d.type = ea.type;
+                stack.back() = {ea.type, (u8)(ea.plain & eb.plain), std::max(ea.pieces, eb.pieces)};  // keeps one branch's pieces
+                pieces -= std::min(ea.pieces, eb.pieces);
+                break;
+            }
+            case YTGPU_EXPR_COMPARE:
+            case YTGPU_EXPR_AND:
+            case YTGPU_EXPR_OR: {
+                if (stack.size() < 2) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: stack underflow", k);
+                const Entry eb = stack.back();
+                stack.pop_back();
+                const Entry ea = stack.back();
+                if (ea.type != eb.type)
+                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: operands of types 0x%x and 0x%x (CAST one of them)", k, ea.type, eb.type);
+                if (N.op == YTGPU_EXPR_COMPARE) {
+                    if (N.column < YTGPU_CMP_LT || N.column > YTGPU_CMP_NE)
+                        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: COMPARE with cmp %d (LT .. NE)", k, N.column);
+                    d.col = (u16)N.column;
+                    pieces -= ea.pieces + eb.pieces;
+                } else if (ea.type != YTGPU_TYPE_BOOLEAN) {
+                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: op %d takes BOOLEANs, not type 0x%x", k, N.op, ea.type);
+                }
+                d.from = ea.type;
+                d.type = YTGPU_TYPE_BOOLEAN;
+                stack.back() = {YTGPU_TYPE_BOOLEAN, 0, 0};
+                break;
+            }
             case YTGPU_EXPR_ADD:
             case YTGPU_EXPR_SUB:
             case YTGPU_EXPR_MUL:
@@ -582,6 +754,7 @@ Status check_expression(const ytgpu_column_view* columns, u32 column_count, bool
         out->max_depth = std::max(out->max_depth, (u32)stack.size());
         out->max_pieces = std::max(out->max_pieces, pieces);
         out->strings_kernel |= d.type == YTGPU_TYPE_STRING || N.op == YTGPU_EXPR_FARM_HASH;
+        out->conditional |= N.op >= YTGPU_EXPR_COMPARE;
         out->nodes.push_back(d);
     }
     if (stack.size() != 1)
@@ -725,22 +898,23 @@ Status evaluate_expression_impl(Context* ctx, const ytgpu_column_view* columns, 
     A.lengths = dlengths;
     A.null_bytes = dnull_bytes;
     // shared memory in the kernel's order: nodes (16 B each), column views, string views (8-byte multiples), the stack
-    // below the top; expression_kernel<true>: the piece stack and, 16-byte aligned, a short-value stage per warp
+    // below the top; expression_kernel<true, true>: the piece stack and, 16-byte aligned, a short-value stage per warp
     static_assert(sizeof(ColumnDev) % 8 == 0 && sizeof(StringDev) % 8 == 0, "shared-memory layout");
     const size_t stack_b = (size_t)(P.max_depth - 1) * kExprThreads * sizeof(u64);
     const u32 blocks = (u32)std::max<u64>(1, std::min<u64>((words * 32 + kExprThreads - 1) / kExprThreads, (u64)kNumSms * 8));
     if (!P.strings_kernel) {
         const size_t smem = nodes_b + cols_b + stack_b;
         KernelTimer t(ctx, KC_DECODE);
-        expression_kernel<false><<<blocks, kExprThreads, smem, ctx->stream>>>(A);
+        if (P.conditional) expression_kernel<false, true><<<blocks, kExprThreads, smem, ctx->stream>>>(A);
+        else expression_kernel<false, false><<<blocks, kExprThreads, smem, ctx->stream>>>(A);
         YTGPU_CUDA_TRY(cudaGetLastError());
     } else {
         const size_t smem = nodes_b + cols_b + strs_b + stack_b + (size_t)P.max_pieces * kExprThreads * 12 + 16 +
                             (size_t)(kExprThreads / 32) * kStageBytes;
         // up to 16 pieces and a 16-deep stack take the stage past the 48 KB default
-        YTGPU_CUDA_TRY(cudaFuncSetAttribute(expression_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        YTGPU_CUDA_TRY(cudaFuncSetAttribute(expression_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         KernelTimer t(ctx, KC_DECODE, string_result ? 4 : 1);
-        expression_kernel<true><<<blocks, kExprThreads, smem, ctx->stream>>>(A);
+        expression_kernel<true, true><<<blocks, kExprThreads, smem, ctx->stream>>>(A);
         if (string_result)  // starts = exclusive scan of the lengths, the total into result[2]
             exclusive_scan_u64(ctx->stream, dstarts, n, scan_sums.p, reinterpret_cast<u64*>(result.p + 2));
         YTGPU_CUDA_TRY(cudaGetLastError());
@@ -778,7 +952,7 @@ Status evaluate_expression_impl(Context* ctx, const ytgpu_column_view* columns, 
         const size_t smem = nodes_b + cols_b + strs_b + stack_b + (size_t)P.max_pieces * kExprThreads * 12 + 16 +
                             (size_t)(kExprThreads / 32) * kStageBytes;
         KernelTimer t(ctx, KC_GATHER);
-        expression_kernel<true><<<blocks, kExprThreads, smem, ctx->stream>>>(A);
+        expression_kernel<true, true><<<blocks, kExprThreads, smem, ctx->stream>>>(A);
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
     if (host) {
