@@ -15,6 +15,8 @@ from CUDA events around the whole call):
   guarded_div   if(b = 0, 0, a / b)            (a division whose zero divisors the IF guards; b has zeros here)
   if_bucket     if(a < 0, 0, if(a < 5 * 10^8, 1, 2))   (a two-level if)
   and_signs     (a > 0) AND (b < 0)            (a BOOLEAN result)
+  in_16         if(k in (16 int64 entries), b, 0)   with k int64 U[0, 64): a quarter of the rows match (the numeric-IN
+                kernel: a binary search over the list staged in shared memory)
 Each leg reports its algorithmic bytes per row — 8 per referenced column read, plus 8 bytes of value and 1/8 byte of null
 bitmap written — and that traffic over the kernel time, against the HBM peak (MEASURED_PEAKS.json's when present, else
 the 3.35 TB/s data-sheet figure of the H100 SXM).
@@ -68,9 +70,13 @@ def main():
     price = torch.rand(n, device="cuda", generator=g, dtype=torch.float64) * 100
     qty = torch.rand(n, device="cuda", generator=g, dtype=torch.float64) * 10
     d = torch.randn(n, device="cuda", generator=g, dtype=torch.float64)
+    k = torch.randint(0, 64, (n,), device="cuda", generator=g)
     cols = [Column(T.Int64, values=a), Column(T.Int64, values=b), Column(T.Double, values=price.view(torch.int64)),
-            Column(T.Double, values=qty.view(torch.int64)), Column(T.Double, values=d.view(torch.int64)), Column(T.Int64, values=bz)]
-    A, B, PRICE, QTY, D, BZ = range(6)
+            Column(T.Double, values=qty.view(torch.int64)), Column(T.Double, values=d.view(torch.int64)), Column(T.Int64, values=bz),
+            Column(T.Int64, values=k)]
+    A, B, PRICE, QTY, D, BZ, K = range(7)
+    in_consts = capi.ExprConstants()
+    in_list = in_consts.in_list(range(0, 64, 4))
     col, const, cast = capi.EXPR_COLUMN, capi.EXPR_CONSTANT, capi.EXPR_CAST
     cmp, iff = capi.EXPR_COMPARE, capi.EXPR_IF
     i64, f64 = int(T.Int64), int(T.Double)
@@ -95,12 +101,13 @@ def main():
                        (cmp, capi.CMP_LT), (const, 0, i64, 1), (const, 0, i64, 2), (iff,), (iff,)], 8 + written),
         "and_signs": ([(col, A), (const, 0, i64, 0), (cmp, capi.CMP_GT), (col, B), (const, 0, i64, 0), (cmp, capi.CMP_LT), (capi.EXPR_AND,)],
                       16 + written),
+        "in_16": ([(col, K), (capi.EXPR_IN, 0, 0, in_list), (col, B), (const, 0, i64, 0), (iff,)], 16 + written, bytes(in_consts)),
     }
     ctx.enable_timers(True)
     results = {}
-    for leg_name, (prog, bytes_per_row) in legs.items():
-        def call(p=prog):
-            return ctx.evaluate_expression(cols, p)
+    for leg_name, (prog, bytes_per_row, *consts) in legs.items():
+        def call(p=prog, c=consts[0] if consts else b""):
+            return ctx.evaluate_expression(cols, p, string_constants=c)
         for _ in range(args.warmup):
             call()
         kernel, calls = [], []
@@ -123,6 +130,7 @@ def main():
     # parity of two legs with torch
     line["add"]["matches_torch"] = bool(torch.equal(results["add"]["values"], a + b))
     line["mod_1000"]["matches_torch"] = bool(torch.equal(results["mod_1000"]["values"], torch.fmod(a, 1000)))
+    line["in_16"]["matches_torch"] = bool(torch.equal(results["in_16"]["values"], torch.where(k % 4 == 0, b, torch.zeros_like(b))))
     safe = torch.where(bz == 0, torch.ones_like(bz), bz)
     line["guarded_div"]["matches_torch"] = bool(torch.equal(results["guarded_div"]["values"],
                                                             torch.where(bz == 0, torch.zeros_like(a), torch.div(a, safe, rounding_mode="trunc"))))

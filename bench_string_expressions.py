@@ -15,10 +15,16 @@ call with a heap sized beforehand, so a size pass, a three-kernel scan and a fil
   farm_hash_a_url_mod   farm_hash(a, url) % 64
   if_a_url_other        if(a > 0, url, 'other')          (a STRING IF: about half the rows keep url's piece)
   url_lt_site5          url < 'https://www.site5'        (a STRING COMPARE, BOOLEAN result)
+  url_like              url like 'https://www.site_.example.com/%q%'   (LIKE over the url leaf: its one piece is matched as
+                        contiguous bytes), beside filter_url_like: the same pattern as a ytgpu_evaluate_filter leaf
+  lower_url_like_site4  lower(url) like '%site4%'        (fused: the matcher walks lower(url)'s piece under its case map),
+                        beside lower_url_then_contains: lower(url) written out, then the filter's CONTAINS 'site4' over it
+  if_substr_api         if(is_substr('/api/', url), 'api', 'web')   (a STRING result)
 Algorithmic bytes per row: a string input reads its 8-byte start, 4-byte length and its bytes (+1 null byte when it has
 NULLs), a numeric one 8 bytes; a STRING result writes its bytes, an 8-byte start, a 4-byte length and a null byte, a
 numeric one 8 bytes and 1/8 byte of null bitmap; a COMPARE against a constant of c bytes reads at most c + 1 bytes of a
-value.  That traffic over the kernel time is set against the HBM peak
+value; LIKE and CONTAINS are counted as reading every byte of the value, the most the matcher consumes.  That traffic over
+the kernel time is set against the HBM peak
 (MEASURED_PEAKS.json's when present, else the 3.35 TB/s data-sheet figure of the H100 SXM).
 GROUP BY leg: COUNT and SUM of a grouped by lower(host), once computed (lower as one call into outputs allocated once, as
 the string legs, then string_value_ids and the GROUP BY) and once over the host names lowered beforehand; both results must
@@ -82,7 +88,11 @@ def main():
     url_nulls = _string_column(heap, starts, lengths, nulls)
     acol = Column(T.Int64, values=a)
     col, const, STR, U64, I64 = capi.EXPR_COLUMN, capi.EXPR_CONSTANT, int(T.String), int(T.Uint64), int(T.Int64)
-    consts = np.frombuffer(b"/xotherhttps://www.site5", np.uint8).copy()  # "/x" at 0, "other" at 2, the URL bound at 7
+    ec = capi.ExprConstants()
+    ec.data += b"/xotherhttps://www.site5"  # "/x" at 0, "other" at 2, the URL bound at 7
+    like_q, site4, api_needle = ec.string(b"https://www.site_.example.com/%q%"), ec.string(b"%site4%"), ec.string(b"/api/")
+    api, web, site4_needle = ec.string(b"api"), ec.string(b"web"), ec.string(b"site4")
+    consts = np.frombuffer(bytes(ec), np.uint8).copy()
 
     out_heap = torch.empty(int(heap.numel()) + 2 * n, dtype=torch.uint8, device="cuda")
     out_starts = torch.empty(n, dtype=torch.int64, device="cuda")
@@ -122,6 +132,10 @@ def main():
                             (capi.EXPR_IF,)], [url], [acol], 8 + 12 + 0.5 * mean_len + (0.5 * mean_len + 0.5 * 5 + 13)),
         "url_lt_site5": ([(col, 0), (const, 0, STR, (7 << 32) | 17), (capi.EXPR_COMPARE, capi.CMP_LT)], [url], (),
                          12 + 18 + numeric_out),
+        "url_like": ([(col, 0), (capi.EXPR_LIKE, -1, 0, like_q)], [url], (), string_in + numeric_out),
+        "lower_url_like_site4": ([(col, 0), (capi.EXPR_LOWER,), (capi.EXPR_LIKE, -1, 0, site4)], [url], (), string_in + numeric_out),
+        "if_substr_api": ([(col, 0), (capi.EXPR_CONTAINS, 0, 0, api_needle), (const, 0, STR, api), (const, 0, STR, web), (capi.EXPR_IF,)],
+                          [url], (), string_in + 3 + 13),
     }
     ctx.enable_timers(True)
     for leg_name, (prog, scols, numeric, bytes_per_row) in legs.items():
@@ -142,7 +156,44 @@ def main():
         line[leg_name] = {"kernel_ms_median": median_ms(kernel), "kernel_ms_min": round(min(kernel), 4), "call_ms_median": median_ms(calls),
                           "result_type": vtype, "heap_bytes": size, "null_count": nul, "bytes_per_row": round(bytes_per_row, 4),
                           "bytes_per_s": rate, "share_of_hbm_peak": round(rate / peak, 4)}
+    # the filter's LIKE over the same column, and lower(url) written out then the filter's CONTAINS: the routes the fused
+    # legs replace
+    def filter_bitmap(scol, op, constant, escape=-1):
+        return ctx.evaluate_filter([], [scol], [(op, 0, 0, escape, constant >> 32, constant & 0xFFFFFFFF)], string_constants=bytes(ec),
+                                   want_bytemap=False, want_rows=False)["bitmap"]
+    routes = {
+        "filter_url_like": (lambda: filter_bitmap((heap, starts, lengths, None), capi.FILTER_LIKE, like_q), string_in + 1 / 8),
+        "lower_url_then_contains": (lambda: (evaluate(legs["lower_url"][0], [url]),
+                                             filter_bitmap((out_heap, out_starts, out_lengths, None), capi.FILTER_CONTAINS, site4_needle))[1],
+                                    (string_in + string_out) + (12 + mean_len + 1 / 8)),
+    }
+    bitmaps = {}
+    for leg_name, (fn, bytes_per_row) in routes.items():
+        for _ in range(args.warmup):
+            fn()
+        kernel, calls = [], []
+        start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        for _ in range(args.steps):
+            ctx.reset_timers()
+            start.record()
+            bitmaps[leg_name] = fn()
+            stop.record()
+            torch.cuda.synchronize()
+            kernel.append(ctx.kernel_ms(capi.KC_DECODE)[0] + ctx.kernel_ms(capi.KC_GATHER)[0])
+            calls.append(start.elapsed_time(stop))
+        km = statistics.median(kernel)
+        rate = n * bytes_per_row / (km * 1e-3)
+        line[leg_name] = {"kernel_ms_median": median_ms(kernel), "kernel_ms_min": round(min(kernel), 4), "call_ms_median": median_ms(calls),
+                          "bytes_per_row": round(bytes_per_row, 4), "bytes_per_s": rate, "share_of_hbm_peak": round(rate / peak, 4)}
     ctx.enable_timers(False)
+    # the fused legs select the rows of the routes they replace (no NULLs here: TRUE rows are the value bits)
+    for leg_name, route in (("url_like", "filter_url_like"), ("lower_url_like_site4", "lower_url_then_contains")):
+        evaluate(legs[leg_name][0], [url])
+        word = torch.arange(64, device="cuda", dtype=torch.int64)
+        vals = torch.zeros((n + 63) // 64 * 64, dtype=torch.int64, device="cuda")
+        vals[:n] = out_values
+        packed = (vals.view(-1, 64) << word).sum(1)
+        line[leg_name]["matches_" + route] = bool(torch.equal(packed, bitmaps[route].view(torch.int64)))
     # lower(url) against torch's ASCII lowering of the same slots
     evaluate(legs["lower_url"][0], [url])
     ref = heap.view(n, -1)[:1_000_000].clone()

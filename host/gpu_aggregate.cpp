@@ -259,6 +259,75 @@ namespace NQueryClient {
 
 namespace {
 
+bool IsPredicate(EExpressionOp op) { return op >= EExpressionOp::In && op <= EExpressionOp::Like; }
+
+// The library node of an expression node.  A String constant, and the list, prefix, needle or pattern of a predicate, are
+// appended to `constants` (the call's string_constants); an In list's entries go at an 8-byte boundary, each its bit
+// pattern or, for a string, (offset << 32) | length of its bytes appended before them.  *listType: the entries' one type
+// (Null for an empty list); entries of several types, or a NULL one, throw.
+ytgpu_expr_node LibraryNode(const TExpressionNode& node, std::string* constants, EValueType* listType) {
+    ytgpu_expr_node x{};
+    x.op = (int32_t)node.Op;
+    x.column = node.Column;
+    x.type = (uint8_t)node.Type;
+    x.constant = node.Bits;
+    *listType = EValueType::Null;
+    auto append = [&](const std::string& bytes) {
+        const uint64_t c = ((uint64_t)constants->size() << 32) | bytes.size();
+        *constants += bytes;
+        return c;
+    };
+    if ((node.Op == EExpressionOp::Constant && node.Type == EValueType::String) ||
+        (IsPredicate(node.Op) && node.Op != EExpressionOp::In))
+        x.constant = append(node.Bytes);
+    if (node.Op != EExpressionOp::In) return x;
+    std::vector<uint64_t> entries;
+    for (size_t e = 0; e < node.List.size(); ++e) {
+        const TExpressionLiteral& v = node.List[e];
+        if (v.Type == EValueType::Null) throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "in: the list holds a NULL");
+        if (*listType != EValueType::Null && v.Type != *listType)
+            throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "in: list entries of different types");
+        *listType = v.Type;
+        entries.push_back(v.Type == EValueType::String ? append(v.Bytes) : v.Bits);
+    }
+    constants->append((8 - constants->size() % 8) % 8, '\0');
+    x.constant = ((uint64_t)constants->size() << 32) | entries.size();
+    constants->append(reinterpret_cast<const char*>(entries.data()), entries.size() * 8);
+    return x;
+}
+
+// Throws INVALID_ARGUMENT when the In node k of `program` has a list of another type than its operand: the operand,
+// compared with a constant of the list's type, must type-check.  `typeQuery` checks a program without evaluating it (a
+// BOOLEAN result: no launch) and returns its ytgpu_error code.  A malformed program is left to the call that evaluates it.
+template <class F>
+void CheckInList(const std::vector<ytgpu_expr_node>& program, size_t k, EValueType listType, F&& typeQuery) {
+    if (listType == EValueType::Null) return;
+    int need = 1;
+    size_t s = k;
+    while (need > 0) {
+        if (s == 0) return;
+        const int op = program[--s].op;
+        const int arity = op == YTGPU_EXPR_COLUMN || op == YTGPU_EXPR_CONSTANT ? 0
+                        : op == YTGPU_EXPR_IF ? 3
+                        : op == YTGPU_EXPR_FARM_HASH ? program[s].column
+                        : (op == YTGPU_EXPR_NEG || op == YTGPU_EXPR_BIT_NOT || op == YTGPU_EXPR_CAST || op == YTGPU_EXPR_LOWER ||
+                           op == YTGPU_EXPR_UPPER || (op >= YTGPU_EXPR_NOT && op <= YTGPU_EXPR_IS_NOT_NULL) || op >= YTGPU_EXPR_IN) ? 1 : 2;
+        need += arity - 1;
+    }
+    std::vector<ytgpu_expr_node> check(program.begin() + (std::ptrdiff_t)s, program.begin() + (std::ptrdiff_t)k);
+    ytgpu_expr_node c{};
+    c.op = YTGPU_EXPR_CONSTANT;
+    c.type = (uint8_t)listType;  // a STRING constant of 0 bytes at offset 0
+    check.push_back(c);
+    ytgpu_expr_node cmp{};
+    cmp.op = YTGPU_EXPR_COMPARE;
+    cmp.column = YTGPU_CMP_EQ;
+    check.push_back(cmp);
+    if (typeQuery(check) != YTGPU_OK)
+        throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "in: list entries of type " + std::to_string((int)listType) +
+                                                              " against an operand of another type");
+}
+
 class TGpuEvaluator : public IEvaluator {
 public:
     TQueryStatistics Run(const TGroupQuery& query, const ISchemalessMultiChunkReaderPtr& reader, const IUnversionedRowsetWriterPtr& writer) override {
@@ -449,7 +518,8 @@ public:
         // An input column without a non-NULL value has no type: it is a STRING where the program reads it as one (an
         // operand of CONCAT, LOWER, UPPER, of IF_NULL or COMPARE with a STRING, or an IF branch beside one; it is passed as
         // an all-NULL string column), a BOOLEAN under AND / OR / NOT or as IF's condition, the other operand's type in a
-        // COMPARE or beside an IF branch, INT64 everywhere else, as view() passes it.  (*leafTypes)[leaf] records the type
+        // COMPARE or beside an IF branch, the list's type under IN, a STRING under IsPrefix / IsSubstr / Like, INT64 everywhere
+        // else, as view() passes it.  (*leafTypes)[leaf] records the type
         // it is read as (Null: INT64).  A malformed program types as INT64 and is refused by the call.
         auto typeComputed = [&](size_t j, std::vector<EValueType>* leafTypes) {
             struct TEntry {
@@ -474,7 +544,7 @@ public:
                                   : node.Op == EExpressionOp::If ? 3
                                   : (node.Op == EExpressionOp::Neg || node.Op == EExpressionOp::BitNot || node.Op == EExpressionOp::Cast ||
                                      node.Op == EExpressionOp::Lower || node.Op == EExpressionOp::Upper || node.Op == EExpressionOp::Not ||
-                                     node.Op == EExpressionOp::IsNull || node.Op == EExpressionOp::IsNotNull) ? 1 : 2;
+                                     node.Op == EExpressionOp::IsNull || node.Op == EExpressionOp::IsNotNull || IsPredicate(node.Op)) ? 1 : 2;
                 if (st.size() < need) return EValueType::Int64;
                 switch (node.Op) {
                     case EExpressionOp::Column: {
@@ -502,6 +572,15 @@ public:
                         asType(st.back(), EValueType::Boolean);
                         break;
                     case EExpressionOp::IsNull: case EExpressionOp::IsNotNull:  // NULL whichever type it is read as
+                        st.back() = {EValueType::Boolean, {}};
+                        break;
+                    case EExpressionOp::In:  // an untyped operand takes the list's type
+                        for (const auto& e : node.List)
+                            if (e.Type != EValueType::Null) asType(st.back(), e.Type);
+                        st.back() = {EValueType::Boolean, {}};
+                        break;
+                    case EExpressionOp::IsPrefix: case EExpressionOp::IsSubstr: case EExpressionOp::Like:
+                        asString(st.back());
                         st.back() = {EValueType::Boolean, {}};
                         break;
                     case EExpressionOp::Compare: case EExpressionOp::And: case EExpressionOp::Or: {
@@ -566,21 +645,58 @@ public:
                 throw TErrorException(YTGPU_ERR_UNSUPPORTED, "sum / avg of a string column");
         }
         std::vector<TUnversionedOwningRow> owned;
-        // a program over output positions; the string functions are not taken there
+        // a program over output positions; the string functions and string predicates are not taken there
+        struct TOutputProgram {
+            std::vector<ytgpu_expr_node> Nodes;
+            std::string Constants;  // In lists
+            std::vector<std::pair<size_t, EValueType>> InLists;
+        };
         auto outputProgram = [&](const TExpression& e, const std::string& what) {
-            std::vector<ytgpu_expr_node> program;
+            TOutputProgram program;
             for (const auto& node : e.Nodes) {
                 if (node.Op == EExpressionOp::Concat || node.Op == EExpressionOp::Lower || node.Op == EExpressionOp::Upper ||
-                    node.Op == EExpressionOp::FarmHash)
+                    node.Op == EExpressionOp::FarmHash || node.Op == EExpressionOp::IsPrefix || node.Op == EExpressionOp::IsSubstr ||
+                    node.Op == EExpressionOp::Like)
                     throw TErrorException(YTGPU_ERR_UNSUPPORTED, what + ": string functions over the output row");
-                ytgpu_expr_node x{};
-                x.op = (int32_t)node.Op;
-                x.column = node.Column;
-                x.type = (uint8_t)node.Type;
-                x.constant = node.Bits;
-                program.push_back(x);
+                EValueType listType;
+                if (node.Op == EExpressionOp::In) {
+                    for (const auto& v : node.List)
+                        if (v.Type == EValueType::String)
+                            throw TErrorException(YTGPU_ERR_UNSUPPORTED, what + ": string functions over the output row");
+                }
+                program.Nodes.push_back(LibraryNode(node, &program.Constants, &listType));
+                if (node.Op == EExpressionOp::In) program.InLists.push_back({program.Nodes.size() - 1, listType});
             }
             return program;
+        };
+        // One call over the output row's views: ytgpu_evaluate_expression, or with In the string entry point without string
+        // columns (it takes the lists in string_constants).
+        auto evaluateOutput = [&](const TOutputProgram& program, const std::vector<ytgpu_column_view>& views, const uint8_t* selection,
+                                  uint64_t* values, uint64_t* nulls, uint8_t* type) {
+            ytgpu_error oerr{};
+            int code;
+            if (program.InLists.empty()) {
+                code = ytgpu_evaluate_expression(GetGpuContext(), views.data(), (uint32_t)views.size(), program.Nodes.data(),
+                                                 (uint32_t)program.Nodes.size(), selection, values, reinterpret_cast<uint8_t*>(nulls), type,
+                                                 nullptr, YTGPU_MEM_HOST, &oerr);
+            } else {
+                auto call = [&](const std::vector<ytgpu_expr_node>& nodes, uint64_t* v, uint64_t* nb, uint8_t* t, ytgpu_error* e) {
+                    uint64_t heapBytes = 0;
+                    return ytgpu_evaluate_expression_strings(
+                        GetGpuContext(), views.data(), (uint32_t)views.size(), nullptr, 0,
+                        reinterpret_cast<const uint8_t*>(program.Constants.data()), program.Constants.size(), nodes.data(),
+                        (uint32_t)nodes.size(), selection, v, reinterpret_cast<uint8_t*>(nb), nullptr, 0, nullptr, nullptr, nullptr,
+                        &heapBytes, t, nullptr, YTGPU_MEM_HOST, e);
+                };
+                for (const auto& [k, listType] : program.InLists)
+                    CheckInList(program.Nodes, k, listType, [&](const std::vector<ytgpu_expr_node>& check) {
+                        ytgpu_error qerr{};
+                        return call(check, nullptr, nullptr, nullptr, &qerr);
+                    });
+                const bool empty = views.empty() || views[0].value_count == 0;
+                code = call(program.Nodes, empty ? nullptr : values, empty ? nullptr : nulls, type, &oerr);
+            }
+            if (code != YTGPU_OK) ThrowFrom(oerr);
         };
         // Having over the output row's views (`groups` rows each) -> its TRUE rows as a selection bitmap in the layout of
         // ytgpu_evaluate_filter's out_bitmap (ceil(groups / 64) words).  With no groups the call only checks the program:
@@ -589,11 +705,7 @@ public:
             const auto program = outputProgram(*query.Having, "having");
             std::vector<uint64_t> values(groups), nulls((groups + 63) / 64), kept((groups + 63) / 64, 0);
             uint8_t type = 0;
-            ytgpu_error herr{};
-            if (ytgpu_evaluate_expression(GetGpuContext(), views.data(), (uint32_t)views.size(), program.data(), (uint32_t)program.size(),
-                                          nullptr, values.data(), reinterpret_cast<uint8_t*>(nulls.data()), &type, nullptr, YTGPU_MEM_HOST,
-                                          &herr) != YTGPU_OK)
-                ThrowFrom(herr);
+            evaluateOutput(program, views, nullptr, values.data(), nulls.data(), &type);
             if (type != (uint8_t)EValueType::Boolean)
                 throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "having: the expression is not a Boolean");
             for (uint64_t g = 0; g < groups; ++g)
@@ -645,17 +757,12 @@ public:
                 std::vector<ytgpu_expr_node> program;
                 std::vector<EValueType> leafTypes(columns.size(), EValueType::Null);  // the types untyped input columns are read as
                 typeComputed(j, &leafTypes);
+                std::vector<std::pair<size_t, EValueType>> inLists;  // In nodes and their lists' types
                 for (size_t k = 0; k < query.Computed[j].Nodes.size(); ++k) {
                     const TExpressionNode& node = query.Computed[j].Nodes[k];
-                    ytgpu_expr_node x{};
-                    x.op = (int32_t)node.Op;
-                    x.type = (uint8_t)node.Type;
-                    x.constant = node.Bits;
-                    if (node.Op == EExpressionOp::FarmHash || node.Op == EExpressionOp::Compare) x.column = node.Column;
-                    if (node.Op == EExpressionOp::Constant && node.Type == EValueType::String) {
-                        x.constant = ((uint64_t)constants.size() << 32) | node.Bytes.size();
-                        constants += node.Bytes;
-                    }
+                    EValueType listType;
+                    ytgpu_expr_node x = LibraryNode(node, &constants, &listType);
+                    if (node.Op == EExpressionOp::In) inLists.push_back({k, listType});
                     const int leaf = leafIndex[j][k];
                     if (leaf >= 0 && slot[leaf] == -1) {
                         if (columns[leaf].Type == EValueType::String || leafTypes[leaf] == EValueType::String) {  // all-NULL: an empty heap
@@ -684,6 +791,15 @@ public:
                     rows.mem = YTGPU_MEM_HOST;
                     inputs.push_back(rows);
                 }
+                for (const auto& [k, listType] : inLists)
+                    CheckInList(program, k, listType, [&](const std::vector<ytgpu_expr_node>& check) {
+                        ytgpu_error qerr{};
+                        uint64_t heapBytes = 0;
+                        return ytgpu_evaluate_expression_strings(
+                            GetGpuContext(), inputs.data(), (uint32_t)inputs.size(), stringInputs.data(), (uint32_t)stringInputs.size(),
+                            reinterpret_cast<const uint8_t*>(constants.data()), constants.size(), check.data(), (uint32_t)check.size(),
+                            nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr, nullptr, &heapBytes, nullptr, nullptr, YTGPU_MEM_HOST, &qerr);
+                    });
                 TFlatColumn& c = columns[i];
                 c.Values.assign(n, 0);
                 c.Nulls.assign((n + 63) / 64 * 8, 0);
@@ -962,12 +1078,7 @@ public:
                         selectValues[s].assign(groups, 0);
                         selectNulls[s].assign((groups + 63) / 64, 0);
                         uint8_t type = 0;
-                        ytgpu_error serr{};
-                        if (ytgpu_evaluate_expression(GetGpuContext(), outViews.data(), (uint32_t)outViews.size(), program.data(),
-                                                      (uint32_t)program.size(), selectSelection, selectValues[s].data(),
-                                                      reinterpret_cast<uint8_t*>(selectNulls[s].data()), &type, nullptr, YTGPU_MEM_HOST,
-                                                      &serr) != YTGPU_OK)
-                            ThrowFrom(serr);
+                        evaluateOutput(program, outViews, selectSelection, selectValues[s].data(), selectNulls[s].data(), &type);
                         selected.push_back({(EValueType)type, nullptr, selectValues[s].data(), nullptr});
                     }
                 }

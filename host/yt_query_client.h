@@ -181,18 +181,26 @@ struct TFilterExpression {
 //! NULLs, wrap-around, division errors and the branches they follow, casts, ASCII case mapping, the fingerprint — are in
 //! include/ytgpu.h).  Nodes are in postfix order; a Column leaf names a position (in the
 //! input rows for TMultiGroupQuery::Computed, in the output row for Select).  Binary operands have one type: there is no
-//! implicit widening, write Cast.  Select takes no string ops.
+//! implicit widening, write Cast.  Select and Having take no string ops; of the predicates they take In over numbers.
 enum class EExpressionOp {
     Column = 1, Constant = 2, Add = 3, Sub = 4, Mul = 5, Div = 6, Mod = 7, Neg = 8, BitAnd = 9, BitOr = 10, BitXor = 11, BitNot = 12,
     Cast = 13, IfNull = 14, Concat = 15, Lower = 16, Upper = 17, FarmHash = 18,
-    Compare = 19, And = 20, Or = 21, Not = 22, IsNull = 23, IsNotNull = 24, If = 25
+    Compare = 19, And = 20, Or = 21, Not = 22, IsNull = 23, IsNotNull = 24, If = 25,
+    In = 26, IsPrefix = 27, IsSubstr = 28, Like = 29
+};
+//! A typed literal: an In list entry.
+struct TExpressionLiteral {
+    EValueType Type = EValueType::Null;
+    uint64_t Bits = 0;                    // Int64 / Uint64 / Double bit pattern, Boolean 0 / 1
+    std::string Bytes = {};               // a String's bytes
 };
 struct TExpressionNode {
     EExpressionOp Op = EExpressionOp::Column;
-    int Column = -1;                      // Column; FarmHash: the operand count; Compare: the EBinaryOp
+    int Column = -1;                      // Column; FarmHash: the operand count; Compare: the EBinaryOp; Like: the escape byte or -1
     EValueType Type = EValueType::Null;   // Constant: its type; Cast: the target type
     uint64_t Bits = 0;                    // Constant: Int64 / Uint64 / Double bit pattern, Boolean 0 / 1
-    std::string Bytes = {};               // Constant: a String's bytes
+    std::string Bytes = {};               // Constant: a String's bytes; IsPrefix / IsSubstr / Like: the prefix, needle or pattern
+    std::vector<TExpressionLiteral> List = {};  // In: the entries
 };
 struct TExpression {
     std::vector<TExpressionNode> Nodes;
@@ -235,8 +243,33 @@ struct TExpression {
     //! if(c, a, b) over the last three values: a where c is true, b where it is false, NULL where c is NULL.  A division or
     //! case-mapping error in the branch not taken does not throw.
     TExpression& If() { return Op(EExpressionOp::If); }
+    //! x in (list): a Boolean, NULL where x is NULL.  The entries have x's type (an all-NULL input column takes theirs) and
+    //! none is NULL: a mistyped entry throws YTGPU_ERR_INVALID_ARGUMENT.  Equality is Compare's: NaN never matches, -0.0 = 0.0.
+    TExpression& In(const std::vector<TUnversionedValue>& list) {
+        TExpressionNode node{EExpressionOp::In, -1, EValueType::Null, 0};
+        for (const auto& v : list) {
+            TExpressionLiteral e{v.Type, 0, {}};
+            if (v.Type == EValueType::String) e.Bytes.assign(v.Data.String, v.Length);
+            else if (v.Type == EValueType::Boolean) e.Bits = v.Data.Boolean ? 1 : 0;
+            else if (v.Type != EValueType::Null) e.Bits = v.Data.Uint64;
+            node.List.push_back(std::move(e));
+        }
+        Nodes.push_back(std::move(node));
+        return *this;
+    }
+    //! is_prefix(prefix, s), is_substr(needle, s) and s like pattern (% any bytes, _ one UTF-8 character, the escape byte
+    //! quotes the next byte) over the string on top: a Boolean, NULL where s is NULL.  An all-NULL input column is a string.
+    TExpression& IsPrefix(const std::string& prefix) { return Text(EExpressionOp::IsPrefix, prefix, -1); }
+    TExpression& IsSubstr(const std::string& needle) { return Text(EExpressionOp::IsSubstr, needle, -1); }
+    TExpression& Like(const std::string& pattern, std::optional<unsigned char> escape = std::nullopt) {
+        return Text(EExpressionOp::Like, pattern, escape ? (int)*escape : -1);
+    }
 
 private:
+    TExpression& Text(EExpressionOp op, const std::string& bytes, int column) {
+        Nodes.push_back({op, column, EValueType::Null, 0, bytes});
+        return *this;
+    }
     TExpression& Op(EExpressionOp op) { Nodes.push_back({op, -1, EValueType::Null, 0}); return *this; }
 };
 

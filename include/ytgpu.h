@@ -787,7 +787,9 @@ typedef enum ytgpu_expr_op {
     YTGPU_EXPR_CONCAT = 15, YTGPU_EXPR_LOWER = 16, YTGPU_EXPR_UPPER = 17, YTGPU_EXPR_FARM_HASH = 18,
     /* conditional expressions, both entry points (see below) */
     YTGPU_EXPR_COMPARE = 19, YTGPU_EXPR_AND = 20, YTGPU_EXPR_OR = 21, YTGPU_EXPR_NOT = 22, YTGPU_EXPR_IS_NULL = 23,
-    YTGPU_EXPR_IS_NOT_NULL = 24, YTGPU_EXPR_IF = 25
+    YTGPU_EXPR_IS_NOT_NULL = 24, YTGPU_EXPR_IF = 25,
+    /* predicates inside expressions, ytgpu_evaluate_expression_strings only (see there) */
+    YTGPU_EXPR_IN = 26, YTGPU_EXPR_STARTS_WITH = 27, YTGPU_EXPR_CONTAINS = 28, YTGPU_EXPR_LIKE = 29
 } ytgpu_expr_op;
 
 #define YTGPU_EXPR_MAX_NODES 64
@@ -799,10 +801,12 @@ typedef enum ytgpu_expr_op {
 typedef struct ytgpu_expr_node {
     int32_t op;          /* ytgpu_expr_op */
     int32_t column;      /* COLUMN: index into columns (++ string_columns); FARM_HASH: its operand count;
-                            COMPARE: the ytgpu_cmp_op */
+                            COMPARE: the ytgpu_cmp_op; LIKE: the escape byte 0..255, or -1 for none */
     uint8_t type;        /* CONSTANT: its value type; CAST: the target type (YTGPU_TYPE_*) */
     uint8_t reserved[7];
-    uint64_t constant;   /* CONSTANT: the bit pattern in `type`; a STRING one: (offset << 32) | length into string_constants */
+    uint64_t constant;   /* CONSTANT: the bit pattern in `type`; a STRING one: (offset << 32) | length into string_constants;
+                            IN: (offset << 32) | count of its list in string_constants; STARTS_WITH, CONTAINS, LIKE: the
+                            prefix, needle or pattern as (offset << 32) | length into string_constants */
 } ytgpu_expr_node;
 
 int ytgpu_evaluate_expression(ytgpu_context* ctx, const ytgpu_column_view* columns, uint32_t column_count,
@@ -870,7 +874,60 @@ int ytgpu_evaluate_expression(ytgpu_context* ctx, const ytgpu_column_view* colum
  * the program reads; no byte outside the heap is read), a result value longer than 2^32 - 1 bytes, out_heap_capacity
  * below the heap size (which is still written), a null out_heap_bytes with a STRING result.  YTGPU_ERR_UNSUPPORTED: a
  * numeric op over a STRING, a non-ASCII LOWER / UPPER operand, a CONCAT / LOWER / UPPER result under FARM_HASH.  After a
- * failure the outputs' contents are unspecified. */
+ * failure the outputs' contents are unspecified.
+ *
+ * Predicates inside expressions (`sum(if(status in (200, 201, 204), 1, 0))`, `group by url like '%/api/%'`,
+ * `group by if(is_prefix('https://', url), 'tls', 'plain')`, `lower(agent) like '%bot%'`), taken by this entry point only
+ * (ytgpu_evaluate_expression refuses them as unknown ops), with or without string columns.  Each takes the value on top of
+ * the stack and gives a BOOLEAN; a NULL operand gives NULL, any other TRUE or FALSE.
+ *   IN                       one operand of type INT64, UINT64, DOUBLE, BOOLEAN or STRING: TRUE when it equals an entry of
+ *                            the list.  `constant` = (offset << 32) | count: count 8-byte little-endian entries at an 8-aligned
+ *                            offset of string_constants.  A number's entry is its bit pattern in the operand's type (a
+ *                            BOOLEAN's 0 or 1); a STRING's is (offset << 32) | length of its bytes in string_constants.
+ *                            Equality is COMPARE's EQ rule: a NaN operand or entry never matches, -0.0 equals +0.0; strings
+ *                            are equal byte for byte.  The list holds no NULL: write is_null(x) OR x IN (...) instead.  An
+ *                            empty list is FALSE for every non-NULL operand; duplicate entries are allowed.
+ *   STARTS_WITH              one STRING (QL is_prefix(prefix, s)): whether its first len(prefix) bytes are the prefix given
+ *                            by `constant` = (offset << 32) | length into string_constants.  An empty prefix matches
+ *                            every non-NULL value.
+ *   CONTAINS                 one STRING (QL is_substr(needle, s)): whether the needle, given as STARTS_WITH's prefix, occurs
+ *                            in it as a contiguous byte sequence.  An empty needle matches every non-NULL value.
+ *   LIKE                     one STRING: whether the WHOLE value matches the pattern given as STARTS_WITH's prefix, with the
+ *                            escape byte in `column` (0..255; -1: no escape).  NOT LIKE is LIKE followed by NOT.  Pattern
+ *                            bytes:
+ *                              %  matches any byte sequence, including the empty one;
+ *                              _  matches one character: one byte outside 0x80..0xBF, followed by any number of bytes in
+ *                                 0x80..0xBF;
+ *                              any other byte matches itself;
+ *                              with an escape byte E, E followed by any byte X matches X literally.  A pattern that ends in
+ *                              a lone E is an error.
+ *                            As a regular expression over bytes, fully matched, % is [\x00-\xff]*, _ is
+ *                            [^\x80-\xbf][\x80-\xbf]* and every other byte is itself.  Newlines are ordinary bytes and
+ *                            matching is case-sensitive.  When the value and the pattern are valid UTF-8 this is exactly
+ *                            "_ = one code point, % = any code-point sequence", the rule ClickHouse documents for LIKE.  YT
+ *                            QL's like compiles to an RE2 expression; how that treats _ on multibyte input and whether % / _
+ *                            cross a newline (RE2's dot_nl) was not read in the reference, so those two rules are unverified
+ *                            against YT QL.  Work per row is bounded as in ytgpu_evaluate_filter: at most (value length) *
+ *                            ceil(positions / 64) + segments steps, no backtracking.  CONTAINS(x) is the pattern %x% without
+ *                            wildcards.
+ * The STRING operand of IN, STARTS_WITH, CONTAINS and LIKE may be any string result (lower(concat(a, '/', b)) like 'x%'): it
+ * is matched against the bytes it would be written as, case maps applied, as COMPARE does.  These ops pass on their
+ * operand's errors, as every op but IF, AND and OR: `if(b = 0, 0, a / b) in (1, 2)` fails nowhere, `(a / b) in (1, 2)`
+ * fails where b = 0.  They consume their operand's pieces and count none toward YTGPU_EXPR_MAX_PIECES.  CONTAINS and LIKE
+ * match values shorter than 2^32 bytes: an operand of 2^32 bytes or more (a CONCAT of long values) in a row where the op
+ * is evaluated fails the call with YTGPU_ERR_INVALID_ARGUMENT, "CONTAINS / LIKE over a value of 2^32 bytes or more".  Like
+ * a value outside its heap this is an input check: it does not follow the data, so it fails in an IF branch not taken
+ * and under FALSE AND too.  STARTS_WITH and IN take any length.
+ * Limits, per call, those of ytgpu_evaluate_filter: at most YTGPU_FILTER_MAX_IN_ENTRIES (65536) IN entries over all IN
+ * nodes, YTGPU_FILTER_MAX_PATTERN_POSITIONS (256) positions per CONTAINS needle or LIKE pattern and
+ * YTGPU_FILTER_MAX_PATTERN_BYTES (32 KiB) of compiled patterns (sizes as stated there).  Lists, prefixes, needles and
+ * patterns live in string_constants, so they count against its 1 MiB.
+ * Launches: as above, one for a numeric or BOOLEAN result and five for a STRING one; the lists and compiled patterns travel
+ * in the one upload of the program.
+ * YTGPU_ERR_INVALID_ARGUMENT, besides the above: an operand type the op does not take (STARTS_WITH, CONTAINS, LIKE over a
+ * non-STRING), an IN list that is not 8-byte aligned or leaves string_constants, a STRING entry outside string_constants, a
+ * BOOLEAN entry other than 0 / 1, a prefix, needle or pattern outside string_constants, a LIKE escape outside -1..255, a
+ * pattern that ends in a lone escape byte, a limit above, a CONTAINS / LIKE operand of 2^32 bytes or more. */
 int ytgpu_evaluate_expression_strings(ytgpu_context* ctx, const ytgpu_column_view* columns, uint32_t column_count,
                                       const ytgpu_string_column* string_columns, uint32_t string_count,
                                       const uint8_t* string_constants /* host */, uint64_t string_constant_bytes,

@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import struct
 
 import numpy as np
 
@@ -171,13 +172,49 @@ class FilterNode(C.Structure):
 (EXPR_COLUMN, EXPR_CONSTANT, EXPR_ADD, EXPR_SUB, EXPR_MUL, EXPR_DIV, EXPR_MOD, EXPR_NEG, EXPR_BIT_AND, EXPR_BIT_OR, EXPR_BIT_XOR,
  EXPR_BIT_NOT, EXPR_CAST, EXPR_IF_NULL, EXPR_CONCAT, EXPR_LOWER, EXPR_UPPER, EXPR_FARM_HASH) = range(1, 19)
 (EXPR_COMPARE, EXPR_AND, EXPR_OR, EXPR_NOT, EXPR_IS_NULL, EXPR_IS_NOT_NULL, EXPR_IF) = range(19, 26)
-EXPR_STRING_OPS = (EXPR_CONCAT, EXPR_LOWER, EXPR_UPPER, EXPR_FARM_HASH)  # ytgpu_evaluate_expression_strings only
+EXPR_IN, EXPR_STARTS_WITH, EXPR_CONTAINS, EXPR_LIKE = range(26, 30)
+# ytgpu_evaluate_expression_strings only
+EXPR_STRING_OPS = (EXPR_CONCAT, EXPR_LOWER, EXPR_UPPER, EXPR_FARM_HASH)
+EXPR_PREDICATE_OPS = (EXPR_IN, EXPR_STARTS_WITH, EXPR_CONTAINS, EXPR_LIKE)
 EXPR_MAX_NODES, EXPR_MAX_DEPTH = 64, 16
 EXPR_MAX_PIECES, EXPR_MAX_HASH_OPERANDS, EXPR_MAX_STRING_CONSTANT_BYTES = 16, 16, 1 << 20
 
 
 class ExprNode(C.Structure):
     _fields_ = [("op", C.c_int32), ("column", C.c_int32), ("type", C.c_uint8), ("reserved", C.c_uint8 * 7), ("constant", C.c_uint64)]
+
+
+class ExprConstants:
+    """The string_constants of ytgpu_evaluate_expression_strings, built node by node: each method appends what a node
+    names and returns that node's `constant`.  bytes(self) is the buffer to pass."""
+
+    def __init__(self):
+        self.data = bytearray()
+
+    def __bytes__(self):
+        return bytes(self.data)
+
+    def string(self, s: bytes) -> int:
+        """A STRING CONSTANT, or the prefix / needle / pattern of STARTS_WITH, CONTAINS and LIKE."""
+        off = len(self.data)
+        self.data += s
+        return (off << 32) | len(s)
+
+    def in_list(self, values) -> int:
+        """An IN list: bytes entries for a STRING operand; otherwise numbers, an int being its bit pattern (taken mod
+        2^64, so -1 is INT64 -1) and a float a DOUBLE's.  The entries go at an 8-byte boundary, the strings before them."""
+        entries = []
+        for v in values:
+            if isinstance(v, (bytes, bytearray)):
+                entries.append(self.string(bytes(v)))
+            elif isinstance(v, float):
+                entries.append(struct.unpack("<Q", struct.pack("<d", v))[0])
+            else:
+                entries.append(int(v) & 0xFFFFFFFFFFFFFFFF)
+        self.data += bytes(-len(self.data) % 8)
+        off = len(self.data)
+        self.data += struct.pack(f"<{len(entries)}Q", *entries)
+        return (off << 32) | len(entries)
 
 
 class GroupByMultiResult(C.Structure):

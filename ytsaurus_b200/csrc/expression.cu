@@ -35,6 +35,15 @@
 // Errors follow the data: each entry carries its error kinds in a bit stack in registers (kEW bits per entry), every op
 // ORs its operands' bits, IF takes the condition's and the taken branch's, FALSE AND x / TRUE OR x drop x's, and only the
 // result's bits reach the error word.  So a program without IF / AND / OR fails on the rows it always failed on.
+//
+// Predicates inside expressions (IN, STARTS_WITH, CONTAINS, LIKE) run in instantiations of their own, chosen by the host
+// from the checked program: expression_kernel<false, true, true> for a numeric IN without strings, <true, true, true> for
+// the rest.  Programs without them launch the other three exactly as before.  The sorted IN lists (strings.cuh
+// prepare_in_list, shared with the filter) and the compiled patterns (compile_pattern) travel in the one upload; the
+// patterns and the head of the lists are staged in shared memory after everything else.  A STRING operand is consumed
+// where its pieces lie: a single piece without a case map is matched as contiguous bytes, as the filter does, a longer
+// list through PieceBytes, which walks the pieces under their case maps for the same matcher; a string IN searches
+// with pieces_compare against the constant bytes.
 #include <algorithm>
 #include <cstring>
 #include <type_traits>
@@ -53,24 +62,28 @@ namespace {
 constexpr int kExprThreads = 256;
 // Errors that follow the data: a bit stack per kind beside the NULL stack, 2 bits per entry in expression_kernel<false, true>,
 // 3 in expression_kernel<true, true>; only the result's bits fail the call.  expression_kernel<false, false> runs programs
-// without conditional ops, where every error reaches the result, so it raises them at once.  The other two are input
+// without conditional ops, where every error reaches the result, so it raises them at once.  The others are input
 // checks, raised at once.
 constexpr u32 kErrDivZero = 1, kErrIntMinByMinusOne = 2, kErrNonAscii = 4;
 constexpr u32 kErrOutOfHeap = 8, kErrTooLong = 16;
+constexpr u32 kErrMatchTooLong = 32;  // CONTAINS / LIKE over 2^32 bytes or more: the matcher counts in 32 bits
 constexpr u32 kModeValues = 0, kModeSize = 1, kModeFill = 2;  // a 64-bit result; a STRING result's two passes
 constexpr u32 kCaseLower = 1, kCaseUpper = 2;
 constexpr u32 kShortValue = 48;                                        // longer values are copied by the whole warp
 constexpr u32 kStageBytes = 32 * kShortValue + 16;                     // a warp's short values and the 16-byte skew
+constexpr u32 kStagedListEntries = 1024;                               // IN entries kept in shared memory per CTA (8 KB)
 
 struct ExprNodeDev {
     u8 op;
     u8 type;  // the node's result type
-    u8 from;  // CAST, COMPARE, IS_NULL, IS_NOT_NULL: the operand's type
+    u8 from;  // CAST, COMPARE, IS_NULL, IS_NOT_NULL, IN: the operand's type
     u8 pad;
     u16 col;  // COLUMN: compact column table (referenced columns only; a STRING leaf: the compact string table);
               // FARM_HASH: its operand count; COMPARE: the ytgpu_cmp_op
     u16 pad2;
-    u64 constant;  // CONSTANT: the bit pattern, a STRING one (offset << 32) | length; FARM_HASH: bit j = operand j is a STRING
+    u64 constant;  // CONSTANT: the bit pattern, a STRING one (offset << 32) | length; FARM_HASH: bit j = operand j is a STRING;
+                   // IN: (first entry in lists << 32) | entries; STARTS_WITH: the prefix as a STRING CONSTANT;
+                   // CONTAINS, LIKE: the compiled pattern's offset in patterns
 };
 static_assert(sizeof(ExprNodeDev) == 16, "ExprNodeDev layout");
 
@@ -95,6 +108,16 @@ struct ExprArgs {
     u32* lengths;
     u8* null_bytes;
     u8* heap;
+};
+
+// expression_pred_kernel only.  A parameter of its own: ExprArgs grown past 128 bytes changed how the compiler reads it,
+// and with that the code of the other kernels.
+struct PredArgs {
+    const u64* lists;             // the sorted IN entries (strings.cuh prepare_in_list), node by node
+    const u8* patterns;           // the compiled CONTAINS / LIKE patterns, node by node
+    u32 staged_list;              // entries of lists staged in shared memory
+    u32 pattern_bytes;            // a multiple of 16, all staged
+    u32 pred_smem;                // the shared-memory offset (16-aligned) of the staged patterns, then the staged entries
 };
 
 __device__ __forceinline__ double as_double(u64 x) { return __longlong_as_double((long long)x); }
@@ -189,11 +212,13 @@ __device__ __forceinline__ void warp_copy(u8* dst, const u8* src, u64 len, u32 c
 }
 
 // A STRING COMPARE: the pieces [a, a + na) against [b, b + nb) of this thread's piece stack (pptr / plen: its entry 0,
-// stride kExprThreads), byte by byte under their case maps: unsigned bytes, then the shorter value first.
-__device__ __forceinline__ int pieces_compare(const u64* pptr, const u32* plen, u32 cases, u32 a, u32 na, u32 b, u32 nb) {
+// stride kExprThreads), byte by byte under their case maps: unsigned bytes, then the shorter value first.  With nb = 0 the
+// right-hand side is the lb contiguous bytes at pb instead (a constant).
+__device__ __forceinline__ int pieces_compare(const u64* pptr, const u32* plen, u32 cases, u32 a, u32 na, u32 b, u32 nb,
+                                              const u8* pb = nullptr, u32 lb = 0) {
     const u32 ea = a + na, eb = b + nb;
-    const u8 *pa = nullptr, *pb = nullptr;
-    u32 la = 0, lb = 0, ca = 0, cb = 0;  // bytes left in the current pieces, their case maps
+    const u8* pa = nullptr;
+    u32 la = 0, ca = 0, cb = 0;  // bytes left in the current pieces (lb: on the right), their case maps
     for (;;) {
         while (la == 0 && a < ea) {
             pa = reinterpret_cast<const u8*>(pptr[a * kExprThreads]);
@@ -214,6 +239,27 @@ __device__ __forceinline__ int pieces_compare(const u64* pptr, const u32* plen, 
     }
 }
 
+// The bytes of the pieces p, p + 1, ... of this thread's piece stack under their case maps, in order: pattern_match's byte
+// source.  The caller asks for no more bytes than the pieces hold.
+struct PieceBytes {
+    const u64* pptr;
+    const u32* plen;
+    u32 cases;
+    u32 p;
+    const u8* cur = nullptr;
+    u32 left = 0, cm = 0;
+    __device__ __forceinline__ u32 operator()(u32) {
+        while (left == 0) {
+            cur = reinterpret_cast<const u8*>(pptr[p * kExprThreads]);
+            left = plen[p * kExprThreads];
+            cm = (cases >> (2 * p)) & 3;
+            ++p;
+        }
+        --left;
+        return case_byte(__ldg(cur++), cm);
+    }
+};
+
 __device__ __forceinline__ bool cmp_holds(u32 cmp, int c) {
     switch (cmp) {
         case YTGPU_CMP_LT: return c < 0;
@@ -227,10 +273,12 @@ __device__ __forceinline__ bool cmp_holds(u32 cmp, int c) {
 
 // kCond: the program may hold COMPARE, AND, OR, NOT, IS_NULL, IS_NOT_NULL or IF.  Without them the scalar instantiation
 // keeps the dispatch and the error handling of a program of arithmetic only (the conditional ops cost the old programs
-// 6-14 % in bench_expressions.py when compiled in); the string one always takes them.
-template <bool kStrings, bool kCond>
-__global__ void __launch_bounds__(kExprThreads) expression_kernel(const ExprArgs A) {
+// 6-14 % in bench_expressions.py when compiled in); the string one always takes them.  kPred: the program may hold IN,
+// STARTS_WITH, CONTAINS or LIKE (the string ones with kStrings only), so the other instantiations do not carry them.
+template <bool kStrings, bool kCond, bool kPred>
+__device__ __forceinline__ void expression_body(const ExprArgs& A, const PredArgs& Q) {
     static_assert(kCond || !kStrings, "expression_kernel<true, false> is not instantiated");
+    static_assert(kCond || !kPred, "the predicates are conditional ops");
     // the error bit stacks: kEW bits per entry, entry d from the top at bit kEW * d (a 16-deep stack fills 32 / 48 bits)
     using ErrStack = typename std::conditional<kStrings, u64, u32>::type;
     constexpr u32 kEW = kStrings ? 3 : 2;
@@ -257,6 +305,17 @@ __global__ void __launch_bounds__(kExprThreads) expression_kernel(const ExprArgs
             dst = reinterpret_cast<u32*>(s_strs);
             for (u32 k = threadIdx.x; k < A.string_count * (u32)(sizeof(StringDev) / 4); k += blockDim.x) dst[k] = src[k];
         }
+    }
+    const u8* s_pat = nullptr;
+    const u64* s_list = nullptr;
+    if constexpr (kPred) {
+        uint4* pat = reinterpret_cast<uint4*>(smem + Q.pred_smem);
+        const uint4* psrc = reinterpret_cast<const uint4*>(Q.patterns);
+        for (u32 k = threadIdx.x; k < Q.pattern_bytes / 16; k += blockDim.x) pat[k] = psrc[k];
+        u64* list = reinterpret_cast<u64*>(smem + Q.pred_smem + Q.pattern_bytes);
+        for (u32 k = threadIdx.x; k < Q.staged_list; k += blockDim.x) list[k] = Q.lists[k];
+        s_pat = smem + Q.pred_smem;
+        s_list = list;
     }
     __syncthreads();
 
@@ -320,6 +379,58 @@ __global__ void __launch_bounds__(kExprThreads) expression_kernel(const ExprArgs
                     if (kStrings && nd.from == YTGPU_TYPE_STRING) np -= (u32)top;  // a NULL string has no pieces
                     top = (nul_stack & 1) ^ (nd.op == YTGPU_EXPR_IS_NULL ? 0u : 1u);
                     nul_stack &= ~1u;
+                } else if (kPred && nd.op == YTGPU_EXPR_IN) {
+                    // lower bound over the sorted entries, then equality on the entry found (a number: the EQ rule)
+                    const u32 first = (u32)(nd.constant >> 32), end = first + (u32)nd.constant;
+                    const bool str = kStrings && nd.from == YTGPU_TYPE_STRING;
+                    const u32 p0 = np - (str ? (u32)top : 0u);
+                    bool r = false;
+                    if (!(nul_stack & 1)) {
+                        const u64 key = str ? 0 : in_key(nd.from, top);
+                        u32 lo = first, cnt = end - first;
+                        int c = 1;
+                        while (cnt > 0) {
+                            const u32 half = cnt >> 1, mid = lo + half;
+                            const u64 e = mid < Q.staged_list ? s_list[mid] : __ldg(Q.lists + mid);
+                            const bool below = str ? pieces_compare(s_pptr, s_plen, cases, p0, (u32)top, 0, 0, A.consts + (e >> 32), (u32)e) > 0
+                                                   : e < key;
+                            if (below) {
+                                lo = mid + 1;
+                                cnt -= half + 1;
+                            } else {
+                                cnt = half;
+                            }
+                        }
+                        if (lo < end) {
+                            const u64 e = lo < Q.staged_list ? s_list[lo] : __ldg(Q.lists + lo);
+                            if (str) c = pieces_compare(s_pptr, s_plen, cases, p0, (u32)top, 0, 0, A.consts + (e >> 32), (u32)e);
+                            r = str ? c == 0 : passes(YTGPU_CMP_EQ, nd.from, top, minmax_decode(nd.from, e));
+                        }
+                    }
+                    np = p0;  // a STRING operand's pieces are dropped
+                    top = r ? 1 : 0;
+                } else if (kStrings && kPred && (nd.op == YTGPU_EXPR_STARTS_WITH || nd.op == YTGPU_EXPR_CONTAINS || nd.op == YTGPU_EXPR_LIKE)) {
+                    const u32 p0 = np - (u32)top;
+                    bool r = false;
+                    if (!(nul_stack & 1)) {
+                        u64 len = 0;
+                        for (u32 p = p0; p < np; ++p) len += s_plen[p * kExprThreads];
+                        PieceBytes src{s_pptr, s_plen, cases, p0};
+                        if (nd.op == YTGPU_EXPR_STARTS_WITH) {
+                            const u8* q = A.consts + (nd.constant >> 32);
+                            const u32 ql = (u32)nd.constant;
+                            r = len >= ql;
+                            for (u32 j = 0; r && j < ql; ++j) r = src(j) == __ldg(q + j);
+                        } else if (len > 0xffffffffull) {
+                            err |= kErrMatchTooLong;
+                        } else if (top == 1 && ((cases >> (2 * p0)) & 3) == 0) {  // one piece as it is: the filter's contiguous scan
+                            r = pattern_match(s_pat + nd.constant, reinterpret_cast<const u8*>(s_pptr[p0 * kExprThreads]), (u32)len);
+                        } else {
+                            r = pattern_match(s_pat + nd.constant, src, (u32)len);
+                        }
+                    }
+                    np = p0;
+                    top = r ? 1 : 0;
                 } else if (kStrings && (nd.op == YTGPU_EXPR_LOWER || nd.op == YTGPU_EXPR_UPPER)) {
                     if (!(nul_stack & 1)) {
                         const u32 first = np - (u32)top;
@@ -524,6 +635,18 @@ __global__ void __launch_bounds__(kExprThreads) expression_kernel(const ExprArgs
     }
 }
 
+template <bool kStrings, bool kCond>
+__global__ void __launch_bounds__(kExprThreads) expression_kernel(const ExprArgs A) {
+    expression_body<kStrings, kCond, false>(A, PredArgs{});
+}
+
+// Programs with IN, STARTS_WITH, CONTAINS or LIKE.  Left to itself ptxas keeps this kernel at the others' 32 / 64 registers
+// and spills; with this budget it has no stack frame and no spills.
+template <bool kStrings>
+__global__ void __launch_bounds__(kExprThreads) __maxnreg__(kStrings ? 80 : 40) expression_pred_kernel(const ExprArgs A, const PredArgs Q) {
+    expression_body<kStrings, true, true>(A, Q);
+}
+
 // ---- host ----
 struct CheckedExpr {
     std::vector<ExprNodeDev> nodes;
@@ -533,6 +656,9 @@ struct CheckedExpr {
     u32 max_pieces = 0;
     bool strings_kernel = false;  // a STRING node or FARM_HASH: expression_kernel<true, true>
     bool conditional = false;     // a conditional op: expression_kernel<false, true> for a scalar program
+    bool predicates = false;      // IN, STARTS_WITH, CONTAINS or LIKE: expression_kernel<*, true, true>
+    std::vector<u64> lists;       // the sorted IN entries, node by node
+    std::vector<u8> patterns;     // the compiled CONTAINS / LIKE patterns, node by node
     u8 type = 0;  // the result type
 };
 
@@ -543,8 +669,8 @@ bool is_number_type(u32 t) { return t == YTGPU_TYPE_INT64 || t == YTGPU_TYPE_UIN
 bool is_integer_type(u32 t) { return t == YTGPU_TYPE_INT64 || t == YTGPU_TYPE_UINT64; }
 
 // `strings`: the program comes through ytgpu_evaluate_expression_strings, which takes string leaves and the string ops.
-Status check_expression(const ytgpu_column_view* columns, u32 column_count, bool strings, u32 string_count, u64 const_bytes,
-                        const ytgpu_expr_node* program, u32 node_count, CheckedExpr* out) {
+Status check_expression(const ytgpu_column_view* columns, u32 column_count, bool strings, u32 string_count, const u8* consts,
+                        u64 const_bytes, const ytgpu_expr_node* program, u32 node_count, CheckedExpr* out) {
     if (node_count == 0 || node_count > (u32)YTGPU_EXPR_MAX_NODES)
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "an expression program has 1 .. %d nodes", YTGPU_EXPR_MAX_NODES);
     if (!program) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null program");
@@ -556,11 +682,13 @@ Status check_expression(const ytgpu_column_view* columns, u32 column_count, bool
     };
     std::vector<Entry> stack;
     u32 pieces = 0;  // on the whole stack
+    u64 in_entries = 0;
     for (u32 k = 0; k < node_count; ++k) {
         const ytgpu_expr_node& N = program[k];
         ExprNodeDev d{};
         d.op = (u8)N.op;
-        const bool string_op = N.op == YTGPU_EXPR_CONCAT || N.op == YTGPU_EXPR_LOWER || N.op == YTGPU_EXPR_UPPER || N.op == YTGPU_EXPR_FARM_HASH;
+        const bool string_op = N.op == YTGPU_EXPR_CONCAT || N.op == YTGPU_EXPR_LOWER || N.op == YTGPU_EXPR_UPPER || N.op == YTGPU_EXPR_FARM_HASH ||
+                               (N.op >= YTGPU_EXPR_IN && N.op <= YTGPU_EXPR_LIKE);
         if (string_op && !strings) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: unknown op %d", k, N.op);
         switch (N.op) {
             case YTGPU_EXPR_COLUMN: {
@@ -709,6 +837,60 @@ Status check_expression(const ytgpu_column_view* columns, u32 column_count, bool
                 stack.back() = {YTGPU_TYPE_BOOLEAN, 0, 0};
                 break;
             }
+            case YTGPU_EXPR_IN: {
+                if (stack.empty()) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: stack underflow", k);
+                const Entry e = stack.back();
+                const u64 off = N.constant >> 32, count = N.constant & 0xffffffffull;
+                if ((off & 7) || off > const_bytes || count * 8 > const_bytes - off)
+                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: IN list outside string_constants or not 8-byte aligned", k);
+                in_entries += count;
+                if (in_entries > (u64)YTGPU_FILTER_MAX_IN_ENTRIES)
+                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "at most %d IN entries per call", YTGPU_FILTER_MAX_IN_ENTRIES);
+                std::vector<u64> entries(count);
+                if (count) memcpy(entries.data(), consts + off, count * 8);
+                if (e.type == YTGPU_TYPE_BOOLEAN)
+                    for (u64 j = 0; j < count; ++j)
+                        if (entries[j] > 1)
+                            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: IN entry %u of a BOOLEAN list is not 0 or 1", k, (u32)j);
+                const u64 first = out->lists.size();
+                const i64 bad = prepare_in_list(e.type, entries.data(), (u32)count, consts, const_bytes, &out->lists);
+                if (bad >= 0) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: IN entry %u outside string_constants", k, (u32)bad);
+                pieces -= e.pieces;
+                d.from = e.type;
+                d.type = YTGPU_TYPE_BOOLEAN;
+                d.constant = (first << 32) | (out->lists.size() - first);
+                stack.back() = {YTGPU_TYPE_BOOLEAN, 0, 0};
+                break;
+            }
+            case YTGPU_EXPR_STARTS_WITH:
+            case YTGPU_EXPR_CONTAINS:
+            case YTGPU_EXPR_LIKE: {
+                if (stack.empty()) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: stack underflow", k);
+                const Entry e = stack.back();
+                if (e.type != YTGPU_TYPE_STRING)
+                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: op %d takes a STRING, not type 0x%x", k, N.op, e.type);
+                const u64 off = N.constant >> 32, len = N.constant & 0xffffffffull;
+                const bool like = N.op == YTGPU_EXPR_LIKE;
+                if (off > const_bytes || len > const_bytes - off)
+                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: %s outside string_constants", k,
+                                       like ? "pattern" : (N.op == YTGPU_EXPR_CONTAINS ? "needle" : "prefix"));
+                d.constant = N.constant;
+                if (N.op != YTGPU_EXPR_STARTS_WITH) {
+                    if (like && (N.column < -1 || N.column > 255))
+                        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: LIKE escape %d outside -1 .. 255", k, N.column);
+                    d.constant = out->patterns.size();
+                    if (const char* why = compile_pattern(consts + off, (u32)len, like, like ? N.column : -1, &out->patterns))
+                        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: %s", k, why);
+                    if (out->patterns.size() > (size_t)YTGPU_FILTER_MAX_PATTERN_BYTES)
+                        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "the patterns of a call compile to more than %d bytes",
+                                           YTGPU_FILTER_MAX_PATTERN_BYTES);
+                }
+                pieces -= e.pieces;
+                d.from = YTGPU_TYPE_STRING;
+                d.type = YTGPU_TYPE_BOOLEAN;
+                stack.back() = {YTGPU_TYPE_BOOLEAN, 0, 0};
+                break;
+            }
             case YTGPU_EXPR_ADD:
             case YTGPU_EXPR_SUB:
             case YTGPU_EXPR_MUL:
@@ -755,6 +937,7 @@ Status check_expression(const ytgpu_column_view* columns, u32 column_count, bool
         out->max_pieces = std::max(out->max_pieces, pieces);
         out->strings_kernel |= d.type == YTGPU_TYPE_STRING || N.op == YTGPU_EXPR_FARM_HASH;
         out->conditional |= N.op >= YTGPU_EXPR_COMPARE;
+        out->predicates |= N.op >= YTGPU_EXPR_IN;
         out->nodes.push_back(d);
     }
     if (stack.size() != 1)
@@ -799,7 +982,7 @@ Status evaluate_expression_impl(Context* ctx, const ytgpu_column_view* columns, 
     if (const_bytes && !consts) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null string_constants");
     if (n >= (1ull << 32)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "fewer than 2^32 rows per call");
     CheckedExpr P;
-    YTGPU_TRY(check_expression(columns, column_count, strings, string_count, const_bytes, program, node_count, &P));
+    YTGPU_TRY(check_expression(columns, column_count, strings, string_count, consts, const_bytes, program, node_count, &P));
     if (out_value_type) *out_value_type = P.type;
     if (out_null_count) *out_null_count = 0;
     const bool string_result = P.type == YTGPU_TYPE_STRING;
@@ -827,13 +1010,20 @@ Status evaluate_expression_impl(Context* ctx, const ytgpu_column_view* columns, 
         YTGPU_TRY(stage_strings(ctx, string_columns[P.strings[k]], &ss[k]));
         hs[k] = ss[k].dev;
     }
-    // one upload: nodes | column views | string views | string constants
+    // one upload: nodes | column views | string views | string constants, then with predicates, 16-byte aligned, the sorted
+    // IN entries | the compiled patterns
     const size_t nodes_b = P.nodes.size() * sizeof(ExprNodeDev), cols_b = hc.size() * sizeof(ColumnDev), strs_b = hs.size() * sizeof(StringDev);
-    std::vector<u8> blob(nodes_b + cols_b + strs_b + const_bytes);
+    auto up16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
+    const size_t base_b = nodes_b + cols_b + strs_b + const_bytes;
+    const size_t list_b = P.lists.size() * 8, pat_b = up16(P.patterns.size());  // patterns are staged in 16-byte units
+    const size_t o_list = up16(base_b), o_pat = o_list + up16(list_b);
+    std::vector<u8> blob(P.predicates ? o_pat + pat_b : base_b, 0);
     memcpy(blob.data(), P.nodes.data(), nodes_b);
     if (cols_b) memcpy(blob.data() + nodes_b, hc.data(), cols_b);
     if (strs_b) memcpy(blob.data() + nodes_b + cols_b, hs.data(), strs_b);
     if (const_bytes) memcpy(blob.data() + nodes_b + cols_b + strs_b, consts, const_bytes);
+    if (list_b) memcpy(blob.data() + o_list, P.lists.data(), list_b);
+    if (!P.patterns.empty()) memcpy(blob.data() + o_pat, P.patterns.data(), P.patterns.size());
     DevBuf<u8> dblob;
     YTGPU_TRY(dblob.allocate(ctx, blob.size()));
     YTGPU_CUDA_TRY(cudaMemcpyAsync(dblob.p, blob.data(), blob.size(), cudaMemcpyHostToDevice, ctx->stream));
@@ -897,24 +1087,36 @@ Status evaluate_expression_impl(Context* ctx, const ytgpu_column_view* columns, 
     A.starts = dstarts;
     A.lengths = dlengths;
     A.null_bytes = dnull_bytes;
+    PredArgs Q{};
+    Q.lists = reinterpret_cast<const u64*>(dblob.p + o_list);
+    Q.patterns = dblob.p + o_pat;
+    Q.staged_list = std::min<u32>((u32)P.lists.size(), kStagedListEntries);
+    Q.pattern_bytes = (u32)pat_b;
     // shared memory in the kernel's order: nodes (16 B each), column views, string views (8-byte multiples), the stack
     // below the top; expression_kernel<true, true>: the piece stack and, 16-byte aligned, a short-value stage per warp
     static_assert(sizeof(ColumnDev) % 8 == 0 && sizeof(StringDev) % 8 == 0, "shared-memory layout");
     const size_t stack_b = (size_t)(P.max_depth - 1) * kExprThreads * sizeof(u64);
     const u32 blocks = (u32)std::max<u64>(1, std::min<u64>((words * 32 + kExprThreads - 1) / kExprThreads, (u64)kNumSms * 8));
-    if (!P.strings_kernel) {
-        const size_t smem = nodes_b + cols_b + stack_b;
-        KernelTimer t(ctx, KC_DECODE);
-        if (P.conditional) expression_kernel<false, true><<<blocks, kExprThreads, smem, ctx->stream>>>(A);
-        else expression_kernel<false, false><<<blocks, kExprThreads, smem, ctx->stream>>>(A);
-        YTGPU_CUDA_TRY(cudaGetLastError());
-    } else {
-        const size_t smem = nodes_b + cols_b + strs_b + stack_b + (size_t)P.max_pieces * kExprThreads * 12 + 16 +
-                            (size_t)(kExprThreads / 32) * kStageBytes;
-        // up to 16 pieces and a 16-deep stack take the stage past the 48 KB default
-        YTGPU_CUDA_TRY(cudaFuncSetAttribute(expression_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    // with predicates, after everything else at a 16-byte boundary: the compiled patterns, then the head of the IN entries
+    size_t smem = P.strings_kernel ? nodes_b + cols_b + strs_b + stack_b + (size_t)P.max_pieces * kExprThreads * 12 + 16 +
+                                         (size_t)(kExprThreads / 32) * kStageBytes
+                                   : nodes_b + cols_b + stack_b;
+    if (P.predicates) {
+        Q.pred_smem = (u32)up16(smem);
+        smem = Q.pred_smem + pat_b + (size_t)Q.staged_list * 8;
+    }
+    // the kernel of the checked program; up to 16 pieces, a 16-deep stack and the predicates' stage exceed the 48 KB default
+    void (*kernel)(ExprArgs) = P.strings_kernel ? expression_kernel<true, true> : (P.conditional ? expression_kernel<false, true> : expression_kernel<false, false>);
+    void (*pred_kernel)(ExprArgs, PredArgs) = P.strings_kernel ? expression_pred_kernel<true> : expression_pred_kernel<false>;
+    auto launch = [&] {
+        if (P.predicates) pred_kernel<<<blocks, kExprThreads, smem, ctx->stream>>>(A, Q);
+        else kernel<<<blocks, kExprThreads, smem, ctx->stream>>>(A);
+    };
+    if (P.predicates) YTGPU_CUDA_TRY(cudaFuncSetAttribute(pred_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    else if (P.strings_kernel) YTGPU_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    {
         KernelTimer t(ctx, KC_DECODE, string_result ? 4 : 1);
-        expression_kernel<true, true><<<blocks, kExprThreads, smem, ctx->stream>>>(A);
+        launch();
         if (string_result)  // starts = exclusive scan of the lengths, the total into result[2]
             exclusive_scan_u64(ctx->stream, dstarts, n, scan_sums.p, reinterpret_cast<u64*>(result.p + 2));
         YTGPU_CUDA_TRY(cudaGetLastError());
@@ -930,6 +1132,8 @@ Status evaluate_expression_impl(Context* ctx, const ytgpu_column_view* columns, 
     if (res[1] & kErrNonAscii)
         return make_status(YTGPU_ERR_UNSUPPORTED, "lower / upper of a value with a byte >= 0x80: Unicode case mapping is not on the GPU path");
     if (res[1] & kErrTooLong) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "a string result is longer than 2^32 - 1 bytes");
+    if (res[1] & kErrMatchTooLong)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "CONTAINS / LIKE over a value of 2^32 bytes or more");
     if (res[1] & kErrDivZero) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "Division by zero");
     if (res[1] & kErrIntMinByMinusOne) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "Division INT_MIN by -1");
     if (out_null_count) *out_null_count = res[0];
@@ -949,10 +1153,8 @@ Status evaluate_expression_impl(Context* ctx, const ytgpu_column_view* columns, 
     A.mode = kModeFill;
     A.heap = dheap;
     {
-        const size_t smem = nodes_b + cols_b + strs_b + stack_b + (size_t)P.max_pieces * kExprThreads * 12 + 16 +
-                            (size_t)(kExprThreads / 32) * kStageBytes;
         KernelTimer t(ctx, KC_GATHER);
-        expression_kernel<true, true><<<blocks, kExprThreads, smem, ctx->stream>>>(A);
+        launch();
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
     if (host) {

@@ -69,12 +69,6 @@ struct FilterArgs {
     unsigned long long* result;  // [0] selected count, [1] error bits
 };
 
-// A value canonicalised for the IN search: -0.0 becomes +0.0 (the EQ rule says they are equal).
-__host__ __device__ __forceinline__ u64 in_key(u8 vtype, u64 bits) {
-    if (vtype == YTGPU_TYPE_DOUBLE && bits == 0x8000000000000000ull) bits = 0;
-    return minmax_encode(vtype, bits);
-}
-
 __device__ __forceinline__ bool cmp_holds(int op, int c) {
     switch (op) {
         case YTGPU_CMP_LT: return c < 0;
@@ -388,28 +382,10 @@ Status check_program(const ytgpu_column_view* columns, u32 column_count, u32 str
                 in_entries += N.length;
                 if (in_entries > (u64)YTGPU_FILTER_MAX_IN_ENTRIES)
                     return make_status(YTGPU_ERR_INVALID_ARGUMENT, "at most %d IN entries per call", YTGPU_FILTER_MAX_IN_ENTRIES);
-                const u64* e = list_values + N.constant;
-                std::vector<u64> sorted;
-                sorted.reserve(N.length);
-                if (str) {
-                    for (u32 j = 0; j < N.length; ++j) {
-                        if (!string_range_ok(e[j] >> 32, e[j] & 0xffffffffu))
-                            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: IN entry %u outside string_constants", k, j);
-                        sorted.push_back(e[j]);
-                    }
-                    auto bytes = [&](u64 x) { return std::string(reinterpret_cast<const char*>(consts) + (x >> 32), (size_t)(x & 0xffffffffu)); };
-                    std::sort(sorted.begin(), sorted.end(), [&](u64 a, u64 b) { return bytes(a) < bytes(b); });  // unsigned bytes
-                } else {
-                    for (u32 j = 0; j < N.length; ++j) {
-                        const u64 x = e[j];
-                        if (vtype == YTGPU_TYPE_DOUBLE && (x & 0x7fffffffffffffffull) > 0x7ff0000000000000ull) continue;  // NaN never matches
-                        sorted.push_back(in_key(vtype, x));
-                    }
-                    std::sort(sorted.begin(), sorted.end());
-                }
                 d.constant = out->lists.size();
-                d.length = (u32)sorted.size();
-                out->lists.insert(out->lists.end(), sorted.begin(), sorted.end());
+                const i64 bad = prepare_in_list(vtype, list_values + N.constant, N.length, consts, const_bytes, &out->lists);
+                if (bad >= 0) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: IN entry %u outside string_constants", k, (u32)bad);
+                d.length = (u32)(out->lists.size() - d.constant);
                 break;
             }
             default:  // IS_NULL / IS_NOT_NULL

@@ -1,12 +1,14 @@
 // strings.cuh — a flat string column (ytgpu_string_column) on the device: bounds-checked value access, QL string order
 // and the upload of HOST columns.  Shared by the string aggregates of groupby_multi.cu and the WHERE evaluator of
-// filter.cu, and the LIKE / substring matcher of filter.cu.  Everything is TU-local (anonymous namespace) so several .cu
+// filter.cu, and the LIKE / substring matcher and the IN lists of filter.cu and expression.cu.  Everything is TU-local (anonymous namespace) so several .cu
 // files may include it.
 #pragma once
 
 #include <algorithm>
+#include <string>
 #include <vector>
 
+#include "columnar.cuh"
 #include "common.cuh"
 #include "context.cuh"
 #include "keys.cuh"
@@ -90,12 +92,20 @@ constexpr u32 kPatternAnchorStart = 1, kPatternAnchorEnd = 2;
 constexpr u32 kPatternMaxWords = (YTGPU_FILTER_MAX_PATTERN_POSITIONS + 63) / 64;
 static_assert(sizeof(PatternHead) == 16 && sizeof(PatternSeg) == 8, "compiled pattern layout");
 
-// Whether the value s[0, len) matches the compiled pattern at pat (8-byte aligned).  Every middle segment takes its
+// The bytes of a contiguous value, for pattern_match.
+struct ContiguousBytes {
+    const u8* s;
+    __device__ __forceinline__ u32 operator()(u32 j) { return __ldg(s + j); }
+};
+
+// Whether the value of len bytes matches the compiled pattern at pat (8-byte aligned).  Every middle segment takes its
 // earliest end: the % that follows it absorbs any gap, so a later end never admits a match an earlier one does not.  The
 // first segment is anchored at 0 when the pattern has no leading %, the last must end at len when it has no trailing %.
 // Each value byte is read by at most one segment scan: at most len * W + segments steps.  kWords >= the pattern's W.
-template <u32 kWords>
-__device__ __forceinline__ bool pattern_match_words(const u8* pat, const u8* s, u32 len) {
+// src(j) is byte j of the value; the scan asks for j = 0, 1, 2, ... in order, each at most once, so a source may walk a
+// list of pieces instead of indexing (ContiguousBytes for a flat value, expression.cu's piece walk).
+template <u32 kWords, class Src>
+__device__ __forceinline__ bool pattern_match_words(const u8* pat, Src& src, u32 len) {
     const PatternHead h = *reinterpret_cast<const PatternHead*>(pat);
     const u8* class_of = pat + sizeof(PatternHead);
     const PatternSeg* segs = reinterpret_cast<const PatternSeg*>(class_of + 256);
@@ -119,7 +129,7 @@ __device__ __forceinline__ bool pattern_match_words(const u8* pat, const u8* s, 
         bool accept = false;
         u32 j = pos;
         while (j < len) {
-            const u32 b = __ldg(s + j);
+            const u32 b = src(j);
             const u64* t = table + (u32)class_of[b] * h.words;
             const u64 loop = (b & 0xC0) == 0x80 ? ~0ull : 0;
             const bool inject = !anchored || j == pos;
@@ -150,10 +160,16 @@ __device__ __forceinline__ bool pattern_match_words(const u8* pat, const u8* s, 
 }
 
 // A pattern of at most 64 positions (every CONTAINS needle of up to 64 bytes, most LIKE patterns) runs the one-word scan.
-__device__ __forceinline__ bool pattern_match(const u8* pat, const u8* s, u32 len) {
+template <class Src>
+__device__ __forceinline__ bool pattern_match(const u8* pat, Src& src, u32 len) {
     const PatternHead h = *reinterpret_cast<const PatternHead*>(pat);
     if (h.segments == 0) return h.flags == 0 || len == 0;  // all %: any value; the empty pattern: the empty value
-    return h.words == 1 ? pattern_match_words<1>(pat, s, len) : pattern_match_words<kPatternMaxWords>(pat, s, len);
+    return h.words == 1 ? pattern_match_words<1>(pat, src, len) : pattern_match_words<kPatternMaxWords>(pat, src, len);
+}
+
+__device__ __forceinline__ bool pattern_match(const u8* pat, const u8* s, u32 len) {
+    ContiguousBytes src{s};
+    return pattern_match(pat, src, len);
 }
 
 // Compiles a LIKE pattern (like = true; escape -1 or 0..255) or a CONTAINS needle (like = false: the pattern %needle%
@@ -227,6 +243,40 @@ inline const char* compile_pattern(const u8* p, u32 len, bool like, int escape, 
     put(any1.data(), any1.size() * 8);
     put(table.data(), table.size() * 8);
     return nullptr;
+}
+
+// ---- IN lists (semantics in ytgpu.h, YTGPU_FILTER_IN and YTGPU_EXPR_IN) ----
+// A value canonicalised for the IN search: -0.0 becomes +0.0 (the EQ rule says they are equal).
+__host__ __device__ __forceinline__ u64 in_key(u8 vtype, u64 bits) {
+    if (vtype == YTGPU_TYPE_DOUBLE && bits == 0x8000000000000000ull) bits = 0;
+    return minmax_encode(vtype, bits);
+}
+
+// Appends the count entries e[] of an IN list over vtype to *out, sorted for the device's binary search: a number's
+// in_key words ascending, NaN entries dropped (they never match); a STRING's (offset << 32) | length entries in unsigned
+// byte order of consts[offset, offset + length).  Returns -1, or the index of a STRING entry outside the const_bytes
+// bytes of consts.
+inline i64 prepare_in_list(u8 vtype, const u64* e, u32 count, const u8* consts, u64 const_bytes, std::vector<u64>* out) {
+    std::vector<u64> sorted;
+    sorted.reserve(count);
+    if (vtype == YTGPU_TYPE_STRING) {
+        for (u32 j = 0; j < count; ++j) {
+            const u64 off = e[j] >> 32, len = e[j] & 0xffffffffu;
+            if (off > const_bytes || len > const_bytes - off) return j;
+            sorted.push_back(e[j]);
+        }
+        auto bytes = [&](u64 x) { return std::string(reinterpret_cast<const char*>(consts) + (x >> 32), (size_t)(x & 0xffffffffu)); };
+        std::sort(sorted.begin(), sorted.end(), [&](u64 a, u64 b) { return bytes(a) < bytes(b); });  // unsigned bytes
+    } else {
+        for (u32 j = 0; j < count; ++j) {
+            const u64 x = e[j];
+            if (vtype == YTGPU_TYPE_DOUBLE && (x & 0x7fffffffffffffffull) > 0x7ff0000000000000ull) continue;  // NaN never matches
+            sorted.push_back(in_key(vtype, x));
+        }
+        std::sort(sorted.begin(), sorted.end());
+    }
+    out->insert(out->end(), sorted.begin(), sorted.end());
+    return -1;
 }
 
 // A string column on the device (HOST inputs are uploaded).

@@ -855,8 +855,9 @@ class GpuContext:
         memory flavour: values n uint64 (int64 on the device), null_bitmap 8 * ceil(n / 64) bytes; `column` is a Column
         over them (without the bitmap when no row is NULL), ready for scan_filter_groupby_multi / evaluate_filter.
         string_columns: (heap, starts, lengths, nulls or None) per column, node column len(columns) + i naming string column
-        i; a STRING constant is (offset << 32) | length into string_constants.  With either, a string op in the program, or a
-        STRING constant in a program with a conditional op, the call is ytgpu_evaluate_expression_strings, made twice: a type and size query, then the call that fills the outputs
+        i; a STRING constant is (offset << 32) | length into string_constants (capi.ExprConstants builds it, IN lists and
+        patterns included).  With either, a string op or an IN / STARTS_WITH / CONTAINS / LIKE in the program, or a STRING
+        constant in a program with a conditional op, the call is ytgpu_evaluate_expression_strings, made twice: a type and size query, then the call that fills the outputs
         of that type, so a STRING result runs its size pass twice (a caller that knows the heap size calls the library once).
         A STRING result comes back as heap / starts / lengths / null_bytemap (values, null_bitmap and column None), ready
         for evaluate_filter's string_columns and string_value_ids."""
@@ -882,11 +883,14 @@ class GpuContext:
         words = (n + 63) // 64
         vtype, nulls = C.c_uint8(0), C.c_uint64(0)
         err = capi.Error()
-        # the string entry point for string columns, constants bytes or ops; a program with a conditional op also for a STRING
+        # the string entry point for string columns, constants bytes, string ops or predicates; a program with a conditional
+        # op also for a STRING
         # constant (`x = ''`, `if(c, '', '')` name no bytes).  Programs of the earlier ops route as they always have.
         ops = [nodes[i].op for i in range(len(program))]
         conditional = any(op >= capi.EXPR_COMPARE for op in ops)
-        strings = (bool(string_columns) or len(string_constants) > 0 or any(op in capi.EXPR_STRING_OPS for op in ops) or
+        string_constants = bytes(string_constants)
+        strings = (bool(string_columns) or len(string_constants) > 0 or
+                   any(op in capi.EXPR_STRING_OPS or op in capi.EXPR_PREDICATE_OPS for op in ops) or
                    (conditional and any(nodes[i].op == capi.EXPR_CONSTANT and nodes[i].type == int(EValueType.String)
                                         for i in range(len(program)))))
         if not strings:
