@@ -272,7 +272,10 @@ int ytgpu_peer_buffer_close(ytgpu_context* ctx, void* dev_ptr, ytgpu_error* err)
 /* Fused slab scatter + exchange.  `in` (DEVICE) holds the rows, partition_index (DEVICE) their partitions as returned
  * by ytgpu_partition_fixed_rows, partition_rows (host) the rows per partition.  Partition p's rows are written in
  * stable order to dest_base[p] (host array of device pointers: local memory or peer-mapped receive buffers).
- * Returns after the kernel completed on this GPU; a cross-rank barrier makes the data visible to its readers. */
+ * partition_count is in [1, 4096]; in->rows and every dest_base[p] are 16-byte aligned.  An index outside
+ * [0, partition_count) or partition_rows that disagree with the index fail with YTGPU_ERR_INVALID_ARGUMENT before any
+ * row is written.  Returns after the kernel completed on this GPU; a cross-rank barrier makes the data visible to its
+ * readers. */
 int ytgpu_scatter_rows_to_peers(ytgpu_context* ctx, const ytgpu_fixed_rows_view* in, const int32_t* partition_index,
                                 int32_t partition_count, const uint64_t* partition_rows, void* const* dest_base,
                                 ytgpu_error* err);

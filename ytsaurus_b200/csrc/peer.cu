@@ -18,16 +18,40 @@ namespace {
 
 constexpr int kMaxScatterPartitions = 4096;
 
-// out position j (rows grouped by partition, stable) -> partition p with start[p] <= j < start[p+1].
+// Rows per partition of the caller-supplied index (per-block shared histogram, then global atomics); a value outside
+// [0, parts) is flagged instead of counted.
+__global__ void __launch_bounds__(256) count_partitions_kernel(const i32* __restrict__ index, u64 n, u32 parts,
+                                                               unsigned long long* __restrict__ counts, u32* __restrict__ err_word) {
+    extern __shared__ u32 s_cnt[];  // [parts]
+    for (u32 i = threadIdx.x; i < parts; i += blockDim.x) s_cnt[i] = 0;
+    __syncthreads();
+    for (u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (u64)gridDim.x * blockDim.x) {
+        const u32 p = (u32)index[r];
+        if (p < parts) atomicAdd(&s_cnt[p], 1u);
+        else atomicOr(err_word, (u32)DE_BAD_PARTITION_INDEX);
+    }
+    __syncthreads();
+    for (u32 i = threadIdx.x; i < parts; i += blockDim.x)
+        if (s_cnt[i]) atomicAdd(&counts[i], (unsigned long long)s_cnt[i]);
+}
+
+// The counted rows of every partition must equal what the caller reserved for it (start[p + 1] - start[p]).
+__global__ void __launch_bounds__(256) check_partition_counts_kernel(const unsigned long long* __restrict__ counts, u32 parts,
+                                                                     const u64* __restrict__ start, u32* __restrict__ err_word) {
+    const u32 p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p < parts && counts[p] != start[p + 1] - start[p]) atomicOr(err_word, (u32)DE_BAD_PARTITION_INDEX);
+}
+
+// out position j (rows grouped by partition, stable) -> partition p with start[p] <= j < start[p+1].  Only start[] is
+// staged in shared memory (32 KiB at 4096 partitions, under the default 48 KiB dynamic limit); the destination pointer
+// is read from global memory, through the read-only cache.
 template <int UNROLL>
 __global__ void __launch_bounds__(256) scatter_rows_to_peers_kernel(const uint4* __restrict__ in, const SortPlan* plan,
                                                                     const u32* __restrict__ pa, const u32* __restrict__ pb,
                                                                     u64 n, u32 gr, u32 parts, const u64* __restrict__ start,
                                                                     uint4* const* __restrict__ dest) {
     extern __shared__ u64 s_start[];  // [parts + 1]
-    uint4** s_dest = reinterpret_cast<uint4**>(s_start + parts + 1);
     for (u32 i = threadIdx.x; i <= parts; i += blockDim.x) s_start[i] = start[i];
-    for (u32 i = threadIdx.x; i < parts; i += blockDim.x) s_dest[i] = dest[i];
     __syncthreads();
     const u32 f = plan->final_idx;
     const u32* perm = f == 1 ? pb : pa;
@@ -50,7 +74,7 @@ __global__ void __launch_bounds__(256) scatter_rows_to_peers_kernel(const uint4*
                     u32 half = cnt >> 1;
                     if (s_start[lo + half] <= j) { lo += half; cnt -= half; } else cnt = half;
                 }
-                dst[k] = s_dest[lo] + (j - s_start[lo]) * gr + g;
+                dst[k] = dest[lo] + (j - s_start[lo]) * gr + g;
             }
         }
 #pragma unroll
@@ -102,12 +126,18 @@ Status scatter_stream(Context* ctx, const ytgpu_fixed_rows_view* in, const i32* 
 
 Status scatter_impl(Context* ctx, const ytgpu_fixed_rows_view* in, const i32* index, i32 parts, const u64* part_rows,
                     void* const* dest_base) {
-    if (!in || !index || !part_rows || !dest_base) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null argument");
+    // an empty input may come with a null index: an empty CUDA tensor has no storage
+    if (!in || (!index && in->row_count) || !part_rows || !dest_base) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null argument");
     if (in->mem != YTGPU_MEM_DEVICE) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "peer scatter needs device-resident rows");
     if (parts <= 0 || parts > kMaxScatterPartitions) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "partition_count must be in [1, %d]", kMaxScatterPartitions);
     const u64 n = in->row_count;
     const u32 rb = in->row_bytes;
     if (rb == 0 || rb % 16) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "row_bytes must be a positive multiple of 16");
+    // both paths move rows as 16-byte vectors: a misaligned pointer (a tensor slice, say) would fault
+    if (reinterpret_cast<uintptr_t>(in->rows) % 16) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "rows must be 16-byte aligned");
+    for (i32 p = 0; p < parts; ++p)
+        if (reinterpret_cast<uintptr_t>(dest_base[p]) % 16)
+            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "destination of partition %d must be 16-byte aligned", p);
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
     std::vector<u64> start(parts + 1, 0);
     for (i32 p = 0; p < parts; ++p) start[p + 1] = start[p] + part_rows[p];
@@ -124,6 +154,18 @@ Status scatter_impl(Context* ctx, const ytgpu_fixed_rows_view* in, const i32* in
     YTGPU_TRY(ddest.allocate(ctx, parts));
     YTGPU_CUDA_TRY(cudaMemcpyAsync(dstart.p, start.data(), (parts + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
     YTGPU_CUDA_TRY(cudaMemcpyAsync(ddest.p, dest_base, parts * sizeof(void*), cudaMemcpyHostToDevice, ctx->stream));
+    {
+        DevBuf<unsigned long long> counts;
+        YTGPU_TRY(counts.allocate(ctx, parts));
+        YTGPU_CUDA_TRY(cudaMemsetAsync(counts.p, 0, parts * sizeof(unsigned long long), ctx->stream));
+        KernelTimer t(ctx, KC_PARTITION, 2);
+        const u32 grid = (u32)std::min<u64>((n + 255) / 256, (u64)kNumSms * 4);
+        count_partitions_kernel<<<grid, 256, parts * sizeof(u32), ctx->stream>>>(index, n, (u32)parts, counts.p, ctx->dev_err);
+        check_partition_counts_kernel<<<(parts + 255) / 256, 256, 0, ctx->stream>>>(counts.p, (u32)parts, dstart.p, ctx->dev_err);
+        YTGPU_CUDA_TRY(cudaGetLastError());
+    }
+    // as on the stream path: caller-supplied indices / counts are validated before any row is written
+    YTGPU_TRY(check_device_errors(ctx));
     YTGPU_TRY(widen_index(ctx, index, n, chunk.p));
     SortScratch scratch;
     PermRef perm;
@@ -135,7 +177,7 @@ Status scatter_impl(Context* ctx, const ytgpu_fixed_rows_view* in, const i32* in
         const u32 gr = rb / 16;
         const u64 items = (n * gr + UNROLL - 1) / UNROLL;
         const u32 grid = (u32)std::max<u64>(1, std::min<u64>((items + 255) / 256, (u64)kNumSms * 8));
-        const size_t smem = (size_t)(parts + 1) * 8 + (size_t)parts * sizeof(void*);
+        const size_t smem = (size_t)(parts + 1) * 8;
         scatter_rows_to_peers_kernel<UNROLL><<<grid, 256, smem, ctx->stream>>>(
             reinterpret_cast<const uint4*>(in->rows), perm.plan, perm.idx[0], perm.idx[1], n, gr, (u32)parts, dstart.p,
             reinterpret_cast<uint4* const*>(ddest.p));
