@@ -43,17 +43,16 @@
 // patterns and the head of the lists are staged in shared memory after everything else.  A STRING operand is consumed
 // where its pieces lie: a single piece without a case map is matched as contiguous bytes, as the filter does, a longer
 // list through PieceBytes, which walks the pieces under their case maps for the same matcher; a string IN searches
-// with pieces_compare against the constant bytes.
+// with pieces_compare against the constant bytes.  The column checks, compact column tables, staging and upload are
+// program.cuh's, shared with filter.cu; the kernel's prologue and IN search stay here, as shared helpers changed its code.
 #include <algorithm>
 #include <cstring>
 #include <type_traits>
 #include <vector>
 
-#include "columnar.cuh"
-#include "context.cuh"
 #include "farmhash.cuh"
+#include "program.cuh"
 #include "scan.cuh"
-#include "strings.cuh"
 
 using namespace ytgpu;
 
@@ -71,7 +70,6 @@ constexpr u32 kModeValues = 0, kModeSize = 1, kModeFill = 2;  // a 64-bit result
 constexpr u32 kCaseLower = 1, kCaseUpper = 2;
 constexpr u32 kShortValue = 48;                                        // longer values are copied by the whole warp
 constexpr u32 kStageBytes = 32 * kShortValue + 16;                     // a warp's short values and the 16-byte skew
-constexpr u32 kStagedListEntries = 1024;                               // IN entries kept in shared memory per CTA (8 KB)
 
 struct ExprNodeDev {
     u8 op;
@@ -259,17 +257,6 @@ struct PieceBytes {
         return case_byte(__ldg(cur++), cm);
     }
 };
-
-__device__ __forceinline__ bool cmp_holds(u32 cmp, int c) {
-    switch (cmp) {
-        case YTGPU_CMP_LT: return c < 0;
-        case YTGPU_CMP_LE: return c <= 0;
-        case YTGPU_CMP_GT: return c > 0;
-        case YTGPU_CMP_GE: return c >= 0;
-        case YTGPU_CMP_EQ: return c == 0;
-        default: return c != 0;
-    }
-}
 
 // kCond: the program may hold COMPARE, AND, OR, NOT, IS_NULL, IS_NOT_NULL or IF.  Without them the scalar instantiation
 // keeps the dispatch and the error handling of a program of arithmetic only (the conditional ops cost the old programs
@@ -650,8 +637,7 @@ __global__ void __launch_bounds__(kExprThreads) __maxnreg__(kStrings ? 80 : 40) 
 // ---- host ----
 struct CheckedExpr {
     std::vector<ExprNodeDev> nodes;
-    std::vector<u32> cols;     // compact slot -> caller column
-    std::vector<u32> strings;  // compact string slot -> caller string column
+    SlotMap cols, strings;  // the referenced columns' compact tables
     u32 max_depth = 0;
     u32 max_pieces = 0;
     bool strings_kernel = false;  // a STRING node or FARM_HASH: expression_kernel<true, true>
@@ -662,9 +648,6 @@ struct CheckedExpr {
     u8 type = 0;  // the result type
 };
 
-bool is_expr_type(u32 t) {
-    return t == YTGPU_TYPE_INT64 || t == YTGPU_TYPE_UINT64 || t == YTGPU_TYPE_DOUBLE || t == YTGPU_TYPE_BOOLEAN;
-}
 bool is_number_type(u32 t) { return t == YTGPU_TYPE_INT64 || t == YTGPU_TYPE_UINT64 || t == YTGPU_TYPE_DOUBLE; }
 bool is_integer_type(u32 t) { return t == YTGPU_TYPE_INT64 || t == YTGPU_TYPE_UINT64; }
 
@@ -674,7 +657,6 @@ Status check_expression(const ytgpu_column_view* columns, u32 column_count, bool
     if (node_count == 0 || node_count > (u32)YTGPU_EXPR_MAX_NODES)
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "an expression program has 1 .. %d nodes", YTGPU_EXPR_MAX_NODES);
     if (!program) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null program");
-    std::vector<int> slot_of(column_count, -1), string_slot_of(string_count, -1);
     struct Entry {
         u8 type;
         u8 plain;     // STRING: one piece without a case map at most (a leaf, a constant or IF_NULL of those)
@@ -695,26 +677,17 @@ Status check_expression(const ytgpu_column_view* columns, u32 column_count, bool
                 if (N.column < 0 || (u64)N.column >= (u64)column_count + (strings ? string_count : 0))
                     return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: column %d out of range", k, N.column);
                 if ((u32)N.column >= column_count) {  // string_columns[column - column_count]
-                    const u32 s = (u32)N.column - column_count;
-                    if (string_slot_of[s] < 0) {
-                        string_slot_of[s] = (int)out->strings.size();
-                        out->strings.push_back(s);
-                    }
-                    d.col = (u16)string_slot_of[s];
+                    d.col = out->strings.slot((u32)N.column - column_count);
                     d.type = YTGPU_TYPE_STRING;
                     stack.push_back({YTGPU_TYPE_STRING, 1, 1});
                     ++pieces;
                     break;
                 }
                 const u8 t = columns[N.column].value_type;
-                if (!is_expr_type(t))
+                if (!is_scalar_type(t))
                     return make_status(YTGPU_ERR_UNSUPPORTED, "node %u: column %d has value type 0x%x (INT64, UINT64, DOUBLE or BOOLEAN)", k,
                                        N.column, t);
-                if (slot_of[N.column] < 0) {
-                    slot_of[N.column] = (int)out->cols.size();
-                    out->cols.push_back((u32)N.column);
-                }
-                d.col = (u16)slot_of[N.column];
+                d.col = out->cols.slot((u32)N.column);
                 d.type = t;
                 stack.push_back({t, 0, 0});
                 break;
@@ -730,7 +703,7 @@ Status check_expression(const ytgpu_column_view* columns, u32 column_count, bool
                     ++pieces;
                     break;
                 }
-                if (!is_expr_type(N.type)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: unknown constant type 0x%x", k, N.type);
+                if (!is_scalar_type(N.type)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: unknown constant type 0x%x", k, N.type);
                 if (N.type == YTGPU_TYPE_BOOLEAN && N.constant > 1)
                     return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: a BOOLEAN constant is 0 or 1", k);
                 d.type = N.type;
@@ -843,18 +816,14 @@ Status check_expression(const ytgpu_column_view* columns, u32 column_count, bool
                 const u64 off = N.constant >> 32, count = N.constant & 0xffffffffull;
                 if ((off & 7) || off > const_bytes || count * 8 > const_bytes - off)
                     return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: IN list outside string_constants or not 8-byte aligned", k);
-                in_entries += count;
-                if (in_entries > (u64)YTGPU_FILTER_MAX_IN_ENTRIES)
-                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "at most %d IN entries per call", YTGPU_FILTER_MAX_IN_ENTRIES);
                 std::vector<u64> entries(count);
                 if (count) memcpy(entries.data(), consts + off, count * 8);
-                if (e.type == YTGPU_TYPE_BOOLEAN)
+                const u64 first = out->lists.size();
+                YTGPU_TRY(add_in_list(k, e.type, entries.data(), (u32)count, consts, const_bytes, &in_entries, &out->lists));
+                if (e.type == YTGPU_TYPE_BOOLEAN)  // after add_in_list: its entry limit is checked first, and it takes any bits
                     for (u64 j = 0; j < count; ++j)
                         if (entries[j] > 1)
                             return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: IN entry %u of a BOOLEAN list is not 0 or 1", k, (u32)j);
-                const u64 first = out->lists.size();
-                const i64 bad = prepare_in_list(e.type, entries.data(), (u32)count, consts, const_bytes, &out->lists);
-                if (bad >= 0) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: IN entry %u outside string_constants", k, (u32)bad);
                 pieces -= e.pieces;
                 d.from = e.type;
                 d.type = YTGPU_TYPE_BOOLEAN;
@@ -876,14 +845,8 @@ Status check_expression(const ytgpu_column_view* columns, u32 column_count, bool
                                        like ? "pattern" : (N.op == YTGPU_EXPR_CONTAINS ? "needle" : "prefix"));
                 d.constant = N.constant;
                 if (N.op != YTGPU_EXPR_STARTS_WITH) {
-                    if (like && (N.column < -1 || N.column > 255))
-                        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: LIKE escape %d outside -1 .. 255", k, N.column);
                     d.constant = out->patterns.size();
-                    if (const char* why = compile_pattern(consts + off, (u32)len, like, like ? N.column : -1, &out->patterns))
-                        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: %s", k, why);
-                    if (out->patterns.size() > (size_t)YTGPU_FILTER_MAX_PATTERN_BYTES)
-                        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "the patterns of a call compile to more than %d bytes",
-                                           YTGPU_FILTER_MAX_PATTERN_BYTES);
+                    YTGPU_TRY(add_pattern(k, consts + off, (u32)len, like, like ? N.column : -1, &out->patterns));
                 }
                 pieces -= e.pieces;
                 d.from = YTGPU_TYPE_STRING;
@@ -961,26 +924,11 @@ Status evaluate_expression_impl(Context* ctx, const ytgpu_column_view* columns, 
                                 const ytgpu_expr_node* program, u32 node_count, const u8* selection, u64* out_values, u8* out_null_bitmap,
                                 u8* out_value_type, u64* out_null_count, int out_mem) {
     const bool strings = sr != nullptr;  // the string entry point
-    if ((column_count && !columns) || (string_count && !string_columns)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null columns");
-    if (column_count + (u64)string_count == 0) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "no columns");
-    if (out_mem != YTGPU_MEM_DEVICE && out_mem != YTGPU_MEM_HOST)
-        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "out_mem must be YTGPU_MEM_DEVICE or YTGPU_MEM_HOST");
-    const u64 n = column_count ? (u64)columns[0].value_count : string_columns[0].row_count;
-    for (u32 c = 0; c < column_count; ++c)
-        if (columns[c].value_count < 0 || (u64)columns[c].value_count != n)
-            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "column %u differs in length", c);
-    for (u32 s = 0; s < string_count; ++s) {
-        const ytgpu_string_column& S = string_columns[s];
-        if (S.row_count != n) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "string column %u differs in length", s);
-        if ((S.heap_bytes && !S.heap) || (n && (!S.starts || !S.lengths)))
-            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "string column %u: null heap, starts or lengths", s);
-        if (S.mem != YTGPU_MEM_DEVICE && S.mem != YTGPU_MEM_HOST)
-            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "string column %u: mem must be YTGPU_MEM_DEVICE or YTGPU_MEM_HOST", s);
-    }
+    u64 n;
+    YTGPU_TRY(check_program_columns(columns, column_count, string_columns, string_count, out_mem, &n));
     if (const_bytes > YTGPU_EXPR_MAX_STRING_CONSTANT_BYTES)
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "more than %u bytes of string_constants", (unsigned)YTGPU_EXPR_MAX_STRING_CONSTANT_BYTES);
     if (const_bytes && !consts) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null string_constants");
-    if (n >= (1ull << 32)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "fewer than 2^32 rows per call");
     CheckedExpr P;
     YTGPU_TRY(check_expression(columns, column_count, strings, string_count, consts, const_bytes, program, node_count, &P));
     if (out_value_type) *out_value_type = P.type;
@@ -998,35 +946,17 @@ Status evaluate_expression_impl(Context* ctx, const ytgpu_column_view* columns, 
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
     if (n == 0) return Status{};
 
-    std::vector<StagedColumn> sc(P.cols.size());
-    std::vector<ColumnDev> hc(P.cols.size());
-    for (size_t k = 0; k < sc.size(); ++k) {
-        YTGPU_TRY(stage_column(ctx, &columns[P.cols[k]], &sc[k]));
-        hc[k] = sc[k].dev;
-    }
-    std::vector<StagedStrings> ss(P.strings.size());
-    std::vector<StringDev> hs(P.strings.size());
-    for (size_t k = 0; k < ss.size(); ++k) {
-        YTGPU_TRY(stage_strings(ctx, string_columns[P.strings[k]], &ss[k]));
-        hs[k] = ss[k].dev;
-    }
-    // one upload: nodes | column views | string views | string constants, then with predicates, 16-byte aligned, the sorted
-    // IN entries | the compiled patterns
-    const size_t nodes_b = P.nodes.size() * sizeof(ExprNodeDev), cols_b = hc.size() * sizeof(ColumnDev), strs_b = hs.size() * sizeof(StringDev);
-    auto up16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
-    const size_t base_b = nodes_b + cols_b + strs_b + const_bytes;
-    const size_t list_b = P.lists.size() * 8, pat_b = up16(P.patterns.size());  // patterns are staged in 16-byte units
-    const size_t o_list = up16(base_b), o_pat = o_list + up16(list_b);
-    std::vector<u8> blob(P.predicates ? o_pat + pat_b : base_b, 0);
-    memcpy(blob.data(), P.nodes.data(), nodes_b);
-    if (cols_b) memcpy(blob.data() + nodes_b, hc.data(), cols_b);
-    if (strs_b) memcpy(blob.data() + nodes_b + cols_b, hs.data(), strs_b);
-    if (const_bytes) memcpy(blob.data() + nodes_b + cols_b + strs_b, consts, const_bytes);
-    if (list_b) memcpy(blob.data() + o_list, P.lists.data(), list_b);
-    if (!P.patterns.empty()) memcpy(blob.data() + o_pat, P.patterns.data(), P.patterns.size());
-    DevBuf<u8> dblob;
-    YTGPU_TRY(dblob.allocate(ctx, blob.size()));
-    YTGPU_CUDA_TRY(cudaMemcpyAsync(dblob.p, blob.data(), blob.size(), cudaMemcpyHostToDevice, ctx->stream));
+    StagedProgramColumns cols;
+    YTGPU_TRY(cols.stage(ctx, columns, P.cols, string_columns, P.strings));
+    // one upload: nodes | column views | string views | string constants | sorted IN entries | compiled patterns
+    ProgramBlob blob;
+    const size_t o_nodes = blob.add(P.nodes.data(), P.nodes.size() * sizeof(ExprNodeDev));
+    const size_t o_cols = blob.add(cols.scalars.data(), cols.scalars.size() * sizeof(ColumnDev));
+    const size_t o_strs = blob.add(cols.strings.data(), cols.strings.size() * sizeof(StringDev));
+    const size_t o_const = blob.add(consts, const_bytes);
+    const size_t o_list = blob.add(P.lists.data(), P.lists.size() * 8);
+    const size_t o_pat = blob.add(P.patterns.data(), P.patterns.size());
+    YTGPU_TRY(blob.upload(ctx));
 
     const u64 words = (n + 63) / 64 * 2;  // 32-bit bitmap words
     const bool host = out_mem == YTGPU_MEM_HOST;
@@ -1069,41 +999,43 @@ Status evaluate_expression_impl(Context* ctx, const ytgpu_column_view* columns, 
     YTGPU_CUDA_TRY(cudaMemsetAsync(result.p, 0, 24, ctx->stream));
 
     ExprArgs A{};
-    A.nodes = reinterpret_cast<const ExprNodeDev*>(dblob.p);
+    A.nodes = blob.at<ExprNodeDev>(o_nodes);
     A.node_count = (u32)P.nodes.size();
-    A.columns = reinterpret_cast<const ColumnDev*>(dblob.p + nodes_b);
-    A.column_count = (u32)hc.size();
+    A.columns = blob.at<ColumnDev>(o_cols);
+    A.column_count = (u32)cols.scalars.size();
     A.selection = dselection;
     A.n = n;
     A.values = dvalues;
     A.nulls = dnulls;
     A.result = result.p;
-    A.strings = reinterpret_cast<const StringDev*>(dblob.p + nodes_b + cols_b);
-    A.string_count = (u32)hs.size();
+    A.strings = blob.at<StringDev>(o_strs);
+    A.string_count = (u32)cols.strings.size();
     A.mode = string_result ? kModeSize : kModeValues;
     A.max_depth = P.max_depth;
     A.max_pieces = P.max_pieces;
-    A.consts = dblob.p + nodes_b + cols_b + strs_b;
+    A.consts = blob.at<u8>(o_const);
     A.starts = dstarts;
     A.lengths = dlengths;
     A.null_bytes = dnull_bytes;
     PredArgs Q{};
-    Q.lists = reinterpret_cast<const u64*>(dblob.p + o_list);
-    Q.patterns = dblob.p + o_pat;
+    Q.lists = blob.at<u64>(o_list);
+    Q.patterns = blob.at<u8>(o_pat);
     Q.staged_list = std::min<u32>((u32)P.lists.size(), kStagedListEntries);
-    Q.pattern_bytes = (u32)pat_b;
+    Q.pattern_bytes = (u32)((P.patterns.size() + 15) & ~(size_t)15);  // staged in 16-byte units, as the blob pads them
     // shared memory in the kernel's order: nodes (16 B each), column views, string views (8-byte multiples), the stack
     // below the top; expression_kernel<true, true>: the piece stack and, 16-byte aligned, a short-value stage per warp
     static_assert(sizeof(ColumnDev) % 8 == 0 && sizeof(StringDev) % 8 == 0, "shared-memory layout");
+    const size_t nodes_b = P.nodes.size() * sizeof(ExprNodeDev), cols_b = cols.scalars.size() * sizeof(ColumnDev),
+                 strs_b = cols.strings.size() * sizeof(StringDev);
     const size_t stack_b = (size_t)(P.max_depth - 1) * kExprThreads * sizeof(u64);
-    const u32 blocks = (u32)std::max<u64>(1, std::min<u64>((words * 32 + kExprThreads - 1) / kExprThreads, (u64)kNumSms * 8));
+    const u32 blocks = blocks_for(words * 32, kExprThreads, 8);  // a warp per 32-row group
     // with predicates, after everything else at a 16-byte boundary: the compiled patterns, then the head of the IN entries
     size_t smem = P.strings_kernel ? nodes_b + cols_b + strs_b + stack_b + (size_t)P.max_pieces * kExprThreads * 12 + 16 +
                                          (size_t)(kExprThreads / 32) * kStageBytes
                                    : nodes_b + cols_b + stack_b;
     if (P.predicates) {
-        Q.pred_smem = (u32)up16(smem);
-        smem = Q.pred_smem + pat_b + (size_t)Q.staged_list * 8;
+        Q.pred_smem = (u32)((smem + 15) & ~(size_t)15);
+        smem = Q.pred_smem + Q.pattern_bytes + (size_t)Q.staged_list * 8;
     }
     // the kernel of the checked program; up to 16 pieces, a 16-deep stack and the predicates' stage exceed the 48 KB default
     void (*kernel)(ExprArgs) = P.strings_kernel ? expression_kernel<true, true> : (P.conditional ? expression_kernel<false, true> : expression_kernel<false, false>);

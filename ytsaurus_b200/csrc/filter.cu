@@ -16,22 +16,19 @@
 //   * CONTAINS and LIKE run the bit-parallel matcher of strings.cuh over patterns compiled on the host and staged in
 //     shared memory after the constants.  The kernel is a template on "the program has pattern nodes", chosen by the host
 //     from the checked program, so programs without them run the same code as before.
+// The column checks, compact column tables, staging and upload are program.cuh's, shared with expression.cu; the IN-list
+// and pattern formats are strings.cuh's.  The IN search stays here: through a shared helper it compiled differently.
 #include <algorithm>
-#include <cstring>
-#include <string>
 #include <vector>
 
-#include "columnar.cuh"
-#include "context.cuh"
+#include "program.cuh"
 #include "scan.cuh"
-#include "strings.cuh"
 
 using namespace ytgpu;
 
 namespace {
 
 constexpr int kFilterThreads = 256;
-constexpr u32 kStagedListEntries = 1024;  // IN entries kept in shared memory per CTA (8 KB)
 constexpr u32 kStagedConstBytes = 4096;   // bytes of string constants kept in shared memory per CTA
 constexpr u32 kMaxFilterColumns = 2 * YTGPU_FILTER_MAX_NODES;  // distinct columns one program can reference
 
@@ -68,17 +65,6 @@ struct FilterArgs {
     u32 bytemap_vec;     // the bytemap is 16-byte aligned: whole 32-row groups are written as two 16-byte stores
     unsigned long long* result;  // [0] selected count, [1] error bits
 };
-
-__device__ __forceinline__ bool cmp_holds(int op, int c) {
-    switch (op) {
-        case YTGPU_CMP_LT: return c < 0;
-        case YTGPU_CMP_LE: return c <= 0;
-        case YTGPU_CMP_GT: return c > 0;
-        case YTGPU_CMP_GE: return c >= 0;
-        case YTGPU_CMP_EQ: return c == 0;
-        default: return c != 0;
-    }
-}
 
 __device__ __forceinline__ u64 load_list(const FilterArgs& A, const u64* s_list, u64 k) {
     return k < A.staged_list ? s_list[k] : __ldg(A.lists + k);
@@ -270,13 +256,8 @@ struct Checked {
     std::vector<NodeDev> nodes;
     std::vector<u64> lists;   // sorted entries of every IN node, node by node
     std::vector<u8> patterns; // compiled CONTAINS / LIKE patterns, node by node (strings.cuh)
-    std::vector<int> scalar_of, string_of;  // caller column -> compact table slot (-1: not referenced)
-    std::vector<u32> scalar_cols, string_cols;  // compact slot -> caller column
+    SlotMap scalars, strings;  // the referenced columns' compact tables
 };
-
-bool is_filter_type(u8 t) {
-    return t == YTGPU_TYPE_INT64 || t == YTGPU_TYPE_UINT64 || t == YTGPU_TYPE_DOUBLE || t == YTGPU_TYPE_BOOLEAN;
-}
 
 Status check_program(const ytgpu_column_view* columns, u32 column_count, u32 string_count, const ytgpu_filter_node* program,
                      u32 node_count, const u64* list_values, u64 list_value_count, const u8* consts, u64 const_bytes,
@@ -289,23 +270,7 @@ Status check_program(const ytgpu_column_view* columns, u32 column_count, u32 str
     if (const_bytes && !consts) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null string_constants");
     if (list_value_count && !list_values) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null list_values");
     const u64 total = (u64)column_count + string_count;
-    out->scalar_of.assign(column_count, -1);
-    out->string_of.assign(string_count, -1);
-    auto slot = [&](u32 c) -> u16 {
-        if (c < column_count) {
-            if (out->scalar_of[c] < 0) {
-                out->scalar_of[c] = (int)out->scalar_cols.size();
-                out->scalar_cols.push_back(c);
-            }
-            return (u16)out->scalar_of[c];
-        }
-        const u32 s = c - column_count;
-        if (out->string_of[s] < 0) {
-            out->string_of[s] = (int)out->string_cols.size();
-            out->string_cols.push_back(s);
-        }
-        return (u16)out->string_of[s];
-    };
+    auto slot = [&](u32 c) { return c < column_count ? out->scalars.slot(c) : out->strings.slot(c - column_count); };
     auto string_range_ok = [&](u64 off, u64 len) { return off <= const_bytes && len <= const_bytes - off; };
     u64 in_entries = 0;
     int depth = 0;
@@ -327,7 +292,7 @@ Status check_program(const ytgpu_column_view* columns, u32 column_count, u32 str
         if (N.column < 0 || (u64)N.column >= total) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: column %d out of range", k, N.column);
         const bool str = (u32)N.column >= column_count;
         const u8 vtype = str ? (u8)YTGPU_TYPE_STRING : columns[N.column].value_type;
-        if (!str && !is_filter_type(vtype))
+        if (!str && !is_scalar_type(vtype))
             return make_status(YTGPU_ERR_UNSUPPORTED, "node %u: column %d has value type 0x%x (INT64, UINT64, DOUBLE or BOOLEAN)", k,
                                N.column, vtype);
         d.is_string = str;
@@ -357,14 +322,8 @@ Status check_program(const ytgpu_column_view* columns, u32 column_count, u32 str
                 if (!str) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: %s on a scalar column", k, like ? "LIKE" : "CONTAINS");
                 if (!string_range_ok(N.constant, N.length))
                     return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: %s outside string_constants", k, like ? "pattern" : "needle");
-                if (like && (N.column2 < -1 || N.column2 > 255))
-                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: LIKE escape %d outside -1 .. 255", k, N.column2);
                 d.constant = out->patterns.size();
-                if (const char* why = compile_pattern(consts + N.constant, N.length, like, like ? N.column2 : -1, &out->patterns))
-                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: %s", k, why);
-                if (out->patterns.size() > (size_t)YTGPU_FILTER_MAX_PATTERN_BYTES)
-                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "the patterns of a call compile to more than %d bytes",
-                                       YTGPU_FILTER_MAX_PATTERN_BYTES);
+                YTGPU_TRY(add_pattern(k, consts + N.constant, N.length, like, like ? N.column2 : -1, &out->patterns));
                 break;
             }
             case YTGPU_FILTER_COMPARE_COLUMNS: {
@@ -379,12 +338,8 @@ Status check_program(const ytgpu_column_view* columns, u32 column_count, u32 str
             case YTGPU_FILTER_IN: {
                 if (N.constant > list_value_count || (u64)N.length > list_value_count - N.constant)
                     return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: IN list outside list_values", k);
-                in_entries += N.length;
-                if (in_entries > (u64)YTGPU_FILTER_MAX_IN_ENTRIES)
-                    return make_status(YTGPU_ERR_INVALID_ARGUMENT, "at most %d IN entries per call", YTGPU_FILTER_MAX_IN_ENTRIES);
                 d.constant = out->lists.size();
-                const i64 bad = prepare_in_list(vtype, list_values + N.constant, N.length, consts, const_bytes, &out->lists);
-                if (bad >= 0) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: IN entry %u outside string_constants", k, (u32)bad);
+                YTGPU_TRY(add_in_list(k, vtype, list_values + N.constant, N.length, consts, const_bytes, &in_entries, &out->lists));
                 d.length = (u32)(out->lists.size() - d.constant);
                 break;
             }
@@ -403,63 +358,27 @@ Status evaluate_filter_impl(Context* ctx, const ytgpu_column_view* columns, u32 
                             u32 string_count, const ytgpu_filter_node* program, u32 node_count, const u64* list_values,
                             u64 list_value_count, const u8* consts, u64 const_bytes, u8* out_bitmap, u8* out_bytemap, u32* out_rows,
                             u64 rows_capacity, u64* out_selected, int out_mem) {
-    if ((column_count && !columns) || (string_count && !string_columns)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null columns");
-    if (column_count + (u64)string_count == 0) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "no columns");
-    if (out_mem != YTGPU_MEM_DEVICE && out_mem != YTGPU_MEM_HOST)
-        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "out_mem must be YTGPU_MEM_DEVICE or YTGPU_MEM_HOST");
-    const u64 n = column_count ? (u64)columns[0].value_count : string_columns[0].row_count;
-    for (u32 c = 0; c < column_count; ++c)
-        if (columns[c].value_count < 0 || (u64)columns[c].value_count != n)
-            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "column %u differs in length", c);
-    for (u32 s = 0; s < string_count; ++s) {
-        const ytgpu_string_column& S = string_columns[s];
-        if (S.row_count != n) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "string column %u differs in length", s);
-        if ((S.heap_bytes && !S.heap) || (n && (!S.starts || !S.lengths)))  // an empty column reads nothing
-            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "string column %u: null heap, starts or lengths", s);
-        if (S.mem != YTGPU_MEM_DEVICE && S.mem != YTGPU_MEM_HOST)
-            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "string column %u: mem must be YTGPU_MEM_DEVICE or YTGPU_MEM_HOST", s);
-    }
-    if (n >= (1ull << 32)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "fewer than 2^32 rows per call");
+    u64 n;
+    YTGPU_TRY(check_program_columns(columns, column_count, string_columns, string_count, out_mem, &n));
     Checked P;
     YTGPU_TRY(check_program(columns, column_count, string_count, program, node_count, list_values, list_value_count, consts, const_bytes, &P));
-    if (P.scalar_cols.size() + P.string_cols.size() > kMaxFilterColumns)
+    if (P.scalars.cols.size() + P.strings.cols.size() > kMaxFilterColumns)
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "too many columns");  // unreachable: 64 nodes reference at most 128
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
     if (out_selected) *out_selected = 0;
     if (n == 0) return Status{};
 
-    // columns the program reads, in compact order
-    std::vector<StagedColumn> sc(P.scalar_cols.size());
-    std::vector<ColumnDev> hc(P.scalar_cols.size());
-    for (size_t k = 0; k < sc.size(); ++k) {
-        YTGPU_TRY(stage_column(ctx, &columns[P.scalar_cols[k]], &sc[k]));
-        hc[k] = sc[k].dev;
-    }
-    std::vector<StagedStrings> ss(P.string_cols.size());
-    std::vector<StringDev> hs(P.string_cols.size());
-    for (size_t k = 0; k < ss.size(); ++k) {
-        YTGPU_TRY(stage_strings(ctx, string_columns[P.string_cols[k]], &ss[k]));
-        hs[k] = ss[k].dev;
-    }
-
-    // one upload: nodes | scalar views | string views | sorted lists | string constants | compiled patterns, then the
-    // outputs' scratch
-    const size_t nodes_b = P.nodes.size() * sizeof(NodeDev), scal_b = hc.size() * sizeof(ColumnDev), str_b = hs.size() * sizeof(StringDev);
-    const size_t list_b = P.lists.size() * 8, const_b = (size_t)const_bytes;
-    auto up16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
-    const size_t o_scal = up16(nodes_b), o_str = o_scal + up16(scal_b), o_list = o_str + up16(str_b), o_const = o_list + up16(list_b);
-    const size_t o_pat = o_const + up16(const_b), pat_b = up16(P.patterns.size());  // staged in 16-byte units
-    const size_t blob_b = o_pat + pat_b;
-    std::vector<u8> blob(blob_b, 0);
-    if (nodes_b) memcpy(blob.data(), P.nodes.data(), nodes_b);
-    if (scal_b) memcpy(blob.data() + o_scal, hc.data(), scal_b);
-    if (str_b) memcpy(blob.data() + o_str, hs.data(), str_b);
-    if (list_b) memcpy(blob.data() + o_list, P.lists.data(), list_b);
-    if (const_b) memcpy(blob.data() + o_const, consts, const_b);
-    if (!P.patterns.empty()) memcpy(blob.data() + o_pat, P.patterns.data(), P.patterns.size());
-    DevBuf<u8> dblob;
-    YTGPU_TRY(dblob.allocate(ctx, blob_b));
-    YTGPU_CUDA_TRY(cudaMemcpyAsync(dblob.p, blob.data(), blob_b, cudaMemcpyHostToDevice, ctx->stream));
+    StagedProgramColumns cols;
+    YTGPU_TRY(cols.stage(ctx, columns, P.scalars, string_columns, P.strings));
+    // one upload: nodes | scalar views | string views | sorted lists | string constants | compiled patterns
+    ProgramBlob blob;
+    const size_t o_nodes = blob.add(P.nodes.data(), P.nodes.size() * sizeof(NodeDev));
+    const size_t o_scal = blob.add(cols.scalars.data(), cols.scalars.size() * sizeof(ColumnDev));
+    const size_t o_str = blob.add(cols.strings.data(), cols.strings.size() * sizeof(StringDev));
+    const size_t o_list = blob.add(P.lists.data(), P.lists.size() * 8);
+    const size_t o_const = blob.add(consts, const_bytes);
+    const size_t o_pat = blob.add(P.patterns.data(), P.patterns.size());
+    YTGPU_TRY(blob.upload(ctx));
 
     const u64 words = (n + 63) / 64 * 2;  // 32-bit bitmap words
     const bool host = out_mem == YTGPU_MEM_HOST;
@@ -482,20 +401,20 @@ Status evaluate_filter_impl(Context* ctx, const ytgpu_column_view* columns, u32 
     YTGPU_CUDA_TRY(cudaMemsetAsync(result.p, 0, 16, ctx->stream));
 
     FilterArgs A{};
-    A.nodes = reinterpret_cast<const NodeDev*>(dblob.p);
+    A.nodes = blob.at<NodeDev>(o_nodes);
     A.node_count = (u32)P.nodes.size();
-    A.scalars = reinterpret_cast<const ColumnDev*>(dblob.p + o_scal);
-    A.scalar_count = (u32)hc.size();
-    A.strings = reinterpret_cast<const StringDev*>(dblob.p + o_str);
-    A.string_count = (u32)hs.size();
-    A.lists = reinterpret_cast<const u64*>(dblob.p + o_list);
+    A.scalars = blob.at<ColumnDev>(o_scal);
+    A.scalar_count = (u32)cols.scalars.size();
+    A.strings = blob.at<StringDev>(o_str);
+    A.string_count = (u32)cols.strings.size();
+    A.lists = blob.at<u64>(o_list);
     A.list_count = (u32)P.lists.size();
     A.staged_list = std::min<u32>(A.list_count, kStagedListEntries);
-    A.consts = dblob.p + o_const;
+    A.consts = blob.at<u8>(o_const);
     A.const_bytes = (u32)const_bytes;
     A.staged_const = std::min<u32>(A.const_bytes, kStagedConstBytes);
-    A.patterns = dblob.p + o_pat;
-    A.pattern_bytes = (u32)pat_b;
+    A.patterns = blob.at<u8>(o_pat);
+    A.pattern_bytes = (u32)((P.patterns.size() + 15) & ~(size_t)15);  // staged in 16-byte units, as the blob pads them
     A.n = n;
     A.bitmap = dbitmap;
     A.bytemap = dbytemap;
@@ -504,13 +423,13 @@ Status evaluate_filter_impl(Context* ctx, const ytgpu_column_view* columns, u32 
     A.result = result.p;
     // shared memory in the kernel's order; every part is a multiple of 8 bytes (NodeDev 24, ColumnDev / StringDev 8-aligned)
     const bool patterns = !P.patterns.empty();
-    size_t smem = nodes_b + scal_b + str_b + (size_t)A.staged_list * 8 + A.staged_const;
-    if (patterns) smem = pattern_smem_offset(smem) + pat_b;
+    size_t smem = P.nodes.size() * sizeof(NodeDev) + A.scalar_count * sizeof(ColumnDev) + A.string_count * sizeof(StringDev) +
+                  (size_t)A.staged_list * 8 + A.staged_const;
+    if (patterns) smem = pattern_smem_offset(smem) + A.pattern_bytes;
     static_assert(sizeof(ColumnDev) % 8 == 0 && sizeof(StringDev) % 8 == 0, "shared-memory layout");
     if (patterns)  // up to 32 KiB of patterns may take the stage past the 48 KB default
         YTGPU_CUDA_TRY(cudaFuncSetAttribute(filter_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const u64 warps = words;
-    const u32 blocks = (u32)std::max<u64>(1, std::min<u64>((warps * 32 + kFilterThreads - 1) / kFilterThreads, (u64)kNumSms * 8));
+    const u32 blocks = blocks_for(words * 32, kFilterThreads, 8);  // a warp per 32-row group
     {
         KernelTimer t(ctx, KC_DECODE);
         if (patterns) filter_kernel<true><<<blocks, kFilterThreads, smem, ctx->stream>>>(A);

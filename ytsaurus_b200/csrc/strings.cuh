@@ -1,7 +1,7 @@
 // strings.cuh — a flat string column (ytgpu_string_column) on the device: bounds-checked value access, QL string order
-// and the upload of HOST columns.  Shared by the string aggregates of groupby_multi.cu and the WHERE evaluator of
-// filter.cu, and the LIKE / substring matcher and the IN lists of filter.cu and expression.cu.  Everything is TU-local (anonymous namespace) so several .cu
-// files may include it.
+// and the upload of HOST columns, for groupby_multi.cu's string aggregates and the program evaluators (filter.cu,
+// expression.cu), and the formats those two share: compiled LIKE / substring patterns and sorted IN lists, with their
+// host checks (add_pattern, add_in_list).  Everything is TU-local (anonymous namespace) so several .cu files may include it.
 #pragma once
 
 #include <algorithm>
@@ -245,7 +245,20 @@ inline const char* compile_pattern(const u8* p, u32 len, bool like, int escape, 
     return nullptr;
 }
 
+// The patterns of one node, compiled and appended to *patterns (LIKE: escape -1 or 0..255; CONTAINS: escape -1), within the
+// per-call limit on compiled bytes.
+inline Status add_pattern(u32 k, const u8* p, u32 len, bool like, int escape, std::vector<u8>* patterns) {
+    if (like && (escape < -1 || escape > 255))
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: LIKE escape %d outside -1 .. 255", k, escape);
+    if (const char* why = compile_pattern(p, len, like, escape, patterns)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: %s", k, why);
+    if (patterns->size() > (size_t)YTGPU_FILTER_MAX_PATTERN_BYTES)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "the patterns of a call compile to more than %d bytes", YTGPU_FILTER_MAX_PATTERN_BYTES);
+    return Status{};
+}
+
 // ---- IN lists (semantics in ytgpu.h, YTGPU_FILTER_IN and YTGPU_EXPR_IN) ----
+constexpr u32 kStagedListEntries = 1024;  // sorted IN entries kept in shared memory per CTA (8 KB)
+
 // A value canonicalised for the IN search: -0.0 becomes +0.0 (the EQ rule says they are equal).
 __host__ __device__ __forceinline__ u64 in_key(u8 vtype, u64 bits) {
     if (vtype == YTGPU_TYPE_DOUBLE && bits == 0x8000000000000000ull) bits = 0;
@@ -278,6 +291,19 @@ inline i64 prepare_in_list(u8 vtype, const u64* e, u32 count, const u8* consts, 
     out->insert(out->end(), sorted.begin(), sorted.end());
     return -1;
 }
+
+// The IN list of node k (count entries e[] over vtype), sorted and appended to *lists; *in_entries counts the entries of
+// the call against its limit.
+inline Status add_in_list(u32 k, u8 vtype, const u64* e, u32 count, const u8* consts, u64 const_bytes, u64* in_entries,
+                          std::vector<u64>* lists) {
+    *in_entries += count;
+    if (*in_entries > (u64)YTGPU_FILTER_MAX_IN_ENTRIES)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "at most %d IN entries per call", YTGPU_FILTER_MAX_IN_ENTRIES);
+    const i64 bad = prepare_in_list(vtype, e, count, consts, const_bytes, lists);
+    if (bad >= 0) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "node %u: IN entry %u outside string_constants", k, (u32)bad);
+    return Status{};
+}
+
 
 // A string column on the device (HOST inputs are uploaded).
 struct StagedStrings {

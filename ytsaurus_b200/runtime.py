@@ -798,6 +798,21 @@ class GpuContext:
         return dict(keys=[k[:g] for k in keys], key_null=[k[:g] for k in kn], values=[v[:g] for v in vals],
                     value_null=[v[:g] for v in vn], count=counts[:g], first_row=first[:g])
 
+    @staticmethod
+    def _program_columns(caller, columns, string_columns):
+        """Column arrays of an evaluator call -> (ColumnView array, views, StringColumn array, mem and n of column 0)."""
+        views = [c.view() for c in columns]
+        sarr = (capi.StringColumn * max(len(string_columns), 1))()
+        for i, column in enumerate(string_columns):
+            sarr[i] = _string_column(*column)
+        if views:
+            mem, n = views[0].mem, int(views[0].value_count)
+        elif string_columns:
+            mem, n = sarr[0].mem, int(sarr[0].row_count)
+        else:
+            raise ValueError(f"{caller} needs at least one column")
+        return (capi.ColumnView * max(len(views), 1))(*views), views, sarr, mem, n
+
     def evaluate_filter(self, columns, string_columns=(), program=(), list_values=(), string_constants=b"",
                         want_bitmap: bool = True, want_bytemap: bool = True, want_rows: bool = True,
                         rows_capacity: int | None = None):
@@ -808,17 +823,7 @@ class GpuContext:
         (offset << 32) | length into string_constants).  The outputs are in the inputs' memory flavour: bitmap
         8 * ceil(n / 64) bytes, bytemap n bytes, rows uint32 (int32 on the device) trimmed to the count; an output not
         wanted is None."""
-        views = [c.view() for c in columns]
-        sarr = (capi.StringColumn * max(len(string_columns), 1))()
-        for i, column in enumerate(string_columns):
-            sarr[i] = _string_column(*column)
-        if views:
-            mem, n = views[0].mem, int(views[0].value_count)
-        elif string_columns:
-            mem, n = sarr[0].mem, int(sarr[0].row_count)
-        else:
-            raise ValueError("evaluate_filter needs at least one column")
-        carr = (capi.ColumnView * max(len(views), 1))(*views)
+        carr, views, sarr, mem, n = self._program_columns("evaluate_filter", columns, string_columns)
         nodes = (capi.FilterNode * max(len(program), 1))()
         for i, node in enumerate(program):
             if isinstance(node, capi.FilterNode):
@@ -861,17 +866,7 @@ class GpuContext:
         of that type, so a STRING result runs its size pass twice (a caller that knows the heap size calls the library once).
         A STRING result comes back as heap / starts / lengths / null_bytemap (values, null_bitmap and column None), ready
         for evaluate_filter's string_columns and string_value_ids."""
-        views = [c.view() for c in columns]
-        sarr = (capi.StringColumn * max(len(string_columns), 1))()
-        for i, column in enumerate(string_columns):
-            sarr[i] = _string_column(*column)
-        if views:
-            mem, n = views[0].mem, int(views[0].value_count)
-        elif string_columns:
-            mem, n = sarr[0].mem, int(sarr[0].row_count)
-        else:
-            raise ValueError("evaluate_expression needs at least one column")
-        carr = (capi.ColumnView * max(len(views), 1))(*views)
+        carr, views, sarr, mem, n = self._program_columns("evaluate_expression", columns, string_columns)
         nodes = (capi.ExprNode * max(len(program), 1))()
         for i, node in enumerate(program):
             if isinstance(node, capi.ExprNode):
