@@ -2,9 +2,9 @@
 
 The scatter writes every row to the slab of its partition, the rows of one partition in input order.  Its destinations
 are plain device pointers, so one GPU runs every path of it with each partition pointed at a local buffer:
-  - up to 32 partitions, the streaming kernel: 64-byte rows through the warp transpose, with ordered or unordered stores
-    (YTGPU_SCATTER_ORDERED=0, read on every call), every other width through the per-row copy loop; tiles of 1024 rows,
-    rounds of 32, partition-bit ballots that change width between 16/17 and 31/32 partitions;
+  - up to 32 partitions, the streaming kernel: 64-byte rows through the warp transpose, which stores each round of 32
+    rows in destination order, every other width through the per-row copy loop; tiles of 1024 rows, rounds of 32,
+    partition-bit ballots that change width between 16/17 and 31/32 partitions;
   - 33 to 4096 partitions, the many-partition path: a radix sort of the index, then a gather that finds each row's
     partition by binary search over the slab starts.  YTGPU_SCATTER_STREAM=0 forces it at any count, but the library
     reads that variable once per process, so those cases run in a child process that imports this module.
@@ -13,7 +13,6 @@ The reference for partition p's slab is the input rows whose index is p, in inpu
 sentinel before the call; after it, the slabs must hold exactly the reference rows and every byte around them must
 still be the sentinel.  A rejected call must leave every destination byte untouched and the context usable.
 """
-import contextlib
 import os
 import subprocess
 import sys
@@ -30,7 +29,6 @@ MANY_PARTS = [33, 257, 3071, 3072, 4096]  # from 3072 on, slab starts and pointe
 ROW_WIDTHS = [16, 32, 48, 64, 80, 128, 256]  # 64: the warp transpose; every other width: the per-row copy loop
 ROW_COUNTS = [0, 1, 31, 32, 33, 1023, 1024, 1025, 4095, 4097, 150_001]
 LAYOUTS = ["tensors", "contiguous", "peer"]
-ORDERINGS = [None, "0"]  # YTGPU_SCATTER_ORDERED unset (ordered stores) and "0" (unordered)
 # all_*: one partition holds every row, so on the many-partition path the index sort skips every digit and returns the
 # identity permutation; sorted: the digit passes run and produce the identity
 SHAPES = ["uniform", "all_first", "all_last", "all_middle", "empty_ends_and_middle", "sorted", "runs_31_32_33", "skew_99"]
@@ -123,22 +121,6 @@ class _Slabs:
             self.peer_ptr = None
 
 
-@contextlib.contextmanager
-def _env(name, value):
-    old = os.environ.get(name)
-    if value is None:
-        os.environ.pop(name, None)
-    else:
-        os.environ[name] = value
-    try:
-        yield
-    finally:
-        if old is None:
-            os.environ.pop(name, None)
-        else:
-            os.environ[name] = old
-
-
 def _dev(a):
     import torch
     return torch.from_numpy(np.ascontiguousarray(a).reshape(-1)).cuda()
@@ -148,24 +130,19 @@ def _random_rows(rng, n, row_bytes):
     return rng.integers(0, 256, (n, row_bytes), dtype=np.uint8)
 
 
-def scatter_and_check(ctx, rows, idx, parts, layout, ordered=None):
+def scatter_and_check(ctx, rows, idx, parts, layout):
     """Scatter host rows [n, row_bytes] by idx into `layout` and compare every destination byte with the reference."""
     row_bytes = rows.shape[1]
     counts = np.bincount(idx, minlength=parts)
     dest = _Slabs(ctx, layout, counts, row_bytes)
     try:
-        with _env("YTGPU_SCATTER_ORDERED", ordered):
-            ctx.scatter_rows_to_peers(_dev(rows), row_bytes, _dev(idx), counts.tolist(), dest.ptrs)
+        ctx.scatter_rows_to_peers(_dev(rows), row_bytes, _dev(idx), counts.tolist(), dest.ptrs)
         got = dest.host_bytes()
     finally:
         dest.close()
     want = expected_buffer(layout, expected_slabs(rows, idx, parts))
     assert got.shape == want.shape and (got == want).all(), (
-        f"{len(rows)} rows x {row_bytes} B, {parts} partitions, {layout}, ordered={ordered}: {_first_difference(got, want)}")
-
-
-def _orderings(row_bytes):
-    return ORDERINGS if row_bytes == 64 else [None]
+        f"{len(rows)} rows x {row_bytes} B, {parts} partitions, {layout}: {_first_difference(got, want)}")
 
 
 def _expect_rejected(ctx, rows, row_bytes, idx, counts, parts, layout="tensors", dest_offsets=None):
@@ -246,11 +223,10 @@ def test_scatter_rows(ctx, parts, row_bytes):
         rows = _random_rows(rng, n, row_bytes)
         idx = make_index("uniform", n, parts, rng)
         layout = LAYOUTS[(i + parts + row_bytes // 16) % len(LAYOUTS)]
-        for ordered in _orderings(row_bytes):
-            try:
-                scatter_and_check(ctx, rows, idx, parts, layout, ordered)
-            except (AssertionError, capi.YtGpuError) as e:
-                failures.append(f"n={n} {layout} ordered={ordered}: {e}")
+        try:
+            scatter_and_check(ctx, rows, idx, parts, layout)
+        except (AssertionError, capi.YtGpuError) as e:
+            failures.append(f"n={n} {layout}: {e}")
     assert not failures, "\n".join(failures)
 
 
@@ -263,8 +239,7 @@ def test_scatter_index_shapes(ctx, parts, shape):
         idx = make_index(shape, n, parts, rng)
         for row_bytes in (48, 64):
             rows = _random_rows(rng, n, row_bytes)
-            for ordered in _orderings(row_bytes):
-                scatter_and_check(ctx, rows, idx, parts, layout, ordered)
+            scatter_and_check(ctx, rows, idx, parts, layout)
 
 
 # ---- the many-partition path at few partitions, in a child process ----
@@ -306,7 +281,6 @@ def forced_many_partition_cases():
 @pytest.mark.gpu
 def test_many_partition_path_at_few_partitions():
     env = dict(os.environ, YTGPU_SCATTER_STREAM="0")
-    env.pop("YTGPU_SCATTER_ORDERED", None)
     here = os.path.dirname(os.path.abspath(__file__))
     code = (f"import sys; sys.path[:0] = [{os.path.dirname(here)!r}, {here!r}]; "
             "import test_peer_scatter as t; t.forced_many_partition_cases()")
@@ -316,7 +290,7 @@ def test_many_partition_path_at_few_partitions():
 
 
 # ---- large inputs, checked on the device ----
-def _scatter_large(ctx, n, parts, row_bytes, ordered):
+def _scatter_large(ctx, n, parts, row_bytes):
     import torch
     g = torch.Generator(device="cuda")
     g.manual_seed(n + parts)
@@ -325,8 +299,7 @@ def _scatter_large(ctx, n, parts, row_bytes, ordered):
     counts = torch.bincount(idx, minlength=parts).cpu().tolist()
     dest = _Slabs(ctx, "contiguous", counts, row_bytes)
     try:
-        with _env("YTGPU_SCATTER_ORDERED", ordered):
-            ctx.scatter_rows_to_peers(rows, row_bytes, idx, counts, dest.ptrs)
+        ctx.scatter_rows_to_peers(rows, row_bytes, idx, counts, dest.ptrs)
         got = dest.bufs[0]
         rows2d = rows.view(n, row_bytes)
         want = torch.cat([rows2d[idx == p] for p in range(parts)]).view(-1)  # boolean masks keep input order
@@ -338,17 +311,15 @@ def _scatter_large(ctx, n, parts, row_bytes, ordered):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("ordered", ORDERINGS, ids=["ordered", "unordered"])
-def test_scatter_bench_exchange_shape(ctx, ordered):
+def test_scatter_bench_exchange_shape(ctx):
     # the row exchange of the 8-GPU sort: 3*10^7 rows of 64 B over 8 partitions
-    _scatter_large(ctx, 30_000_000, 8, 64, ordered)
+    _scatter_large(ctx, 30_000_000, 8, 64)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("ordered", ORDERINGS, ids=["ordered", "unordered"])
-def test_scatter_large_many_partitions(ctx, ordered):
+def test_scatter_large_many_partitions(ctx):
     # 10^7 rows: the index sort takes the radix sort's hybrid schedule
-    _scatter_large(ctx, 10_000_000, 4096, 64, ordered)
+    _scatter_large(ctx, 10_000_000, 4096, 64)
 
 
 # ---- fed by the partition step ----
@@ -378,18 +349,16 @@ def test_scatter_matches_partition_slabs(ctx, kind, parts):
         idx, hist, slabs = ctx.partition_fixed_rows(src, row_bytes, spec, want_index=True, want_slabs=True)
         counts = hist.cpu().numpy().view(np.uint64).tolist()
         assert sum(counts) == n and sum(c > 0 for c in counts) > parts // 2
-        for ordered in _orderings(row_bytes):
-            dest = _Slabs(ctx, "contiguous", counts, row_bytes)
-            try:
-                with _env("YTGPU_SCATTER_ORDERED", ordered):
-                    ctx.scatter_rows_to_peers(src, row_bytes, idx, counts, dest.ptrs)
-                got = dest.host_bytes()
-            finally:
-                dest.close()
-            want = np.concatenate([np.full(GUARD, SENTINEL, np.uint8), slabs.cpu().numpy(), np.full(GUARD, SENTINEL, np.uint8)])
-            assert (got == want).all(), f"{row_bytes} B, ordered={ordered}: {_first_difference(got, want)}"
-            ref = expected_buffer("contiguous", expected_slabs(rows, idx.cpu().numpy(), parts))
-            assert (got == ref).all()
+        dest = _Slabs(ctx, "contiguous", counts, row_bytes)
+        try:
+            ctx.scatter_rows_to_peers(src, row_bytes, idx, counts, dest.ptrs)
+            got = dest.host_bytes()
+        finally:
+            dest.close()
+        want = np.concatenate([np.full(GUARD, SENTINEL, np.uint8), slabs.cpu().numpy(), np.full(GUARD, SENTINEL, np.uint8)])
+        assert (got == want).all(), f"{row_bytes} B: {_first_difference(got, want)}"
+        ref = expected_buffer("contiguous", expected_slabs(rows, idx.cpu().numpy(), parts))
+        assert (got == ref).all()
 
 
 # ---- rejected calls ----
@@ -410,9 +379,7 @@ def test_scatter_rejects_bad_index(ctx, parts, case):
         counts[(src + 1) % parts] += 1
     else:
         idx[[0, n // 2, n - 1]] = [parts, 2**31 - 1, parts + 7] if case == "index_past_end" else [-1, -2**31, -parts]
-    for ordered in ORDERINGS:
-        with _env("YTGPU_SCATTER_ORDERED", ordered):
-            _expect_rejected(ctx, _dev(rows), 64, _dev(idx), counts, parts)
+    _expect_rejected(ctx, _dev(rows), 64, _dev(idx), counts, parts)
     _still_usable(ctx, parts, parts)
 
 

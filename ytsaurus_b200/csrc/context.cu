@@ -1,7 +1,6 @@
 // context.cu — context lifetime, status plumbing, timers.
 #include <cstdarg>
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <new>
 
@@ -101,10 +100,6 @@ int ytgpu_context_create(int device, void* cuda_stream, ytgpu_context** out, ytg
             return fill_error(err, cuda_status(e, "cudaStreamCreate"));
         }
         c->owns_stream = true;
-    }
-    if (const char* e = getenv("YTGPU_L2_FETCH")) {
-        // experiment knob: L2 fetch granularity hint (32/64/128 bytes) for the random row/key gathers
-        cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)atoi(e));
     }
     // keep freed scratch cached in the stream-ordered pool between calls
     cudaMemPool_t pool;

@@ -150,7 +150,7 @@ struct CtxLock {
 };
 
 // Kernel families whose launches need cudaFuncSetAttribute(MaxDynamicSharedMemorySize) on each device.
-enum FuncAttrFamily : u32 { FA_SORT_PASS = 1u << 0, FA_GROUPBY = 1u << 2, FA_SHUFFLE = 1u << 3 };
+enum FuncAttrFamily : u32 { FA_SORT_PASS = 1u << 0, FA_GROUPBY = 1u << 2 };
 
 // Reads and clears the device error word (synchronises the stream).
 Status check_device_errors(Context* ctx);

@@ -18,6 +18,37 @@ namespace {
 
 constexpr int kMaxScatterPartitions = 4096;
 
+// Rows per partition in every tile of the streaming scatter (TileCounts).
+__global__ void __launch_bounds__(kStreamThreads) tile_count_kernel(const i32* __restrict__ index, u64 n, u32 parts, u64 tiles,
+                                                                    u64* __restrict__ counts /*[parts][tiles]*/, u32* __restrict__ err_word) {
+    __shared__ u32 s_cnt[kStreamMaxParts];
+    if (threadIdx.x < kStreamMaxParts) s_cnt[threadIdx.x] = 0;
+    __syncthreads();
+    const u64 base = (u64)blockIdx.x * kStreamTile;
+#pragma unroll
+    for (int i = 0; i < kStreamItems; ++i) {
+        const u64 r = base + (u64)i * kStreamThreads + threadIdx.x;
+        if (r < n) {
+            u32 p = (u32)index[r];
+            if (p >= parts) {  // caller-supplied index outside [0, parts): flag it, never index shared memory with it
+                atomicOr(err_word, (u32)DE_BAD_PARTITION_INDEX);
+                p = 0;
+            }
+            atomicAdd(&s_cnt[p], 1u);
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x < parts) counts[(u64)threadIdx.x * tiles + blockIdx.x] = s_cnt[threadIdx.x];
+}
+
+// The per-partition totals of the counting pass must equal what the caller said it would send: otherwise rows would land
+// outside the slabs reserved in the destination buffers.
+__global__ void check_partition_totals_kernel(const u64* __restrict__ scanned /*[parts][tiles]*/, u64 tiles, u64 n, u32 parts,
+                                              const u64* __restrict__ expected_start /*[parts + 1]*/, u32* __restrict__ err_word) {
+    const u32 p = threadIdx.x;
+    if (p < parts && scanned[(u64)p * tiles] != expected_start[p]) atomicOr(err_word, (u32)DE_BAD_PARTITION_INDEX);
+}
+
 // Rows per partition of the caller-supplied index (per-block shared histogram, then global atomics); a value outside
 // [0, parts) is flagged instead of counted.
 __global__ void __launch_bounds__(256) count_partitions_kernel(const i32* __restrict__ index, u64 n, u32 parts,
@@ -86,38 +117,27 @@ __global__ void __launch_bounds__(256) scatter_rows_to_peers_kernel(const uint4*
 Status scatter_stream(Context* ctx, const ytgpu_fixed_rows_view* in, const i32* index, u32 parts, const std::vector<u64>& start,
                       void* const* dest_base) {
     const u64 n = in->row_count;
-    const u32 gr = in->row_bytes / 16;
-    const u64 tiles = (n + kStreamTile - 1) / kStreamTile;
-    const u64 cells = (u64)parts * tiles;
-    const u64 nblocks = (cells + 1023) / 1024;
-    DevBuf<u64> counts, sums;
-    YTGPU_TRY(counts.allocate(ctx, cells));
-    YTGPU_TRY(sums.allocate(ctx, nblocks));
+    TileCounts counts;
+    YTGPU_TRY(counts.allocate(ctx, n, parts));
     DestTable D{};
     for (u32 p = 0; p < parts; ++p) {
         D.base[p] = reinterpret_cast<uint4*>(dest_base[p]);
         D.start[p] = start[p];
     }
-    u32 bits = 0;
-    while ((1u << bits) < parts) ++bits;
     DevBuf<u64> dstart;
     YTGPU_TRY(dstart.allocate(ctx, parts + 1));
     YTGPU_CUDA_TRY(cudaMemcpyAsync(dstart.p, start.data(), (parts + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
     {
         KernelTimer t(ctx, KC_PARTITION, 5);
-        tile_count_kernel<<<(u32)tiles, kStreamThreads, 0, ctx->stream>>>(index, n, parts, tiles, counts.p, ctx->dev_err);
-        pscan_blocks_kernel<false><<<(u32)nblocks, 256, 0, ctx->stream>>>(counts.p, cells, sums.p);
-        pscan_sums_kernel<<<1, 256, 0, ctx->stream>>>(sums.p, nblocks);
-        pscan_blocks_kernel<true><<<(u32)nblocks, 256, 0, ctx->stream>>>(counts.p, cells, sums.p);
-        check_partition_totals_kernel<<<1, 32, 0, ctx->stream>>>(counts.p, tiles, n, parts, dstart.p, ctx->dev_err);
+        tile_count_kernel<<<(u32)counts.tiles, kStreamThreads, 0, ctx->stream>>>(index, n, parts, counts.tiles, counts.cells.p, ctx->dev_err);
+        counts.scan(ctx->stream);
+        check_partition_totals_kernel<<<1, 32, 0, ctx->stream>>>(counts.cells.p, counts.tiles, n, parts, dstart.p, ctx->dev_err);
     }
     // caller-supplied indices / counts are validated BEFORE anything is written into another GPU's memory
     YTGPU_TRY(check_device_errors(ctx));
-    const char* ord = getenv("YTGPU_SCATTER_ORDERED");
     {
         KernelTimer t(ctx, KC_SCATTER);
-        scatter_stream_kernel<<<(u32)tiles, kStreamThreads, 0, ctx->stream>>>(reinterpret_cast<const uint4*>(in->rows), index, n, gr, parts,
-                                                                             bits, tiles, counts.p, D, (ord && ord[0] == '0') ? 0u : 1u);
+        launch_scatter_stream(ctx->stream, in->rows, index, n, in->row_bytes, parts, counts, D);
     }
     YTGPU_CUDA_TRY(cudaGetLastError());
     YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));

@@ -3,7 +3,10 @@
 // Kernels are `static` (TU-local) so both translation units may include it.
 #pragma once
 
+#include <algorithm>
+
 #include "context.cuh"
+#include "scan.cuh"
 
 namespace ytgpu {
 
@@ -19,99 +22,6 @@ constexpr int kStreamItems = 4;
 constexpr int kStreamTile = kStreamThreads * kStreamItems;  // rows per tile
 constexpr int kStreamMaxParts = 32;
 
-static __global__ void __launch_bounds__(kStreamThreads) tile_count_kernel(const i32* __restrict__ index, u64 n, u32 parts,
-                                                                    u64 tiles, u64* __restrict__ counts /*[parts][tiles]*/,
-                                                                    u32* __restrict__ err_word) {
-    __shared__ u32 s_cnt[kStreamMaxParts];
-    if (threadIdx.x < kStreamMaxParts) s_cnt[threadIdx.x] = 0;
-    __syncthreads();
-    const u64 base = (u64)blockIdx.x * kStreamTile;
-#pragma unroll
-    for (int i = 0; i < kStreamItems; ++i) {
-        const u64 r = base + (u64)i * kStreamThreads + threadIdx.x;
-        if (r < n) {
-            u32 p = (u32)index[r];
-            if (p >= parts) {  // caller-supplied index outside [0, parts): flag it, never index shared memory with it
-                atomicOr(err_word, (u32)DE_BAD_PARTITION_INDEX);
-                p = 0;
-            }
-            atomicAdd(&s_cnt[p], 1u);
-        }
-    }
-    __syncthreads();
-    if (threadIdx.x < parts) counts[(u64)threadIdx.x * tiles + blockIdx.x] = s_cnt[threadIdx.x];
-}
-
-// three-phase exclusive scan of u64 (1024 elements per block), in place
-static __device__ __forceinline__ u64 scan_block_excl(u64 v, u64* s_warp, u64* total) {
-    const u32 lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    u64 inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        u64 t = __shfl_up_sync(0xffffffffu, inc, o);
-        if (lane >= (u32)o) inc += t;
-    }
-    if (lane == 31) s_warp[warp] = inc;
-    __syncthreads();
-    u64 wp = 0, tot = 0;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) {
-        u64 x = s_warp[w];
-        if (w < (int)warp) wp += x;
-        tot += x;
-    }
-    __syncthreads();
-    *total = tot;
-    return inc - v + wp;
-}
-template <bool WRITE>
-static __global__ void __launch_bounds__(256) pscan_blocks_kernel(u64* data, u64 n, u64* block_sums) {
-    __shared__ u64 s_warp[8];
-    const u64 base = (u64)blockIdx.x * 1024 + (u64)threadIdx.x * 4;
-    u64 v[4], sum = 0;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        v[i] = base + i < n ? data[base + i] : 0;
-        sum += v[i];
-    }
-    u64 total;
-    const u64 ex = scan_block_excl(sum, s_warp, &total);
-    if (!WRITE) {
-        if (threadIdx.x == 0) block_sums[blockIdx.x] = total;
-    } else {
-        u64 run = ex + block_sums[blockIdx.x];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            if (base + i < n) data[base + i] = run;
-            run += v[i];
-        }
-    }
-}
-static __global__ void __launch_bounds__(256) pscan_sums_kernel(u64* sums, u64 nblocks) {
-    __shared__ u64 s_warp[8];
-    __shared__ u64 s_carry;
-    if (threadIdx.x == 0) s_carry = 0;
-    __syncthreads();
-    for (u64 base = 0; base < nblocks; base += 256) {
-        const u64 i = base + threadIdx.x;
-        const u64 v = i < nblocks ? sums[i] : 0;
-        u64 total;
-        const u64 ex = scan_block_excl(v, s_warp, &total);
-        if (i < nblocks) sums[i] = ex + s_carry;
-        __syncthreads();
-        if (threadIdx.x == 0) s_carry += total;
-        __syncthreads();
-    }
-}
-
-// The per-partition totals of the counting pass must equal what the caller said it would send: otherwise rows would land
-// outside the slabs reserved in the destination buffers.
-static __global__ void check_partition_totals_kernel(const u64* __restrict__ scanned /*[parts][tiles]*/, u64 tiles, u64 n, u32 parts,
-                                                     const u64* __restrict__ expected_start /*[parts + 1]*/, u32* __restrict__ err_word) {
-    const u32 p = threadIdx.x;
-    if (p < parts && scanned[(u64)p * tiles] != expected_start[p]) atomicOr(err_word, (u32)DE_BAD_PARTITION_INDEX);
-}
-
 struct DestTable {
     uint4* base[kStreamMaxParts];  // destination of partition p's slab
     u64 start[kStreamMaxParts];    // global slot of its first row (scan value of tile 0)
@@ -120,7 +30,7 @@ struct DestTable {
 static __global__ void __launch_bounds__(kStreamThreads) scatter_stream_kernel(const uint4* __restrict__ in, const i32* __restrict__ index,
                                                                         u64 n, u32 gr, u32 parts, u32 part_bits, u64 tiles,
                                                                         const u64* __restrict__ tile_base /*[parts][tiles]*/,
-                                                                        const DestTable D, u32 ordered) {
+                                                                        const DestTable D) {
     constexpr int WARPS = kStreamThreads / 32;
     __shared__ u32 s_wcnt[WARPS][kStreamMaxParts];  // running per-warp counts -> warp offsets inside the tile
     __shared__ u64 s_slot[kStreamMaxParts];         // first slot of this tile per partition
@@ -193,8 +103,10 @@ static __global__ void __launch_bounds__(kStreamThreads) scatter_stream_kernel(c
             }
             // Rows leave in destination order: rows of one partition sit next to each other in its slab, so a store
             // instruction writes runs of whole rows (128 B and more) instead of isolated 64-byte rows — fewer, larger
-            // NVLink write packets.
-            s_order[warp][ordered ? pos[i] : lane] = (u8)lane;
+            // NVLink write packets.  With one partition pos[i] == lane; the select on `parts` only steers ptxas (nvcc 12.9):
+            // without it the partition-bit sweep above loses its uniform-register loop counters and the kernel measured
+            // about 1 % slower on an H100 80GB HBM3 at 700 W (10^8 rows of 64 B, 2 to 32 partitions).
+            s_order[warp][parts > 1 ? pos[i] : lane] = (u8)lane;
             __syncwarp();
 #pragma unroll
             for (u32 s = 0; s < 4; ++s) {
@@ -220,97 +132,29 @@ static __global__ void __launch_bounds__(kStreamThreads) scatter_stream_kernel(c
     __threadfence_system();
 }
 
+// The [partition][tile] count matrix.  A counting pass over the partition index (tile_count_kernel in peer.cu,
+// partition_count_kernel in shuffle.cu) stores the rows of partition p in tile t at cells[p * tiles + t]; scan() turns
+// every cell into the global slot of that tile's first row of partition p, which scatter_stream_kernel reads.
+struct TileCounts {
+    u64 tiles = 0;
+    DevBuf<u64> cells;
+    DevBuf<u64> sums;  // the scan's block sums, then its grand total
+    Status allocate(Context* ctx, u64 n, u32 parts) {
+        tiles = std::max<u64>(1, (n + kStreamTile - 1) / kStreamTile);
+        YTGPU_TRY(cells.allocate(ctx, (u64)parts * tiles));
+        return sums.allocate(ctx, scan_block_count(cells.n) + 1);
+    }
+    void scan(cudaStream_t st) { exclusive_scan_u64(st, cells.p, cells.n, sums.p, sums.p + sums.n - 1); }  // three launches
+};
 
-// ---------------------------------------------------------------------------------------------
-// Tile-staged scatter for 64-byte rows: the whole 1024-row tile is staged in shared memory IN DESTINATION ORDER, then
-// written out with consecutive threads -> consecutive 16-byte granules.  A store instruction then covers 512 contiguous
-// bytes of ONE destination slab (the per-warp variant above writes runs of ~32/g rows: 256 B at g = 8), i.e. fewer and
-// larger NVLink write packets: what limits the exchange at 4-8 GPUs.
-// ---------------------------------------------------------------------------------------------
-constexpr size_t kScatterTileSmem = (size_t)kStreamTile * 64;
-
-static __global__ void __launch_bounds__(kStreamThreads) scatter_tile_kernel(const uint4* __restrict__ in, const i32* __restrict__ index, u64 n,
-                                                                             u32 parts, u32 part_bits, u64 tiles,
-                                                                             const u64* __restrict__ tile_base /*[parts][tiles]*/, const DestTable D) {
-    constexpr int WARPS = kStreamThreads / 32;
-    extern __shared__ __align__(16) uint4 s_tile[];         // [kStreamTile][4]
-    __shared__ u32 s_wcnt[WARPS][kStreamMaxParts];           // per-warp counts -> warp offsets inside the partition's tile segment
-    __shared__ u32 s_pstart[kStreamMaxParts + 1];            // first tile slot of every partition
-    __shared__ uint4* s_gptr[kStreamMaxParts];               // where this tile's rows of partition p start in p's destination slab
-    __shared__ u8 s_dest[kStreamTile];                       // partition of every tile slot
-    const u32 tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid < WARPS * kStreamMaxParts) (&s_wcnt[0][0])[tid] = 0;
-    __syncthreads();
-    const u64 tile = blockIdx.x;
-    const u64 wbase = tile * kStreamTile + (u64)warp * (32 * kStreamItems) + lane;  // warp-striped: stable (item, lane) order
-    u32 part[kStreamItems], rank[kStreamItems];
-    u32 lt;
-    asm("mov.u32 %0, %%lanemask_lt;" : "=r"(lt));
-#pragma unroll
-    for (int i = 0; i < kStreamItems; ++i) {
-        const u64 r = wbase + (u64)i * 32;
-        const bool valid = r < n;
-        part[i] = valid ? min((u32)index[r], parts - 1) : 0u;
-        const u32 kk = valid ? part[i] : (1u << part_bits);
-        u32 m = 0xffffffffu;
-        for (int b = (int)part_bits; b >= 0; --b) {
-            const bool bit = (kk >> b) & 1;
-            const u32 v = __ballot_sync(0xffffffffu, bit);
-            m &= bit ? v : ~v;
-        }
-        const u32 prev = s_wcnt[warp][part[i]];
-        __syncwarp();
-        if (valid && (m & lt) == 0) s_wcnt[warp][part[i]] = prev + __popc(m);
-        rank[i] = prev + __popc(m & lt);
-        __syncwarp();
-    }
-    __syncthreads();
-    if (tid < parts) {
-        u32 run = 0;
-#pragma unroll
-        for (int w = 0; w < WARPS; ++w) {
-            const u32 c = s_wcnt[w][tid];
-            s_wcnt[w][tid] = run;
-            run += c;
-        }
-        s_pstart[tid + 1] = run;  // counts for now
-        s_gptr[tid] = D.base[tid] + (tile_base[(u64)tid * tiles + tile] - D.start[tid]) * 4;
-    }
-    __syncthreads();
-    if (tid == 0) {
-        u32 run = 0;
-        s_pstart[0] = 0;
-        for (u32 p = 0; p < parts; ++p) {
-            const u32 c = s_pstart[p + 1];
-            s_pstart[p + 1] = run + c;
-            run += c;
-        }
-    }
-    __syncthreads();
-    // stage: the 32 rows of a round are contiguous in the input (one coalesced 2 KB read); row `row` of the round goes to
-    // the tile slot its owner lane computed
-#pragma unroll
-    for (int i = 0; i < kStreamItems; ++i) {
-        const u64 r = wbase + (u64)i * 32;
-        const u32 p = part[i];
-        const u32 myslot = r < n ? s_pstart[p] + s_wcnt[warp][p] + rank[i] : 0xffffffffu;
-        if (r < n) s_dest[myslot] = (u8)p;
-        const u64 round_row0 = r - lane;
-#pragma unroll
-        for (u32 s4 = 0; s4 < 4; ++s4) {
-            const u32 q = s4 * 32 + lane, row = q >> 2, g = q & 3;
-            const u32 slot = __shfl_sync(0xffffffffu, myslot, row);
-            if (slot != 0xffffffffu) s_tile[slot * 4 + g] = ld_stream_u128(in + round_row0 * 4 + q);
-        }
-    }
-    __syncthreads();
-    const u32 total = s_pstart[parts] * 4;  // granules
-    for (u32 q = tid; q < total; q += kStreamThreads) {
-        const u32 slot = q >> 2, g = q & 3;
-        const u32 p = s_dest[slot];
-        s_gptr[p][(size_t)(slot - s_pstart[p]) * 4 + g] = s_tile[q];
-    }
-    __threadfence_system();  // peer stores are ordered before whatever signals completion to the other GPU
+// Row r of rows[n][row_bytes] goes to D.base[p] + (slot - D.start[p]) rows, p = index[r], its slot taken from the
+// scanned counts plus its rank among the tile's rows of partition p.
+static inline void launch_scatter_stream(cudaStream_t st, const void* rows, const i32* index, u64 n, u32 row_bytes, u32 parts,
+                                         const TileCounts& counts, const DestTable& D) {
+    u32 part_bits = 0;
+    while ((1u << part_bits) < parts) ++part_bits;
+    scatter_stream_kernel<<<(u32)counts.tiles, kStreamThreads, 0, st>>>(reinterpret_cast<const uint4*>(rows), index, n, row_bytes / 16, parts,
+                                                                       part_bits, counts.tiles, counts.cells.p, D);
 }
 
 }  // namespace ytgpu

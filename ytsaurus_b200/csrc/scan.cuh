@@ -1,5 +1,6 @@
-// scan.cuh — exclusive scan of u64 in place (three phases over 4096-element blocks), shared by the block codec and
-// the column writer.  Everything is TU-local (static) so several .cu files may include it.
+// scan.cuh — exclusive scan of u64 in place (three phases over 4096-element blocks), shared by the block codec, the
+// column writers, the evaluators, the sorts and the count matrix of the row exchange (peer_kernels.cuh).  Everything is
+// TU-local (static) so several .cu files may include it.
 #pragma once
 
 #include "common.cuh"

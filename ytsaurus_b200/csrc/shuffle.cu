@@ -17,7 +17,6 @@
 //                   buffer over NVLink (peer_kernels.cuh), barrier
 //   local sort   -> the rank's key range (capi_sort.cu)
 // The host takes part once per sort (it reads the count matrix to size the local sort); no NCCL, no host barrier.
-#include <cstdlib>
 #include <cstring>
 #include <new>
 #include <vector>
@@ -339,27 +338,25 @@ Status shuffle_sort_impl(Shuffle* s, const ytgpu_fixed_rows_view* in, const ytgp
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
     // ---- 3. partition index + per-tile counts, scan, publish the counts, barrier ----
-    const u64 tiles = std::max<u64>(1, (n + kStreamTile - 1) / kStreamTile);
-    const u64 cells = (u64)parts * tiles;
-    const u64 nblocks = (cells + 1023) / 1024;
     DevBuf<i32> index;
-    DevBuf<u64> counts, sums;
+    TileCounts counts;
     YTGPU_TRY(index.allocate(ctx, std::max<u64>(n, 1)));
-    YTGPU_TRY(counts.allocate(ctx, cells));
-    YTGPU_TRY(sums.allocate(ctx, nblocks));
+    YTGPU_TRY(counts.allocate(ctx, n, parts));
     {
         KernelTimer t(ctx, KC_PARTITION);  // one timed unit: the partition/count pass + the three tiny scan launches
         ctx->count_launch(3);
-        if (scalar8) partition_count_kernel<true><<<(u32)tiles, kStreamThreads, 0, st>>>(L, in->rows, n, rb, s->pivots, parts, tiles, index.p, counts.p);
-        else partition_count_kernel<false><<<(u32)tiles, kStreamThreads, 0, st>>>(L, in->rows, n, rb, s->pivots, parts, tiles, index.p, counts.p);
-        pscan_blocks_kernel<false><<<(u32)nblocks, 256, 0, st>>>(counts.p, cells, sums.p);
-        pscan_sums_kernel<<<1, 256, 0, st>>>(sums.p, nblocks);
-        pscan_blocks_kernel<true><<<(u32)nblocks, 256, 0, st>>>(counts.p, cells, sums.p);
+        if (scalar8)
+            partition_count_kernel<true><<<(u32)counts.tiles, kStreamThreads, 0, st>>>(L, in->rows, n, rb, s->pivots, parts, counts.tiles,
+                                                                                        index.p, counts.cells.p);
+        else
+            partition_count_kernel<false><<<(u32)counts.tiles, kStreamThreads, 0, st>>>(L, in->rows, n, rb, s->pivots, parts, counts.tiles,
+                                                                                         index.p, counts.cells.p);
+        counts.scan(st);
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
     {
         KernelTimer t(ctx, KC_SHUFFLE_SYNC, 2);
-        publish_counts_kernel<<<1, 32, 0, st>>>(counts.p, tiles, n, parts, s->peers, world, rank);
+        publish_counts_kernel<<<1, 32, 0, st>>>(counts.cells.p, counts.tiles, n, parts, s->peers, world, rank);
         YTGPU_TRY(barrier(s));
     }
     // ---- 4. the host's one look at the data: the g x g count matrix ----
@@ -404,24 +401,8 @@ Status shuffle_sort_impl(Shuffle* s, const ytgpu_fixed_rows_view* in, const ytgp
             D.start[p] = startp;
             startp += hc->counts[rank][p];
         }
-        u32 bits = 0;
-        while ((1u << bits) < parts) ++bits;
         KernelTimer t(ctx, KC_SCATTER);
-        // The tile-staged scatter (rows regrouped by destination in shared memory first) is opt-in: measured at 2 ranks it
-        // is SLOWER than the streaming one (6.64 vs 4.97 ms for 5*10^7 rows out: the streaming kernel's 64-byte row
-        // stores already fill whole NVLink packets, staging only adds a shared-memory round trip and a barrier).
-        static const int tile_scatter = [] { const char* e = getenv("YTGPU_SCATTER_TILE"); return e ? atoi(e) : 0; }();
-        if (rb == 64 && tile_scatter) {
-            if (!(ctx->func_attrs_done & FA_SHUFFLE)) {
-                cudaFuncSetAttribute(scatter_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kScatterTileSmem);
-                ctx->func_attrs_done |= FA_SHUFFLE;
-            }
-            scatter_tile_kernel<<<(u32)tiles, kStreamThreads, kScatterTileSmem, st>>>(reinterpret_cast<const uint4*>(in->rows), index.p, n, parts, bits,
-                                                                                      tiles, counts.p, D);
-        } else {
-            scatter_stream_kernel<<<(u32)tiles, kStreamThreads, 0, st>>>(reinterpret_cast<const uint4*>(in->rows), index.p, n, rb / 16, parts, bits,
-                                                                        tiles, counts.p, D, 1u);
-        }
+        launch_scatter_stream(st, in->rows, index.p, n, rb, parts, counts, D);
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
     {
