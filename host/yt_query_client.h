@@ -294,6 +294,21 @@ struct TMultiGroupQuery {
     //! division by zero in a dropped group does not throw.  The program is checked whatever the data: a Having that is not
     //! a Boolean throws on an empty input too.  Without it every group is written.
     std::optional<TExpression> Having;
+    //! JOIN (JoinOpHelper, cg_routines/registry.cpp): an inner or left equi-join of the reader's rows (the primary side)
+    //! with Foreign's rows on SelfColumns[k] = ForeignColumns[k].  With Join set, every position above that names an input
+    //! column names a column of the JOINED row: a primary position as without it, or ForeignColumn(j) for position j of the
+    //! foreign rows.  Select and Having keep naming output positions.  A LEFT join's primary row without a match gets NULL
+    //! in every foreign column.  Join keys compare as the GROUP BY keys do: NULL equals NULL, doubles by bit pattern.
+    struct TJoinClause {
+        ISchemalessMultiChunkReaderPtr Foreign;   // the foreign table's rows, in the order the reference fetches them
+        std::vector<int> SelfColumns;             // join key positions in the primary rows (1..8)
+        std::vector<int> ForeignColumns;          // the matching positions in the foreign rows
+        bool IsLeft = false;
+    };
+    std::optional<TJoinClause> Join;
+    static constexpr int kForeignColumnBase = 1 << 24;
+    static constexpr int ForeignColumn(int j) { return kForeignColumnBase + j; }
+    static constexpr bool IsForeignColumn(int position) { return position >= kForeignColumnBase; }
 };
 
 struct TQueryStatistics {
@@ -321,6 +336,13 @@ struct IEvaluator {
     //! a string column to every consumer (group item, string aggregate argument, WHERE leaf); lower / upper of a non-ASCII
     //! value throws YTGPU_ERR_UNSUPPORTED.  Errors of the calls (a division by zero, a mistyped expression:
     //! YTGPU_ERR_INVALID_ARGUMENT) throw TErrorException.  A query without computed columns and Select runs as before.
+    //! With Join, both sides are flattened, the join keys typed (an all-NULL key column takes the other side's type; any
+    //! other mismatch, Int64 against Uint64 included, throws YTGPU_ERR_INVALID_ARGUMENT: the caller casts first; string keys
+    //! go through one joint ytgpu_string_value_ids call), ytgpu_hash_join makes the pairs (a count query, then the fill), and
+    //! every flattened column is replaced by its gather at the pairs' primary or foreign rows.  Everything above then runs
+    //! unchanged over the joined rows: WHERE filters joined rows, the SQL meaning for both kinds.  So, beside the note on
+    //! division errors: a computed column or WHERE is not evaluated over a primary row that an INNER join drops.  RowsRead
+    //! counts primary rows.  A query without Join runs exactly as before.
     virtual TQueryStatistics Run(const TMultiGroupQuery& query, const ISchemalessMultiChunkReaderPtr& reader,
                                  const IUnversionedRowsetWriterPtr& writer) = 0;
 };

@@ -64,7 +64,8 @@ uint64_t ytgpu_context_launch_count(const ytgpu_context* ctx);
  * gather / peer scatter, 2 key extraction, 3 histogram / tie fix-up, 4 partition, 5 group-by, 6 decode / block
  * codec, 7 radix pass launches that were skipped on the device (inactive digit), 8 the in-box
  * shuffle's row scatter over NVLink, 9 its sampling / pivot selection / count exchange / peer barriers (includes the
- * time spent WAITING for the other ranks), 10 sorted-input segmented reduce.
+ * time spent WAITING for the other ranks), 10 sorted-input segmented reduce, 11 hash join: build, probe, pair write and
+ * gathers.
  * launches (nullable) receives the number of launches behind the returned time. */
 double ytgpu_context_kernel_ms(ytgpu_context* ctx, int which, uint64_t* launches);
 void ytgpu_context_reset_timers(ytgpu_context* ctx);
@@ -587,6 +588,69 @@ int ytgpu_scan_filter_groupby_multi_strings(ytgpu_context* ctx, const ytgpu_colu
                                             uint64_t group_count_hint, ytgpu_groupby_multi_result* out, int out_mem,
                                             const ytgpu_string_column* string_columns, uint32_t string_count,
                                             ytgpu_error* err);
+
+/* ---- hash JOIN: inner and left equi-joins over key tuples ----
+ * The join of YT QL's JoinOpHelper (library/query/engine/cg_routines/registry.cpp), which collects the primary rows' join
+ * keys, fetches the foreign rows and joins them row by row through a hash lookup keyed on the join key.  Here the foreign
+ * side is always the built one: its key tuples go into the open-addressing table of the GROUP BY calls, every primary row
+ * probes it, and the result is a list of (primary row, foreign row) PAIRS; ytgpu_gather_column and
+ * ytgpu_gather_string_column turn the pairs into columns every other call takes.
+ * Keys.  Key k of the two sides has one value_type: INT64, UINT64, DOUBLE or BOOLEAN, in any encoding the GROUP BY calls take.
+ * There is no implicit widening: different types are INVALID_ARGUMENT, the caller casts.  Tuples compare exactly as the GROUP
+ * BY calls compare them, as (is-null, 64-bit payload) per column: doubles by bit pattern, so -0.0 does not match +0.0 and a
+ * NaN matches only the same NaN bits; NULL EQUALS NULL.  That rule is shared with GROUP BY and with the unversioned value
+ * comparator; that YT QL's join lookup treats NULL keys this way is recalled, not read.  The SQL rule of ClickHouse and YQL,
+ * where NULL never matches, is not offered: a SQL caller drops the rows with NULL keys first (ytgpu_evaluate_filter) for an
+ * INNER join, and has no way to do so for a LEFT one.
+ * String keys go through ytgpu_string_value_ids: call it ONCE over one string column holding the F foreign values followed
+ * by the P primary values.  Then ids[0, F) is the foreign key column and ids[F, F + P) the primary one, both UINT64 with the
+ * null bytemap as their NULLs: equal strings on either side get the same first-row id.  The join itself is numeric only.
+ * Pairs.  INNER: one pair (p, f) for every primary row p and foreign row f with equal key tuples.  LEFT: in addition one pair
+ * (p, YTGPU_JOIN_NO_ROW) for every primary row without a match.  The pairs are ordered by ascending primary row, then
+ * ascending foreign row, the LEFT pair of an unmatched row at its place: the row-by-row order of JoinOpHelper when the
+ * foreign rows come in their fetched order (that order is recalled, not read).  The output is fully deterministic.
+ * Capacity protocol (that of ytgpu_evaluate_filter's out_rows): *out_pair_count is always written once the call gets that
+ * far.  Both outputs NULL is a count query and launches no write pass; exactly one NULL is INVALID_ARGUMENT.  A
+ * pairs_capacity below the count fails with INVALID_ARGUMENT, the count still written.  Outputs are in out_mem.
+ * Limits and errors: 1 .. YTGPU_JOIN_MAX_KEYS key columns; at most 2^30 primary rows and 2^30 - 1 foreign rows (slots and
+ * rows are 32-bit, and the foreign rows go through the radix sort, which takes fewer than 2^30), checked before any access
+ * (UNSUPPORTED); the key columns of one side have one length (INVALID_ARGUMENT); an unknown kind is
+ * INVALID_ARGUMENT; a key type other than the four scalars is UNSUPPORTED.
+ * Launches: the build (one assign pass of the GROUP BY calls, sized for the foreign row count so that no retry is expected,
+ * and a read of its error word), one probe kernel over the primary rows, a three-kernel scan of the per-row pair counts and
+ * a read of the total; with outputs, a three-kernel scan of the per-key counts, one stable radix sort of the foreign rows by
+ * their slot (which reads its plan back once from 2^18 foreign rows), the output-partitioned pair write and a closing
+ * synchronisation of the context's stream: the outputs are complete when the call returns, whichever stream the caller
+ * reads them on (a context may run on a private stream), as with the GROUP BY calls.  HOST inputs are copied to the device
+ * first. */
+typedef enum ytgpu_join_kind { YTGPU_JOIN_INNER = 0, YTGPU_JOIN_LEFT = 1 } ytgpu_join_kind;
+#define YTGPU_JOIN_NO_ROW 0xffffffffu
+#define YTGPU_JOIN_MAX_KEYS 8
+
+int ytgpu_hash_join(ytgpu_context* ctx, const ytgpu_column_view* primary_keys, const ytgpu_column_view* foreign_keys,
+                    uint32_t key_count, int kind, uint32_t* out_primary_rows, uint32_t* out_foreign_rows,
+                    uint64_t pairs_capacity, uint64_t* out_pair_count /* host */, int out_mem, ytgpu_error* err);
+
+/* Gathers.  ytgpu_gather_column decodes `column` at rows[i] into out_values[i] and bit i of out_null_bitmap, for i < count,
+ * in the layout of ytgpu_evaluate_expression: out_values count 64-bit bit patterns (a NULL row holds 0), out_null_bitmap
+ * 8 * ceil(count / 64) bytes (LSB first, the bits past count zero), *out_null_count (host, nullable) the NULL rows.  So
+ * {value_type = column->value_type, bit_width = 64, has_values = 1, values = out_values, values_count = count, value_count
+ * = count, null_bitmap = out_null_bitmap} is a column every other call takes.  rows[i] = YTGPU_JOIN_NO_ROW gives NULL: that
+ * is how the missing foreign side of a LEFT join becomes NULL.
+ * ytgpu_gather_string_column gathers starts, lengths and the null bytemap (count entries each; a NULL row gets start 0,
+ * length 0, null byte 1).  The heap is not copied: {column->heap, column->heap_bytes, out_starts, out_lengths,
+ * out_null_bytemap, count, out_mem} is the gathered column.  rows, like the outputs, are in out_mem; the column in its own.
+ * INVALID_ARGUMENT: a row index neither below the column's length (value_count / row_count) nor YTGPU_JOIN_NO_ROW (checked
+ * on the device: no byte outside the column is read), a null output, a column as the other calls refuse it.  UNSUPPORTED: a
+ * value_type other than INT64, UINT64, DOUBLE or BOOLEAN.  One gather kernel, then one read of the error word (and the NULL
+ * count).  out_null_bitmap is written in 4-byte words: 4-byte aligned in DEVICE memory. */
+int ytgpu_gather_column(ytgpu_context* ctx, const ytgpu_column_view* column, const uint32_t* rows /* out_mem */,
+                        uint64_t count, uint64_t* out_values, uint8_t* out_null_bitmap,
+                        uint64_t* out_null_count /* host, nullable */, int out_mem, ytgpu_error* err);
+
+int ytgpu_gather_string_column(ytgpu_context* ctx, const ytgpu_string_column* column, const uint32_t* rows /* out_mem */,
+                               uint64_t count, uint64_t* out_starts, uint32_t* out_lengths, uint8_t* out_null_bytemap,
+                               int out_mem, ytgpu_error* err);
 
 /* ---- WHERE expressions: a selection over several columns ----
  * The filter of YT QL's ScanOpHelper / FilterOpHelper (the WHERE clause compiled by the query evaluator) and of

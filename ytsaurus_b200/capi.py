@@ -25,7 +25,7 @@ TYPE_NULL, TYPE_INT64, TYPE_UINT64, TYPE_DOUBLE, TYPE_BOOLEAN, TYPE_STRING = 0x0
 CMP_NONE, CMP_LT, CMP_LE, CMP_GT, CMP_GE, CMP_EQ, CMP_NE = range(7)
 
 KC_RADIX_PASS, KC_GATHER, KC_EXTRACT, KC_HISTOGRAM, KC_PARTITION, KC_GROUPBY, KC_DECODE, KC_PASS_SKIPPED, KC_SCATTER, \
-    KC_SHUFFLE_SYNC, KC_REDUCE = range(11)
+    KC_SHUFFLE_SYNC, KC_REDUCE, KC_JOIN = range(12)
 MAX_SHUFFLE_RANKS = 32
 
 
@@ -120,6 +120,7 @@ EXPORTED_SYMBOLS = [
     "ytgpu_block_agg_state_init", "ytgpu_block_combine_all",
     "ytgpu_build_bitmap_from_flags", "ytgpu_build_bytemap_from_flags", "ytgpu_count_flags", "ytgpu_build_dictionary_indexes",
     "ytgpu_count_total_string_length", "ytgpu_translate_rle_indexes", "ytgpu_context_get_option", "ytgpu_convert_ch_column_to_values", "ytgpu_convert_string_column_to_ch", "ytgpu_decode_column_typed",
+    "ytgpu_hash_join", "ytgpu_gather_column", "ytgpu_gather_string_column",
 ]
 
 FLAGS_DICTIONARY_ZERO, FLAGS_BITMAP = 0, 1
@@ -147,6 +148,9 @@ class FlagSource(C.Structure):
 
 
 AGG_SUM, AGG_MIN, AGG_MAX, AGG_COUNT, AGG_AVG, AGG_ARGMIN, AGG_ARGMAX, AGG_FIRST = range(8)
+JOIN_INNER, JOIN_LEFT = 0, 1
+JOIN_NO_ROW = 0xFFFFFFFF
+JOIN_MAX_KEYS = 8
 
 
 class Aggregate(C.Structure):
@@ -365,6 +369,12 @@ def load() -> C.CDLL:
                                                 C.POINTER(Error)]
     lib.ytgpu_string_value_ids.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p,
                                            C.c_void_p, C.c_int, C.POINTER(Error)]
+    lib.ytgpu_hash_join.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_int, C.c_void_p, C.c_void_p, C.c_uint64,
+                                    C.POINTER(C.c_uint64), C.c_int, C.POINTER(Error)]
+    lib.ytgpu_gather_column.argtypes = [C.c_void_p, C.POINTER(ColumnView), C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
+                                        C.POINTER(C.c_uint64), C.c_int, C.POINTER(Error)]
+    lib.ytgpu_gather_string_column.argtypes = [C.c_void_p, C.POINTER(StringColumn), C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
+                                               C.c_void_p, C.c_int, C.POINTER(Error)]
     lib.ytgpu_extract_column.argtypes = [C.c_void_p, C.POINTER(RowsetView), C.c_uint32, C.c_uint8, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_int, C.POINTER(Error)]
     lib.ytgpu_block_agg_state_init.argtypes = [C.POINTER(BlockAggState), C.c_uint8, C.c_uint8]

@@ -20,7 +20,7 @@ constexpr int kNumSms = 132;  // H100 SXM
 // Kernel classes for the per-context CUDA-event timers (ytgpu_context_kernel_ms).
 enum KernelClass { KC_RADIX_PASS = 0, KC_GATHER = 1, KC_EXTRACT = 2, KC_HISTOGRAM = 3, KC_PARTITION = 4,
                    KC_GROUPBY = 5, KC_DECODE = 6, KC_PASS_SKIPPED = 7, KC_SCATTER = 8, KC_SHUFFLE_SYNC = 9,
-                   KC_REDUCE = 10, KC_COUNT = 11 };
+                   KC_REDUCE = 10, KC_JOIN = 11, KC_COUNT = 12 };
 
 struct Status {
     int code = YTGPU_OK;
@@ -57,6 +57,7 @@ enum DevErr : u32 {
     DE_PEER_TIMEOUT = 1u << 8,       // a peer GPU did not reach the in-box shuffle's barrier in time
     DE_BAD_PARTITION_INDEX = 1u << 9,  // caller-supplied partition index outside [0, partition_count)
     DE_STRING_OUT_OF_HEAP = 1u << 10,  // a string value's [start, start + length) leaves its heap
+    DE_ROW_OUT_OF_RANGE = 1u << 11,    // a gather's row index is neither below the column's length nor YTGPU_JOIN_NO_ROW
 };
 
 struct Context;  // context.cu

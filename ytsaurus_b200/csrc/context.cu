@@ -65,6 +65,8 @@ Status check_device_errors(Context* ctx) {
     if (e & DE_BAD_PARTITION_INDEX)
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "partition index outside [0, partition_count) or partition row counts that disagree with it");
     if (e & DE_STRING_OUT_OF_HEAP) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "a string value runs past the end of its heap");
+    if (e & DE_ROW_OUT_OF_RANGE)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "a row index is neither below the column's length nor YTGPU_JOIN_NO_ROW");
     return make_status(YTGPU_ERR_CUDA, "unknown device error word 0x%x", e);
 }
 

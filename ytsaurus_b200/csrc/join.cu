@@ -1,0 +1,515 @@
+// join.cu — hash JOIN: inner and left equi-joins over key tuples, and the gathers that turn its pairs into columns.
+//
+// Replaces the row-by-row hash lookup of YT QL's JoinOpHelper (library/query/engine/cg_routines/registry.cpp): the foreign
+// rows are built into a table keyed on the join key, every primary row looks its key up there.  Five steps:
+//   1. build: the GROUP BY assign step (key_tuple.cuh) over the foreign keys, sized for the foreign row count: rep[slot] =
+//      a foreign row holding the tuple, counts[slot] = the foreign rows of the tuple, slot_of_row[f] = f's slot.
+//   2. per-key lists: the counts, scanned, give each slot's start; one stable radix sort of the foreign rows by slot lists
+//      every slot's rows in ascending order (an atomic scatter would not be stable, and the order is part of the result).
+//   3. probe: each primary row loads and hashes its tuple with the same hash_tuple, walks the table comparing against the
+//      FOREIGN columns at the slot's row and stops at an empty slot: its slot, and its pair count.
+//   4. offsets: the pair counts, scanned; the total is read back (the count query ends here, before steps 2 and 5).
+//   5. write: each CTA owns a fixed range of output positions, finds its first primary row by binary search over the
+//      offsets and walks the rows and their slot lists from there, galloping over rows without pairs.  So a key with 10^6
+//      foreign rows spreads over about 245 CTAs, and a run of r unmatched rows costs a thread about 2 log2(r) loads:
+//      neither serialises on one thread.
+#include <algorithm>
+
+#include "columnar.cuh"
+#include "context.cuh"
+#include "key_tuple.cuh"
+#include "radix_sort.cuh"
+#include "scan.cuh"
+
+using namespace ytgpu;
+
+namespace {
+
+constexpr u32 kNoRow = YTGPU_JOIN_NO_ROW;
+// Rows per side: slots and rows are 32-bit.  The foreign side is also sorted by slot, and the radix sort takes fewer than
+// 2^30 rows (its look-back words carry 30-bit counts).
+constexpr u64 kMaxPrimaryRows = 1ull << 30;
+constexpr u64 kMaxForeignRows = (1ull << 30) - 1;
+
+// Step 3, with the two-rows-in-flight structure of mg_assign_kernel: the probe is a chain of dependent loads (key -> slot ->
+// the foreign row's key), so both rows' loads are issued before either is used.  DIRECT: every key column of BOTH sides is
+// a plain 64-bit vector; NK: 1, 2 or 0 (K.count columns).
+template <bool DIRECT, int NK>
+__global__ void __launch_bounds__(256) hj_probe_kernel(const KeyColumns P, const KeyColumns F, u64 n, const u32* __restrict__ rep, u64 mask,
+                                                       const unsigned long long* __restrict__ counts, int left, u32* __restrict__ probe_slot,
+                                                       u64* __restrict__ pair_counts) {
+    constexpr int R = NK ? 2 : 1;  // 3+ key columns: four 8-word tuples in flight would cost the occupancy
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    u64 base = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    KeyTuple ahead[R];
+#pragma unroll
+    for (int j = 0; j < R; ++j)
+        if (base + (u64)j * stride < n) ahead[j] = load_tuple<DIRECT, NK>(P, base + (u64)j * stride);
+    for (; base < n; base += stride * R) {
+        u64 row[R], b[R];
+        u32 r[R], slot[R];
+        bool valid[R];
+        KeyTuple mine[R], cand[R];
+#pragma unroll
+        for (int j = 0; j < R; ++j) {
+            mine[j] = ahead[j];
+            const u64 nxt = base + stride * R + (u64)j * stride;
+            if (nxt < n) ahead[j] = load_tuple<DIRECT, NK>(P, nxt);
+        }
+#pragma unroll
+        for (int j = 0; j < R; ++j) {
+            row[j] = base + (u64)j * stride;
+            valid[j] = row[j] < n;
+            slot[j] = kNoSlot;
+            b[j] = valid[j] ? hash_tuple<NK>(P, mine[j]) & mask : 0;
+            r[j] = valid[j] ? rep[b[j]] : kNoSlot;
+        }
+#pragma unroll
+        for (int j = 0; j < R; ++j)
+            if (valid[j] && r[j] != kNoSlot) cand[j] = load_tuple<DIRECT, NK>(F, r[j]);
+#pragma unroll
+        for (int j = 0; j < R; ++j) {
+            if (!valid[j]) continue;
+            u32 rr = r[j];
+            bool have = true;  // cand[j] holds the key of foreign row rr
+            u64 bb = b[j];
+            for (u64 probes = 0; probes <= mask && rr != kNoSlot; ++probes) {
+                if (same_tuple<NK>(P, mine[j], have ? cand[j] : load_tuple<DIRECT, NK>(F, rr))) {
+                    slot[j] = (u32)bb;
+                    break;
+                }
+                bb = (bb + 1) & mask;
+                rr = rep[bb];
+                have = false;
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < R; ++j) {
+            if (!valid[j]) continue;
+            probe_slot[row[j]] = slot[j];
+            pair_counts[row[j]] = slot[j] != kNoSlot ? (u64)counts[slot[j]] : (left ? 1 : 0);
+        }
+    }
+}
+
+// The sort key of step 2: a foreign row's slot.
+__global__ void __launch_bounds__(256) hj_slot_keys_kernel(const u32* __restrict__ slot_of_row, u64 n, u64* __restrict__ keys) {
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) keys[i] = slot_of_row[i];
+}
+
+// Step 5: CTA c writes output positions [c * kWriteTile, (c + 1) * kWriteTile), thread t the kWriteItems consecutive ones
+// from c * kWriteTile + t * kWriteItems, into shared memory first so that the global stores are coalesced.
+constexpr int kWriteThreads = 256;
+constexpr int kWriteItems = 16;
+constexpr int kWriteTile = kWriteThreads * kWriteItems;
+__device__ __forceinline__ u32 tile_index(u32 i) { return i + i / kWriteItems; }  // one pad word per thread: no bank conflicts
+
+__global__ void __launch_bounds__(kWriteThreads) hj_write_pairs_kernel(const u64* __restrict__ offsets, u64 n, u64 total,
+                                                                       const u32* __restrict__ probe_slot, const u64* __restrict__ slot_start,
+                                                                       const SortPlan* plan, const u32* pa, const u32* pb,
+                                                                       u32* __restrict__ out_primary, u32* __restrict__ out_foreign) {
+    __shared__ u32 s_p[kWriteTile + kWriteThreads], s_f[kWriteTile + kWriteThreads];
+    const u64 tile0 = (u64)blockIdx.x * kWriteTile;
+    const u64 first = tile0 + (u64)threadIdx.x * kWriteItems;
+    if (first < total) {
+        u64 lo = 0, hi = n;  // the last row p with offsets[p] <= first (offsets[0] = 0): it has a pair there
+        while (hi - lo > 1) {
+            const u64 mid = (lo + hi) >> 1;
+            if (offsets[mid] <= first) lo = mid;
+            else hi = mid;
+        }
+        u64 p = lo, start = offsets[p], end = p + 1 < n ? offsets[p + 1] : total;
+#pragma unroll 1
+        for (u32 k = 0; k < (u32)kWriteItems; ++k) {
+            const u64 o = first + k;
+            if (o >= total) break;
+            if (o >= end) {
+                const u64 next_end = p + 2 < n ? offsets[p + 2] : total;
+                if (o < next_end) {  // the next row: the common case, one load
+                    ++p;
+                    start = end;
+                    end = next_end;
+                } else {
+                    // A run of rows without pairs (INNER misses; a sorted primary table against a dimension that covers
+                    // part of its key range): the last q with offsets[q] <= o by a gallop from p + 2 (offsets[p + 2] =
+                    // next_end <= o) and a binary search inside the last step, O(log run) loads rather than one per row,
+                    // so no thread does more than kWriteItems such searches.
+                    u64 q = p + 2, step = 1;
+                    while (q + step < n && offsets[q + step] <= o) {
+                        q += step;
+                        step <<= 1;
+                    }
+                    u64 qe = q + step < n ? q + step : n;  // offsets[qe] > o, or qe == n
+                    while (qe - q > 1) {
+                        const u64 mid = (q + qe) >> 1;
+                        if (offsets[mid] <= o) q = mid;
+                        else qe = mid;
+                    }
+                    p = q;
+                    start = offsets[p];
+                    end = p + 1 < n ? offsets[p + 1] : total;
+                }
+            }
+            const u32 s = probe_slot[p];
+            const u32 i = tile_index(threadIdx.x * kWriteItems + k);
+            s_p[i] = (u32)p;
+            s_f[i] = s == kNoSlot ? kNoRow : perm_at(plan, pa, pb, slot_start[s] + (o - start));
+        }
+    }
+    __syncthreads();
+    const u32 m = (u32)std::min<u64>((u64)kWriteTile, total - tile0);
+    for (u32 i = threadIdx.x; i < m; i += kWriteThreads) {
+        out_primary[tile0 + i] = s_p[tile_index(i)];
+        out_foreign[tile0 + i] = s_f[tile_index(i)];
+    }
+}
+
+// ytgpu_gather_column: one row per thread; each warp writes its 32 null bits as one word.  The grid covers whole 64-row
+// words, so the bits past `count` are written as zeros.
+__global__ void __launch_bounds__(256) hj_gather_kernel(const ColumnDev c, u64 column_rows, const u32* __restrict__ rows, u64 count,
+                                                        u64* __restrict__ out, u32* __restrict__ out_bits, unsigned long long* null_count,
+                                                        u32* err_word) {
+    const u64 padded = (count + 63) / 64 * 64;
+    u32 bad = 0, nulls = 0;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < padded; i += (u64)gridDim.x * blockDim.x) {
+        bool nul = false;
+        if (i < count) {
+            const u32 r = rows[i];
+            u64 v = 0;
+            if (r == kNoRow) {
+                nul = true;
+            } else if ((u64)r >= column_rows) {
+                bad = 1;
+                nul = true;
+            } else {
+                v = decode_at(c, (i64)r, &nul);
+            }
+            out[i] = nul ? 0 : v;
+        }
+        const u32 m = __ballot_sync(0xffffffffu, nul);
+        if ((threadIdx.x & 31) == 0) {
+            out_bits[i >> 5] = m;
+            nulls += __popc(m);
+        }
+    }
+    if (bad) atomicOr(err_word, (u32)DE_ROW_OUT_OF_RANGE);
+    if ((threadIdx.x & 31) == 0 && nulls) atomicAdd(null_count, (unsigned long long)nulls);
+}
+
+__global__ void __launch_bounds__(256) hj_gather_strings_kernel(const u64* __restrict__ starts, const u32* __restrict__ lengths,
+                                                                const u8* __restrict__ nulls, u64 column_rows, const u32* __restrict__ rows,
+                                                                u64 count, u64* __restrict__ out_starts, u32* __restrict__ out_lengths,
+                                                                u8* __restrict__ out_nulls, u32* err_word) {
+    u32 bad = 0;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (u64)gridDim.x * blockDim.x) {
+        const u32 r = rows[i];
+        bool nul = r == kNoRow;
+        if (!nul && (u64)r >= column_rows) {
+            bad = 1;
+            nul = true;
+        }
+        nul = nul || (nulls && nulls[r]);
+        out_starts[i] = nul ? 0 : starts[r];
+        out_lengths[i] = nul ? 0 : lengths[r];
+        out_nulls[i] = nul ? 1 : 0;
+    }
+    if (bad) atomicOr(err_word, (u32)DE_ROW_OUT_OF_RANGE);
+}
+
+bool join_key_type(u8 t) { return t == YTGPU_TYPE_INT64 || t == YTGPU_TYPE_UINT64 || t == YTGPU_TYPE_DOUBLE || t == YTGPU_TYPE_BOOLEAN; }
+
+Status check_side(const ytgpu_column_view* keys, u32 key_count, const char* side, u64 max_rows, u64* rows) {
+    for (u32 k = 0; k < key_count; ++k) {
+        if (keys[k].value_count < 0 || keys[k].start_index < 0) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "%s key %u: negative column range", side, k);
+        if (keys[k].value_count != keys[0].value_count)
+            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "%s key columns differ in length", side);
+        if (!join_key_type(keys[k].value_type))
+            return make_status(YTGPU_ERR_UNSUPPORTED, "%s key %u: value type 0x%x is not INT64, UINT64, DOUBLE or BOOLEAN", side, k,
+                               keys[k].value_type);
+    }
+    *rows = (u64)keys[0].value_count;
+    if (*rows > max_rows)
+        return make_status(YTGPU_ERR_UNSUPPORTED, "%s side: at most %llu rows (slots and rows are 32-bit)", side, (unsigned long long)max_rows);
+    return Status{};
+}
+
+Status hash_join_impl(Context* ctx, const ytgpu_column_view* primary_keys, const ytgpu_column_view* foreign_keys, u32 key_count, int kind,
+                      u32* out_primary, u32* out_foreign, u64 pairs_capacity, u64* out_pair_count, int out_mem) {
+    if (!primary_keys || !foreign_keys || !out_pair_count) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null argument");
+    if (key_count == 0 || key_count > (u32)YTGPU_JOIN_MAX_KEYS)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "key column count must be in [1, %d]", YTGPU_JOIN_MAX_KEYS);
+    if (kind != YTGPU_JOIN_INNER && kind != YTGPU_JOIN_LEFT) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "unknown join kind %d", kind);
+    if ((out_primary == nullptr) != (out_foreign == nullptr))
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "both outputs or neither (a count query) must be given");
+    if (out_mem != YTGPU_MEM_DEVICE && out_mem != YTGPU_MEM_HOST)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "out_mem must be YTGPU_MEM_DEVICE or YTGPU_MEM_HOST");
+    u64 np = 0, nf = 0;
+    YTGPU_TRY(check_side(primary_keys, key_count, "primary", kMaxPrimaryRows, &np));
+    YTGPU_TRY(check_side(foreign_keys, key_count, "foreign", kMaxForeignRows, &nf));
+    for (u32 k = 0; k < key_count; ++k)
+        if (primary_keys[k].value_type != foreign_keys[k].value_type)
+            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "key %u: primary type 0x%x differs from foreign type 0x%x (no implicit widening)", k,
+                               primary_keys[k].value_type, foreign_keys[k].value_type);
+    *out_pair_count = 0;
+    YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (np == 0) return Status{};
+
+    std::vector<StagedColumn> sp(key_count), sf(key_count);
+    KeyColumns KP{}, KF{};
+    KP.count = KF.count = key_count;
+    bool direct = true;  // plain 64-bit key vectors on both sides: one load per column
+    for (u32 k = 0; k < key_count; ++k) {
+        YTGPU_TRY(stage_column(ctx, &primary_keys[k], &sp[k]));
+        YTGPU_TRY(stage_column(ctx, &foreign_keys[k], &sf[k]));
+        KP.col[k] = sp[k].dev;
+        KF.col[k] = sf[k].dev;
+        for (const ColumnDev* c : {&sp[k].dev, &sf[k].dev}) direct = direct && is_direct64(*c) && c->base == 0 && !c->zigzag;
+    }
+    bool foreign_direct = true;
+    for (u32 k = 0; k < key_count; ++k) foreign_direct = foreign_direct && is_direct64(sf[k].dev) && sf[k].dev.base == 0 && !sf[k].dev.zigzag;
+
+    // step 1 (an empty foreign side: a one-slot empty table, so every probe ends at once)
+    KeyTable T;
+    if (nf > 0) {
+        YTGPU_TRY(assign_key_slots(ctx, KC_JOIN, KF, foreign_direct, ColumnDev{}, YTGPU_CMP_NONE, 0, nf, nf, &T));
+    } else {
+        T.cap = 1;
+        YTGPU_TRY(T.rep.allocate(ctx, 1));
+        YTGPU_TRY(T.counts.allocate(ctx, 1));
+        YTGPU_CUDA_TRY(cudaMemsetAsync(T.rep.p, 0xff, 4, ctx->stream));
+        YTGPU_CUDA_TRY(cudaMemsetAsync(T.counts.p, 0, 8, ctx->stream));
+    }
+
+    // step 3
+    DevBuf<u32> probe_slot;
+    DevBuf<u64> offsets, scan_sums, total;
+    YTGPU_TRY(probe_slot.allocate(ctx, np));
+    YTGPU_TRY(offsets.allocate(ctx, np));
+    YTGPU_TRY(scan_sums.allocate(ctx, scan_block_count(std::max<u64>(np, T.cap))));
+    YTGPU_TRY(total.allocate(ctx, 2));
+    {
+        KernelTimer t(ctx, KC_JOIN);
+        const int left = kind == YTGPU_JOIN_LEFT;
+        const u32 blocks = blocks_for((np + 1) / 2, 256, 16);
+#define YTGPU_HJ_PROBE(D, N)                                                                                                    \
+    hj_probe_kernel<D, N><<<blocks, 256, 0, ctx->stream>>>(KP, KF, np, T.rep.p, T.cap - 1, T.counts.p, left, probe_slot.p, offsets.p)
+        if (direct && key_count == 1) YTGPU_HJ_PROBE(true, 1);
+        else if (direct && key_count == 2) YTGPU_HJ_PROBE(true, 2);
+        else if (direct) YTGPU_HJ_PROBE(true, 0);
+        else if (key_count == 1) YTGPU_HJ_PROBE(false, 1);
+        else if (key_count == 2) YTGPU_HJ_PROBE(false, 2);
+        else YTGPU_HJ_PROBE(false, 0);
+#undef YTGPU_HJ_PROBE
+        YTGPU_CUDA_TRY(cudaGetLastError());
+    }
+    // step 4
+    {
+        KernelTimer t(ctx, KC_JOIN, 3);
+        exclusive_scan_u64(ctx->stream, offsets.p, np, scan_sums.p, total.p);
+        YTGPU_CUDA_TRY(cudaGetLastError());
+    }
+    u64 pairs = 0;
+    YTGPU_CUDA_TRY(cudaMemcpyAsync(&pairs, total.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    *out_pair_count = pairs;
+    if (!out_primary) return Status{};
+    if (pairs > pairs_capacity)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "the join has %llu pairs, pairs_capacity is %llu", (unsigned long long)pairs,
+                           (unsigned long long)pairs_capacity);
+    if (pairs == 0) return Status{};
+
+    // step 2 (only a foreign side with rows can have matches)
+    DevBuf<u64> slot_start, sort_keys;
+    SortScratch scratch;
+    PermRef perm;
+    if (nf > 0) {
+        YTGPU_TRY(slot_start.allocate(ctx, T.cap));
+        YTGPU_CUDA_TRY(cudaMemcpyAsync(slot_start.p, T.counts.p, T.cap * 8, cudaMemcpyDeviceToDevice, ctx->stream));
+        YTGPU_TRY(sort_keys.allocate(ctx, nf));
+        {
+            KernelTimer t(ctx, KC_JOIN, 4);
+            exclusive_scan_u64(ctx->stream, slot_start.p, T.cap, scan_sums.p, total.p + 1);
+            hj_slot_keys_kernel<<<blocks_for(nf, 256, 8), 256, 0, ctx->stream>>>(T.slot_of_row.p, nf, sort_keys.p);
+            YTGPU_CUDA_TRY(cudaGetLastError());
+        }
+        const u64* chunk[1] = {sort_keys.p};
+        YTGPU_TRY(radix_sort_chunks(ctx, chunk, 1, nf, &scratch, &perm));
+    }
+
+    // step 5
+    const bool host = out_mem == YTGPU_MEM_HOST;
+    DevBuf<u32> tp, tf;
+    u32 *dp = out_primary, *df = out_foreign;
+    if (host) {
+        YTGPU_TRY(tp.allocate(ctx, pairs));
+        YTGPU_TRY(tf.allocate(ctx, pairs));
+        dp = tp.p;
+        df = tf.p;
+    }
+    {
+        KernelTimer t(ctx, KC_JOIN);
+        const u64 tiles = (pairs + kWriteTile - 1) / kWriteTile;
+        hj_write_pairs_kernel<<<(u32)tiles, kWriteThreads, 0, ctx->stream>>>(offsets.p, np, pairs, probe_slot.p, slot_start.p, perm.plan,
+                                                                             perm.idx[0], perm.idx[1], dp, df);
+        YTGPU_CUDA_TRY(cudaGetLastError());
+    }
+    if (host) {
+        YTGPU_TRY(copy_out(ctx, out_primary, dp, pairs * 4, YTGPU_MEM_HOST));
+        YTGPU_TRY(copy_out(ctx, out_foreign, df, pairs * 4, YTGPU_MEM_HOST));
+    }
+    YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return Status{};
+}
+
+// The row indexes of a gather, on the device.
+Status stage_rows(Context* ctx, const u32* rows, u64 count, int mem, DevBuf<u32>* staged, const u32** dev) {
+    if (mem != YTGPU_MEM_HOST) {
+        *dev = rows;
+        return Status{};
+    }
+    YTGPU_TRY(staged->allocate(ctx, count));
+    YTGPU_TRY(copy_in(ctx, staged->p, rows, count * 4, YTGPU_MEM_HOST));
+    *dev = staged->p;
+    return Status{};
+}
+
+Status gather_column_impl(Context* ctx, const ytgpu_column_view* column, const u32* rows, u64 count, u64* out_values, u8* out_null_bitmap,
+                          u64* out_null_count, int out_mem) {
+    if (!column) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null column");
+    if (out_mem != YTGPU_MEM_DEVICE && out_mem != YTGPU_MEM_HOST)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "out_mem must be YTGPU_MEM_DEVICE or YTGPU_MEM_HOST");
+    if (count && (!rows || !out_values || !out_null_bitmap)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null rows or output");
+    if (!join_key_type(column->value_type))
+        return make_status(YTGPU_ERR_UNSUPPORTED, "value type 0x%x is not INT64, UINT64, DOUBLE or BOOLEAN", column->value_type);
+    if (out_null_count) *out_null_count = 0;
+    YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (count == 0) return Status{};
+    StagedColumn sc;
+    YTGPU_TRY(stage_column(ctx, column, &sc));
+    DevBuf<u32> staged_rows;
+    const u32* drows = nullptr;
+    YTGPU_TRY(stage_rows(ctx, rows, count, out_mem, &staged_rows, &drows));
+    const u64 words = (count + 63) / 64;
+    const bool host = out_mem == YTGPU_MEM_HOST;
+    DevBuf<u64> tv, tb;
+    DevBuf<unsigned long long> nulls;
+    u64* dv = out_values;
+    u32* db = reinterpret_cast<u32*>(out_null_bitmap);
+    if (host) {
+        YTGPU_TRY(tv.allocate(ctx, count));
+        YTGPU_TRY(tb.allocate(ctx, words));
+        dv = tv.p;
+        db = reinterpret_cast<u32*>(tb.p);
+    }
+    YTGPU_TRY(nulls.allocate(ctx, 1));
+    YTGPU_CUDA_TRY(cudaMemsetAsync(nulls.p, 0, 8, ctx->stream));
+    {
+        KernelTimer t(ctx, KC_JOIN);
+        hj_gather_kernel<<<blocks_for(words * 64, 256, 16), 256, 0, ctx->stream>>>(sc.dev, (u64)column->value_count, drows, count, dv, db,
+                                                                                   nulls.p, ctx->dev_err);
+        YTGPU_CUDA_TRY(cudaGetLastError());
+    }
+    if (host) {
+        YTGPU_TRY(copy_out(ctx, out_values, dv, count * 8, YTGPU_MEM_HOST));
+        YTGPU_TRY(copy_out(ctx, out_null_bitmap, db, words * 8, YTGPU_MEM_HOST));
+    }
+    unsigned long long null_count = 0;
+    YTGPU_CUDA_TRY(cudaMemcpyAsync(&null_count, nulls.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    YTGPU_TRY(check_device_errors(ctx));  // synchronises
+    if (out_null_count) *out_null_count = null_count;
+    return Status{};
+}
+
+Status gather_string_column_impl(Context* ctx, const ytgpu_string_column* column, const u32* rows, u64 count, u64* out_starts,
+                                 u32* out_lengths, u8* out_null_bytemap, int out_mem) {
+    if (!column) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null column");
+    if (out_mem != YTGPU_MEM_DEVICE && out_mem != YTGPU_MEM_HOST)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "out_mem must be YTGPU_MEM_DEVICE or YTGPU_MEM_HOST");
+    if (column->mem != YTGPU_MEM_DEVICE && column->mem != YTGPU_MEM_HOST)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "column mem must be YTGPU_MEM_DEVICE or YTGPU_MEM_HOST");
+    const u64 n = column->row_count;
+    if (n && (!column->starts || !column->lengths)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null starts or lengths");
+    if (count && (!rows || !out_starts || !out_lengths || !out_null_bytemap))
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null rows or output");
+    YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (count == 0) return Status{};
+    // the heap is never read: only starts, lengths and the null bytemap move
+    DevBuf<u64> cs;
+    DevBuf<u32> cl;
+    DevBuf<u8> cn;
+    const u64* ds = column->starts;
+    const u32* dl = column->lengths;
+    const u8* dn = column->null_bytemap;
+    if (column->mem == YTGPU_MEM_HOST && n) {
+        YTGPU_TRY(cs.allocate(ctx, n));
+        YTGPU_TRY(cl.allocate(ctx, n));
+        YTGPU_TRY(copy_in(ctx, cs.p, column->starts, n * 8, YTGPU_MEM_HOST));
+        YTGPU_TRY(copy_in(ctx, cl.p, column->lengths, n * 4, YTGPU_MEM_HOST));
+        ds = cs.p;
+        dl = cl.p;
+        if (dn) {
+            YTGPU_TRY(cn.allocate(ctx, n));
+            YTGPU_TRY(copy_in(ctx, cn.p, column->null_bytemap, n, YTGPU_MEM_HOST));
+            dn = cn.p;
+        }
+    }
+    DevBuf<u32> staged_rows;
+    const u32* drows = nullptr;
+    YTGPU_TRY(stage_rows(ctx, rows, count, out_mem, &staged_rows, &drows));
+    const bool host = out_mem == YTGPU_MEM_HOST;
+    DevBuf<u64> ts;
+    DevBuf<u32> tl;
+    DevBuf<u8> tn;
+    u64* os = out_starts;
+    u32* ol = out_lengths;
+    u8* on = out_null_bytemap;
+    if (host) {
+        YTGPU_TRY(ts.allocate(ctx, count));
+        YTGPU_TRY(tl.allocate(ctx, count));
+        YTGPU_TRY(tn.allocate(ctx, count));
+        os = ts.p;
+        ol = tl.p;
+        on = tn.p;
+    }
+    {
+        KernelTimer t(ctx, KC_JOIN);
+        hj_gather_strings_kernel<<<blocks_for(count, 256, 16), 256, 0, ctx->stream>>>(ds, dl, dn, n, drows, count, os, ol, on, ctx->dev_err);
+        YTGPU_CUDA_TRY(cudaGetLastError());
+    }
+    if (host) {
+        YTGPU_TRY(copy_out(ctx, out_starts, os, count * 8, YTGPU_MEM_HOST));
+        YTGPU_TRY(copy_out(ctx, out_lengths, ol, count * 4, YTGPU_MEM_HOST));
+        YTGPU_TRY(copy_out(ctx, out_null_bytemap, on, count, YTGPU_MEM_HOST));
+    }
+    return check_device_errors(ctx);  // synchronises
+}
+
+}  // namespace
+
+extern "C" {
+
+int ytgpu_hash_join(ytgpu_context* h, const ytgpu_column_view* primary_keys, const ytgpu_column_view* foreign_keys, uint32_t key_count,
+                    int kind, uint32_t* out_primary_rows, uint32_t* out_foreign_rows, uint64_t pairs_capacity, uint64_t* out_pair_count,
+                    int out_mem, ytgpu_error* err) {
+    if (!h) return fill_error(err, make_status(YTGPU_ERR_INVALID_ARGUMENT, "null context"));
+    CtxLock lock(h);
+    return fill_error(err, hash_join_impl(as_context(h), primary_keys, foreign_keys, key_count, kind, out_primary_rows, out_foreign_rows,
+                                          pairs_capacity, out_pair_count, out_mem));
+}
+
+int ytgpu_gather_column(ytgpu_context* h, const ytgpu_column_view* column, const uint32_t* rows, uint64_t count, uint64_t* out_values,
+                        uint8_t* out_null_bitmap, uint64_t* out_null_count, int out_mem, ytgpu_error* err) {
+    if (!h) return fill_error(err, make_status(YTGPU_ERR_INVALID_ARGUMENT, "null context"));
+    CtxLock lock(h);
+    return fill_error(err, gather_column_impl(as_context(h), column, rows, count, out_values, out_null_bitmap, out_null_count, out_mem));
+}
+
+int ytgpu_gather_string_column(ytgpu_context* h, const ytgpu_string_column* column, const uint32_t* rows, uint64_t count,
+                               uint64_t* out_starts, uint32_t* out_lengths, uint8_t* out_null_bytemap, int out_mem, ytgpu_error* err) {
+    if (!h) return fill_error(err, make_status(YTGPU_ERR_INVALID_ARGUMENT, "null context"));
+    CtxLock lock(h);
+    return fill_error(err, gather_string_column_impl(as_context(h), column, rows, count, out_starts, out_lengths, out_null_bytemap,
+                                                     out_mem));
+}
+
+}  // extern "C"

@@ -798,6 +798,70 @@ class GpuContext:
         return dict(keys=[k[:g] for k in keys], key_null=[k[:g] for k in kn], values=[v[:g] for v in vals],
                     value_null=[v[:g] for v in vn], count=counts[:g], first_row=first[:g])
 
+    def hash_join(self, primary_keys, foreign_keys, kind: int = capi.JOIN_INNER, count_only: bool = False,
+                  capacity: int | None = None, out_mem: int | None = None):
+        """Hash JOIN of key tuples (ytgpu_hash_join): primary_keys and foreign_keys are lists of Column, key k of one type on
+        both sides.  -> (primary rows, foreign rows): the pairs in ascending (primary, foreign) order, a LEFT join's unmatched
+        primary row paired with capi.JOIN_NO_ROW, as uint32 arrays (int32 tensors in DEVICE memory); with count_only, the
+        pair count.  The outputs are in out_mem (default: the primary keys' memory).  Without a capacity a count query sizes
+        them first; a capacity below the count raises YtGpuError with .pair_count set."""
+        pviews = [c.view() for c in primary_keys]
+        fviews = [c.view() for c in foreign_keys]
+        if out_mem is None:
+            out_mem = pviews[0].mem if pviews else capi.MEM_HOST
+        parr = (capi.ColumnView * max(len(pviews), 1))(*pviews)
+        farr = (capi.ColumnView * max(len(fviews), 1))(*fviews)
+        count = C.c_uint64(0)
+        err = capi.Error()
+
+        def call(prim=None, fore=None, cap=0):
+            code = self.lib.ytgpu_hash_join(self.handle, C.cast(parr, C.c_void_p), C.cast(farr, C.c_void_p), len(pviews), kind,
+                                            _ptr_mem(prim)[0], _ptr_mem(fore)[0], cap, C.byref(count), out_mem, C.byref(err))
+            if code != capi.OK:
+                e = capi.YtGpuError(code, err.message.decode(errors="replace"), err.cuda_error)
+                e.pair_count = int(count.value)  # the needed capacity when that was too small
+                raise e
+        if count_only or capacity is None:
+            call()
+            if count_only:
+                return int(count.value)
+            capacity = int(count.value)
+        prim = self._out((max(capacity, 1),), np.uint32, out_mem)
+        fore = self._out((max(capacity, 1),), np.uint32, out_mem)
+        call(prim, fore, capacity)
+        pairs = int(count.value)
+        return prim[:pairs], fore[:pairs]
+
+    def gather_column(self, column: "Column", rows):
+        """ytgpu_gather_column: `column` decoded at rows (uint32; capi.JOIN_NO_ROW gives NULL) -> dict(values, null_bitmap,
+        null_count, column) in the rows' memory flavour, laid out as evaluate_expression's result: `column` is a Column over
+        them (without the bitmap when no row is NULL)."""
+        view = column.view()
+        rp, mem = _ptr_mem(rows)
+        count = rows.numel() if _is_tensor(rows) else rows.size
+        values = self._out((count,), np.uint64, mem)
+        null_bitmap = self._out(((count + 63) // 64 * 8,), np.uint8, mem)
+        nulls = C.c_uint64(0)
+        err = capi.Error()
+        capi.check(self.lib.ytgpu_gather_column(self.handle, C.byref(view), rp, count, _ptr_mem(values)[0], _ptr_mem(null_bitmap)[0],
+                                                C.byref(nulls), mem, C.byref(err)), err)
+        out = Column(column.value_type, values=values, value_count=count, null_bitmap=null_bitmap if nulls.value else None)
+        return dict(values=values, null_bitmap=null_bitmap, null_count=int(nulls.value), column=out)
+
+    def gather_string_column(self, heap, starts, lengths, nulls, rows):
+        """ytgpu_gather_string_column: the string column (heap, starts, lengths, nulls or None) at rows -> (heap, starts,
+        lengths, null_bytemap), the gathered arrays in the rows' memory flavour and the heap itself, not copied."""
+        scol = _string_column(heap, starts, lengths, nulls)
+        rp, mem = _ptr_mem(rows)
+        count = rows.numel() if _is_tensor(rows) else rows.size
+        ostarts = self._out((count,), np.uint64, mem)
+        olengths = self._out((count,), np.uint32, mem)
+        onulls = self._out((count,), np.uint8, mem)
+        err = capi.Error()
+        capi.check(self.lib.ytgpu_gather_string_column(self.handle, C.byref(scol), rp, count, _ptr_mem(ostarts)[0], _ptr_mem(olengths)[0],
+                                                       _ptr_mem(onulls)[0], mem, C.byref(err)), err)
+        return heap, ostarts, olengths, onulls
+
     @staticmethod
     def _program_columns(caller, columns, string_columns):
         """Column arrays of an evaluator call -> (ColumnView array, views, StringColumn array, mem and n of column 0)."""
