@@ -410,7 +410,18 @@ public:
     TQueryStatistics Run(const TMultiGroupQuery& query, const ISchemalessMultiChunkReaderPtr& reader,
                          const IUnversionedRowsetWriterPtr& writer) override {
         TQueryStatistics stats;
-        if (query.GroupColumns.empty() || query.GroupColumns.size() > 8) throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "1..8 group items");
+        const bool project = !query.Project.empty();
+        if (project) {
+            if (!query.GroupColumns.empty() || !query.AggregateItems.empty())
+                throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "Project is the output row of a query without GROUP BY: no group or aggregate items");
+            if (query.Having) throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "Having without GROUP BY");
+        } else if (query.GroupColumns.empty() || query.GroupColumns.size() > 8) {
+            throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "1..8 group items");
+        }
+        if (!query.OrderBy.empty() && !query.Limit) throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "ORDER BY used without LIMIT");
+        if (query.Offset != 0 && query.OrderBy.empty()) throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "OFFSET used without ORDER BY");
+        if (query.Offset < 0 || (query.Limit && *query.Limit < 0)) throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "negative OFFSET or LIMIT");
+        if (query.OrderBy.size() > 32) throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "at most 32 ORDER BY items");
         // the columns the query touches, each flattened once: 64-bit payloads + a null bitmap, or (strings) one heap with
         // starts, lengths and a null bytemap
         struct TFlatColumn {
@@ -434,6 +445,8 @@ public:
         };
         std::vector<int> keyIndex, aggIndex, byIndex;
         for (int position : query.GroupColumns) keyIndex.push_back(columnIndex(position));
+        std::vector<int> projectIndex;
+        for (int position : query.Project) projectIndex.push_back(columnIndex(position));
         for (const auto& item : query.AggregateItems) {
             aggIndex.push_back(columnIndex(item.Column));
             const bool arg = item.Function == EAggregateFunction::ArgMin || item.Function == EAggregateFunction::ArgMax;
@@ -443,11 +456,12 @@ public:
         const int whereIndex = query.WhereOp != EBinaryOp::None ? columnIndex(query.WhereColumn) : -1;
         if (query.Where && query.WhereOp != EBinaryOp::None)
             throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "a query has either Where or WhereColumn / WhereOp");
-        // with computed columns the WhereOp form runs as a one-node COMPARE program: the WHERE is then one filter pass that
-        // comes before the computed columns it does not read (its constant gets the column's type once that is known)
+        // with computed columns, or without GROUP BY, the WhereOp form runs as a one-node COMPARE program: the WHERE is then
+        // one filter pass that comes before the computed columns it does not read (its constant gets the column's type once
+        // that is known)
         std::optional<TFilterExpression> where = query.Where;
         const bool whereOpAsProgram = query.WhereOp != EBinaryOp::None &&
-            std::any_of(columns.begin(), columns.end(), [](const TFlatColumn& c) { return TMultiGroupQuery::IsComputedColumn(c.Position); });
+            (project || std::any_of(columns.begin(), columns.end(), [](const TFlatColumn& c) { return TMultiGroupQuery::IsComputedColumn(c.Position); }));
         if (whereOpAsProgram) {
             where = TFilterExpression().Compare(query.WhereColumn, query.WhereOp, query.WhereConstant);
             where->Nodes[0].Constant.Bits = query.WhereConstant.Data.Uint64;  // the built-in predicate's bits
@@ -834,6 +848,139 @@ public:
                 if (values[g] == 1 && !((nulls[g >> 6] >> (g & 63)) & 1)) kept[g >> 6] |= 1ull << (g & 63);
             return kept;
         };
+        // ORDER BY, OFFSET and LIMIT over the output row -> the rows written, in order.  `views` are the output row's positions
+        // (rowCount rows each; a string position's view has value_type STRING), strings[p] position p as a flat string column
+        // when it holds strings, `selection` the rows WHERE / HAVING keep and `kept` their list (nullptr: every row).  The items
+        // are evaluated over the kept rows only; one ytgpu_order_rows call orders the kept rows and cuts the window.  Without
+        // ORDER BY the window is the first Limit kept rows.  With an empty window the items are checked over zero rows, so a
+        // malformed item is refused whatever the data.
+        auto orderWindow = [&](const std::vector<ytgpu_column_view>& views, const std::vector<std::optional<ytgpu_string_column>>& strings,
+                               const uint8_t* selection, const std::vector<uint32_t>* kept, uint64_t rowCount) {
+            const uint64_t candidates = kept ? kept->size() : rowCount;
+            const uint64_t offset = (uint64_t)query.Offset, limit = query.Limit ? (uint64_t)*query.Limit : candidates;
+            const uint64_t count = std::min(limit, candidates - std::min(offset, candidates));
+            std::vector<uint32_t> window(count);
+            if (query.OrderBy.empty()) {
+                for (uint64_t i = 0; i < count; ++i) window[i] = kept ? (*kept)[i] : (uint32_t)i;
+                return window;
+            }
+            std::vector<ytgpu_column_view> none;  // the views over zero rows
+            if (count == 0) {
+                none = views;
+                for (auto& v : none) {
+                    v.value_count = 0;
+                    v.values_count = 0;
+                    v.has_values = 0;
+                    v.values = nullptr;
+                    v.null_bitmap = nullptr;
+                }
+                rowCount = 0;
+                selection = nullptr;
+            }
+            const auto& itemViews = count == 0 ? none : views;
+            std::vector<ytgpu_column_view> orderColumns;
+            std::vector<ytgpu_string_column> orderStrings;
+            std::vector<ytgpu_order_item> items;
+            std::vector<std::vector<uint64_t>> values, nulls;  // the evaluated items
+            values.reserve(query.OrderBy.size());
+            nulls.reserve(query.OrderBy.size());
+            for (size_t i = 0; i < query.OrderBy.size(); ++i) {
+                const auto& item = query.OrderBy[i];
+                const uint8_t descending = item.Descending ? 1 : 0;
+                const auto& nodes = item.Expression.Nodes;
+                if (nodes.size() == 1 && nodes[0].Op == EExpressionOp::Column) {
+                    const int p = nodes[0].Column;
+                    if (p < 0 || (size_t)p >= views.size())
+                        throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "order by item " + std::to_string(i) + ": no output position " + std::to_string(p));
+                    if (strings[p]) {
+                        items.push_back({(uint32_t)orderStrings.size(), 1, descending, 0});
+                        orderStrings.push_back(*strings[p]);
+                    } else {
+                        items.push_back({(uint32_t)orderColumns.size(), 0, descending, 0});
+                        orderColumns.push_back(itemViews[p]);
+                    }
+                    continue;
+                }
+                const auto program = outputProgram(item.Expression, "order by item " + std::to_string(i));
+                values.emplace_back(rowCount);
+                nulls.emplace_back((rowCount + 63) / 64);
+                uint8_t type = 0;
+                evaluateOutput(program, itemViews, selection, values.back().data(), nulls.back().data(), &type);
+                ytgpu_column_view v{};
+                v.value_count = (int64_t)rowCount;
+                v.value_type = type;
+                v.has_values = 1;
+                v.bit_width = 64;
+                v.values = values.back().data();
+                v.values_count = rowCount;
+                v.null_bitmap = reinterpret_cast<const uint8_t*>(nulls.back().data());
+                v.mem = YTGPU_MEM_HOST;
+                items.push_back({(uint32_t)orderColumns.size(), 0, descending, 0});
+                orderColumns.push_back(v);
+            }
+            if (count == 0) return window;
+            uint64_t got = 0;
+            ytgpu_error err{};
+            if (ytgpu_order_rows(GetGpuContext(), orderColumns.data(), (uint32_t)orderColumns.size(), orderStrings.data(), (uint32_t)orderStrings.size(),
+                                 items.data(), (uint32_t)items.size(), kept ? kept->data() : nullptr, candidates, offset, limit, window.data(), &got,
+                                 YTGPU_MEM_HOST, &err) != YTGPU_OK)
+                ThrowFrom(err);
+            return window;
+        };
+        // a string result (and a string key) is the index of a row that holds it
+        auto make = [&](const TFlatColumn* strings, EValueType type, uint64_t bits, bool null, int id) {
+            if (null) return MakeUnversionedNullValue(id);
+            if (strings) return MakeUnversionedStringValue(strings->StringAt(bits), id);
+            switch (type) {
+                case EValueType::Uint64: return MakeUnversionedUint64Value(bits, id);
+                case EValueType::Double: { double d; std::memcpy(&d, &bits, 8); return MakeUnversionedDoubleValue(d, id); }
+                case EValueType::Boolean: return MakeUnversionedBooleanValue(bits != 0, id);
+                default: return MakeUnversionedInt64Value((int64_t)bits, id);
+            }
+        };
+        // the output row's positions
+        struct TOutput {
+            EValueType Type;
+            const TFlatColumn* Strings;
+            const uint64_t* Values;
+            const uint8_t* Null;  // bytemap
+        };
+        // Select over the output row's positions (`rows` rows each) -> the written row's positions.  A bare Column passes its
+        // position through; every other item is one ytgpu_evaluate_expression call over the views (a string position is
+        // refused by the call as UNSUPPORTED), over `selection` only.  selectValues / selectNulls hold the results.
+        std::vector<std::vector<uint64_t>> selectValues, selectNulls;  // selectNulls: null bitmaps
+        auto evaluateSelect = [&](const std::vector<TOutput>& outputs, const std::vector<ytgpu_column_view>& outViews, const uint8_t* selection,
+                                  uint64_t rows) {
+            std::vector<TOutput> selected;
+            selectValues.assign(query.Select->size(), {});
+            selectNulls.assign(query.Select->size(), {});
+            for (size_t s = 0; s < query.Select->size(); ++s) {
+                const auto& nodes = (*query.Select)[s].Nodes;
+                if (nodes.size() == 1 && nodes[0].Op == EExpressionOp::Column) {
+                    if (nodes[0].Column < 0 || (size_t)nodes[0].Column >= outputs.size())
+                        throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "select item " + std::to_string(s) + ": no output position " +
+                                                                              std::to_string(nodes[0].Column));
+                    selected.push_back(outputs[nodes[0].Column]);
+                    continue;
+                }
+                const auto program = outputProgram((*query.Select)[s], "select item " + std::to_string(s));
+                selectValues[s].assign(rows, 0);
+                selectNulls[s].assign((rows + 63) / 64, 0);
+                uint8_t type = 0;
+                evaluateOutput(program, outViews, selection, selectValues[s].data(), selectNulls[s].data(), &type);
+                selected.push_back({(EValueType)type, nullptr, selectValues[s].data(), nullptr});
+            }
+            return selected;
+        };
+        auto writeRow = [&](const std::vector<TOutput>& selected, uint64_t g) {
+            TUnversionedOwningRowBuilder b;
+            for (size_t s = 0; s < selected.size(); ++s) {
+                const TOutput& o = selected[s];
+                const bool null = o.Null ? o.Null[g] != 0 : ((selectNulls[s][g >> 6] >> (g & 63)) & 1) != 0;
+                b.AddValue(make(o.Strings, o.Type, o.Values[g], null, (int)s));
+            }
+            owned.push_back(b.FinishRow());
+        };
         if (n == 0 && query.Having) {  // no rows, no groups: the output row's types from the columns' (NULL: INT64)
             std::vector<ytgpu_column_view> views;
             auto add = [&](EValueType type) {
@@ -849,6 +996,24 @@ public:
                 add(f == EAggregateFunction::Count ? EValueType::Int64 : f == EAggregateFunction::Avg ? EValueType::Double : columns[aggIndex[a]].Type);
             }
             evaluateHaving(views, 0);
+        }
+        if (n == 0 && project) {  // no rows: ORDER BY and Select are still checked, over zero-row views of the output row
+            std::vector<ytgpu_column_view> views;
+            std::vector<std::optional<ytgpu_string_column>> strings;
+            std::vector<TOutput> outputs;
+            for (int i : projectIndex) {
+                const TFlatColumn& c = columns[i];
+                const bool str = c.Type == EValueType::String;
+                ytgpu_column_view v{};
+                v.value_type = (uint8_t)(str ? EValueType::String : c.Type == EValueType::Null ? EValueType::Int64 : c.Type);
+                v.bit_width = 64;
+                v.mem = YTGPU_MEM_HOST;
+                views.push_back(v);
+                strings.push_back(str ? std::optional(ytgpu_string_column{nullptr, 0, nullptr, nullptr, nullptr, 0, YTGPU_MEM_HOST, 0}) : std::nullopt);
+                outputs.push_back({c.Type, str ? &c : nullptr, nullptr, nullptr});
+            }
+            orderWindow(views, strings, nullptr, nullptr, 0);
+            if (query.Select) evaluateSelect(outputs, views, nullptr, 0);
         }
         if (n > 0) {
             auto view = [&](const TFlatColumn& c) {
@@ -1103,9 +1268,72 @@ public:
                 aggregates.push_back(ytgpu_aggregate{ops[(int)query.AggregateItems[a].Function], argIndex[aggIndex[a]],
                                                      byIndex[a] >= 0 ? argIndex[byIndex[a]] : -1, 0});
             }
+            if (project) {
+                // the output row: the projected columns over all rows; the WHERE's rows are the ones ordered
+                std::vector<ytgpu_column_view> projected;
+                std::vector<std::optional<ytgpu_string_column>> strings;
+                for (int i : projectIndex) {
+                    const TFlatColumn& c = columns[i];
+                    projected.push_back(view(c));
+                    strings.push_back(std::nullopt);
+                    if (c.Type == EValueType::String) {
+                        projected.back().value_type = (uint8_t)EValueType::String;
+                        strings.back() = stringView(c);
+                    }
+                }
+                std::vector<uint32_t> kept;
+                if (where)
+                    for (uint64_t r = 0; r < n; ++r)
+                        if ((selection[r >> 3] >> (r & 7)) & 1) kept.push_back((uint32_t)r);
+                const std::vector<uint32_t> rows = orderWindow(projected, strings, where ? selection.data() : nullptr, where ? &kept : nullptr, n);
+                // the output columns gathered at the window's rows: Select sees those rows only.  A string position keeps the
+                // row index into its flat column.
+                const uint64_t m = rows.size();
+                const size_t np = projectIndex.size();
+                std::vector<uint64_t> rowIds(rows.begin(), rows.end());
+                std::vector<std::vector<uint64_t>> gathered(np);
+                std::vector<std::vector<uint8_t>> bitmaps(np), nullBytes(np);
+                std::vector<TOutput> outputs;
+                std::vector<ytgpu_column_view> outViews;
+                for (size_t p = 0; p < np; ++p) {
+                    const TFlatColumn& c = columns[projectIndex[p]];
+                    bitmaps[p].assign((m + 63) / 64 * 8, 0);
+                    nullBytes[p].assign(m, 0);
+                    if (c.Type == EValueType::String) {
+                        for (uint64_t i = 0; i < m; ++i) nullBytes[p][i] = c.NullBytes[rows[i]];
+                    } else if (m > 0) {
+                        gathered[p].assign(m, 0);
+                        const ytgpu_column_view source = view(c);
+                        uint64_t nullCount = 0;
+                        ytgpu_error err{};
+                        if (ytgpu_gather_column(GetGpuContext(), &source, rows.data(), m, gathered[p].data(), bitmaps[p].data(), &nullCount,
+                                                YTGPU_MEM_HOST, &err) != YTGPU_OK)
+                            ThrowFrom(err);
+                    }
+                    for (uint64_t i = 0; i < m; ++i) {
+                        if (c.Type != EValueType::String) nullBytes[p][i] = (bitmaps[p][i >> 3] >> (i & 7)) & 1;
+                        else if (nullBytes[p][i]) bitmaps[p][i >> 3] |= (uint8_t)(1u << (i & 7));
+                    }
+                    const bool str = c.Type == EValueType::String;
+                    outputs.push_back({c.Type, str ? &c : nullptr, str ? rowIds.data() : gathered[p].data(), nullBytes[p].data()});
+                    ytgpu_column_view v{};
+                    v.value_count = (int64_t)m;
+                    v.value_type = (uint8_t)(str ? EValueType::String : c.Type == EValueType::Null ? EValueType::Int64 : c.Type);
+                    v.has_values = m > 0;
+                    v.bit_width = 64;
+                    v.values = m == 0 ? nullptr : str ? rowIds.data() : gathered[p].data();
+                    v.values_count = m;
+                    v.null_bitmap = bitmaps[p].data();
+                    v.mem = YTGPU_MEM_HOST;
+                    outViews.push_back(v);
+                }
+                const std::vector<TOutput> selected = query.Select ? evaluateSelect(outputs, outViews, nullptr, m) : outputs;
+                owned.reserve(m);
+                for (uint64_t i = 0; i < m; ++i) writeRow(selected, i);
+            }
             const size_t nk = keyViews.size(), na = aggregates.size();
             uint64_t cap = std::min<uint64_t>(n, 1 << 16);
-            for (;;) {
+            while (!project) {  // the GROUP BY call, again with the capacity it reports when its first guess was too small
                 std::vector<std::vector<uint64_t>> keys(nk, std::vector<uint64_t>(cap)), values(na, std::vector<uint64_t>(cap));
                 std::vector<std::vector<uint8_t>> keyNull(nk, std::vector<uint8_t>(cap)), valueNull(na, std::vector<uint8_t>(cap));
                 std::vector<uint64_t*> pk, pv;
@@ -1126,25 +1354,8 @@ public:
                     continue;
                 }
                 if (code != YTGPU_OK) ThrowFrom(err);
-                // a string result (and a string key) is the index of a row that holds it
-                auto make = [&](const TFlatColumn* strings, EValueType type, uint64_t bits, bool null, int id) {
-                    if (null) return MakeUnversionedNullValue(id);
-                    if (strings) return MakeUnversionedStringValue(strings->StringAt(bits), id);
-                    switch (type) {
-                        case EValueType::Uint64: return MakeUnversionedUint64Value(bits, id);
-                        case EValueType::Double: { double d; std::memcpy(&d, &bits, 8); return MakeUnversionedDoubleValue(d, id); }
-                        case EValueType::Boolean: return MakeUnversionedBooleanValue(bits != 0, id);
-                        default: return MakeUnversionedInt64Value((int64_t)bits, id);
-                    }
-                };
                 auto stringsOf = [&](int index) { return columns[index].Type == EValueType::String ? &columns[index] : nullptr; };
                 // the output row's positions: group items, then aggregates
-                struct TOutput {
-                    EValueType Type;
-                    const TFlatColumn* Strings;
-                    const uint64_t* Values;
-                    const uint8_t* Null;  // bytemap
-                };
                 std::vector<TOutput> outputs;
                 for (size_t k = 0; k < nk; ++k)
                     outputs.push_back({columns[keyIndex[k]].Type, stringsOf(keyIndex[k]), keys[k].data(), keyNull[k].data()});
@@ -1155,14 +1366,12 @@ public:
                     outputs.push_back({type, f == EAggregateFunction::Count ? nullptr : stringsOf(aggIndex[a]), values[a].data(), valueNull[a].data()});
                 }
                 const uint64_t groups = res.group_count;
-                // Select: a bare Column passes its position through; every other item, and Having, is one
-                // ytgpu_evaluate_expression call over the result arrays (a string position is refused by the call as UNSUPPORTED)
-                std::vector<std::vector<uint64_t>> selectValues, selectNulls;  // selectNulls: null bitmaps
+                // Select, Having and the ORDER BY items are evaluated over the result arrays (evaluateSelect)
                 std::vector<TOutput> selected;
                 std::vector<uint64_t> having;  // Having: bit g set where group g is written
                 std::vector<std::vector<uint8_t>> bitmaps(outputs.size());
                 std::vector<ytgpu_column_view> outViews;
-                if (query.Select || query.Having) {
+                if (query.Select || query.Having || !query.OrderBy.empty()) {
                     for (size_t p = 0; p < outputs.size(); ++p) {
                         bitmaps[p].assign((groups + 63) / 64 * 8, 0);
                         for (uint64_t g = 0; g < groups; ++g)
@@ -1181,44 +1390,50 @@ public:
                     }
                 }
                 if (query.Having) having = evaluateHaving(outViews, groups);
-                // Select is evaluated over the groups Having keeps only, as QL projects after HAVING: a division by zero in a
-                // dropped group does not throw
-                const uint8_t* selectSelection = query.Having ? reinterpret_cast<const uint8_t*>(having.data()) : nullptr;
-                if (query.Select) {
-                    selectValues.resize(query.Select->size());
-                    selectNulls.resize(query.Select->size());
-                    for (size_t s = 0; s < query.Select->size(); ++s) {
-                        const auto& nodes = (*query.Select)[s].Nodes;
-                        if (nodes.size() == 1 && nodes[0].Op == EExpressionOp::Column) {
-                            if (nodes[0].Column < 0 || (size_t)nodes[0].Column >= outputs.size())
-                                throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "select item " + std::to_string(s) + ": no output position " +
-                                                                                      std::to_string(nodes[0].Column));
-                            selected.push_back(outputs[nodes[0].Column]);
-                            continue;
-                        }
-                        const auto program = outputProgram((*query.Select)[s], "select item " + std::to_string(s));
-                        selectValues[s].assign(groups, 0);
-                        selectNulls[s].assign((groups + 63) / 64, 0);
-                        uint8_t type = 0;
-                        evaluateOutput(program, outViews, selectSelection, selectValues[s].data(), selectNulls[s].data(), &type);
-                        selected.push_back({(EValueType)type, nullptr, selectValues[s].data(), nullptr});
+                // ORDER BY, OFFSET and LIMIT over the groups Having keeps: the window's groups, in order
+                const bool windowed = !query.OrderBy.empty() || query.Limit;
+                std::vector<uint32_t> window;
+                std::vector<uint64_t> windowBits;
+                if (windowed) {
+                    std::vector<uint32_t> kept;
+                    for (uint64_t g = 0; query.Having && g < groups; ++g)
+                        if ((having[g >> 6] >> (g & 63)) & 1) kept.push_back((uint32_t)g);
+                    // a string position as a flat column over the groups: its rows' starts and lengths
+                    std::vector<std::optional<ytgpu_string_column>> strings(outputs.size());
+                    std::vector<std::vector<uint64_t>> starts(outputs.size());
+                    std::vector<std::vector<uint32_t>> lengths(outputs.size());
+                    for (size_t p = 0; p < outputs.size() && !query.OrderBy.empty(); ++p) {
+                        const TFlatColumn* S = outputs[p].Strings;
+                        if (!S) continue;
+                        starts[p].assign(groups, 0);
+                        lengths[p].assign(groups, 0);
+                        for (uint64_t g = 0; g < groups; ++g)
+                            if (!outputs[p].Null[g]) {
+                                starts[p][g] = S->Starts[outputs[p].Values[g]];
+                                lengths[p][g] = S->Lengths[outputs[p].Values[g]];
+                            }
+                        strings[p] = ytgpu_string_column{reinterpret_cast<const uint8_t*>(S->Heap.data()), S->Heap.size(), starts[p].data(),
+                                                         lengths[p].data(), outputs[p].Null, groups, YTGPU_MEM_HOST, 0};
                     }
+                    window = orderWindow(outViews, strings, query.Having ? reinterpret_cast<const uint8_t*>(having.data()) : nullptr,
+                                         query.Having ? &kept : nullptr, groups);
+                    windowBits.assign((groups + 63) / 64, 0);
+                    for (uint32_t g : window) windowBits[g >> 6] |= 1ull << (g & 63);
+                }
+                // Select is evaluated over the groups written only, as QL projects after HAVING and LIMIT: a division by zero
+                // in a dropped group does not throw
+                const uint8_t* selectSelection = windowed ? reinterpret_cast<const uint8_t*>(windowBits.data())
+                                               : query.Having ? reinterpret_cast<const uint8_t*>(having.data()) : nullptr;
+                selected = query.Select ? evaluateSelect(outputs, outViews, selectSelection, groups) : outputs;
+                if (windowed) {
+                    owned.reserve(window.size());
+                    for (uint32_t g : window) writeRow(selected, g);
+                    break;
                 }
                 owned.reserve(groups);
                 for (uint64_t g = 0; g < groups; ++g) {  // already in first-seen order
                     if (query.Having && !((having[g >> 6] >> (g & 63)) & 1)) continue;
-                    TUnversionedOwningRowBuilder b;
-                    if (query.Select) {
-                        for (size_t s = 0; s < selected.size(); ++s) {
-                            const TOutput& o = selected[s];
-                            const bool null = o.Null ? o.Null[g] != 0 : ((selectNulls[s][g >> 6] >> (g & 63)) & 1) != 0;
-                            b.AddValue(make(o.Strings, o.Type, o.Values[g], null, (int)s));
-                        }
-                    } else {
-                        for (size_t p = 0; p < outputs.size(); ++p)
-                            b.AddValue(make(outputs[p].Strings, outputs[p].Type, outputs[p].Values[g], outputs[p].Null[g], (int)p));
-                    }
-                    owned.push_back(b.FinishRow());
+                    writeRow(selected, g);
                 }
                 break;
             }

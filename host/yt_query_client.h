@@ -309,6 +309,21 @@ struct TMultiGroupQuery {
     static constexpr int kForeignColumnBase = 1 << 24;
     static constexpr int ForeignColumn(int j) { return kForeignColumnBase + j; }
     static constexpr bool IsForeignColumn(int position) { return position >= kForeignColumnBase; }
+    //! A query WITHOUT GROUP BY: the output row is these positions of the (joined) input rows, input, computed (string
+    //! results included) or foreign columns.  Non-empty exactly when GroupColumns and AggregateItems are empty.  Select then
+    //! names positions of this output row, as it names group / aggregate positions otherwise; Having is refused.
+    std::vector<int> Project;
+    //! ORDER BY: expressions over output-row positions, as Having's, compared in turn.  A bare Column item may name a string
+    //! position (a string group item, a string MIN / MAX, a projected string); any other item is a numeric expression.
+    struct TOrderItem {
+        TExpression Expression;
+        bool Descending = false;
+    };
+    std::vector<TOrderItem> OrderBy;
+    //! LIMIT and OFFSET: the rows written are positions [Offset, Offset + Limit) of the ordered rows.  OrderBy needs a Limit
+    //! and a non-zero Offset needs OrderBy, as QL's query preparer requires.
+    std::optional<int64_t> Limit;
+    int64_t Offset = 0;
 };
 
 struct TQueryStatistics {
@@ -343,6 +358,13 @@ struct IEvaluator {
     //! unchanged over the joined rows: WHERE filters joined rows, the SQL meaning for both kinds.  So, beside the note on
     //! division errors: a computed column or WHERE is not evaluated over a primary row that an INNER join drops.  RowsRead
     //! counts primary rows.  A query without Join runs exactly as before.
+    //! Evaluation order, as QL plans it: scan (+ JOIN) -> WHERE -> computed columns -> GROUP BY -> HAVING -> ORDER BY, OFFSET
+    //! and LIMIT -> SELECT -> write.  ORDER BY items are evaluated over the rows WHERE keeps (a projection) or the groups
+    //! HAVING keeps only; one ytgpu_order_rows call over those rows gives the window.  Without ORDER BY, LIMIT keeps the first
+    //! rows WHERE keeps in input (joined) order, or the first groups HAVING keeps in first-seen order.  SELECT is evaluated
+    //! over the window only: a projection's output columns are gathered at the window rows first, a grouped query's Select
+    //! runs over the window's groups; so a division by zero outside the window does not throw.  RowsWritten counts the rows
+    //! written.  A query that sets none of Project, OrderBy, Limit and Offset runs exactly as before.
     virtual TQueryStatistics Run(const TMultiGroupQuery& query, const ISchemalessMultiChunkReaderPtr& reader,
                                  const IUnversionedRowsetWriterPtr& writer) = 0;
 };

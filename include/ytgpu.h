@@ -652,6 +652,44 @@ int ytgpu_gather_string_column(ytgpu_context* ctx, const ytgpu_string_column* co
                                uint64_t count, uint64_t* out_starts, uint32_t* out_lengths, uint8_t* out_null_bytemap,
                                int out_mem, ytgpu_error* err);
 
+/* ---- ORDER BY ... OFFSET ... LIMIT over typed columns ----
+ * The order of YT QL's OrderOpHelper (library/query/engine/cg_routines/registry.cpp:1948) and its TTopCollector
+ * (engine_api/top_collector.h), computed as ONE stable sort of the rows being ordered followed by a window.
+ * Inputs.  Item k names columns[column] (INT64, UINT64, DOUBLE or BOOLEAN, in any encoding the GROUP BY calls take:
+ * plain widths, bit-packed, dictionary, RLE, boolean bitmap, Arrow validity, start_index windows) or, with is_string,
+ * string_columns[column] (flat string columns; each may have its own heap).  Every item column holds the same number of
+ * rows L.  Columns not named by an item are not read.
+ * Order.  Items are compared in turn, each in the unversioned value order of ytgpu_sort_rowset (compare-inl.h:49-66):
+ * NULL below every value; false below true; a NaN above +inf, all NaNs equal; -0.0 equal to +0.0; strings as unsigned
+ * bytes, a prefix first.  `descending` reverses one item, its NULLs then come last.  Rows equal on every item keep their
+ * order in `rows` (ascending row index when `rows` is NULL): the sort is stable, which is one of the orders the
+ * reference's heap may produce.  That QL's generated ORDER BY comparer orders NaN and NULL this way is recalled, not read.
+ * Output.  out_rows[i] is the ROW INDEX (not the position in `rows`) of the row at position offset + i of that order,
+ * for i < *out_count = min(limit, row_count - min(offset, row_count)).  out_rows NULL is a count query: *out_count is
+ * written and nothing is launched; so is a window of 0 rows (limit == 0, offset >= row_count).
+ * Limits and errors.  row_count < 2^30 (the radix sort's bound), checked before any access: UNSUPPORTED otherwise.
+ * 1 .. 32 items.  INVALID_ARGUMENT: a row index >= L (checked on the device, no byte outside a column is read); item
+ * columns of different lengths; an item naming a missing column; a non-zero `reserved`; a null out_count; a string
+ * value whose [start, start + length) leaves its heap (checked on the device).  UNSUPPORTED: another value type.
+ * Memory and launches.  `rows` and out_rows are in out_mem, each column in its own mem (HOST columns are copied to the
+ * device first).  One kernel writes the rows in `rows` order as a device rowset of item_count values each (numeric
+ * items decoded, string starts rebased into one heap: the string heaps concatenated), the stable sort of
+ * ytgpu_sort_rowset runs over it (keys of any length, "last_sort_refine_rounds" as there), one kernel writes the window.
+ * The call synchronises the context's stream before returning. */
+typedef struct ytgpu_order_item {
+    uint32_t column;     /* index into columns[], or into string_columns[] when is_string */
+    uint8_t is_string;
+    uint8_t descending;
+    uint16_t reserved;   /* 0 */
+} ytgpu_order_item;
+
+int ytgpu_order_rows(ytgpu_context* ctx, const ytgpu_column_view* columns, uint32_t column_count,
+                     const ytgpu_string_column* string_columns, uint32_t string_column_count,
+                     const ytgpu_order_item* items /* host */, uint32_t item_count,
+                     const uint32_t* rows /* out_mem, nullable: rows 0 .. row_count - 1 */, uint64_t row_count,
+                     uint64_t offset, uint64_t limit, uint32_t* out_rows, uint64_t* out_count /* host */,
+                     int out_mem, ytgpu_error* err);
+
 /* ---- WHERE expressions: a selection over several columns ----
  * The filter of YT QL's ScanOpHelper / FilterOpHelper (the WHERE clause compiled by the query evaluator) and of
  * ClickHouse's FilterTransform, for expressions built of comparisons, IN lists, NULL tests, prefix and substring tests and

@@ -120,7 +120,7 @@ EXPORTED_SYMBOLS = [
     "ytgpu_block_agg_state_init", "ytgpu_block_combine_all",
     "ytgpu_build_bitmap_from_flags", "ytgpu_build_bytemap_from_flags", "ytgpu_count_flags", "ytgpu_build_dictionary_indexes",
     "ytgpu_count_total_string_length", "ytgpu_translate_rle_indexes", "ytgpu_context_get_option", "ytgpu_convert_ch_column_to_values", "ytgpu_convert_string_column_to_ch", "ytgpu_decode_column_typed",
-    "ytgpu_hash_join", "ytgpu_gather_column", "ytgpu_gather_string_column",
+    "ytgpu_hash_join", "ytgpu_gather_column", "ytgpu_gather_string_column", "ytgpu_order_rows",
 ]
 
 FLAGS_DICTIONARY_ZERO, FLAGS_BITMAP = 0, 1
@@ -160,6 +160,14 @@ class Aggregate(C.Structure):
 class StringColumn(C.Structure):
     _fields_ = [("heap", C.c_void_p), ("heap_bytes", C.c_uint64), ("starts", C.c_void_p), ("lengths", C.c_void_p),
                 ("null_bytemap", C.c_void_p), ("row_count", C.c_uint64), ("mem", C.c_int32), ("reserved", C.c_int32)]
+
+
+ORDER_MAX_ITEMS = 32
+ORDER_MAX_ROWS = 1 << 30  # exclusive
+
+
+class OrderItem(C.Structure):
+    _fields_ = [("column", C.c_uint32), ("is_string", C.c_uint8), ("descending", C.c_uint8), ("reserved", C.c_uint16)]
 
 
 (FILTER_COMPARE, FILTER_COMPARE_COLUMNS, FILTER_IN, FILTER_STARTS_WITH, FILTER_IS_NULL, FILTER_IS_NOT_NULL, FILTER_AND, FILTER_OR,
@@ -375,6 +383,9 @@ def load() -> C.CDLL:
                                         C.POINTER(C.c_uint64), C.c_int, C.POINTER(Error)]
     lib.ytgpu_gather_string_column.argtypes = [C.c_void_p, C.POINTER(StringColumn), C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
                                                C.c_void_p, C.c_int, C.POINTER(Error)]
+    lib.ytgpu_order_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(OrderItem), C.c_uint32,
+                                     C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p, C.POINTER(C.c_uint64), C.c_int,
+                                     C.POINTER(Error)]
     lib.ytgpu_extract_column.argtypes = [C.c_void_p, C.POINTER(RowsetView), C.c_uint32, C.c_uint8, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_int, C.POINTER(Error)]
     lib.ytgpu_block_agg_state_init.argtypes = [C.POINTER(BlockAggState), C.c_uint8, C.c_uint8]

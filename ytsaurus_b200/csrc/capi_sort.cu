@@ -1,6 +1,7 @@
 // capi_sort.cu — C ABI: sort / merge entry points (see include/ytgpu.h for the reference interfaces).
 #include <vector>
 
+#include "columnar.cuh"
 #include "context.cuh"
 #include "keys.cuh"
 #include "long_keys.cuh"
@@ -430,3 +431,225 @@ int ytgpu_join_sorted_runs(ytgpu_context* h, const ytgpu_rowset_view* in, const 
 }
 
 }  // extern "C"
+
+// ---- ORDER BY ... OFFSET ... LIMIT over typed columns (ytgpu_order_rows) ----
+// The rows to order are written as a device rowset, one 16-byte value per item, and sorted by RowsetSort: the order, the
+// string widths, the packed / hybrid schedules and the long-key refinement are those of ytgpu_sort_rowset.
+namespace {
+
+constexpr u64 kMaxOrderRows = 1ull << 30;  // the radix sort's bound
+
+struct OrderItemDev {
+    ColumnDev col;          // numeric item
+    const u64* starts;      // string item
+    const u32* lengths;
+    const u8* nulls;        // nullable
+    u64 heap_base;          // offset of the column's heap in the concatenated heap
+    u64 heap_bytes;
+    u8 is_string;
+    u8 type;                // the declared type of the sort key
+};
+
+// Position i of the rowset holds row rows[i] (or i): value k is item k of that row, NULL when the row's value is NULL.
+// A row index past the columns writes NULLs and flags DE_ROW_OUT_OF_RANGE; a string past its heap, DE_STRING_OUT_OF_HEAP.
+__global__ void __launch_bounds__(256) order_materialize_kernel(const OrderItemDev* __restrict__ items, u32 item_count, u64 column_rows,
+                                                                const u32* __restrict__ rows, u64 count, ytgpu_value* __restrict__ out,
+                                                                u32* err_word) {
+    u32 err = 0;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (u64)gridDim.x * blockDim.x) {
+        const u64 r = rows ? rows[i] : i;
+        const bool bad = r >= column_rows;
+        if (bad) err |= DE_ROW_OUT_OF_RANGE;
+        for (u32 k = 0; k < item_count; ++k) {
+            const OrderItemDev& it = items[k];
+            ytgpu_value v{};
+            v.id = (u16)k;
+            v.type = YTGPU_TYPE_NULL;
+            if (!bad) {
+                if (it.is_string) {
+                    if (!(it.nulls && it.nulls[r])) {
+                        const u64 s = it.starts[r];
+                        const u32 len = it.lengths[r];
+                        if (s > it.heap_bytes || len > it.heap_bytes - s) {
+                            err |= DE_STRING_OUT_OF_HEAP;
+                        } else {
+                            v.type = YTGPU_TYPE_STRING;
+                            v.length = len;
+                            v.data = it.heap_base + s;
+                        }
+                    }
+                } else {
+                    bool nul = false;
+                    const u64 x = decode_at(it.col, (i64)r, &nul);
+                    if (!nul) {
+                        v.type = it.type;
+                        v.data = it.type == YTGPU_TYPE_BOOLEAN ? (x != 0) : x;
+                    }
+                }
+            }
+            out[i * item_count + k] = v;
+        }
+    }
+    if (err) atomicOr(err_word, err);
+}
+
+// out[i] = the row at sorted position offset + i.
+__global__ void __launch_bounds__(256) order_window_kernel(const SortPlan* plan, const u32* pa, const u32* pb, const u32* __restrict__ rows,
+                                                           u64 offset, u64 count, u32* __restrict__ out) {
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (u64)gridDim.x * blockDim.x) {
+        const u32 p = perm_at(plan, pa, pb, offset + i);
+        out[i] = rows ? rows[p] : p;
+    }
+}
+
+bool order_numeric_type(u8 t) { return t == YTGPU_TYPE_INT64 || t == YTGPU_TYPE_UINT64 || t == YTGPU_TYPE_DOUBLE || t == YTGPU_TYPE_BOOLEAN; }
+
+Status order_rows_impl(Context* ctx, const ytgpu_column_view* columns, u32 column_count, const ytgpu_string_column* string_columns,
+                       u32 string_column_count, const ytgpu_order_item* items, u32 item_count, const u32* rows, u64 row_count, u64 offset,
+                       u64 limit, u32* out_rows, u64* out_count, int out_mem) {
+    if (row_count >= kMaxOrderRows)
+        return make_status(YTGPU_ERR_UNSUPPORTED, "at most 2^30 - 1 rows are ordered (the radix sort's bound), got %llu",
+                           (unsigned long long)row_count);
+    if (!out_count) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null out_count");
+    if (!items || item_count == 0 || item_count > (u32)kMaxKeyColumns)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "item count must be in [1, %d]", kMaxKeyColumns);
+    if (out_mem != YTGPU_MEM_DEVICE && out_mem != YTGPU_MEM_HOST)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "out_mem must be YTGPU_MEM_DEVICE or YTGPU_MEM_HOST");
+    i64 column_rows = -1;
+    for (u32 k = 0; k < item_count; ++k) {
+        const ytgpu_order_item& it = items[k];
+        if (it.reserved != 0) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "item %u: reserved must be 0", k);
+        i64 len;
+        if (it.is_string) {
+            if (!string_columns || it.column >= string_column_count)
+                return make_status(YTGPU_ERR_INVALID_ARGUMENT, "item %u: no string column %u", k, it.column);
+            const ytgpu_string_column& s = string_columns[it.column];
+            if (s.mem != YTGPU_MEM_DEVICE && s.mem != YTGPU_MEM_HOST)
+                return make_status(YTGPU_ERR_INVALID_ARGUMENT, "item %u: string column mem must be YTGPU_MEM_DEVICE or YTGPU_MEM_HOST", k);
+            if (s.row_count && (!s.starts || !s.lengths))
+                return make_status(YTGPU_ERR_INVALID_ARGUMENT, "item %u: null starts or lengths", k);
+            if (s.heap_bytes && !s.heap) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "item %u: null heap", k);
+            len = (i64)s.row_count;
+        } else {
+            if (!columns || it.column >= column_count) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "item %u: no column %u", k, it.column);
+            const ytgpu_column_view& c = columns[it.column];
+            if (!order_numeric_type(c.value_type))
+                return make_status(YTGPU_ERR_UNSUPPORTED, "item %u: value type 0x%x is not INT64, UINT64, DOUBLE or BOOLEAN", k, c.value_type);
+            if (c.value_count < 0 || c.start_index < 0) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "item %u: negative column range", k);
+            len = c.value_count;
+        }
+        if (column_rows >= 0 && len != column_rows) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "item columns differ in length");
+        column_rows = len;
+    }
+    if (!rows && row_count > (u64)column_rows)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "without rows, row_count (%llu) exceeds the columns' length (%lld)",
+                           (unsigned long long)row_count, (long long)column_rows);
+    const u64 n = row_count;
+    const u64 window = std::min(limit, n - std::min(offset, n));
+    *out_count = window;
+    if (!out_rows || window == 0) return Status{};
+    ctx->last_sort_refine_rounds = 0;
+    YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
+
+    DevBuf<u32> staged_rows;
+    const u32* drows = rows;
+    if (rows && out_mem == YTGPU_MEM_HOST) {
+        YTGPU_TRY(staged_rows.allocate(ctx, n));
+        YTGPU_TRY(copy_in(ctx, staged_rows.p, rows, n * 4, YTGPU_MEM_HOST));
+        drows = staged_rows.p;
+    }
+    // the item columns on the device; each string heap at its offset in one concatenated heap
+    std::vector<StagedColumn> staged(item_count);
+    std::vector<DevBuf<u64>> sstarts(item_count);
+    std::vector<DevBuf<u32>> slengths(item_count);
+    std::vector<DevBuf<u8>> snulls(item_count);
+    std::vector<OrderItemDev> host_items(item_count);
+    std::vector<ytgpu_key_column> keys(item_count);
+    u64 heap_total = 0;
+    for (u32 k = 0; k < item_count; ++k) {
+        OrderItemDev& d = host_items[k];
+        d = OrderItemDev{};
+        keys[k] = ytgpu_key_column{k, 0, 0, items[k].descending ? (u8)1 : (u8)0, 0, 0};
+        if (!items[k].is_string) {
+            YTGPU_TRY(stage_column(ctx, &columns[items[k].column], &staged[k]));
+            d.col = staged[k].dev;
+            d.type = columns[items[k].column].value_type;
+            keys[k].type = d.type;
+            continue;
+        }
+        const ytgpu_string_column& s = string_columns[items[k].column];
+        d.is_string = 1;
+        d.type = YTGPU_TYPE_STRING;
+        keys[k].type = YTGPU_TYPE_STRING;
+        d.heap_base = heap_total;
+        d.heap_bytes = s.heap_bytes;
+        heap_total += s.heap_bytes;
+        d.starts = s.starts;
+        d.lengths = s.lengths;
+        d.nulls = s.null_bytemap;
+        if (s.mem == YTGPU_MEM_HOST && s.row_count) {
+            YTGPU_TRY(sstarts[k].allocate(ctx, s.row_count));
+            YTGPU_TRY(slengths[k].allocate(ctx, s.row_count));
+            YTGPU_TRY(copy_in(ctx, sstarts[k].p, s.starts, s.row_count * 8, YTGPU_MEM_HOST));
+            YTGPU_TRY(copy_in(ctx, slengths[k].p, s.lengths, s.row_count * 4, YTGPU_MEM_HOST));
+            d.starts = sstarts[k].p;
+            d.lengths = slengths[k].p;
+            if (s.null_bytemap) {
+                YTGPU_TRY(snulls[k].allocate(ctx, s.row_count));
+                YTGPU_TRY(copy_in(ctx, snulls[k].p, s.null_bytemap, s.row_count, YTGPU_MEM_HOST));
+                d.nulls = snulls[k].p;
+            }
+        }
+    }
+    DevBuf<u8> heap;
+    YTGPU_TRY(heap.allocate(ctx, heap_total));
+    for (u32 k = 0; k < item_count; ++k)
+        if (host_items[k].is_string)
+            YTGPU_TRY(copy_in(ctx, heap.p + host_items[k].heap_base, string_columns[items[k].column].heap, host_items[k].heap_bytes,
+                              string_columns[items[k].column].mem));
+    DevBuf<OrderItemDev> dev_items;
+    YTGPU_TRY(dev_items.allocate(ctx, item_count));
+    YTGPU_TRY(copy_in(ctx, dev_items.p, host_items.data(), item_count * sizeof(OrderItemDev), YTGPU_MEM_HOST));
+    DevBuf<ytgpu_value> values;
+    YTGPU_TRY(values.allocate(ctx, n * item_count));
+    {
+        KernelTimer t(ctx, KC_EXTRACT);
+        order_materialize_kernel<<<blocks_for(n, 256, 16), 256, 0, ctx->stream>>>(dev_items.p, item_count, (u64)column_rows, drows, n,
+                                                                                   values.p, ctx->dev_err);
+        YTGPU_CUDA_TRY(cudaGetLastError());
+    }
+    YTGPU_TRY(check_device_errors(ctx));  // synchronises
+
+    const ytgpu_rowset_view view{values.p, n, item_count, 0, heap.p, heap_total, YTGPU_MEM_DEVICE};
+    const ytgpu_sort_spec spec{keys.data(), item_count};
+    RowsetSort rs;
+    YTGPU_TRY(rs.run(ctx, &view, &spec));
+
+    DevBuf<u32> out_stage;
+    u32* dst = out_rows;
+    if (out_mem == YTGPU_MEM_HOST) {
+        YTGPU_TRY(out_stage.allocate(ctx, window));
+        dst = out_stage.p;
+    }
+    {
+        KernelTimer t(ctx, KC_GATHER);
+        order_window_kernel<<<blocks_for(window, 256, 16), 256, 0, ctx->stream>>>(rs.perm.plan, rs.perm.idx[0], rs.perm.idx[1], drows,
+                                                                                  std::min(offset, n), window, dst);
+        YTGPU_CUDA_TRY(cudaGetLastError());
+    }
+    if (out_mem == YTGPU_MEM_HOST) YTGPU_TRY(copy_out(ctx, out_rows, dst, window * 4, YTGPU_MEM_HOST));
+    YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return Status{};
+}
+
+}  // namespace
+
+extern "C" int ytgpu_order_rows(ytgpu_context* h, const ytgpu_column_view* columns, uint32_t column_count,
+                                const ytgpu_string_column* string_columns, uint32_t string_column_count, const ytgpu_order_item* items,
+                                uint32_t item_count, const uint32_t* rows, uint64_t row_count, uint64_t offset, uint64_t limit,
+                                uint32_t* out_rows, uint64_t* out_count, int out_mem, ytgpu_error* err) {
+    if (!h) return fill_error(err, make_status(YTGPU_ERR_INVALID_ARGUMENT, "null context"));
+    CtxLock lock(h);
+    return fill_error(err, order_rows_impl(as_context(h), columns, column_count, string_columns, string_column_count, items, item_count,
+                                           rows, row_count, offset, limit, out_rows, out_count, out_mem));
+}

@@ -862,6 +862,50 @@ class GpuContext:
                                                        _ptr_mem(onulls)[0], mem, C.byref(err)), err)
         return heap, ostarts, olengths, onulls
 
+    def order_rows(self, columns, string_columns=(), items=(), rows=None, offset: int = 0, limit: int | None = None,
+                   count_only: bool = False, out_mem: int | None = None, row_count: int | None = None):
+        """ORDER BY ... OFFSET ... LIMIT (ytgpu_order_rows).  columns: Column objects; string_columns: (heap, starts, lengths,
+        nulls or None) per column; items: (column, is_string, descending) per ORDER BY item, column indexing columns or
+        string_columns.  rows (uint32; None: every row of the item columns) are the rows to order.  -> the row indexes of
+        sorted positions [offset, offset + limit) as uint32 (int32 tensors in DEVICE memory); with count_only, their number.
+        The output is in the rows' memory; without rows in out_mem (default: the first item column's).  row_count overrides
+        the number of rows passed to the call."""
+        views = [c.view() for c in columns]
+        sarr = (capi.StringColumn * max(len(string_columns), 1))()
+        for i, column in enumerate(string_columns):
+            sarr[i] = _string_column(*column)
+        iarr = (capi.OrderItem * max(len(items), 1))()
+        for i, (column, is_string, descending) in enumerate(items):
+            iarr[i] = capi.OrderItem(column, int(bool(is_string)), int(bool(descending)), 0)
+        first = items[0] if items else None
+        column_mem, column_rows = capi.MEM_HOST, 0
+        if first is not None and first[1] and first[0] < len(string_columns):
+            column_mem, column_rows = sarr[first[0]].mem, int(sarr[first[0]].row_count)
+        elif first is not None and not first[1] and first[0] < len(views):
+            column_mem, column_rows = views[first[0]].mem, int(views[first[0]].value_count)
+        if rows is not None:
+            rp, rows_mem = _ptr_mem(rows)
+            n = rows.numel() if _is_tensor(rows) else rows.size
+        else:
+            rp, rows_mem, n = None, column_mem, column_rows
+        if row_count is not None:
+            n = row_count
+        if rows is not None or out_mem is None:
+            out_mem = rows_mem
+        if limit is None:
+            limit = n
+        count = C.c_uint64(0)
+        err = capi.Error()
+        window = min(limit, n - min(offset, n))
+        out = None if count_only else self._out((max(window, 1),), np.uint32, out_mem)
+        arr = (capi.ColumnView * max(len(views), 1))(*views)
+        capi.check(self.lib.ytgpu_order_rows(self.handle, C.cast(arr, C.c_void_p), len(views), C.cast(sarr, C.c_void_p),
+                                             len(string_columns), iarr, len(items), rp, n, offset, limit,
+                                             _ptr_mem(out)[0] if out is not None else None, C.byref(count), out_mem, C.byref(err)), err)
+        if count_only:
+            return int(count.value)
+        return out[:int(count.value)]
+
     @staticmethod
     def _program_columns(caller, columns, string_columns):
         """Column arrays of an evaluator call -> (ColumnView array, views, StringColumn array, mem and n of column 0)."""
