@@ -507,7 +507,7 @@ __global__ void __launch_bounds__(256, 8) tie_fix_runs_kernel(const u64* __restr
                 u32 r = s_out[l];
                 if (r == kNoSlot && (int)l >= lo && (int)l < hi) r = s_idx[l];
                 ok[k] = r != kNoSlot;
-                if (ok[k]) v[k] = ld_stream_u128(G.rows + (u64)r * G.gr + (q - l * G.gr));
+                if (ok[k]) v[k] = ld_l2_u128(G.rows + (u64)r * G.gr + (q - l * G.gr));
             }
 #pragma unroll
             for (int k = 0; k < kTailGatherUnroll; ++k)

@@ -25,7 +25,7 @@ __global__ void __launch_bounds__(256) extract_scalar_key_kernel(const u8* __res
         const bool valid = i < n;
         u64 v = 0;
         if (valid) {
-            v = ld_stream_u64(reinterpret_cast<const u64*>(rows + i * row_bytes + offset));
+            v = ld_l2_u64(reinterpret_cast<const u64*>(rows + i * row_bytes + offset));
             if (type == YTGPU_TYPE_INT64) v ^= 0x8000000000000000ull;
             else if (type == YTGPU_TYPE_DOUBLE) v = normalize_double_bits(v);
             if (desc) v = ~v;
