@@ -278,7 +278,7 @@ ytgpu_expr_node LibraryNode(const TExpressionNode& node, std::string* constants,
         return c;
     };
     if ((node.Op == EExpressionOp::Constant && node.Type == EValueType::String) ||
-        (IsPredicate(node.Op) && node.Op != EExpressionOp::In))
+        (IsPredicate(node.Op) && node.Op != EExpressionOp::In) || node.Op == EExpressionOp::FormatTimestamp)
         x.constant = append(node.Bytes);
     if (node.Op != EExpressionOp::In) return x;
     std::vector<uint64_t> entries;
@@ -680,7 +680,8 @@ public:
                                   : node.Op == EExpressionOp::If ? 3
                                   : (node.Op == EExpressionOp::Neg || node.Op == EExpressionOp::BitNot || node.Op == EExpressionOp::Cast ||
                                      node.Op == EExpressionOp::Lower || node.Op == EExpressionOp::Upper || node.Op == EExpressionOp::Not ||
-                                     node.Op == EExpressionOp::IsNull || node.Op == EExpressionOp::IsNotNull || IsPredicate(node.Op)) ? 1 : 2;
+                                     node.Op == EExpressionOp::IsNull || node.Op == EExpressionOp::IsNotNull || IsPredicate(node.Op) ||
+                                     node.Op == EExpressionOp::TimestampFloor || node.Op == EExpressionOp::FormatTimestamp) ? 1 : 2;
                 if (st.size() < need) return EValueType::Int64;
                 switch (node.Op) {
                     case EExpressionOp::Column: {
@@ -699,6 +700,13 @@ public:
                     case EExpressionOp::Cast:
                         asNumber(st.back());
                         st.back().Type = node.Type;
+                        break;
+                    case EExpressionOp::TimestampFloor:  // an untyped operand is an Int64
+                        asNumber(st.back());
+                        break;
+                    case EExpressionOp::FormatTimestamp:
+                        asNumber(st.back());
+                        st.back().Type = EValueType::String;
                         break;
                     case EExpressionOp::FarmHash:  // a NULL hashes alike whichever type it is read as
                         st.resize(st.size() - need);
@@ -792,7 +800,7 @@ public:
             for (const auto& node : e.Nodes) {
                 if (node.Op == EExpressionOp::Concat || node.Op == EExpressionOp::Lower || node.Op == EExpressionOp::Upper ||
                     node.Op == EExpressionOp::FarmHash || node.Op == EExpressionOp::IsPrefix || node.Op == EExpressionOp::IsSubstr ||
-                    node.Op == EExpressionOp::Like)
+                    node.Op == EExpressionOp::Like || node.Op == EExpressionOp::FormatTimestamp)
                     throw TErrorException(YTGPU_ERR_UNSUPPORTED, what + ": string functions over the output row");
                 EValueType listType;
                 if (node.Op == EExpressionOp::In) {

@@ -181,12 +181,14 @@ struct TFilterExpression {
 //! NULLs, wrap-around, division errors and the branches they follow, casts, ASCII case mapping, the fingerprint — are in
 //! include/ytgpu.h).  Nodes are in postfix order; a Column leaf names a position (in the
 //! input rows for TMultiGroupQuery::Computed, in the output row for Select).  Binary operands have one type: there is no
-//! implicit widening, write Cast.  Select and Having take no string ops; of the predicates they take In over numbers.
+//! implicit widening, write Cast.  Select and Having take no string ops; of the predicates they take In over numbers; of
+//! the timestamp functions they take the floors.
 enum class EExpressionOp {
     Column = 1, Constant = 2, Add = 3, Sub = 4, Mul = 5, Div = 6, Mod = 7, Neg = 8, BitAnd = 9, BitOr = 10, BitXor = 11, BitNot = 12,
     Cast = 13, IfNull = 14, Concat = 15, Lower = 16, Upper = 17, FarmHash = 18,
     Compare = 19, And = 20, Or = 21, Not = 22, IsNull = 23, IsNotNull = 24, If = 25,
-    In = 26, IsPrefix = 27, IsSubstr = 28, Like = 29
+    In = 26, IsPrefix = 27, IsSubstr = 28, Like = 29,
+    TimestampFloor = 30, FormatTimestamp = 31
 };
 //! A typed literal: an In list entry.
 struct TExpressionLiteral {
@@ -196,10 +198,12 @@ struct TExpressionLiteral {
 };
 struct TExpressionNode {
     EExpressionOp Op = EExpressionOp::Column;
-    int Column = -1;                      // Column; FarmHash: the operand count; Compare: the EBinaryOp; Like: the escape byte or -1
+    int Column = -1;                      // Column; FarmHash: the operand count; Compare: the EBinaryOp; Like: the escape byte or -1;
+                                          // TimestampFloor: the ytgpu_timestamp_unit
     EValueType Type = EValueType::Null;   // Constant: its type; Cast: the target type
     uint64_t Bits = 0;                    // Constant: Int64 / Uint64 / Double bit pattern, Boolean 0 / 1
-    std::string Bytes = {};               // Constant: a String's bytes; IsPrefix / IsSubstr / Like: the prefix, needle or pattern
+    std::string Bytes = {};               // Constant: a String's bytes; IsPrefix / IsSubstr / Like: the prefix, needle or pattern;
+                                          // FormatTimestamp: the format
     std::vector<TExpressionLiteral> List = {};  // In: the entries
 };
 struct TExpression {
@@ -264,6 +268,17 @@ struct TExpression {
     TExpression& Like(const std::string& pattern, std::optional<unsigned char> escape = std::nullopt) {
         return Text(EExpressionOp::Like, pattern, escape ? (int)*escape : -1);
     }
+    //! timestamp_floor_hour / day / week (from Monday) / month / year of an Int64 or Uint64 of seconds since the epoch, UTC:
+    //! the operand's type (an all-NULL input column is an Int64).  A value outside [0, 9999-12-31T23:59:59Z] that is
+    //! evaluated, or a week floor before 1970-01-05, throws YTGPU_ERR_UNSUPPORTED.
+    TExpression& TimestampFloorHour() { return Floor(0); }
+    TExpression& TimestampFloorDay() { return Floor(1); }
+    TExpression& TimestampFloorWeek() { return Floor(2); }
+    TExpression& TimestampFloorMonth() { return Floor(3); }
+    TExpression& TimestampFloorYear() { return Floor(4); }
+    //! format_timestamp(t, format): a String, C-locale strftime of t in UTC (the conversions in include/ytgpu.h).  Computed
+    //! columns only; the range rule of the floors applies.
+    TExpression& FormatTimestamp(const std::string& format) { return Text(EExpressionOp::FormatTimestamp, format, -1); }
 
 private:
     TExpression& Text(EExpressionOp op, const std::string& bytes, int column) {
@@ -271,6 +286,7 @@ private:
         return *this;
     }
     TExpression& Op(EExpressionOp op) { Nodes.push_back({op, -1, EValueType::Null, 0}); return *this; }
+    TExpression& Floor(int unit) { Nodes.push_back({EExpressionOp::TimestampFloor, unit, EValueType::Null, 0}); return *this; }
 };
 
 struct TMultiGroupQuery {

@@ -894,24 +894,34 @@ typedef enum ytgpu_expr_op {
     YTGPU_EXPR_COMPARE = 19, YTGPU_EXPR_AND = 20, YTGPU_EXPR_OR = 21, YTGPU_EXPR_NOT = 22, YTGPU_EXPR_IS_NULL = 23,
     YTGPU_EXPR_IS_NOT_NULL = 24, YTGPU_EXPR_IF = 25,
     /* predicates inside expressions, ytgpu_evaluate_expression_strings only (see there) */
-    YTGPU_EXPR_IN = 26, YTGPU_EXPR_STARTS_WITH = 27, YTGPU_EXPR_CONTAINS = 28, YTGPU_EXPR_LIKE = 29
+    YTGPU_EXPR_IN = 26, YTGPU_EXPR_STARTS_WITH = 27, YTGPU_EXPR_CONTAINS = 28, YTGPU_EXPR_LIKE = 29,
+    /* timestamps: TIMESTAMP_FLOOR both entry points, FORMAT_TIMESTAMP ytgpu_evaluate_expression_strings only (see there) */
+    YTGPU_EXPR_TIMESTAMP_FLOOR = 30, YTGPU_EXPR_FORMAT_TIMESTAMP = 31
 } ytgpu_expr_op;
+
+/* TIMESTAMP_FLOOR's unit, in the node's `column` */
+typedef enum ytgpu_timestamp_unit {
+    YTGPU_TIMESTAMP_HOUR = 0, YTGPU_TIMESTAMP_DAY = 1, YTGPU_TIMESTAMP_WEEK = 2, YTGPU_TIMESTAMP_MONTH = 3, YTGPU_TIMESTAMP_YEAR = 4
+} ytgpu_timestamp_unit;
 
 #define YTGPU_EXPR_MAX_NODES 64
 #define YTGPU_EXPR_MAX_DEPTH 16
 #define YTGPU_EXPR_MAX_PIECES 16
 #define YTGPU_EXPR_MAX_HASH_OPERANDS 16
 #define YTGPU_EXPR_MAX_STRING_CONSTANT_BYTES (1u << 20)
+#define YTGPU_EXPR_MAX_FORMATTED_BYTES 64
 
 typedef struct ytgpu_expr_node {
     int32_t op;          /* ytgpu_expr_op */
     int32_t column;      /* COLUMN: index into columns (++ string_columns); FARM_HASH: its operand count;
-                            COMPARE: the ytgpu_cmp_op; LIKE: the escape byte 0..255, or -1 for none */
+                            COMPARE: the ytgpu_cmp_op; LIKE: the escape byte 0..255, or -1 for none;
+                            TIMESTAMP_FLOOR: the ytgpu_timestamp_unit */
     uint8_t type;        /* CONSTANT: its value type; CAST: the target type (YTGPU_TYPE_*) */
     uint8_t reserved[7];
     uint64_t constant;   /* CONSTANT: the bit pattern in `type`; a STRING one: (offset << 32) | length into string_constants;
                             IN: (offset << 32) | count of its list in string_constants; STARTS_WITH, CONTAINS, LIKE: the
-                            prefix, needle or pattern as (offset << 32) | length into string_constants */
+                            prefix, needle or pattern as (offset << 32) | length into string_constants; FORMAT_TIMESTAMP:
+                            the format, likewise */
 } ytgpu_expr_node;
 
 int ytgpu_evaluate_expression(ytgpu_context* ctx, const ytgpu_column_view* columns, uint32_t column_count,
@@ -1032,7 +1042,33 @@ int ytgpu_evaluate_expression(ytgpu_context* ctx, const ytgpu_column_view* colum
  * YTGPU_ERR_INVALID_ARGUMENT, besides the above: an operand type the op does not take (STARTS_WITH, CONTAINS, LIKE over a
  * non-STRING), an IN list that is not 8-byte aligned or leaves string_constants, a STRING entry outside string_constants, a
  * BOOLEAN entry other than 0 / 1, a prefix, needle or pattern outside string_constants, a LIKE escape outside -1..255, a
- * pattern that ends in a lone escape byte, a limit above, a CONTAINS / LIKE operand of 2^32 bytes or more. */
+ * pattern that ends in a lone escape byte, a limit above, a CONTAINS / LIKE operand of 2^32 bytes or more.
+ *
+ * Timestamps (`group by timestamp_floor_day(ts)`, `group by format_timestamp(ts, '%Y-%m')`).  A timestamp is seconds since
+ * the Unix epoch, UTC, proleptic Gregorian, no leap seconds, in an INT64 or UINT64 operand; a NULL operand gives NULL.
+ *   TIMESTAMP_FLOOR(unit)    both entry points; `column` the ytgpu_timestamp_unit -> the operand's type: HOUR t - t % 3600,
+ *                            DAY t - t % 86400, WEEK the Monday 00:00 of t's week ((d - (d + 3) % 7) * 86400 with
+ *                            d = t / 86400), MONTH the first day of t's month at 00:00, YEAR January 1 of t's year at 00:00.
+ *                            That QL's week starts on Monday is recalled, not read.
+ *   FORMAT_TIMESTAMP         this entry point only (ytgpu_evaluate_expression refuses it as an unknown op) -> STRING: byte
+ *                            for byte what C-locale strftime(format, gmtime(t)) writes.  `constant` = (offset << 32) |
+ *                            length of the format in string_constants.  Conversions: %a %A %b %B %h %p (the C locale's
+ *                            English names), %C %d %e %H %I %j %m %M %S %u %w %y %Y, %D %F %R %T, %U %W, the ISO %G %g %V,
+ *                            %n %t %%; every other byte is itself; an empty format gives "".  That QL's format_timestamp
+ *                            is the C library's strftime is recalled, not read.  The format is compiled when the program
+ *                            is checked and travels in the program's one upload.  A formatted value is a STRING operand
+ *                            like any other (CONCAT, COMPARE, IN, STARTS_WITH, CONTAINS, LIKE, IF, IF_NULL, LOWER, UPPER,
+ *                            the result) and one piece toward YTGPU_EXPR_MAX_PIECES; under FARM_HASH it is
+ *                            YTGPU_ERR_UNSUPPORTED, as a CONCAT result is.
+ * A timestamp is accepted in [0, 253402300799] (9999-12-31T23:59:59Z).  An evaluated row outside it, or a WEEK floor whose
+ * result would be negative (t before 1970-01-05), fails the call with YTGPU_ERR_UNSUPPORTED: the reference's result there
+ * is not known (it is recalled to go through an unsigned instant).  This error follows the data as a division error does:
+ * a row outside the selection, an IF branch not taken and FALSE AND x raise nothing.  YTGPU_ERR_UNSUPPORTED whatever the
+ * data: another conversion (%c %x %X %r %Z %z %s %k %l %P %+ ...), an E / O modifier, a flag or width (%-d, %10Y), a lone %
+ * at the end, a format whose longest output exceeds YTGPU_EXPR_MAX_FORMATTED_BYTES (64; a bound chosen to be safe, as the
+ * reference's buffer size was not read).  YTGPU_ERR_INVALID_ARGUMENT: an operand other than INT64 / UINT64, a unit outside
+ * 0 .. 4, a format outside string_constants.  Device scratch: 64 bytes per thread of the grid and FORMAT_TIMESTAMP node
+ * (about 17 MB each on a 132-SM H100 at 10^6 rows or more). */
 int ytgpu_evaluate_expression_strings(ytgpu_context* ctx, const ytgpu_column_view* columns, uint32_t column_count,
                                       const ytgpu_string_column* string_columns, uint32_t string_count,
                                       const uint8_t* string_constants /* host */, uint64_t string_constant_bytes,

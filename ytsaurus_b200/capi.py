@@ -185,11 +185,14 @@ class FilterNode(C.Structure):
  EXPR_BIT_NOT, EXPR_CAST, EXPR_IF_NULL, EXPR_CONCAT, EXPR_LOWER, EXPR_UPPER, EXPR_FARM_HASH) = range(1, 19)
 (EXPR_COMPARE, EXPR_AND, EXPR_OR, EXPR_NOT, EXPR_IS_NULL, EXPR_IS_NOT_NULL, EXPR_IF) = range(19, 26)
 EXPR_IN, EXPR_STARTS_WITH, EXPR_CONTAINS, EXPR_LIKE = range(26, 30)
+EXPR_TIMESTAMP_FLOOR, EXPR_FORMAT_TIMESTAMP = 30, 31  # FORMAT_TIMESTAMP: ytgpu_evaluate_expression_strings only
+TIMESTAMP_HOUR, TIMESTAMP_DAY, TIMESTAMP_WEEK, TIMESTAMP_MONTH, TIMESTAMP_YEAR = range(5)  # TIMESTAMP_FLOOR's `column`
 # ytgpu_evaluate_expression_strings only
 EXPR_STRING_OPS = (EXPR_CONCAT, EXPR_LOWER, EXPR_UPPER, EXPR_FARM_HASH)
 EXPR_PREDICATE_OPS = (EXPR_IN, EXPR_STARTS_WITH, EXPR_CONTAINS, EXPR_LIKE)
 EXPR_MAX_NODES, EXPR_MAX_DEPTH = 64, 16
 EXPR_MAX_PIECES, EXPR_MAX_HASH_OPERANDS, EXPR_MAX_STRING_CONSTANT_BYTES = 16, 16, 1 << 20
+EXPR_MAX_FORMATTED_BYTES = 64
 
 
 class ExprNode(C.Structure):

@@ -969,7 +969,7 @@ class GpuContext:
         over them (without the bitmap when no row is NULL), ready for scan_filter_groupby_multi / evaluate_filter.
         string_columns: (heap, starts, lengths, nulls or None) per column, node column len(columns) + i naming string column
         i; a STRING constant is (offset << 32) | length into string_constants (capi.ExprConstants builds it, IN lists and
-        patterns included).  With either, a string op or an IN / STARTS_WITH / CONTAINS / LIKE in the program, or a STRING
+        patterns and FORMAT_TIMESTAMP formats included).  With either, a string op, FORMAT_TIMESTAMP or an IN / STARTS_WITH / CONTAINS / LIKE in the program, or a STRING
         constant in a program with a conditional op, the call is ytgpu_evaluate_expression_strings, made twice: a type and size query, then the call that fills the outputs
         of that type, so a STRING result runs its size pass twice (a caller that knows the heap size calls the library once).
         A STRING result comes back as heap / starts / lengths / null_bytemap (values, null_bitmap and column None), ready
@@ -993,7 +993,7 @@ class GpuContext:
         conditional = any(op >= capi.EXPR_COMPARE for op in ops)
         string_constants = bytes(string_constants)
         strings = (bool(string_columns) or len(string_constants) > 0 or
-                   any(op in capi.EXPR_STRING_OPS or op in capi.EXPR_PREDICATE_OPS for op in ops) or
+                   any(op in capi.EXPR_STRING_OPS or op in capi.EXPR_PREDICATE_OPS or op == capi.EXPR_FORMAT_TIMESTAMP for op in ops) or
                    (conditional and any(nodes[i].op == capi.EXPR_CONSTANT and nodes[i].type == int(EValueType.String)
                                         for i in range(len(program)))))
         if not strings:
