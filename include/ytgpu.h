@@ -1086,7 +1086,9 @@ int ytgpu_evaluate_expression_strings(ytgpu_context* ctx, const ytgpu_column_vie
  * rows whose 8-byte key column at key_offset is non-decreasing (only equality of neighbours is used); the value column
  * at value_offset is INT64 / UINT64 (sums wrap mod 2^64) or DOUBLE.  out_* (DEVICE, `capacity` entries) receive one
  * entry per group in input order, *out_group_count (host) the number of groups; INVALID_ARGUMENT when it exceeds
- * capacity.  Same sums / counts as ytgpu_scan_filter_groupby over the same rows. */
+ * capacity.  `in->rows` and out_* must be 8-byte aligned (INVALID_ARGUMENT otherwise).  Same sums / counts as
+ * ytgpu_scan_filter_groupby over the same rows: double sums are added in arbitrary order starting from +0.0, so a
+ * group of only -0.0 sums to +0.0, and a group holding a NaN, or both infinities, sums to a NaN. */
 int ytgpu_reduce_sorted_fixed_rows(ytgpu_context* ctx, const ytgpu_fixed_rows_view* in, uint32_t key_offset,
                                    uint32_t value_offset, uint8_t value_type, uint64_t* out_keys, uint64_t* out_sums,
                                    uint64_t* out_counts, uint64_t capacity, uint64_t* out_group_count, ytgpu_error* err);
@@ -1126,7 +1128,9 @@ void ytgpu_block_agg_state_init(ytgpu_block_agg_state* state, uint8_t value_type
  * 697-770, mkql_block_agg_count.cpp) in ONE pass over the block: folds the batch into *state (host).  `filter`
  * (nullable) is the non-nullable bool filter column, one byte per row.  Same IsValid rules as the reference,
  * including its quirks (a filtered batch without nulls raises sum's IsValid even if no row passed).  Floating point:
- * the sum is a tree reduction (reproducible for a given length), min/max follow AggLess (NaN is the biggest). */
+ * the sum is a tree reduction (reproducible for a given length), min/max follow AggLess (NaN is the biggest, all NaNs
+ * are equal, -0.0 == +0.0): of AggLess-equal values the last in row order stays, with its own bits, so the state is
+ * the reference's bit for bit.  DEVICE `values` must be 8-byte aligned (INVALID_ARGUMENT otherwise). */
 int ytgpu_block_combine_all(ytgpu_context* ctx, const ytgpu_arrow_array* column, const uint8_t* filter,
                             ytgpu_block_agg_state* state, ytgpu_error* err);
 

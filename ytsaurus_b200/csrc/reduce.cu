@@ -139,6 +139,9 @@ Status reduce_impl(Context* ctx, const ytgpu_fixed_rows_view* in, u32 key_off, u
                    u64* out_counts, u64 capacity, u64* out_group_count) {
     if (!in || !out_keys || !out_sums || !out_counts || !out_group_count) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null argument");
     if (in->mem != YTGPU_MEM_DEVICE) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "the sorted reduce reads device-resident rows");
+    const void* words[] = {in->rows, out_keys, out_sums, out_counts};
+    for (const void* w : words)
+        if (reinterpret_cast<uintptr_t>(w) % 8) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "rows and outputs must be 8-byte aligned");
     const u32 rb = in->row_bytes;
     if (rb == 0 || rb % 8 || key_off % 8 || val_off % 8 || (u64)key_off + 8 > rb || (u64)val_off + 8 > rb)
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "key/value offsets must be 8-byte aligned and inside the row");
