@@ -17,6 +17,12 @@ rows by default):
   star_groupby    star's join, a gather of one foreign column (region U[0, 100)), a gather of a primary column (amount) and
                   GROUP BY region with SUM(amount): SELECT d.region, sum(f.amount) FROM f JOIN d ON f.k = d.id GROUP BY
                   d.region, end to end
+  snowflake_groupby  the evaluator's device call sequence for SELECT r.name, sum(f.amount) FROM f JOIN u ON f.user_id =
+                  u.id JOIN r ON u.region_id = r.id GROUP BY r.name: N facts with user ids U[0, 10^6); 10^6 users with
+                  unique ids and a region id U[0, 10^3); 10^3 regions with a string name.  Join, a gather of the users'
+                  region id at the joined rows (clause 2's key), join, composition of the two row maps (gathers of the
+                  maps as UINT64 columns), the final gathers (amount through the facts' map, the name through the regions'),
+                  the name's string ids and GROUP BY them with SUM(amount)
 Each leg reports the median call time (CUDA events around the call, after warm-up), primary rows / s, the time of timer
 class 11 (build, probe, pair write and gathers; the stable sort of the foreign rows times itself under the sort classes)
 and a byte floor computed from the shapes: 8 B per key column and row read on both sides, 8 B per pair written, and
@@ -25,7 +31,7 @@ write: 8 B offset + 4 B slot read).  floor_fraction is that floor at 3.35 TB/s (
 time: a lower bound on the share of bandwidth the call uses, not a roofline.
 Parity: every leg checks a seeded sample of primary rows (10^6 rows; 10^4 for fanout, whose rows carry ~100 pairs each)
 against a numpy reference (the foreign rows of each sampled row's key in ascending order, or NO_ROW), and star_groupby its
-sums against torch's index_add over all rows.  The project has no CPU port of the reference's JoinOpHelper, so there is no
+sums (and snowflake_groupby its sums by region name) against torch's index_add over all rows.  The project has no CPU port of the reference's JoinOpHelper, so there is no
 CPU baseline and the line says so.  One JSON line on stdout, with the card's name and power limit; nothing is written to
 the source tree.
 """
@@ -193,6 +199,50 @@ def main():
     line["legs"]["star_groupby"] = {"primary_rows": N, "foreign_rows": D, "pairs": N, "median_ms": round(ms, 3),
                                     "rows_per_s": N / (ms / 1e3), "join_class_ms": round(join_ms, 3), "floor_bytes": floor,
                                     "floor_fraction": floor / DATASHEET_HBM_BPS / (ms / 1e3), "parity_rows": N, "parity": ok}
+
+    # snowflake_groupby: two clauses, the second keyed on a column of the first clause's table
+    R = 1000
+    user_region = ri(0, R, D)
+    region_ids = torch.randperm(R, device="cuda", generator=g)
+    names = [b"region-%04d" % i for i in region_ids.tolist()]
+    name_heap = torch.tensor(list(b"".join(names)), dtype=torch.uint8, device="cuda")
+    name_lengths = torch.tensor([len(x) for x in names], dtype=torch.int32, device="cuda")
+    name_starts = (torch.cumsum(name_lengths.to(torch.int64), 0) - name_lengths.to(torch.int64)).contiguous()
+    ucol, rcol = col(user_region), col(region_ids)
+    wide = lambda rows: Column(T.Uint64, values=rows.to(torch.int64))  # a row map as a UINT64 column
+    narrow = lambda gathered: gathered["values"].to(torch.int32)
+
+    def snowflake():
+        p1, f1 = ctx.hash_join(pcols, fcols, capi.JOIN_INNER, capacity=N)
+        key = ctx.gather_column(ucol, f1)["column"]
+        pairs = ctx.hash_join([key], [rcol], capi.JOIN_INNER, count_only=True)
+        p2, f2 = ctx.hash_join([key], [rcol], capi.JOIN_INNER, capacity=pairs)
+        fact_map = narrow(ctx.gather_column(wide(p1), p2))
+        narrow(ctx.gather_column(wide(f1), p2))  # the users' map, composed as the evaluator composes every earlier map
+        amount_col = ctx.gather_column(acol, fact_map)["column"]
+        _, starts, lengths, nulls = ctx.gather_string_column(name_heap, name_starts, name_lengths, None, f2)
+        ids, _ = ctx.string_value_ids(name_heap, starts, lengths, nulls)
+        res = ctx.scan_filter_groupby_multi([Column(T.Uint64, values=ids.view(torch.int64))], [amount_col], [(capi.AGG_SUM, 0)],
+                                            group_count_hint=R, capacity=2 * R)
+        return res, starts, lengths
+    (res, starts, lengths), ms, join_ms = timed(snowflake)
+    # every fact has its user and every user its region: the sum of region id r is the amounts of the facts whose user's
+    # region is r
+    want = torch.zeros(R, dtype=torch.int64, device="cuda").index_add_(0, user_region[where[pkeys]], amount).cpu().numpy()
+    heap = bytes(name_heap.cpu().numpy())
+    first = res["keys"][0].cpu().numpy().view(np.int64)
+    got_starts, got_lengths = starts.cpu().numpy()[first], lengths.cpu().numpy()[first]
+    sums = res["values"][0].cpu().numpy().view(np.int64)
+    got = {int(heap[s:s + n].split(b"-")[1]): int(v) for s, n, v in zip(got_starts, got_lengths, sums)}
+    present = np.unique(user_region.cpu().numpy())
+    ok = len(got) == len(first) == present.size and all(got.get(int(r)) == int(want[r]) for r in present)
+    # per fact row: both joins as the other legs count them, the key gather, the amount gather (4 B row in, 8 B out each),
+    # two map compositions (4 B row + 8 B map value in, 8 B out each), the name gather (4 B row in, 13 B out), the string ids
+    # (13 B in, 9 B out) and the GROUP BY read (16 B); the dimension-sized terms of the builds
+    floor = 8 * (D + R) + (8 + 8 + 40) * 2 * N + 2 * 12 * N + 2 * 20 * N + 17 * N + 22 * N + 16 * N
+    line["legs"]["snowflake_groupby"] = {"primary_rows": N, "foreign_rows": [D, R], "pairs": N, "median_ms": round(ms, 3),
+                                         "rows_per_s": N / (ms / 1e3), "join_class_ms": round(join_ms, 3), "floor_bytes": floor,
+                                         "floor_fraction": floor / DATASHEET_HBM_BPS / (ms / 1e3), "parity_rows": N, "parity": ok}
     line["parity"] = all(v["parity"] for v in line["legs"].values())
     print(json.dumps(line), flush=True)
     ctx.close()

@@ -315,16 +315,36 @@ struct TMultiGroupQuery {
     //! column names a column of the JOINED row: a primary position as without it, or ForeignColumn(j) for position j of the
     //! foreign rows.  Select and Having keep naming output positions.  A LEFT join's primary row without a match gets NULL
     //! in every foreign column.  Join keys compare as the GROUP BY keys do: NULL equals NULL, doubles by bit pattern.
+    //! Join is the FIRST clause; NextJoins holds clauses 2..N (at most kMaxJoinClauses in all), applied left to right:
+    //! clause c joins the joined rows of clauses 0..c-1 with its foreign rows, and ForeignColumn(c, j) names position j of
+    //! clause c's foreign rows.  The joined rows are ordered by (primary row, foreign row of clause 0, of clause 1, ...).
+    //! A key is a column or an expression (ON f.k % 1000 = d.id, ON cast(f.u as int64) = d.id, ON lower(f.host) = d.host):
+    //! ComputedColumn(e) in SelfColumns / ForeignColumns names SelfExpressions[e] / ForeignExpressions[e].  A self key
+    //! (column or expression leaf) reads primary positions and foreign positions of EARLIER clauses; a foreign expression
+    //! reads positions of this clause's foreign rows (plain j).  No key reads a query.Computed position.  Each key
+    //! expression is evaluated once over every row of its side, before its join and so before WHERE: a division by zero
+    //! in any row throws, even in a row a later WHERE drops.  Keys keep one type per key pair (an all-NULL column takes the
+    //! other side's type).  Because NULL equals NULL in every clause, a row that a LEFT clause left without a match, NULL
+    //! in that clause's columns, matches a foreign NULL key of a later clause that keys on those columns.  That YT QL
+    //! allows several clauses whose keys read the tables joined before, and expressions as join keys evaluated before
+    //! WHERE, is recalled, not read.
     struct TJoinClause {
         ISchemalessMultiChunkReaderPtr Foreign;   // the foreign table's rows, in the order the reference fetches them
-        std::vector<int> SelfColumns;             // join key positions in the primary rows (1..8)
+        std::vector<int> SelfColumns;             // join key positions in the (joined) primary rows (1..8)
         std::vector<int> ForeignColumns;          // the matching positions in the foreign rows
         bool IsLeft = false;
+        std::vector<TExpression> SelfExpressions = {};     // the self keys that are expressions: ComputedColumn(e)
+        std::vector<TExpression> ForeignExpressions = {};  // the foreign keys that are expressions: ComputedColumn(e)
     };
     std::optional<TJoinClause> Join;
+    std::vector<TJoinClause> NextJoins;          // clauses 2..N, in order; they need Join
+    static constexpr int kMaxJoinClauses = 8;
     static constexpr int kForeignColumnBase = 1 << 24;
     static constexpr int ForeignColumn(int j) { return kForeignColumnBase + j; }
+    static constexpr int ForeignColumn(int clause, int j) { return (clause + 1) * kForeignColumnBase + j; }
     static constexpr bool IsForeignColumn(int position) { return position >= kForeignColumnBase; }
+    static constexpr int ForeignClause(int position) { return position / kForeignColumnBase - 1; }
+    static constexpr int ForeignIndex(int position) { return position % kForeignColumnBase; }
     //! A query WITHOUT GROUP BY: the output row is these positions of the (joined) input rows, input, computed (string
     //! results included) or foreign columns.  Non-empty exactly when GroupColumns and AggregateItems are empty.  Select then
     //! names positions of this output row, as it names group / aggregate positions otherwise; Having is refused.
@@ -369,11 +389,17 @@ struct IEvaluator {
     //! YTGPU_ERR_INVALID_ARGUMENT) throw TErrorException.  A query without computed columns and Select runs as before.
     //! With Join, both sides are flattened, the join keys typed (an all-NULL key column takes the other side's type; any
     //! other mismatch, Int64 against Uint64 included, throws YTGPU_ERR_INVALID_ARGUMENT: the caller casts first; string keys
-    //! go through one joint ytgpu_string_value_ids call), ytgpu_hash_join makes the pairs (a count query, then the fill), and
-    //! every flattened column is replaced by its gather at the pairs' primary or foreign rows.  Everything above then runs
-    //! unchanged over the joined rows: WHERE filters joined rows, the SQL meaning for both kinds.  So, beside the note on
-    //! division errors: a computed column or WHERE is not evaluated over a primary row that an INNER join drops.  RowsRead
-    //! counts primary rows.  A query without Join runs exactly as before.
+    //! go through one joint ytgpu_string_value_ids call per clause and key), ytgpu_hash_join makes the pairs (a count query,
+    //! then the fill), and every column the query reads is gathered at the joined rows.  With several clauses each side is
+    //! flattened once and one row map per table is kept: per clause only the self key inputs are gathered at the current
+    //! joined rows, the key expressions of both sides are evaluated (ytgpu_evaluate_expression_strings), the clause joins,
+    //! and the earlier maps are composed through the pairs' primary rows (ytgpu_gather_column); after the last clause every
+    //! column is gathered once from its table.  The joined rows stay below 2^30 (checked after each clause's count query:
+    //! YTGPU_ERR_UNSUPPORTED).  Everything above then runs unchanged over the joined rows: WHERE filters joined rows, the SQL
+    //! meaning for both kinds.  So, beside the note on division errors: a computed column or WHERE is not evaluated over a
+    //! primary row that an INNER join drops, while a join key expression is evaluated over every row of its side before its
+    //! join, so its division by zero throws even in a row a later WHERE drops.  RowsRead counts primary rows.  A query
+    //! without Join runs exactly as before.
     //! Evaluation order, as QL plans it: scan (+ JOIN) -> WHERE -> computed columns -> GROUP BY -> HAVING -> ORDER BY, OFFSET
     //! and LIMIT -> SELECT -> write.  ORDER BY items are evaluated over the rows WHERE keeps (a projection) or the groups
     //! HAVING keeps only; one ytgpu_order_rows call over those rows gives the window.  Without ORDER BY, LIMIT keeps the first
