@@ -1674,21 +1674,7 @@ public:
 
     void AddBlock(const TArrowColumn& keys, const TArrowColumn& values) override {
         if (keys.Length != values.Length) throw NYT::NTableClient::TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "Block columns differ in length");
-        auto view = [](const TArrowColumn& a) {
-            ytgpu_column_view v{};
-            v.start_index = a.Offset;
-            v.value_count = a.Length;
-            v.value_type = a.ValueType;
-            v.has_values = 1;
-            v.bit_width = 64;
-            v.values = a.Values;
-            v.values_count = (uint64_t)(a.Offset + a.Length);
-            v.null_bitmap = a.Validity;
-            v.reserved = a.Validity ? YTGPU_COLUMN_ARROW_VALIDITY : 0;
-            v.mem = YTGPU_MEM_HOST;
-            return v;
-        };
-        States_.AddBatch(view(keys), view(values), YTGPU_CMP_NONE, 0, Rows_);
+        States_.AddBatch(NDetail::ArrowColumnView(keys), NDetail::ArrowColumnView(values), YTGPU_CMP_NONE, 0, Rows_);
         Rows_ += (uint64_t)keys.Length;
     }
 

@@ -1,4 +1,5 @@
-// gpu_internal.h — helpers shared by the adapter translation units (gpu_adapters.cpp, gpu_shuffle.cpp).
+// gpu_internal.h — helpers shared by the adapter translation units (gpu_adapters.cpp, gpu_shuffle.cpp, gpu_aggregate.cpp,
+// gpu_map_join.cpp).
 #pragma once
 
 #include <cstdlib>
@@ -7,6 +8,7 @@
 #include <vector>
 
 #include "../include/ytgpu.h"
+#include "yt_query_client.h"
 #include "yt_table_client.h"
 
 namespace NYT::NTableClient::NDetail {
@@ -136,3 +138,24 @@ inline int64_t GetDataWeight(TUnversionedRow row) {  // unversioned_row.cpp:601-
 }
 
 }  // namespace NYT::NTableClient::NDetail
+
+namespace NYql::NMiniKQL::NDetail {
+
+//! A fixed-width Arrow column (host memory) as the column view of the C ABI: its offset as start_index, its validity
+//! bitmap (if any) as an Arrow validity bitmap.
+inline ytgpu_column_view ArrowColumnView(const TArrowColumn& a) {
+    ytgpu_column_view v{};
+    v.start_index = a.Offset;
+    v.value_count = a.Length;
+    v.value_type = a.ValueType;
+    v.has_values = 1;
+    v.bit_width = 64;
+    v.values = a.Values;
+    v.values_count = (uint64_t)(a.Offset + a.Length);
+    v.null_bitmap = a.Validity;
+    v.reserved = a.Validity ? YTGPU_COLUMN_ARROW_VALIDITY : 0;
+    v.mem = YTGPU_MEM_HOST;
+    return v;
+}
+
+}  // namespace NYql::NMiniKQL::NDetail

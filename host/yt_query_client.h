@@ -489,4 +489,30 @@ struct IBlockCombineHashed {
 };
 std::unique_ptr<IBlockCombineHashed> CreateGpuBlockCombineHashed(uint64_t groupCountHint, bool withMinMax = false);
 
+//! BlockMapJoinCore (mkql_block_map_join.cpp, in the same comp_nodes directory): a map join of Arrow blocks, the right
+//! (dimension) side held in a hash table, every left block probed against it.  The operator's name, its kinds and its
+//! output order below are RECALLED, NOT READ: SURVEY.md read only the block-aggregate files of comp_nodes.
+//!   * AddRightBlock adds a block of right key columns (as many blocks as needed, before the first probe).  The right
+//!     side is built into one GPU join table (ytgpu_join_table_build) on the first ProbeBlock; every later probe reuses it.
+//!   * ProbeBlock joins one left block.  LeftRows are rows of that block; RightRows index the right rows over all right
+//!     blocks in the order they were added.  Inner / Left: the pairs in ascending (left, right) order, a Left miss as
+//!     (l, YTGPU_JOIN_NO_ROW).  LeftSemi / LeftOnly: each left row with / without a match, once, ascending; RightRows empty.
+//!   * NULLs follow SQL: a key tuple with a NULL component matches nothing (YTGPU_JOIN_NULLS_NEVER_MATCH), so a NULL left
+//!     key is a Left miss and a LeftOnly row.  Doubles compare by bit pattern (-0.0 is not +0.0, a NaN matches only the
+//!     same NaN bits): what YQL's map join does with such keys is not known here.
+//!   * Key types INT64, UINT64 and DOUBLE; another type throws UNSUPPORTED, a key count or type that differs between the
+//!     blocks throws INVALID_ARGUMENT.  String keys are refused: their ids (ytgpu_string_value_ids) need both sides in one
+//!     call, and the table outlives a call.
+enum class EBlockJoinKind { Inner, Left, LeftSemi, LeftOnly };
+
+struct IBlockMapJoin {
+    virtual ~IBlockMapJoin() = default;
+    virtual void AddRightBlock(const std::vector<TArrowColumn>& keys) = 0;
+    struct TResult {
+        std::vector<uint32_t> LeftRows, RightRows;
+    };
+    virtual TResult ProbeBlock(const std::vector<TArrowColumn>& leftKeys) = 0;
+};
+std::unique_ptr<IBlockMapJoin> CreateGpuBlockMapJoin(EBlockJoinKind kind, uint32_t keyCount);
+
 }  // namespace NYql::NMiniKQL

@@ -589,7 +589,7 @@ int ytgpu_scan_filter_groupby_multi_strings(ytgpu_context* ctx, const ytgpu_colu
                                             const ytgpu_string_column* string_columns, uint32_t string_count,
                                             ytgpu_error* err);
 
-/* ---- hash JOIN: inner and left equi-joins over key tuples ----
+/* ---- hash JOIN: inner, left, left semi and left only equi-joins over key tuples ----
  * The join of YT QL's JoinOpHelper (library/query/engine/cg_routines/registry.cpp), which collects the primary rows' join
  * keys, fetches the foreign rows and joins them row by row through a hash lookup keyed on the join key.  Here the foreign
  * side is always the built one: its key tuples go into the open-addressing table of the GROUP BY calls, every primary row
@@ -600,8 +600,7 @@ int ytgpu_scan_filter_groupby_multi_strings(ytgpu_context* ctx, const ytgpu_colu
  * BY calls compare them, as (is-null, 64-bit payload) per column: doubles by bit pattern, so -0.0 does not match +0.0 and a
  * NaN matches only the same NaN bits; NULL EQUALS NULL.  That rule is shared with GROUP BY and with the unversioned value
  * comparator; that YT QL's join lookup treats NULL keys this way is recalled, not read.  The SQL rule of ClickHouse and YQL,
- * where NULL never matches, is not offered: a SQL caller drops the rows with NULL keys first (ytgpu_evaluate_filter) for an
- * INNER join, and has no way to do so for a LEFT one.
+ * where NULL never matches, is the join table's YTGPU_JOIN_NULLS_NEVER_MATCH (below); ytgpu_hash_join keeps the rule above.
  * String keys go through ytgpu_string_value_ids: call it ONCE over one string column holding the F foreign values followed
  * by the P primary values.  Then ids[0, F) is the foreign key column and ids[F, F + P) the primary one, both UINT64 with the
  * null bytemap as their NULLs: equal strings on either side get the same first-row id.  The join itself is numeric only.
@@ -616,20 +615,70 @@ int ytgpu_scan_filter_groupby_multi_strings(ytgpu_context* ctx, const ytgpu_colu
  * rows are 32-bit, and the foreign rows go through the radix sort, which takes fewer than 2^30), checked before any access
  * (UNSUPPORTED); the key columns of one side have one length (INVALID_ARGUMENT); an unknown kind is
  * INVALID_ARGUMENT; a key type other than the four scalars is UNSUPPORTED.
- * Launches: the build (one assign pass of the GROUP BY calls, sized for the foreign row count so that no retry is expected,
+ * ytgpu_hash_join takes INNER and LEFT only (any other kind is INVALID_ARGUMENT); it is the join table below built, probed
+ * once and destroyed, with every argument check of both sides made before the first launch.
+ * Launches: the build (a decode pass of the foreign keys, one assign pass of the GROUP BY calls, sized for the foreign row count so that no retry is expected,
  * and a read of its error word), one probe kernel over the primary rows, a three-kernel scan of the per-row pair counts and
- * a read of the total; with outputs, a three-kernel scan of the per-key counts, one stable radix sort of the foreign rows by
- * their slot (which reads its plan back once from 2^18 foreign rows), the output-partitioned pair write and a closing
+ * a read of the total; with outputs, a three-kernel scan of the per-key counts and one stable radix sort of the foreign rows
+ * by their slot (which reads its plan back once from 2^18 foreign rows) before the probe, the output-partitioned pair write and a closing
  * synchronisation of the context's stream: the outputs are complete when the call returns, whichever stream the caller
  * reads them on (a context may run on a private stream), as with the GROUP BY calls.  HOST inputs are copied to the device
  * first. */
-typedef enum ytgpu_join_kind { YTGPU_JOIN_INNER = 0, YTGPU_JOIN_LEFT = 1 } ytgpu_join_kind;
+typedef enum ytgpu_join_kind {
+    YTGPU_JOIN_INNER = 0,
+    YTGPU_JOIN_LEFT = 1,
+    YTGPU_JOIN_SEMI = 2,  /* LEFT SEMI: each primary row with at least one match, once (join table only) */
+    YTGPU_JOIN_ANTI = 3   /* LEFT ONLY: each primary row without a match, once (join table only) */
+} ytgpu_join_kind;
 #define YTGPU_JOIN_NO_ROW 0xffffffffu
 #define YTGPU_JOIN_MAX_KEYS 8
 
 int ytgpu_hash_join(ytgpu_context* ctx, const ytgpu_column_view* primary_keys, const ytgpu_column_view* foreign_keys,
                     uint32_t key_count, int kind, uint32_t* out_primary_rows, uint32_t* out_foreign_rows,
                     uint64_t pairs_capacity, uint64_t* out_pair_count /* host */, int out_mem, ytgpu_error* err);
+
+/* Join table: the foreign (right) side built once and probed any number of times, one block of primary rows at a time.
+ * Build.  foreign_keys as ytgpu_hash_join takes them (1 .. YTGPU_JOIN_MAX_KEYS columns of one length, INT64 / UINT64 / DOUBLE /
+ * BOOLEAN in any encoding the GROUP BY calls take, fewer than 2^30 rows, HOST or DEVICE memory).  The table owns a device
+ * copy of the foreign key tuples, decoded to 64-bit payloads plus a null mask per row: the caller may free or overwrite the
+ * foreign key buffers as soon as the build returns, and no probe reads them.  The build also runs every step that depends
+ * on the foreign side only (the assign step of the GROUP BY calls, the per-key counts and their scan, the stable radix
+ * sort of the foreign rows by slot), so no probe repeats them.  The table records its context, key count and key types; it
+ * is immutable, may be probed from any thread that may use its context, and must be destroyed before its context.
+ * NULL rules.  YTGPU_JOIN_NULLS_EQUAL: NULL equals NULL, exactly as ytgpu_hash_join (YT QL).  YTGPU_JOIN_NULLS_NEVER_MATCH:
+ * the SQL rule of YQL and ClickHouse, a key tuple with any NULL component matches nothing: such a foreign row does not
+ * enter the table, and such a primary row gives no INNER pair, the LEFT pair (p, YTGPU_JOIN_NO_ROW), no SEMI row and an
+ * ANTI row.  DOUBLE keys compare by bit pattern under both rules (-0.0 does not match +0.0, a NaN matches only the same
+ * NaN bits).  SQL value equality of doubles is not offered; what YQL's map join does with -0.0 and NaN keys is not known
+ * here, so a YQL caller with such keys sees this difference: a known limit.
+ * Probe.  primary_keys: key_count columns of the table's key count and types, at most 2^30 rows; primary row indexes are
+ * the rows of these columns, foreign row indexes the rows of the build's columns.  INNER and LEFT give exactly the pairs
+ * and the order of ytgpu_hash_join (ascending primary row, then ascending foreign row; a LEFT miss as (p,
+ * YTGPU_JOIN_NO_ROW) at its place) into out_primary_rows / out_foreign_rows.  SEMI and ANTI give ascending primary row
+ * indexes in out_primary_rows; out_foreign_rows must be NULL.  Capacity protocol of ytgpu_hash_join: *out_count is
+ * written once the call gets that far; no outputs is a count query; a capacity below the count is INVALID_ARGUMENT with the
+ * count written.  A SEMI / ANTI count is at most the primary row count, so that capacity always suffices.
+ * Errors.  INVALID_ARGUMENT: a null context, table or argument; a table of another context; a key count or key type
+ * other than the table's; an unknown kind or NULL rule; a SEMI / ANTI probe with out_foreign_rows, an INNER / LEFT one
+ * with exactly one output.  UNSUPPORTED: a side over its row limit (checked from the views, before any access) or a key
+ * type other than the four scalars.  ytgpu_join_table_destroy(NULL) is a no-op.
+ * Synchronisations.  Build: the read of the assign step's error word (again when a full table doubles), the sort's plan
+ * read from 2^18 foreign rows, and a closing synchronisation.  SEMI / ANTI probe: one read-back (the row count, after the
+ * rows are listed), and a copy after it when out_mem is HOST or the capacity is below the primary row count.  INNER /
+ * LEFT probe: the read of the pair count and, with outputs, a closing synchronisation.  Bit-packed DEVICE columns cost one
+ * more read of their header word, as in every call. */
+typedef enum ytgpu_join_nulls {
+    YTGPU_JOIN_NULLS_EQUAL = 0,       /* QL: NULL equals NULL, exactly as ytgpu_hash_join */
+    YTGPU_JOIN_NULLS_NEVER_MATCH = 1  /* SQL: a key tuple with any NULL component matches nothing */
+} ytgpu_join_nulls;
+typedef struct ytgpu_join_table ytgpu_join_table;
+
+int ytgpu_join_table_build(ytgpu_context* ctx, const ytgpu_column_view* foreign_keys, uint32_t key_count, int nulls,
+                           ytgpu_join_table** out, ytgpu_error* err);
+int ytgpu_join_table_probe(ytgpu_context* ctx, const ytgpu_join_table* table, const ytgpu_column_view* primary_keys,
+                           uint32_t key_count, int kind, uint32_t* out_primary_rows, uint32_t* out_foreign_rows,
+                           uint64_t capacity, uint64_t* out_count /* host */, int out_mem, ytgpu_error* err);
+int ytgpu_join_table_destroy(ytgpu_join_table* table, ytgpu_error* err);
 
 /* Gathers.  ytgpu_gather_column decodes `column` at rows[i] into out_values[i] and bit i of out_null_bitmap, for i < count,
  * in the layout of ytgpu_evaluate_expression: out_values count 64-bit bit patterns (a NULL row holds 0), out_null_bitmap

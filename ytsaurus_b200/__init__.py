@@ -9,7 +9,7 @@ from .rowset import EValueType, ESortOrder, Rowset, U64, Sentinel, make_rowset, 
 
 
 def __getattr__(name):
-    if name in ("GpuContext", "Column"):
+    if name in ("GpuContext", "Column", "JoinTable"):
         from . import runtime
         return getattr(runtime, name)
     raise AttributeError(name)

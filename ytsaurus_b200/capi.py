@@ -121,6 +121,7 @@ EXPORTED_SYMBOLS = [
     "ytgpu_build_bitmap_from_flags", "ytgpu_build_bytemap_from_flags", "ytgpu_count_flags", "ytgpu_build_dictionary_indexes",
     "ytgpu_count_total_string_length", "ytgpu_translate_rle_indexes", "ytgpu_context_get_option", "ytgpu_convert_ch_column_to_values", "ytgpu_convert_string_column_to_ch", "ytgpu_decode_column_typed",
     "ytgpu_hash_join", "ytgpu_gather_column", "ytgpu_gather_string_column", "ytgpu_order_rows",
+    "ytgpu_join_table_build", "ytgpu_join_table_probe", "ytgpu_join_table_destroy",
 ]
 
 FLAGS_DICTIONARY_ZERO, FLAGS_BITMAP = 0, 1
@@ -148,7 +149,8 @@ class FlagSource(C.Structure):
 
 
 AGG_SUM, AGG_MIN, AGG_MAX, AGG_COUNT, AGG_AVG, AGG_ARGMIN, AGG_ARGMAX, AGG_FIRST = range(8)
-JOIN_INNER, JOIN_LEFT = 0, 1
+JOIN_INNER, JOIN_LEFT, JOIN_SEMI, JOIN_ANTI = 0, 1, 2, 3
+JOIN_NULLS_EQUAL, JOIN_NULLS_NEVER_MATCH = 0, 1
 JOIN_NO_ROW = 0xFFFFFFFF
 JOIN_MAX_KEYS = 8
 
@@ -382,6 +384,10 @@ def load() -> C.CDLL:
                                            C.c_void_p, C.c_int, C.POINTER(Error)]
     lib.ytgpu_hash_join.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_int, C.c_void_p, C.c_void_p, C.c_uint64,
                                     C.POINTER(C.c_uint64), C.c_int, C.POINTER(Error)]
+    lib.ytgpu_join_table_build.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_int, C.POINTER(C.c_void_p), C.POINTER(Error)]
+    lib.ytgpu_join_table_probe.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_int, C.c_void_p, C.c_void_p, C.c_uint64,
+                                           C.POINTER(C.c_uint64), C.c_int, C.POINTER(Error)]
+    lib.ytgpu_join_table_destroy.argtypes = [C.c_void_p, C.POINTER(Error)]
     lib.ytgpu_gather_column.argtypes = [C.c_void_p, C.POINTER(ColumnView), C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
                                         C.POINTER(C.c_uint64), C.c_int, C.POINTER(Error)]
     lib.ytgpu_gather_string_column.argtypes = [C.c_void_p, C.POINTER(StringColumn), C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,

@@ -1,19 +1,29 @@
-// join.cu — hash JOIN: inner and left equi-joins over key tuples, and the gathers that turn its pairs into columns.
+// join.cu — hash JOIN: the join table (built once from the foreign keys, probed any number of times) with inner, left,
+// left semi and left only joins over key tuples, the one-shot ytgpu_hash_join over it, and the gathers that turn its pairs
+// into columns.
 //
 // Replaces the row-by-row hash lookup of YT QL's JoinOpHelper (library/query/engine/cg_routines/registry.cpp): the foreign
-// rows are built into a table keyed on the join key, every primary row looks its key up there.  Five steps:
-//   1. build: the GROUP BY assign step (key_tuple.cuh) over the foreign keys, sized for the foreign row count: rep[slot] =
-//      a foreign row holding the tuple, counts[slot] = the foreign rows of the tuple, slot_of_row[f] = f's slot.
+// rows are built into a table keyed on the join key, every primary row looks its key up there.  The build (steps 0-2)
+// depends on the foreign side only; a probe (steps 3-5) on the table and one set of primary rows:
+//   0. decode: the foreign key tuples, decoded to 64-bit payloads plus a null mask per row, into the table's own memory: a
+//      probe compares against them with one plain load per column, and never reads the caller's foreign columns.
+//   1. assign: the GROUP BY assign step (key_tuple.cuh) over the foreign keys, sized for the foreign row count: rep[slot] =
+//      a foreign row holding the tuple, counts[slot] = the foreign rows of the tuple, slot_of_row[f] = f's slot.  Under
+//      the SQL NULL rule the assign step's predicate (null mask == 0) keeps the rows with a NULL component out.
 //   2. per-key lists: the counts, scanned, give each slot's start; one stable radix sort of the foreign rows by slot lists
 //      every slot's rows in ascending order (an atomic scatter would not be stable, and the order is part of the result).
 //   3. probe: each primary row loads and hashes its tuple with the same hash_tuple, walks the table comparing against the
-//      FOREIGN columns at the slot's row and stops at an empty slot: its slot, and its pair count.
-//   4. offsets: the pair counts, scanned; the total is read back (the count query ends here, before steps 2 and 5).
+//      table's decoded tuples at the slot's row and stops at an empty slot: its slot, and its pair count.  SEMI / ANTI
+//      run the existence probe instead: one flag per primary row, no slot and no count.
+//   4. offsets: the pair counts (or flags), scanned; the total is read back (a count query ends here).  SEMI / ANTI list
+//      the flagged rows through the scanned flags.
 //   5. write: each CTA owns a fixed range of output positions, finds its first primary row by binary search over the
 //      offsets and walks the rows and their slot lists from there, galloping over rows without pairs.  So a key with 10^6
 //      foreign rows spreads over about 245 CTAs, and a run of r unmatched rows costs a thread about 2 log2(r) loads:
 //      neither serialises on one thread.
 #include <algorithm>
+#include <new>
+#include <vector>
 
 #include "columnar.cuh"
 #include "context.cuh"
@@ -31,13 +41,46 @@ constexpr u32 kNoRow = YTGPU_JOIN_NO_ROW;
 constexpr u64 kMaxPrimaryRows = 1ull << 30;
 constexpr u64 kMaxForeignRows = (1ull << 30) - 1;
 
+// The table's own copy of the foreign key tuples (step 0): payload of key k of row f at w[k * rows + f], NULL as 0.
+struct TableKeys {
+    const u64* w;
+    const u8* nulls;  // bit k: key k of the row is NULL; nullptr when no row in the table has a NULL component
+    u64 rows;
+};
+
+template <int NK>
+__device__ __forceinline__ KeyTuple load_table_tuple(const TableKeys& F, u32 count, u32 row) {
+    KeyTuple t;
+    t.nulls = F.nulls ? F.nulls[row] : 0u;
+#pragma unroll
+    for (u32 k = 0; k < (u32)(NK ? NK : kMaxGroupKeys); ++k) t.w[k] = (NK || k < count) ? F.w[(u64)k * F.rows + row] : 0;
+    return t;
+}
+
+// Step 0: every foreign row's tuple, decoded once.  DIRECT: every key column is a plain 64-bit vector.
+template <bool DIRECT>
+__global__ void __launch_bounds__(256) hj_decode_keys_kernel(const KeyColumns K, u64 n, u64* __restrict__ w, u8* __restrict__ nulls) {
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
+        u32 m = 0;
+#pragma unroll 1
+        for (u32 k = 0; k < K.count; ++k) {
+            bool nul = false;
+            const u64 v = DIRECT ? reinterpret_cast<const u64*>(K.col[k].values)[(u64)K.col[k].start + i] : decode_at(K.col[k], (i64)i, &nul);
+            w[(u64)k * n + i] = nul ? 0 : v;
+            m |= (u32)nul << k;
+        }
+        nulls[i] = (u8)m;
+    }
+}
+
 // Step 3, with the two-rows-in-flight structure of mg_assign_kernel: the probe is a chain of dependent loads (key -> slot ->
-// the foreign row's key), so both rows' loads are issued before either is used.  DIRECT: every key column of BOTH sides is
-// a plain 64-bit vector; NK: 1, 2 or 0 (K.count columns).
-template <bool DIRECT, int NK>
-__global__ void __launch_bounds__(256) hj_probe_kernel(const KeyColumns P, const KeyColumns F, u64 n, const u32* __restrict__ rep, u64 mask,
-                                                       const unsigned long long* __restrict__ counts, int left, u32* __restrict__ probe_slot,
-                                                       u64* __restrict__ pair_counts) {
+// the foreign row's key), so both rows' loads are issued before either is used.  DIRECT: every primary key column is a
+// plain 64-bit vector (the foreign side is always the table's decoded copy); NK: 1, 2 or 0 (P.count columns).  emit(row,
+// slot) runs once per primary row, slot = kNoSlot without a match.  never_match: a primary tuple with a NULL component
+// matches nothing (the SQL rule) and does not touch the table.
+template <bool DIRECT, int NK, class Emit>
+__device__ __forceinline__ void probe_rows(const KeyColumns& P, const TableKeys& F, u64 n, const u32* __restrict__ rep, u64 mask,
+                                           bool never_match, Emit emit) {
     constexpr int R = NK ? 2 : 1;  // 3+ key columns: four 8-word tuples in flight would cost the occupancy
     const u64 stride = (u64)gridDim.x * blockDim.x;
     u64 base = (u64)blockIdx.x * blockDim.x + threadIdx.x;
@@ -48,7 +91,7 @@ __global__ void __launch_bounds__(256) hj_probe_kernel(const KeyColumns P, const
     for (; base < n; base += stride * R) {
         u64 row[R], b[R];
         u32 r[R], slot[R];
-        bool valid[R];
+        bool valid[R], look[R];
         KeyTuple mine[R], cand[R];
 #pragma unroll
         for (int j = 0; j < R; ++j) {
@@ -60,21 +103,22 @@ __global__ void __launch_bounds__(256) hj_probe_kernel(const KeyColumns P, const
         for (int j = 0; j < R; ++j) {
             row[j] = base + (u64)j * stride;
             valid[j] = row[j] < n;
+            look[j] = valid[j] && !(never_match && mine[j].nulls);
             slot[j] = kNoSlot;
-            b[j] = valid[j] ? hash_tuple<NK>(P, mine[j]) & mask : 0;
-            r[j] = valid[j] ? rep[b[j]] : kNoSlot;
+            b[j] = look[j] ? hash_tuple<NK>(P, mine[j]) & mask : 0;
+            r[j] = look[j] ? rep[b[j]] : kNoSlot;
         }
 #pragma unroll
         for (int j = 0; j < R; ++j)
-            if (valid[j] && r[j] != kNoSlot) cand[j] = load_tuple<DIRECT, NK>(F, r[j]);
+            if (r[j] != kNoSlot) cand[j] = load_table_tuple<NK>(F, P.count, r[j]);
 #pragma unroll
         for (int j = 0; j < R; ++j) {
-            if (!valid[j]) continue;
+            if (!look[j]) continue;
             u32 rr = r[j];
             bool have = true;  // cand[j] holds the key of foreign row rr
             u64 bb = b[j];
             for (u64 probes = 0; probes <= mask && rr != kNoSlot; ++probes) {
-                if (same_tuple<NK>(P, mine[j], have ? cand[j] : load_tuple<DIRECT, NK>(F, rr))) {
+                if (same_tuple<NK>(P, mine[j], have ? cand[j] : load_table_tuple<NK>(F, P.count, rr))) {
                     slot[j] = (u32)bb;
                     break;
                 }
@@ -84,11 +128,36 @@ __global__ void __launch_bounds__(256) hj_probe_kernel(const KeyColumns P, const
             }
         }
 #pragma unroll
-        for (int j = 0; j < R; ++j) {
-            if (!valid[j]) continue;
-            probe_slot[row[j]] = slot[j];
-            pair_counts[row[j]] = slot[j] != kNoSlot ? (u64)counts[slot[j]] : (left ? 1 : 0);
-        }
+        for (int j = 0; j < R; ++j)
+            if (valid[j]) emit(row[j], slot[j]);
+    }
+}
+
+// Step 3 of INNER / LEFT: the slot and the pair count of every primary row.
+template <bool DIRECT, int NK>
+__global__ void __launch_bounds__(256) hj_probe_kernel(const KeyColumns P, const TableKeys F, u64 n, const u32* __restrict__ rep, u64 mask,
+                                                       const unsigned long long* __restrict__ counts, int left, int never_match,
+                                                       u32* __restrict__ probe_slot, u64* __restrict__ pair_counts) {
+    probe_rows<DIRECT, NK>(P, F, n, rep, mask, never_match, [&](u64 row, u32 slot) {
+        probe_slot[row] = slot;
+        pair_counts[row] = slot != kNoSlot ? (u64)counts[slot] : (left ? 1 : 0);
+    });
+}
+
+// Step 3 of SEMI / ANTI, the existence probe: it stops at the first match, reads neither the counts nor the per-key lists,
+// and writes one flag per primary row: 1 when the row is listed (SEMI: it has a match; ANTI: it has none).
+template <bool DIRECT, int NK>
+__global__ void __launch_bounds__(256) hj_exists_kernel(const KeyColumns P, const TableKeys F, u64 n, const u32* __restrict__ rep, u64 mask,
+                                                        int never_match, int anti, u64* __restrict__ flags) {
+    probe_rows<DIRECT, NK>(P, F, n, rep, mask, never_match, [&](u64 row, u32 slot) { flags[row] = (slot != kNoSlot) != (anti != 0); });
+}
+
+// Step 4 of SEMI / ANTI: the scanned flags -> the ascending list of flagged rows.
+__global__ void __launch_bounds__(256) hj_list_rows_kernel(const u64* __restrict__ offsets, u64 n, const u64* __restrict__ total,
+                                                           u32* __restrict__ out) {
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
+        const u64 end = i + 1 < n ? offsets[i + 1] : *total;
+        if (end != offsets[i]) out[offsets[i]] = (u32)i;
     }
 }
 
@@ -106,8 +175,8 @@ __device__ __forceinline__ u32 tile_index(u32 i) { return i + i / kWriteItems; }
 
 __global__ void __launch_bounds__(kWriteThreads) hj_write_pairs_kernel(const u64* __restrict__ offsets, u64 n, u64 total,
                                                                        const u32* __restrict__ probe_slot, const u64* __restrict__ slot_start,
-                                                                       const SortPlan* plan, const u32* pa, const u32* pb,
-                                                                       u32* __restrict__ out_primary, u32* __restrict__ out_foreign) {
+                                                                       const u32* __restrict__ rows_by_slot, u32* __restrict__ out_primary,
+                                                                       u32* __restrict__ out_foreign) {
     __shared__ u32 s_p[kWriteTile + kWriteThreads], s_f[kWriteTile + kWriteThreads];
     const u64 tile0 = (u64)blockIdx.x * kWriteTile;
     const u64 first = tile0 + (u64)threadIdx.x * kWriteItems;
@@ -153,7 +222,7 @@ __global__ void __launch_bounds__(kWriteThreads) hj_write_pairs_kernel(const u64
             const u32 s = probe_slot[p];
             const u32 i = tile_index(threadIdx.x * kWriteItems + k);
             s_p[i] = (u32)p;
-            s_f[i] = s == kNoSlot ? kNoRow : perm_at(plan, pa, pb, slot_start[s] + (o - start));
+            s_f[i] = s == kNoSlot ? kNoRow : rows_by_slot[slot_start[s] + (o - start)];
         }
     }
     __syncthreads();
@@ -233,6 +302,229 @@ Status check_side(const ytgpu_column_view* keys, u32 key_count, const char* side
     return Status{};
 }
 
+bool known_kind(int kind) {
+    return kind == YTGPU_JOIN_INNER || kind == YTGPU_JOIN_LEFT || kind == YTGPU_JOIN_SEMI || kind == YTGPU_JOIN_ANTI;
+}
+
+// A built table (ytgpu_join_table): the foreign side after steps 0-2.  Immutable once built; its buffers are the
+// context's stream-ordered memory.
+struct JoinTable {
+    Context* ctx = nullptr;
+    u32 key_count = 0;
+    u8 types[kMaxGroupKeys] = {};
+    int nulls = YTGPU_JOIN_NULLS_EQUAL;
+    u64 rows = 0;                // foreign rows
+    bool null_keys = false;      // a row in the table may have a NULL component: the probe loads the null masks
+    bool listed = false;         // step 2 ran (a one-shot count query skips it: it writes no pairs)
+    DevBuf<u64> keys;            // step 0: key_count * rows payloads, column by column
+    DevBuf<u8> null_mask;        // step 0: bit k = key k of the row is NULL
+    KeyTable T;                  // step 1: rep and counts (slot_of_row and first are released after step 2)
+    DevBuf<u64> slot_start;      // step 2: exclusive scan of counts
+    DevBuf<u32> rows_by_slot;    // step 2: the foreign rows stable-sorted by slot, slot s at [slot_start[s], + counts[s])
+
+    TableKeys dev() const { return TableKeys{keys.p, null_keys ? null_mask.p : nullptr, rows}; }
+};
+
+// Steps 0-2 over the staged foreign key columns KF (nf rows).  list_rows = false skips step 2: the table then answers
+// counts and SEMI / ANTI probes, not INNER / LEFT pair writes.  Synchronises once for the assign step's error word (more
+// when a full table doubles), and the sort reads its plan back once from 2^18 rows.
+Status build_table(Context* ctx, const KeyColumns& KF, bool foreign_direct, u64 nf, int nulls, bool list_rows, JoinTable* J) {
+    J->ctx = ctx;
+    J->key_count = KF.count;
+    for (u32 k = 0; k < KF.count; ++k) J->types[k] = KF.col[k].value_type;
+    J->nulls = nulls;
+    J->rows = nf;
+    const bool never_match = nulls == YTGPU_JOIN_NULLS_NEVER_MATCH;
+    // under the SQL rule no row with a NULL component enters the table; plain 64-bit columns have no NULLs at all
+    J->null_keys = !never_match && !foreign_direct;
+    YTGPU_TRY(J->keys.allocate(ctx, nf * KF.count));
+    YTGPU_TRY(J->null_mask.allocate(ctx, nf));
+    if (nf == 0) {  // a one-slot empty table: every probe ends at once
+        J->T.cap = 1;
+        YTGPU_TRY(J->T.rep.allocate(ctx, 1));
+        YTGPU_TRY(J->T.counts.allocate(ctx, 1));
+        YTGPU_CUDA_TRY(cudaMemsetAsync(J->T.rep.p, 0xff, 4, ctx->stream));
+        YTGPU_CUDA_TRY(cudaMemsetAsync(J->T.counts.p, 0, 8, ctx->stream));
+        J->listed = true;
+        return Status{};
+    }
+    {  // step 0
+        KernelTimer t(ctx, KC_JOIN);
+        const u32 blocks = blocks_for(nf, 256, 8);
+        if (foreign_direct) hj_decode_keys_kernel<true><<<blocks, 256, 0, ctx->stream>>>(KF, nf, J->keys.p, J->null_mask.p);
+        else hj_decode_keys_kernel<false><<<blocks, 256, 0, ctx->stream>>>(KF, nf, J->keys.p, J->null_mask.p);
+        YTGPU_CUDA_TRY(cudaGetLastError());
+    }
+    // step 1; the SQL rule keeps the rows whose null mask is not 0 out through the assign step's predicate
+    ColumnDev mask_col{};
+    int op = YTGPU_CMP_NONE;
+    if (never_match) {
+        mask_col.count = (i64)nf;
+        mask_col.values = J->null_mask.p;
+        mask_col.values_count = nf;
+        mask_col.bit_width = 8;
+        mask_col.has_values = 1;
+        mask_col.value_type = YTGPU_TYPE_UINT64;
+        op = YTGPU_CMP_EQ;
+    }
+    YTGPU_TRY(assign_key_slots(ctx, KC_JOIN, KF, foreign_direct, mask_col, op, 0, nf, nf, &J->T));
+    J->T.first.reset();
+    if (!list_rows) return Status{};
+
+    // step 2 (rows kept out by the SQL rule have slot kNoSlot: they sort behind every listed row)
+    DevBuf<u64> sort_keys, scan_sums, total;
+    YTGPU_TRY(J->slot_start.allocate(ctx, J->T.cap));
+    YTGPU_TRY(scan_sums.allocate(ctx, scan_block_count(J->T.cap)));
+    YTGPU_TRY(total.allocate(ctx, 1));
+    YTGPU_CUDA_TRY(cudaMemcpyAsync(J->slot_start.p, J->T.counts.p, J->T.cap * 8, cudaMemcpyDeviceToDevice, ctx->stream));
+    YTGPU_TRY(sort_keys.allocate(ctx, nf));
+    {
+        KernelTimer t(ctx, KC_JOIN, 4);
+        exclusive_scan_u64(ctx->stream, J->slot_start.p, J->T.cap, scan_sums.p, total.p);
+        hj_slot_keys_kernel<<<blocks_for(nf, 256, 8), 256, 0, ctx->stream>>>(J->T.slot_of_row.p, nf, sort_keys.p);
+        YTGPU_CUDA_TRY(cudaGetLastError());
+    }
+    J->T.slot_of_row.reset();
+    SortScratch scratch;
+    PermRef perm;
+    const u64* chunk[1] = {sort_keys.p};
+    YTGPU_TRY(radix_sort_chunks(ctx, chunk, 1, nf, &scratch, &perm));
+    YTGPU_TRY(J->rows_by_slot.allocate(ctx, nf));
+    YTGPU_TRY(materialize_perm(ctx, perm, nf, J->rows_by_slot.p));
+    J->listed = true;
+    return Status{};
+}
+
+// Steps 3-5 of one probe: the staged primary key columns KP (np >= 1 rows) against table J.  The caller has checked the
+// arguments and written *out_count = 0.
+Status probe_table(Context* ctx, const JoinTable& J, const KeyColumns& KP, bool primary_direct, u64 np, int kind, u32* out_primary,
+                   u32* out_foreign, u64 capacity, u64* out_count, int out_mem) {
+    const TableKeys F = J.dev();
+    const u64 mask = J.T.cap - 1;
+    const int never_match = J.nulls == YTGPU_JOIN_NULLS_NEVER_MATCH;
+    const u32 key_count = KP.count;
+    const u32 blocks = blocks_for((np + 1) / 2, 256, 16);
+    const bool host = out_mem == YTGPU_MEM_HOST;
+    DevBuf<u64> offsets, scan_sums, total;
+    YTGPU_TRY(offsets.allocate(ctx, np));
+    YTGPU_TRY(scan_sums.allocate(ctx, scan_block_count(np)));
+    YTGPU_TRY(total.allocate(ctx, 1));
+#define YTGPU_HJ_DISPATCH(LAUNCH)                           \
+    if (primary_direct && key_count == 1) LAUNCH(true, 1);  \
+    else if (primary_direct && key_count == 2) LAUNCH(true, 2); \
+    else if (primary_direct) LAUNCH(true, 0);               \
+    else if (key_count == 1) LAUNCH(false, 1);              \
+    else if (key_count == 2) LAUNCH(false, 2);              \
+    else LAUNCH(false, 0)
+
+    if (kind == YTGPU_JOIN_SEMI || kind == YTGPU_JOIN_ANTI) {
+        {  // steps 3 and 4: flags, their scan, and the list of flagged rows
+            KernelTimer t(ctx, KC_JOIN, out_primary ? 5 : 4);
+            const int anti = kind == YTGPU_JOIN_ANTI;
+#define YTGPU_HJ_EXISTS(D, N) \
+    hj_exists_kernel<D, N><<<blocks, 256, 0, ctx->stream>>>(KP, F, np, J.T.rep.p, mask, never_match, anti, offsets.p)
+            YTGPU_HJ_DISPATCH(YTGPU_HJ_EXISTS);
+#undef YTGPU_HJ_EXISTS
+            exclusive_scan_u64(ctx->stream, offsets.p, np, scan_sums.p, total.p);
+            YTGPU_CUDA_TRY(cudaGetLastError());
+        }
+        // the list has at most np rows: with that much DEVICE capacity it goes straight to the output, and the count is
+        // the one read-back
+        DevBuf<u32> staged;
+        u32* dst = out_primary;
+        if (out_primary && (host || capacity < np)) {
+            YTGPU_TRY(staged.allocate(ctx, np));
+            dst = staged.p;
+        }
+        if (out_primary) {
+            hj_list_rows_kernel<<<blocks_for(np, 256, 16), 256, 0, ctx->stream>>>(offsets.p, np, total.p, dst);
+            YTGPU_CUDA_TRY(cudaGetLastError());
+        }
+        u64 rows = 0;
+        YTGPU_CUDA_TRY(cudaMemcpyAsync(&rows, total.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
+        YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+        *out_count = rows;
+        if (!out_primary) return Status{};
+        if (rows > capacity)
+            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "the join lists %llu rows, capacity is %llu", (unsigned long long)rows,
+                               (unsigned long long)capacity);
+        if (dst != out_primary && rows) {
+            YTGPU_TRY(copy_out(ctx, out_primary, dst, rows * 4, out_mem));
+            YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+        }
+        return Status{};
+    }
+
+    // step 3
+    DevBuf<u32> probe_slot;
+    YTGPU_TRY(probe_slot.allocate(ctx, np));
+    {
+        KernelTimer t(ctx, KC_JOIN);
+        const int left = kind == YTGPU_JOIN_LEFT;
+#define YTGPU_HJ_PROBE(D, N)                                                                                                    \
+    hj_probe_kernel<D, N><<<blocks, 256, 0, ctx->stream>>>(KP, F, np, J.T.rep.p, mask, J.T.counts.p, left, never_match, probe_slot.p, \
+                                                           offsets.p)
+        YTGPU_HJ_DISPATCH(YTGPU_HJ_PROBE);
+#undef YTGPU_HJ_PROBE
+        YTGPU_CUDA_TRY(cudaGetLastError());
+    }
+#undef YTGPU_HJ_DISPATCH
+    // step 4
+    {
+        KernelTimer t(ctx, KC_JOIN, 3);
+        exclusive_scan_u64(ctx->stream, offsets.p, np, scan_sums.p, total.p);
+        YTGPU_CUDA_TRY(cudaGetLastError());
+    }
+    u64 pairs = 0;
+    YTGPU_CUDA_TRY(cudaMemcpyAsync(&pairs, total.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    *out_count = pairs;
+    if (!out_primary) return Status{};
+    if (pairs > capacity)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "the join has %llu pairs, pairs_capacity is %llu", (unsigned long long)pairs,
+                           (unsigned long long)capacity);
+    if (pairs == 0) return Status{};
+    if (!J.listed) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "the table was built without its per-key row lists");
+
+    // step 5
+    DevBuf<u32> tp, tf;
+    u32 *dp = out_primary, *df = out_foreign;
+    if (host) {
+        YTGPU_TRY(tp.allocate(ctx, pairs));
+        YTGPU_TRY(tf.allocate(ctx, pairs));
+        dp = tp.p;
+        df = tf.p;
+    }
+    {
+        KernelTimer t(ctx, KC_JOIN);
+        const u64 tiles = (pairs + kWriteTile - 1) / kWriteTile;
+        hj_write_pairs_kernel<<<(u32)tiles, kWriteThreads, 0, ctx->stream>>>(offsets.p, np, pairs, probe_slot.p, J.slot_start.p,
+                                                                             J.rows_by_slot.p, dp, df);
+        YTGPU_CUDA_TRY(cudaGetLastError());
+    }
+    if (host) {
+        YTGPU_TRY(copy_out(ctx, out_primary, dp, pairs * 4, YTGPU_MEM_HOST));
+        YTGPU_TRY(copy_out(ctx, out_foreign, df, pairs * 4, YTGPU_MEM_HOST));
+    }
+    YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return Status{};
+}
+
+// Stages key_count columns into staged (key_count entries) and reports whether each is a plain 64-bit vector without base
+// or zig-zag.
+Status stage_keys(Context* ctx, const ytgpu_column_view* keys, u32 key_count, std::vector<StagedColumn>* staged, KeyColumns* K,
+                  bool* direct) {
+    *K = KeyColumns{};
+    K->count = key_count;
+    *direct = true;
+    for (u32 k = 0; k < key_count; ++k) {
+        YTGPU_TRY(stage_column(ctx, &keys[k], &(*staged)[k]));
+        K->col[k] = (*staged)[k].dev;
+        *direct = *direct && is_direct64(K->col[k]) && K->col[k].base == 0 && !K->col[k].zigzag;
+    }
+    return Status{};
+}
+
 Status hash_join_impl(Context* ctx, const ytgpu_column_view* primary_keys, const ytgpu_column_view* foreign_keys, u32 key_count, int kind,
                       u32* out_primary, u32* out_foreign, u64 pairs_capacity, u64* out_pair_count, int out_mem) {
     if (!primary_keys || !foreign_keys || !out_pair_count) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null argument");
@@ -254,111 +546,74 @@ Status hash_join_impl(Context* ctx, const ytgpu_column_view* primary_keys, const
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
     if (np == 0) return Status{};
 
+    // both sides staged (and their column checks made) before the first launch; then one build, one probe
     std::vector<StagedColumn> sp(key_count), sf(key_count);
-    KeyColumns KP{}, KF{};
-    KP.count = KF.count = key_count;
-    bool direct = true;  // plain 64-bit key vectors on both sides: one load per column
-    for (u32 k = 0; k < key_count; ++k) {
-        YTGPU_TRY(stage_column(ctx, &primary_keys[k], &sp[k]));
-        YTGPU_TRY(stage_column(ctx, &foreign_keys[k], &sf[k]));
-        KP.col[k] = sp[k].dev;
-        KF.col[k] = sf[k].dev;
-        for (const ColumnDev* c : {&sp[k].dev, &sf[k].dev}) direct = direct && is_direct64(*c) && c->base == 0 && !c->zigzag;
-    }
-    bool foreign_direct = true;
-    for (u32 k = 0; k < key_count; ++k) foreign_direct = foreign_direct && is_direct64(sf[k].dev) && sf[k].dev.base == 0 && !sf[k].dev.zigzag;
+    KeyColumns KP, KF;
+    bool primary_direct = false, foreign_direct = false;
+    YTGPU_TRY(stage_keys(ctx, primary_keys, key_count, &sp, &KP, &primary_direct));
+    YTGPU_TRY(stage_keys(ctx, foreign_keys, key_count, &sf, &KF, &foreign_direct));
+    JoinTable J;
+    YTGPU_TRY(build_table(ctx, KF, foreign_direct, nf, YTGPU_JOIN_NULLS_EQUAL, out_primary != nullptr, &J));
+    return probe_table(ctx, J, KP, primary_direct, np, kind, out_primary, out_foreign, pairs_capacity, out_pair_count, out_mem);
+}
 
-    // step 1 (an empty foreign side: a one-slot empty table, so every probe ends at once)
-    KeyTable T;
-    if (nf > 0) {
-        YTGPU_TRY(assign_key_slots(ctx, KC_JOIN, KF, foreign_direct, ColumnDev{}, YTGPU_CMP_NONE, 0, nf, nf, &T));
-    } else {
-        T.cap = 1;
-        YTGPU_TRY(T.rep.allocate(ctx, 1));
-        YTGPU_TRY(T.counts.allocate(ctx, 1));
-        YTGPU_CUDA_TRY(cudaMemsetAsync(T.rep.p, 0xff, 4, ctx->stream));
-        YTGPU_CUDA_TRY(cudaMemsetAsync(T.counts.p, 0, 8, ctx->stream));
+Status join_table_build_impl(Context* ctx, const ytgpu_column_view* foreign_keys, u32 key_count, int nulls, JoinTable** out) {
+    if (!foreign_keys || !out) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null argument");
+    *out = nullptr;
+    if (key_count == 0 || key_count > (u32)YTGPU_JOIN_MAX_KEYS)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "key column count must be in [1, %d]", YTGPU_JOIN_MAX_KEYS);
+    if (nulls != YTGPU_JOIN_NULLS_EQUAL && nulls != YTGPU_JOIN_NULLS_NEVER_MATCH)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "unknown NULL rule %d", nulls);
+    u64 nf = 0;
+    YTGPU_TRY(check_side(foreign_keys, key_count, "foreign", kMaxForeignRows, &nf));
+    YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
+    std::vector<StagedColumn> sf(key_count);
+    KeyColumns KF;
+    bool foreign_direct = false;
+    YTGPU_TRY(stage_keys(ctx, foreign_keys, key_count, &sf, &KF, &foreign_direct));
+    JoinTable* J = new (std::nothrow) JoinTable();
+    if (!J) return make_status(YTGPU_ERR_OUT_OF_MEMORY, "host allocation failed");
+    Status s = build_table(ctx, KF, foreign_direct, nf, nulls, true, J);
+    if (s.code == YTGPU_OK) {
+        const cudaError_t e = cudaStreamSynchronize(ctx->stream);
+        if (e != cudaSuccess) s = cuda_status(e, "cudaStreamSynchronize");
     }
-
-    // step 3
-    DevBuf<u32> probe_slot;
-    DevBuf<u64> offsets, scan_sums, total;
-    YTGPU_TRY(probe_slot.allocate(ctx, np));
-    YTGPU_TRY(offsets.allocate(ctx, np));
-    YTGPU_TRY(scan_sums.allocate(ctx, scan_block_count(std::max<u64>(np, T.cap))));
-    YTGPU_TRY(total.allocate(ctx, 2));
-    {
-        KernelTimer t(ctx, KC_JOIN);
-        const int left = kind == YTGPU_JOIN_LEFT;
-        const u32 blocks = blocks_for((np + 1) / 2, 256, 16);
-#define YTGPU_HJ_PROBE(D, N)                                                                                                    \
-    hj_probe_kernel<D, N><<<blocks, 256, 0, ctx->stream>>>(KP, KF, np, T.rep.p, T.cap - 1, T.counts.p, left, probe_slot.p, offsets.p)
-        if (direct && key_count == 1) YTGPU_HJ_PROBE(true, 1);
-        else if (direct && key_count == 2) YTGPU_HJ_PROBE(true, 2);
-        else if (direct) YTGPU_HJ_PROBE(true, 0);
-        else if (key_count == 1) YTGPU_HJ_PROBE(false, 1);
-        else if (key_count == 2) YTGPU_HJ_PROBE(false, 2);
-        else YTGPU_HJ_PROBE(false, 0);
-#undef YTGPU_HJ_PROBE
-        YTGPU_CUDA_TRY(cudaGetLastError());
+    if (s.code != YTGPU_OK) {
+        delete J;
+        return s;
     }
-    // step 4
-    {
-        KernelTimer t(ctx, KC_JOIN, 3);
-        exclusive_scan_u64(ctx->stream, offsets.p, np, scan_sums.p, total.p);
-        YTGPU_CUDA_TRY(cudaGetLastError());
-    }
-    u64 pairs = 0;
-    YTGPU_CUDA_TRY(cudaMemcpyAsync(&pairs, total.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
-    YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    *out_pair_count = pairs;
-    if (!out_primary) return Status{};
-    if (pairs > pairs_capacity)
-        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "the join has %llu pairs, pairs_capacity is %llu", (unsigned long long)pairs,
-                           (unsigned long long)pairs_capacity);
-    if (pairs == 0) return Status{};
-
-    // step 2 (only a foreign side with rows can have matches)
-    DevBuf<u64> slot_start, sort_keys;
-    SortScratch scratch;
-    PermRef perm;
-    if (nf > 0) {
-        YTGPU_TRY(slot_start.allocate(ctx, T.cap));
-        YTGPU_CUDA_TRY(cudaMemcpyAsync(slot_start.p, T.counts.p, T.cap * 8, cudaMemcpyDeviceToDevice, ctx->stream));
-        YTGPU_TRY(sort_keys.allocate(ctx, nf));
-        {
-            KernelTimer t(ctx, KC_JOIN, 4);
-            exclusive_scan_u64(ctx->stream, slot_start.p, T.cap, scan_sums.p, total.p + 1);
-            hj_slot_keys_kernel<<<blocks_for(nf, 256, 8), 256, 0, ctx->stream>>>(T.slot_of_row.p, nf, sort_keys.p);
-            YTGPU_CUDA_TRY(cudaGetLastError());
-        }
-        const u64* chunk[1] = {sort_keys.p};
-        YTGPU_TRY(radix_sort_chunks(ctx, chunk, 1, nf, &scratch, &perm));
-    }
-
-    // step 5
-    const bool host = out_mem == YTGPU_MEM_HOST;
-    DevBuf<u32> tp, tf;
-    u32 *dp = out_primary, *df = out_foreign;
-    if (host) {
-        YTGPU_TRY(tp.allocate(ctx, pairs));
-        YTGPU_TRY(tf.allocate(ctx, pairs));
-        dp = tp.p;
-        df = tf.p;
-    }
-    {
-        KernelTimer t(ctx, KC_JOIN);
-        const u64 tiles = (pairs + kWriteTile - 1) / kWriteTile;
-        hj_write_pairs_kernel<<<(u32)tiles, kWriteThreads, 0, ctx->stream>>>(offsets.p, np, pairs, probe_slot.p, slot_start.p, perm.plan,
-                                                                             perm.idx[0], perm.idx[1], dp, df);
-        YTGPU_CUDA_TRY(cudaGetLastError());
-    }
-    if (host) {
-        YTGPU_TRY(copy_out(ctx, out_primary, dp, pairs * 4, YTGPU_MEM_HOST));
-        YTGPU_TRY(copy_out(ctx, out_foreign, df, pairs * 4, YTGPU_MEM_HOST));
-    }
-    YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    *out = J;
     return Status{};
+}
+
+Status join_table_probe_impl(Context* ctx, const JoinTable* J, const ytgpu_column_view* primary_keys, u32 key_count, int kind,
+                             u32* out_primary, u32* out_foreign, u64 capacity, u64* out_count, int out_mem) {
+    if (!J || !primary_keys || !out_count) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null argument");
+    if (J->ctx != ctx) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "the table was built on another context");
+    if (key_count != J->key_count)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "%u key columns, the table has %u", key_count, J->key_count);
+    if (!known_kind(kind)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "unknown join kind %d", kind);
+    const bool rows_only = kind == YTGPU_JOIN_SEMI || kind == YTGPU_JOIN_ANTI;
+    if (rows_only && out_foreign)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "a SEMI or ANTI join lists primary rows only: out_foreign_rows must be NULL");
+    if (!rows_only && (out_primary == nullptr) != (out_foreign == nullptr))
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "both outputs or neither (a count query) must be given");
+    if (out_mem != YTGPU_MEM_DEVICE && out_mem != YTGPU_MEM_HOST)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "out_mem must be YTGPU_MEM_DEVICE or YTGPU_MEM_HOST");
+    u64 np = 0;
+    YTGPU_TRY(check_side(primary_keys, key_count, "primary", kMaxPrimaryRows, &np));
+    for (u32 k = 0; k < key_count; ++k)
+        if (primary_keys[k].value_type != J->types[k])
+            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "key %u: primary type 0x%x differs from the table's type 0x%x (no implicit widening)",
+                               k, primary_keys[k].value_type, J->types[k]);
+    *out_count = 0;
+    YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (np == 0) return Status{};
+    std::vector<StagedColumn> sp(key_count);
+    KeyColumns KP;
+    bool primary_direct = false;
+    YTGPU_TRY(stage_keys(ctx, primary_keys, key_count, &sp, &KP, &primary_direct));
+    return probe_table(ctx, *J, KP, primary_direct, np, kind, out_primary, out_foreign, capacity, out_count, out_mem);
 }
 
 // The row indexes of a gather, on the device.
@@ -495,6 +750,35 @@ int ytgpu_hash_join(ytgpu_context* h, const ytgpu_column_view* primary_keys, con
     CtxLock lock(h);
     return fill_error(err, hash_join_impl(as_context(h), primary_keys, foreign_keys, key_count, kind, out_primary_rows, out_foreign_rows,
                                           pairs_capacity, out_pair_count, out_mem));
+}
+
+int ytgpu_join_table_build(ytgpu_context* h, const ytgpu_column_view* foreign_keys, uint32_t key_count, int nulls, ytgpu_join_table** out,
+                           ytgpu_error* err) {
+    if (!h) return fill_error(err, make_status(YTGPU_ERR_INVALID_ARGUMENT, "null context"));
+    CtxLock lock(h);
+    JoinTable* t = nullptr;
+    const int code = fill_error(err, join_table_build_impl(as_context(h), foreign_keys, key_count, nulls, &t));
+    if (out) *out = reinterpret_cast<ytgpu_join_table*>(t);
+    return code;
+}
+
+int ytgpu_join_table_probe(ytgpu_context* h, const ytgpu_join_table* table, const ytgpu_column_view* primary_keys, uint32_t key_count,
+                           int kind, uint32_t* out_primary_rows, uint32_t* out_foreign_rows, uint64_t capacity, uint64_t* out_count,
+                           int out_mem, ytgpu_error* err) {
+    if (!h) return fill_error(err, make_status(YTGPU_ERR_INVALID_ARGUMENT, "null context"));
+    CtxLock lock(h);
+    return fill_error(err, join_table_probe_impl(as_context(h), reinterpret_cast<const JoinTable*>(table), primary_keys, key_count, kind,
+                                                 out_primary_rows, out_foreign_rows, capacity, out_count, out_mem));
+}
+
+int ytgpu_join_table_destroy(ytgpu_join_table* table, ytgpu_error* err) {
+    if (!table) return fill_error(err, Status{});
+    JoinTable* t = reinterpret_cast<JoinTable*>(table);
+    Context* ctx = t->ctx;
+    std::unique_lock<std::mutex> lock(ctx->mu);
+    const cudaError_t e = cudaSetDevice(ctx->device);
+    delete t;  // stream-ordered frees on the context's stream
+    return fill_error(err, e == cudaSuccess ? Status{} : cuda_status(e, "cudaSetDevice"));
 }
 
 int ytgpu_gather_column(ytgpu_context* h, const ytgpu_column_view* column, const uint32_t* rows, uint64_t count, uint64_t* out_values,

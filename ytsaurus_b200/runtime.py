@@ -8,6 +8,7 @@ CUDA torch tensors (DEVICE flavour: zero-copy).
 from __future__ import annotations
 
 import ctypes as C
+import weakref
 
 import numpy as np
 
@@ -85,6 +86,8 @@ class GpuContext:
 
     def close(self):
         if getattr(self, "handle", None):
+            for table in list(getattr(self, "_join_tables", ())):  # a join table is destroyed before its context
+                table.close()
             self.lib.ytgpu_context_destroy(self.handle)
             self.handle = None
 
@@ -832,6 +835,13 @@ class GpuContext:
         pairs = int(count.value)
         return prim[:pairs], fore[:pairs]
 
+    def join_table(self, foreign_keys, nulls: int = capi.JOIN_NULLS_EQUAL) -> "JoinTable":
+        """ytgpu_join_table_build: a join table over foreign_keys (a list of Column), built once and probed any number of
+        times (JoinTable.probe).  nulls: capi.JOIN_NULLS_EQUAL (NULL equals NULL, as hash_join) or
+        capi.JOIN_NULLS_NEVER_MATCH (a tuple with a NULL component matches nothing).  The table owns a copy of the keys:
+        the columns may be freed or overwritten once this returns."""
+        return JoinTable(self, foreign_keys, nulls)
+
     def gather_column(self, column: "Column", rows):
         """ytgpu_gather_column: `column` decoded at rows (uint32; capi.JOIN_NO_ROW gives NULL) -> dict(values, null_bitmap,
         null_count, column) in the rows' memory flavour, laid out as evaluate_expression's result: `column` is a Column over
@@ -1035,6 +1045,83 @@ class GpuContext:
             call(heap=heap, capacity=size, starts=starts, lengths=lengths, null_bytemap=null_bytemap)
         return dict(values=None, null_bitmap=None, null_count=int(nulls.value), value_type=int(vtype.value), column=None,
                     heap=heap[:size], starts=starts, lengths=lengths, null_bytemap=null_bytemap)
+
+
+class JoinTable:
+    """A built join table (ytgpu_join_table); see GpuContext.join_table.  close() or a with block destroys it."""
+
+    def __init__(self, ctx: GpuContext, foreign_keys, nulls: int):
+        self.ctx, self.handle = ctx, None
+        views = [c.view() for c in foreign_keys]
+        arr = (capi.ColumnView * max(len(views), 1))(*views)
+        h = C.c_void_p()
+        err = capi.Error()
+        capi.check(ctx.lib.ytgpu_join_table_build(ctx.handle, C.cast(arr, C.c_void_p), len(views), nulls, C.byref(h), C.byref(err)), err)
+        self.handle = h
+        if not hasattr(ctx, "_join_tables"):
+            ctx._join_tables = weakref.WeakSet()
+        ctx._join_tables.add(self)
+
+    def probe(self, primary_keys, kind: int = capi.JOIN_INNER, count_only: bool = False, capacity: int | None = None,
+              out_mem: int | None = None):
+        """ytgpu_join_table_probe with primary_keys (a list of Column).  INNER / LEFT -> (primary rows, foreign rows) as
+        GpuContext.hash_join returns them; SEMI / ANTI -> the ascending primary rows (uint32; int32 tensors in DEVICE
+        memory); with count_only, the count.  The outputs are in out_mem (default: the primary keys' memory).  Without a
+        capacity, SEMI / ANTI size the output for every primary row and INNER / LEFT run a count query first; a capacity
+        below the count raises YtGpuError with .pair_count set."""
+        if self.handle is None:
+            raise ValueError("the join table is closed")
+        views = [c.view() for c in primary_keys]
+        if out_mem is None:
+            out_mem = views[0].mem if views else capi.MEM_HOST
+        arr = (capi.ColumnView * max(len(views), 1))(*views)
+        rows_only = kind in (capi.JOIN_SEMI, capi.JOIN_ANTI)
+        count = C.c_uint64(0)
+        err = capi.Error()
+
+        def call(prim=None, fore=None, cap=0):
+            code = self.ctx.lib.ytgpu_join_table_probe(self.ctx.handle, self.handle, C.cast(arr, C.c_void_p), len(views), kind,
+                                                       _ptr_mem(prim)[0], _ptr_mem(fore)[0], cap, C.byref(count), out_mem, C.byref(err))
+            if code != capi.OK:
+                e = capi.YtGpuError(code, err.message.decode(errors="replace"), err.cuda_error)
+                e.pair_count = int(count.value)
+                raise e
+        if count_only:
+            call()
+            return int(count.value)
+        if capacity is None:
+            if rows_only:
+                capacity = views[0].value_count if views else 0
+            else:
+                call()
+                capacity = int(count.value)
+        prim = self.ctx._out((max(capacity, 1),), np.uint32, out_mem)
+        if rows_only:
+            call(prim, None, capacity)
+            return prim[:int(count.value)]
+        fore = self.ctx._out((max(capacity, 1),), np.uint32, out_mem)
+        call(prim, fore, capacity)
+        pairs = int(count.value)
+        return prim[:pairs], fore[:pairs]
+
+    def close(self):
+        if self.handle is not None:
+            if getattr(self.ctx, "handle", None):
+                err = capi.Error()
+                capi.check(self.ctx.lib.ytgpu_join_table_destroy(self.handle, C.byref(err)), err)
+            self.handle = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 class Column:
