@@ -101,10 +101,25 @@ __device__ __forceinline__ bool same_string(const Input& in, u64 a, u64 b) {
     return true;
 }
 
+// Every segment has its own table: a power of two >= 2 x the segment's rows, at least 8 slots.  table_at[s] <- its slot
+// count, and table_at[nseg] <- 0 so that the exclusive scan turns table_at into the first slots plus the total.  Sizing by
+// the segment's own rows keeps a column cut into many short segments by the buffer rule as small as its rows.
+__global__ void __launch_bounds__(256) table_sizes_kernel(const u64* __restrict__ seg_start, u32 nseg, u64* __restrict__ table_at) {
+    for (u32 s = blockIdx.x * blockDim.x + threadIdx.x; s <= nseg; s += gridDim.x * blockDim.x) {
+        u64 cap = 0;
+        if (s < nseg) {
+            const u64 rows = seg_start[s + 1] - seg_start[s];
+            cap = 8;
+            while (cap < 2 * rows) cap <<= 1;
+        }
+        table_at[s] = cap;
+    }
+}
+
 // 1. insert: slot word = (fingerprint << 32) | row index inside the segment.
 __global__ void __launch_bounds__(256) insert_kernel(const Input in, const u64* __restrict__ seg_start, const u32* __restrict__ seg_of_row,
-                                                     u64* table, u32 cap, u32* __restrict__ slot_of_row, u32* __restrict__ max_len) {
-    const u32 mask = cap - 1;
+                                                     u64* table, const u64* __restrict__ table_at, u32* __restrict__ slot_of_row,
+                                                     u32* __restrict__ max_len) {
     const u64 lo = (u64)blockIdx.x * kRowsPerBlock, hi = min(in.n, lo + kRowsPerBlock);
     for (u64 g = lo + threadIdx.x; g < hi; g += blockDim.x) {
         u32 found = kNone;
@@ -119,7 +134,8 @@ __global__ void __launch_bounds__(256) insert_kernel(const Input in, const u64* 
             const u64 mx = mix64(hsh);
             const u32 fp = (u32)(mx >> 32);
             const u64 want = ((u64)fp << 32) | (u64)i;
-            u64* slots = table + (u64)s * cap;
+            u64* slots = table + table_at[s];
+            const u32 mask = (u32)(table_at[s + 1] - table_at[s]) - 1;
             u32 h = (u32)mx & mask;
             for (;;) {
                 u64 cur = *reinterpret_cast<volatile u64*>(slots + h);
@@ -142,7 +158,8 @@ __global__ void __launch_bounds__(256) insert_kernel(const Input in, const u64* 
 
 // 2. flags.  counts: low 32 bits = first occurrence, high 32 = run start.
 __global__ void __launch_bounds__(256) flags_kernel(const Input in, const u64* __restrict__ seg_start, const u32* __restrict__ seg_of_row,
-                                                    const u64* __restrict__ table, u32 cap, const u32* __restrict__ slot_of_row,
+                                                    const u64* __restrict__ table, const u64* __restrict__ table_at,
+                                                    const u32* __restrict__ slot_of_row,
                                                     u32* __restrict__ first_of, u64* __restrict__ counts, u64* __restrict__ dict_bytes,
                                                     u64* __restrict__ run_bytes) {
     const u64 lo = (u64)blockIdx.x * kRowsPerBlock, hi = min(in.n + 1, lo + kRowsPerBlock);
@@ -162,7 +179,7 @@ __global__ void __launch_bounds__(256) flags_kernel(const Input in, const u64* _
             run_start = pnl != nl || (!nl && slot_of_row[g - 1] != slot);
         }
         u32 f = kNone;
-        if (!nl) f = (u32)table[(u64)s * cap + slot];  // the slot's row converged to the first row of the value
+        if (!nl) f = (u32)table[table_at[s] + slot];  // the slot's row converged to the first row of the value
         first_of[g] = f;
         const u64 len = nl ? 0 : in.lengths[g];
         counts[g] = ((u64)run_start << 32) | (u64)(f == i);
@@ -541,9 +558,17 @@ Status encode_string_impl(Context* ctx, const u8* heap, u64 heap_bytes, const u6
     *out_seg_count = nseg;
 
     // 1.-3.
-    const u64 seg_rows = std::min<u64>(max_values, n);
-    u32 cap = 8;
-    while ((u64)cap < 2 * seg_rows) cap <<= 1;
+    DevBuf<u64> table_at;
+    YTGPU_TRY(table_at.allocate(ctx, (u64)nseg + 1));
+    {
+        KernelTimer t(ctx, KC_DECODE, 4);
+        table_sizes_kernel<<<grid_for((u64)nseg + 1, 256, 4), 256, 0, ctx->stream>>>(seg_start.p, nseg, table_at.p);
+        exclusive_scan_u64(ctx->stream, table_at.p, (u64)nseg + 1, sums.p, totals.p + 1);
+        YTGPU_CUDA_TRY(cudaGetLastError());
+    }
+    u64 table_slots = 0;
+    YTGPU_CUDA_TRY(cudaMemcpyAsync(&table_slots, totals.p + 1, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     DevBuf<u32> seg_of_row, slot_of_row, first_of, dict_row, run_row, max_len;
     DevBuf<u64> table, counts, D, Q;
     DevBuf<SegWork> work;
@@ -554,22 +579,22 @@ Status encode_string_impl(Context* ctx, const u8* heap, u64 heap_bytes, const u6
     YTGPU_TRY(dict_row.allocate(ctx, n));
     YTGPU_TRY(run_row.allocate(ctx, n));
     YTGPU_TRY(max_len.allocate(ctx, nseg));
-    YTGPU_TRY(table.allocate(ctx, (u64)nseg * cap));
+    YTGPU_TRY(table.allocate(ctx, table_slots));
     YTGPU_TRY(counts.allocate(ctx, n + 1));
     YTGPU_TRY(D.allocate(ctx, n + 1));
     YTGPU_TRY(Q.allocate(ctx, n + 1));
     YTGPU_TRY(work.allocate(ctx, nseg));
     YTGPU_TRY(segs.allocate(ctx, nseg));
-    YTGPU_CUDA_TRY(cudaMemsetAsync(table.p, 0xff, (u64)nseg * cap * 8, ctx->stream));
+    YTGPU_CUDA_TRY(cudaMemsetAsync(table.p, 0xff, table_slots * 8, ctx->stream));
     YTGPU_CUDA_TRY(cudaMemsetAsync(max_len.p, 0, (u64)nseg * 4, ctx->stream));
     const Scans S{P.p, counts.p, D.p, Q.p};
     {
         KernelTimer t(ctx, KC_DECODE, 17);
         const u32 row_blocks = (u32)((n + kRowsPerBlock - 1) / kRowsPerBlock);
         segment_of_row_kernel<<<grid_for(n, 256, 8), 256, 0, ctx->stream>>>(seg_start.p, nseg, n, seg_of_row.p);
-        insert_kernel<<<row_blocks, 256, 0, ctx->stream>>>(in, seg_start.p, seg_of_row.p, table.p, cap, slot_of_row.p, max_len.p);
-        flags_kernel<<<(u32)((n + kRowsPerBlock) / kRowsPerBlock), 256, 0, ctx->stream>>>(in, seg_start.p, seg_of_row.p, table.p, cap, slot_of_row.p,
-                                                                                         first_of.p, counts.p, D.p, Q.p);
+        insert_kernel<<<row_blocks, 256, 0, ctx->stream>>>(in, seg_start.p, seg_of_row.p, table.p, table_at.p, slot_of_row.p, max_len.p);
+        flags_kernel<<<(u32)((n + kRowsPerBlock) / kRowsPerBlock), 256, 0, ctx->stream>>>(in, seg_start.p, seg_of_row.p, table.p, table_at.p,
+                                                                                         slot_of_row.p, first_of.p, counts.p, D.p, Q.p);
         exclusive_scan_u64(ctx->stream, counts.p, n + 1, sums.p, totals.p + 1);
         exclusive_scan_u64(ctx->stream, D.p, n + 1, sums.p, totals.p + 1);
         exclusive_scan_u64(ctx->stream, Q.p, n + 1, sums.p, totals.p + 1);
@@ -656,15 +681,15 @@ Status string_value_ids_impl(Context* ctx, const u8* heap, u64 heap_bytes, const
     DevBuf<u64> table, seg_start;
     DevBuf<u32> seg_of_row, slot_of_row, max_len;
     YTGPU_TRY(table.allocate(ctx, cap));
-    YTGPU_TRY(seg_start.allocate(ctx, 2));
+    YTGPU_TRY(seg_start.allocate(ctx, 4));  // the segment's rows [0, n), then its table's slots [0, cap)
     YTGPU_TRY(seg_of_row.allocate(ctx, n));
     YTGPU_TRY(slot_of_row.allocate(ctx, n));
     YTGPU_TRY(max_len.allocate(ctx, 1));
     YTGPU_CUDA_TRY(cudaMemsetAsync(table.p, 0xff, (u64)cap * 8, ctx->stream));
     YTGPU_CUDA_TRY(cudaMemsetAsync(seg_of_row.p, 0, n * 4, ctx->stream));  // one segment: every row belongs to segment 0
     YTGPU_CUDA_TRY(cudaMemsetAsync(max_len.p, 0, 4, ctx->stream));
-    const u64 bounds[2] = {0, n};
-    YTGPU_CUDA_TRY(cudaMemcpyAsync(seg_start.p, bounds, 16, cudaMemcpyHostToDevice, ctx->stream));
+    const u64 bounds[4] = {0, n, 0, cap};
+    YTGPU_CUDA_TRY(cudaMemcpyAsync(seg_start.p, bounds, 32, cudaMemcpyHostToDevice, ctx->stream));
     u64* dids = out_ids;
     u8* dnull = out_null;
     if (mem == YTGPU_MEM_HOST) {
@@ -677,7 +702,7 @@ Status string_value_ids_impl(Context* ctx, const u8* heap, u64 heap_bytes, const
     }
     {
         KernelTimer t(ctx, KC_GROUPBY, 2);
-        insert_kernel<<<(u32)((n + kRowsPerBlock - 1) / kRowsPerBlock), 256, 0, ctx->stream>>>(in, seg_start.p, seg_of_row.p, table.p, cap,
+        insert_kernel<<<(u32)((n + kRowsPerBlock - 1) / kRowsPerBlock), 256, 0, ctx->stream>>>(in, seg_start.p, seg_of_row.p, table.p, seg_start.p + 2,
                                                                                              slot_of_row.p, max_len.p);
         value_ids_kernel<<<grid_for(n, 256, 8), 256, 0, ctx->stream>>>(in, table.p, cap, slot_of_row.p, dids, dnull);
         YTGPU_CUDA_TRY(cudaGetLastError());
