@@ -19,9 +19,21 @@ around the calls, after warm-up.  Legs (N = 10^8 primary rows by default):
                  measured time, a lower bound on the bandwidth share, not a roofline.
   star           the star leg of bench_join.py (N primary keys U[0, 10^6) against a shuffled 0 .. 10^6 - 1, INNER) as one
                  ytgpu_hash_join call against ytgpu_join_table_build + one ytgpu_join_table_probe, both with capacity N
+String legs (ytgpu_join_table_build_strings / _probe_strings; --strings 0 leaves them out).  A key k of the legs above
+becomes the 24 bytes "key-" + k in 20 zero-padded decimal digits, each row its own bytes in one device heap:
+  build_string   the 10^6 foreign keys of build as strings: the median build time
+  probe_string_<kind>_<block>  the N primary keys as strings, INNER and SEMI in blocks of 2^20 and 2^24 rows, as the probe
+                 legs; floor_bytes: the int64 leg's floor plus, per row, the 24 string bytes, 12 B of start and length, and
+                 the 8 B id written and read again
+  probe_url_inner_16777216  INNER in blocks of 2^24 rows over keys of 20-120 bytes: key k is its 20-digit rendering
+                 followed by filler up to a length of 20 + (k * 2654435761 mod 101) bytes; every row points at its key's
+                 bytes in one heap of the 2 * 10^6 possible keys
+  star_string    the star leg with its keys as strings: ytgpu_string_value_ids over foreign + primary and ytgpu_hash_join
+                 over the ids (joint_ids) against the string table built and probed once (build_probe)
 Parity: each probe kind's first 2^24-row block against numpy on a seeded sample of 10^5 rows (membership of the row's key
 in the foreign keys, and the foreign row of each INNER pair), and star's two ways against each other (every pair) and
-against numpy on the sample.  One JSON line on stdout with the card's name and power limit; nothing is written to the
+against numpy on the sample.  Each string probe leg's first block equals the int64 probe of the same keys (every row and
+pair), and star_string's two ways give star's pairs.  One JSON line on stdout with the card's name and power limit; nothing is written to the
 source tree.
 """
 from __future__ import annotations
@@ -57,11 +69,150 @@ def device_info():
     return torch.cuda.get_device_properties(0).name, power
 
 
+def render24(keys):
+    """Non-negative int64 keys (a CUDA tensor) -> (heap, starts, lengths): row i is b"key-" + keys[i] in 20 decimal digits."""
+    import torch
+    n = keys.numel()
+    heap = torch.empty((n, 24), dtype=torch.uint8, device="cuda")
+    heap[:, :4] = torch.tensor(list(b"key-"), dtype=torch.uint8, device="cuda")
+    pow10 = torch.tensor([10 ** (18 - i) for i in range(19)], dtype=torch.int64, device="cuda")
+    for s in range(0, n, 1 << 24):  # the digits in chunks: (rows, 20) int64 temporaries
+        k = keys[s:s + (1 << 24)]
+        heap[s:s + k.numel(), 4] = 48  # keys < 10^19
+        heap[s:s + k.numel(), 5:] = ((k[:, None] // pow10) % 10 + 48).to(torch.uint8)
+    starts = torch.arange(n, device="cuda", dtype=torch.int64) * 24
+    return heap.reshape(-1), starts, torch.full((n,), 24, dtype=torch.int32, device="cuda")
+
+
+def time_blocks(fn, blocks, steps, warmup):
+    """fn(start, rows) over every block, warmup + steps times -> (median ms of a whole block, the first call's outputs)."""
+    import torch
+    per_block, first = [], None
+    for i in range(warmup + steps):
+        spans = []
+        for s, n in blocks:
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            out = fn(s, n)
+            b.record()
+            spans.append((a, b, n))
+            if i == 0 and s == 0:
+                first = out
+        torch.cuda.synchronize()
+        if i >= warmup:
+            per_block += [a.elapsed_time(b) for a, b, n in spans if n == blocks[0][1]]
+    return statistics.median(per_block), first
+
+
+def string_legs(ctx, args, line, parity, fkeys, pkeys, itable):
+    import torch
+
+    from ytsaurus_b200 import Column, capi
+    from ytsaurus_b200.rowset import EValueType as T
+    N, D = pkeys.numel(), fkeys.numel()
+    fstr = render24(fkeys) + (None,)
+    times = []
+    for i in range(args.warmup + args.steps):
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        t = ctx.join_table([], capi.JOIN_NULLS_NEVER_MATCH, string_keys=[fstr])
+        b.record()
+        b.synchronize()
+        if i >= args.warmup:
+            times.append(a.elapsed_time(b))
+        t.close()
+    ms = statistics.median(times)
+    line["legs"]["build_string"] = {"foreign_rows": D, "key_bytes": 24, "median_ms": round(ms, 3), "rows_per_s": D / (ms / 1e3),
+                                    "floor_bytes": D * (2 * (24 + 12) + 16)}
+    heap, starts, lengths = render24(pkeys)
+    stable = ctx.join_table([], capi.JOIN_NULLS_NEVER_MATCH, string_keys=[fstr])
+    kinds = {"inner": capi.JOIN_INNER, "semi": capi.JOIN_SEMI}
+    for kname, kind in kinds.items():
+        for B in (1 << 20, 1 << 24):
+            blocks = [(s, min(B, N - s)) for s in range(0, N, B)]
+            ms, first = time_blocks(lambda s, n: stable.probe([], kind, capacity=n, out_mem=capi.MEM_DEVICE,
+                                                               string_keys=[(heap, starts[s:s + n], lengths[s:s + n], None)]),
+                                    blocks, args.steps, args.warmup)
+            n0 = blocks[0][1]
+            want = itable.probe([Column(T.Int64, values=pkeys[:n0].contiguous())], kind, capacity=n0, out_mem=capi.MEM_DEVICE)
+            same = all(torch.equal(x, y) for x, y in zip(first, want)) if kind == capi.JOIN_INNER else torch.equal(first, want)
+            parity.append(bool(same))
+            listed = (first[0] if kind == capi.JOIN_INNER else first).numel()
+            per_row = 8 + (12 + 16 + 12 if kind == capi.JOIN_INNER else 8 + 16 + 8) + 24 + 12 + 16
+            floor = per_row * n0 + (8 if kind == capi.JOIN_INNER else 4) * listed
+            line["legs"][f"probe_string_{kname}_{B}"] = {"block_rows": B, "blocks": len(blocks), "median_block_ms": round(ms, 4),
+                                                         "rows_per_s": B / (ms / 1e3), "floor_bytes": floor,
+                                                         "floor_fraction": floor / DATASHEET_HBM_BPS / (ms / 1e3), "same_as_int64": bool(same)}
+    stable.close()
+    del heap, starts, lengths
+    # URL-like keys of 20-120 bytes: one heap row of 120 bytes per possible key, each row pointing at its key's
+    dom = torch.arange(2 * D, device="cuda", dtype=torch.int64)
+    ulen = (20 + (dom * 2654435761) % 101).to(torch.int32)
+    uheap = (97 + (dom[:, None] + torch.arange(120, device="cuda")) % 26).to(torch.uint8)
+    uheap[:, :20] = render24(dom)[0].reshape(-1, 24)[:, 4:]  # the 20 digits first: unique within every key's 20 or more bytes
+    uheap = uheap.reshape(-1)
+    ufor = (uheap, fkeys * 120, ulen[fkeys].contiguous(), None)
+    B = 1 << 24
+    with ctx.join_table([], capi.JOIN_NULLS_NEVER_MATCH, string_keys=[ufor]) as utable:
+        blocks = [(s, min(B, N - s)) for s in range(0, N, B)]
+        ustarts, ulens = pkeys * 120, ulen[pkeys].contiguous()
+        ms, first = time_blocks(lambda s, n: utable.probe([], capi.JOIN_INNER, capacity=n, out_mem=capi.MEM_DEVICE,
+                                                           string_keys=[(uheap, ustarts[s:s + n], ulens[s:s + n], None)]),
+                                blocks, args.steps, args.warmup)
+        n0 = blocks[0][1]
+        want = itable.probe([Column(T.Int64, values=pkeys[:n0].contiguous())], capi.JOIN_INNER, capacity=n0, out_mem=capi.MEM_DEVICE)
+        same = all(torch.equal(x, y) for x, y in zip(first, want))
+        parity.append(bool(same))
+        mean_len = float(ulens[:n0].float().mean())
+        floor = round((8 + 12 + 16 + 12 + mean_len + 12 + 16) * n0 + 8 * first[0].numel())
+        line["legs"][f"probe_url_inner_{B}"] = {"block_rows": B, "blocks": len(blocks), "mean_key_bytes": round(mean_len, 1),
+                                                "median_block_ms": round(ms, 4), "rows_per_s": B / (ms / 1e3), "floor_bytes": floor,
+                                                "floor_fraction": floor / DATASHEET_HBM_BPS / (ms / 1e3), "same_as_int64": bool(same)}
+
+
+def star_string(ctx, args, line, parity, skeys, spk, want):
+    """The star leg over 24-byte string keys: joint value ids + ytgpu_hash_join against the string table built and probed."""
+    import torch
+
+    from ytsaurus_b200 import Column, capi
+    from ytsaurus_b200.rowset import EValueType as T
+    N, D = spk.numel(), skeys.numel()
+    fh, fs, fl = render24(skeys)
+    ph, ps, pl = render24(spk)
+    jh, js, jl = torch.cat([fh, ph]), torch.cat([fs, ps + fh.numel()]), torch.cat([fl, pl])  # foreign + primary, one column
+
+    def joint_ids():
+        ids, _ = ctx.string_value_ids(jh, js, jl)
+        return ctx.hash_join([Column(T.Uint64, values=ids[D:])], [Column(T.Uint64, values=ids[:D])], capi.JOIN_INNER, capacity=N)
+
+    def build_probe():
+        with ctx.join_table([], capi.JOIN_NULLS_EQUAL, string_keys=[(fh, fs, fl, None)]) as t:
+            return t.probe([], capi.JOIN_INNER, capacity=N, string_keys=[(ph, ps, pl, None)])
+    leg = {"primary_rows": N, "foreign_rows": D, "key_bytes": 24}
+    for name, fn in (("joint_ids", joint_ids), ("build_probe", build_probe)):
+        times = []
+        for i in range(args.warmup + args.steps):
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            out = fn()
+            b.record()
+            b.synchronize()
+            if i >= args.warmup:
+                times.append(a.elapsed_time(b))
+        same = all(torch.equal(x, y) for x, y in zip(out, want))
+        parity.append(bool(same))
+        leg[name + "_median_ms"] = round(statistics.median(times), 3)
+        leg[name + "_same_pairs"] = bool(same)
+        del out
+    line["legs"]["star_string"] = leg
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rows", type=int, default=100_000_000)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=1)
+    ap.add_argument("--strings", type=int, default=1)
     args = ap.parse_args()
     import torch
 
@@ -143,6 +294,8 @@ def main():
                                                   "rows_per_s": B / (ms / 1e3), "listed_rows_per_block": round(listed * B / N),
                                                   "floor_bytes": round(floor),
                                                   "floor_fraction": floor / DATASHEET_HBM_BPS / (ms / 1e3)}
+    if args.strings:
+        string_legs(ctx, args, line, parity, fkeys, pkeys, table)
     table.close()
     del member, where
 
@@ -171,6 +324,8 @@ def main():
                 times.append(a.elapsed_time(b))
         outs[leg] = out
         star[leg + "_median_ms"] = round(statistics.median(times), 3)
+    if args.strings:
+        star_string(ctx, args, line, parity, skeys, spk, outs["one_shot"])
     same = all(torch.equal(x, y) for x, y in zip(outs["one_shot"], outs["build_probe"]))
     where = torch.empty(D, dtype=torch.int64, device="cuda")
     where[skeys] = torch.arange(D, device="cuda")

@@ -465,13 +465,16 @@ std::unique_ptr<IAggregatingSource> CreateGpuAggregatingSource(IColumnarReaderPt
 
 namespace NYql::NMiniKQL {
 
-//! A fixed-width arrow::ArrayData as TArrowBlock hands it to an aggregator (buffers[0] validity, buffers[1] values).
+//! A fixed-width arrow::ArrayData as TArrowBlock hands it to an aggregator (buffers[0] validity, buffers[1] values), or
+//! an Arrow binary / utf8 array (buffers[1] offsets, buffers[2] data): element i is then the bytes [Offsets[Offset + i],
+//! Offsets[Offset + i + 1]) of Values.  That YQL's block String / Utf8 columns use these 32-bit offsets is recalled, not read.
 struct TArrowColumn {
     const void* Values = nullptr;
     const uint8_t* Validity = nullptr;  // LSB bit order, 1 = valid; null = no nulls
     int64_t Offset = 0;
     int64_t Length = 0;
-    uint8_t ValueType = 0;  // YTGPU_TYPE_INT64 / UINT64 / DOUBLE
+    uint8_t ValueType = 0;  // YTGPU_TYPE_INT64 / UINT64 / DOUBLE, or YTGPU_TYPE_STRING with Offsets
+    const int32_t* Offsets = nullptr;  // STRING only: Offset + Length + 1 entries
 };
 
 //! BlockCombineHashed with one key column and the sum / count aggregators (mkql_block_agg.cpp:1234-1400 drives
@@ -500,9 +503,13 @@ std::unique_ptr<IBlockCombineHashed> CreateGpuBlockCombineHashed(uint64_t groupC
 //!   * NULLs follow SQL: a key tuple with a NULL component matches nothing (YTGPU_JOIN_NULLS_NEVER_MATCH), so a NULL left
 //!     key is a Left miss and a LeftOnly row.  Doubles compare by bit pattern (-0.0 is not +0.0, a NaN matches only the
 //!     same NaN bits): what YQL's map join does with such keys is not known here.
-//!   * Key types INT64, UINT64 and DOUBLE; another type throws UNSUPPORTED, a key count or type that differs between the
-//!     blocks throws INVALID_ARGUMENT.  String keys are refused: their ids (ytgpu_string_value_ids) need both sides in one
-//!     call, and the table outlives a call.
+//!   * Key types INT64, UINT64, DOUBLE and STRING.  A STRING key is an Arrow binary / utf8 array with 32-bit Offsets;
+//!     keys compare by their bytes (that YQL's map join compares string keys by bytes is recalled, not read).  The table
+//!     keeps the right side's strings in its own dictionary (ytgpu_join_table_build_strings); a left block passes its bytes
+//!     from Offsets[Offset] on, with starts and lengths made on the host.  A STRING key without Offsets (views, dictionary
+//!     arrays, large_binary) and any other type throw UNSUPPORTED; a key count, a type that differs between the right
+//!     blocks, a position that is a string key in one block and numeric in another, and decreasing offsets throw
+//!     INVALID_ARGUMENT.
 enum class EBlockJoinKind { Inner, Left, LeftSemi, LeftOnly };
 
 struct IBlockMapJoin {

@@ -604,6 +604,7 @@ int ytgpu_scan_filter_groupby_multi_strings(ytgpu_context* ctx, const ytgpu_colu
  * String keys go through ytgpu_string_value_ids: call it ONCE over one string column holding the F foreign values followed
  * by the P primary values.  Then ids[0, F) is the foreign key column and ids[F, F + P) the primary one, both UINT64 with the
  * null bytemap as their NULLs: equal strings on either side get the same first-row id.  The join itself is numeric only.
+ * A join table takes string keys itself (ytgpu_join_table_build_strings, below).
  * Pairs.  INNER: one pair (p, f) for every primary row p and foreign row f with equal key tuples.  LEFT: in addition one pair
  * (p, YTGPU_JOIN_NO_ROW) for every primary row without a match.  The pairs are ordered by ascending primary row, then
  * ascending foreign row, the LEFT pair of an unmatched row at its place: the row-by-row order of JoinOpHelper when the
@@ -679,6 +680,35 @@ int ytgpu_join_table_probe(ytgpu_context* ctx, const ytgpu_join_table* table, co
                            uint32_t key_count, int kind, uint32_t* out_primary_rows, uint32_t* out_foreign_rows,
                            uint64_t capacity, uint64_t* out_count /* host */, int out_mem, ytgpu_error* err);
 int ytgpu_join_table_destroy(ytgpu_join_table* table, ytgpu_error* err);
+
+/* Join tables with string keys.  The key tuple is the key_count numeric keys followed by the string_key_count string keys
+ * (flat string columns, HOST or DEVICE, each with its own heap): 1 .. YTGPU_JOIN_MAX_KEYS components in all, key_count may
+ * be 0.  With string_key_count = 0 these are exactly ytgpu_join_table_build / _probe.  Two string values are equal when
+ * they have the same length and the same bytes: no collation, and "" is not NULL.  Both NULL rules apply per component, as
+ * for numbers.  Pairs, rows, their order, the kinds and the capacity protocol are those of ytgpu_join_table_probe.
+ * Build.  The table owns its string keys: the caller may free or overwrite the foreign heaps, starts, lengths and null
+ * bytemaps once the build returns.  Per string key it keeps a dictionary in device memory: the bytes of the non-NULL
+ * values, compacted; 12 B per foreign row of starts and lengths; and a hash table of a power of two >= 2 x the foreign
+ * rows (at least 8) 8-byte slots, 16 to 32 B per row.  Each foreign value becomes the id of the first foreign row with
+ * its bytes, and the numeric build runs on those ids.
+ * Probe.  primary_keys and primary_string_keys must have the table's numeric key count and types and its string key count.
+ * Each primary string value is looked up in its key's dictionary (FNV-1a + mix64 hash, fingerprint, then length and
+ * bytes); a value no foreign row holds matches nothing.  Key columns without NULLs (string columns without a null
+ * bytemap) keep the probe's fast path.
+ * Errors: as ytgpu_join_table_build / _probe, and INVALID_ARGUMENT for a string count other than the table's, string
+ * columns whose row_count differs from the other keys', a null starts or lengths, a null heap with heap_bytes > 0, a mem
+ * that is neither DEVICE nor HOST, and a non-NULL value whose [start, start + length) leaves its heap (checked on the
+ * device for every value on either side: no byte outside a heap is read).  Row limits are checked from the views
+ * (row_count without numeric keys), before any access.  After such a refusal the context and the table stay usable.
+ * Synchronisations.  Build: one more than ytgpu_join_table_build, which reads the dictionaries' byte totals and the bounds
+ * checks together.  Probe: none more; the bounds checks are read with the count. */
+int ytgpu_join_table_build_strings(ytgpu_context* ctx, const ytgpu_column_view* foreign_keys, uint32_t key_count,
+                                   const ytgpu_string_column* foreign_string_keys, uint32_t string_key_count, int nulls,
+                                   ytgpu_join_table** out, ytgpu_error* err);
+int ytgpu_join_table_probe_strings(ytgpu_context* ctx, const ytgpu_join_table* table, const ytgpu_column_view* primary_keys,
+                                   uint32_t key_count, const ytgpu_string_column* primary_string_keys, uint32_t string_key_count,
+                                   int kind, uint32_t* out_primary_rows, uint32_t* out_foreign_rows, uint64_t capacity,
+                                   uint64_t* out_count /* host */, int out_mem, ytgpu_error* err);
 
 /* Gathers.  ytgpu_gather_column decodes `column` at rows[i] into out_values[i] and bit i of out_null_bitmap, for i < count,
  * in the layout of ytgpu_evaluate_expression: out_values count 64-bit bit patterns (a NULL row holds 0), out_null_bitmap

@@ -122,6 +122,7 @@ EXPORTED_SYMBOLS = [
     "ytgpu_count_total_string_length", "ytgpu_translate_rle_indexes", "ytgpu_context_get_option", "ytgpu_convert_ch_column_to_values", "ytgpu_convert_string_column_to_ch", "ytgpu_decode_column_typed",
     "ytgpu_hash_join", "ytgpu_gather_column", "ytgpu_gather_string_column", "ytgpu_order_rows",
     "ytgpu_join_table_build", "ytgpu_join_table_probe", "ytgpu_join_table_destroy",
+    "ytgpu_join_table_build_strings", "ytgpu_join_table_probe_strings",
 ]
 
 FLAGS_DICTIONARY_ZERO, FLAGS_BITMAP = 0, 1
@@ -388,6 +389,10 @@ def load() -> C.CDLL:
     lib.ytgpu_join_table_probe.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_int, C.c_void_p, C.c_void_p, C.c_uint64,
                                            C.POINTER(C.c_uint64), C.c_int, C.POINTER(Error)]
     lib.ytgpu_join_table_destroy.argtypes = [C.c_void_p, C.POINTER(Error)]
+    lib.ytgpu_join_table_build_strings.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_int,
+                                                   C.POINTER(C.c_void_p), C.POINTER(Error)]
+    lib.ytgpu_join_table_probe_strings.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_int,
+                                                   C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.c_int, C.POINTER(Error)]
     lib.ytgpu_gather_column.argtypes = [C.c_void_p, C.POINTER(ColumnView), C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
                                         C.POINTER(C.c_uint64), C.c_int, C.POINTER(Error)]
     lib.ytgpu_gather_string_column.argtypes = [C.c_void_p, C.POINTER(StringColumn), C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,

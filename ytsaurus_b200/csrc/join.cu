@@ -21,6 +21,10 @@
 //      offsets and walks the rows and their slot lists from there, galloping over rows without pairs.  So a key with 10^6
 //      foreign rows spreads over about 245 CTAs, and a run of r unmatched rows costs a thread about 2 log2(r) loads:
 //      neither serialises on one thread.
+// String key components become UINT64 id columns before step 0 and step 3, and the steps above run on them unchanged.  The
+// build keeps a string dictionary per string key (string_dict.cuh): a compacted copy of the foreign values and the hash
+// table of their first rows.  A foreign value's id is the first foreign row holding its bytes; a primary value's id is what
+// the dictionary lookup finds, or kStringDictMiss, which no foreign id equals.  NULL stays NULL.
 #include <algorithm>
 #include <new>
 #include <vector>
@@ -30,6 +34,7 @@
 #include "key_tuple.cuh"
 #include "radix_sort.cuh"
 #include "scan.cuh"
+#include "string_dict.cuh"
 
 using namespace ytgpu;
 
@@ -302,6 +307,35 @@ Status check_side(const ytgpu_column_view* keys, u32 key_count, const char* side
     return Status{};
 }
 
+// The string keys of one side: one length, which is the numeric keys' when there are any (have_rows: *rows holds it).
+Status check_string_side(const ytgpu_string_column* strings, u32 count, bool have_rows, const char* side, u64 max_rows, u64* rows) {
+    for (u32 s = 0; s < count; ++s) {
+        const ytgpu_string_column& c = strings[s];
+        if (s == 0 && !have_rows) *rows = c.row_count;
+        if (c.row_count != *rows) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "%s string key %u differs in length from the other keys", side, s);
+        if (c.mem != YTGPU_MEM_DEVICE && c.mem != YTGPU_MEM_HOST)
+            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "%s string key %u: mem must be YTGPU_MEM_DEVICE or YTGPU_MEM_HOST", side, s);
+        if ((c.row_count && (!c.starts || !c.lengths)) || (c.heap_bytes && !c.heap))  // an empty heap (all "" / NULL) is never read
+            return make_status(YTGPU_ERR_INVALID_ARGUMENT, "%s string key %u: null heap, starts or lengths", side, s);
+    }
+    if (*rows > max_rows)
+        return make_status(YTGPU_ERR_UNSUPPORTED, "%s side: at most %llu rows (slots and rows are 32-bit)", side, (unsigned long long)max_rows);
+    return Status{};
+}
+
+// A string key's ids as a key column: plain 64-bit values, with a null bitmap only when the strings have NULLs.
+ColumnDev id_column(const u64* ids, const u32* null_bits, u64 n) {
+    ColumnDev c{};
+    c.count = (i64)n;
+    c.values = ids;
+    c.values_count = n;
+    c.bitmap = reinterpret_cast<const u8*>(null_bits);
+    c.bit_width = 64;
+    c.has_values = 1;
+    c.value_type = YTGPU_TYPE_UINT64;
+    return c;
+}
+
 bool known_kind(int kind) {
     return kind == YTGPU_JOIN_INNER || kind == YTGPU_JOIN_LEFT || kind == YTGPU_JOIN_SEMI || kind == YTGPU_JOIN_ANTI;
 }
@@ -310,7 +344,8 @@ bool known_kind(int kind) {
 // context's stream-ordered memory.
 struct JoinTable {
     Context* ctx = nullptr;
-    u32 key_count = 0;
+    u32 key_count = 0;           // the tuple's components: the numeric keys, then string_count string keys
+    u32 string_count = 0;
     u8 types[kMaxGroupKeys] = {};
     int nulls = YTGPU_JOIN_NULLS_EQUAL;
     u64 rows = 0;                // foreign rows
@@ -321,6 +356,7 @@ struct JoinTable {
     KeyTable T;                  // step 1: rep and counts (slot_of_row and first are released after step 2)
     DevBuf<u64> slot_start;      // step 2: exclusive scan of counts
     DevBuf<u32> rows_by_slot;    // step 2: the foreign rows stable-sorted by slot, slot s at [slot_start[s], + counts[s])
+    StringDict dicts[kMaxGroupKeys];  // string key s: dicts[s]
 
     TableKeys dev() const { return TableKeys{keys.p, null_keys ? null_mask.p : nullptr, rows}; }
 };
@@ -397,8 +433,9 @@ Status build_table(Context* ctx, const KeyColumns& KF, bool foreign_direct, u64 
 
 // Steps 3-5 of one probe: the staged primary key columns KP (np >= 1 rows) against table J.  The caller has checked the
 // arguments and written *out_count = 0.
+// read_errors: the device error word is read with the count (the string lookups' bounds checks).
 Status probe_table(Context* ctx, const JoinTable& J, const KeyColumns& KP, bool primary_direct, u64 np, int kind, u32* out_primary,
-                   u32* out_foreign, u64 capacity, u64* out_count, int out_mem) {
+                   u32* out_foreign, u64 capacity, u64* out_count, int out_mem, bool read_errors = false) {
     const TableKeys F = J.dev();
     const u64 mask = J.T.cap - 1;
     const int never_match = J.nulls == YTGPU_JOIN_NULLS_NEVER_MATCH;
@@ -442,7 +479,8 @@ Status probe_table(Context* ctx, const JoinTable& J, const KeyColumns& KP, bool 
         }
         u64 rows = 0;
         YTGPU_CUDA_TRY(cudaMemcpyAsync(&rows, total.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
-        YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+        if (read_errors) YTGPU_TRY(check_device_errors(ctx));  // synchronises
+        else YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
         *out_count = rows;
         if (!out_primary) return Status{};
         if (rows > capacity)
@@ -477,7 +515,8 @@ Status probe_table(Context* ctx, const JoinTable& J, const KeyColumns& KP, bool 
     }
     u64 pairs = 0;
     YTGPU_CUDA_TRY(cudaMemcpyAsync(&pairs, total.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
-    YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    if (read_errors) YTGPU_TRY(check_device_errors(ctx));  // synchronises
+    else YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     *out_count = pairs;
     if (!out_primary) return Status{};
     if (pairs > capacity)
@@ -557,15 +596,18 @@ Status hash_join_impl(Context* ctx, const ytgpu_column_view* primary_keys, const
     return probe_table(ctx, J, KP, primary_direct, np, kind, out_primary, out_foreign, pairs_capacity, out_pair_count, out_mem);
 }
 
-Status join_table_build_impl(Context* ctx, const ytgpu_column_view* foreign_keys, u32 key_count, int nulls, JoinTable** out) {
-    if (!foreign_keys || !out) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null argument");
+Status join_table_build_impl(Context* ctx, const ytgpu_column_view* foreign_keys, u32 key_count, const ytgpu_string_column* strings,
+                             u32 string_count, int nulls, JoinTable** out) {
+    if ((key_count && !foreign_keys) || (string_count && !strings) || !out) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null argument");
     *out = nullptr;
-    if (key_count == 0 || key_count > (u32)YTGPU_JOIN_MAX_KEYS)
+    const u64 total = (u64)key_count + string_count;
+    if (total == 0 || total > (u64)YTGPU_JOIN_MAX_KEYS)
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "key column count must be in [1, %d]", YTGPU_JOIN_MAX_KEYS);
     if (nulls != YTGPU_JOIN_NULLS_EQUAL && nulls != YTGPU_JOIN_NULLS_NEVER_MATCH)
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "unknown NULL rule %d", nulls);
     u64 nf = 0;
-    YTGPU_TRY(check_side(foreign_keys, key_count, "foreign", kMaxForeignRows, &nf));
+    if (key_count) YTGPU_TRY(check_side(foreign_keys, key_count, "foreign", kMaxForeignRows, &nf));
+    YTGPU_TRY(check_string_side(strings, string_count, key_count != 0, "foreign", kMaxForeignRows, &nf));
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
     std::vector<StagedColumn> sf(key_count);
     KeyColumns KF;
@@ -573,8 +615,21 @@ Status join_table_build_impl(Context* ctx, const ytgpu_column_view* foreign_keys
     YTGPU_TRY(stage_keys(ctx, foreign_keys, key_count, &sf, &KF, &foreign_direct));
     JoinTable* J = new (std::nothrow) JoinTable();
     if (!J) return make_status(YTGPU_ERR_OUT_OF_MEMORY, "host allocation failed");
-    Status s = build_table(ctx, KF, foreign_direct, nf, nulls, true, J);
+    // the string keys' ids: read by step 0 only, so they are freed when the build returns
+    DevBuf<u64> ids[kMaxGroupKeys];
+    DevBuf<u32> null_bits[kMaxGroupKeys];
+    Status s = string_dicts_build(ctx, strings, string_count, nf, J->dicts, ids, null_bits);
     if (s.code == YTGPU_OK) {
+        KF.count = (u32)total;
+        for (u32 c = 0; c < string_count; ++c) {
+            KF.col[key_count + c] = id_column(ids[c].p, null_bits[c].p, nf);
+            foreign_direct = foreign_direct && !strings[c].null_bytemap;
+        }
+        s = build_table(ctx, KF, foreign_direct, nf, nulls, true, J);
+    }
+    if (s.code == YTGPU_OK) {
+        J->string_count = string_count;
+        for (u32 c = 0; c < string_count; ++c) J->types[key_count + c] = YTGPU_TYPE_STRING;
         const cudaError_t e = cudaStreamSynchronize(ctx->stream);
         if (e != cudaSuccess) s = cuda_status(e, "cudaStreamSynchronize");
     }
@@ -586,12 +641,17 @@ Status join_table_build_impl(Context* ctx, const ytgpu_column_view* foreign_keys
     return Status{};
 }
 
-Status join_table_probe_impl(Context* ctx, const JoinTable* J, const ytgpu_column_view* primary_keys, u32 key_count, int kind,
-                             u32* out_primary, u32* out_foreign, u64 capacity, u64* out_count, int out_mem) {
-    if (!J || !primary_keys || !out_count) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null argument");
+Status join_table_probe_impl(Context* ctx, const JoinTable* J, const ytgpu_column_view* primary_keys, u32 key_count,
+                             const ytgpu_string_column* strings, u32 string_count, int kind, u32* out_primary, u32* out_foreign, u64 capacity,
+                             u64* out_count, int out_mem) {
+    if (!J || (key_count && !primary_keys) || (string_count && !strings) || !out_count)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null argument");
     if (J->ctx != ctx) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "the table was built on another context");
-    if (key_count != J->key_count)
-        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "%u key columns, the table has %u", key_count, J->key_count);
+    const u32 table_numeric = J->key_count - J->string_count;
+    if (key_count != table_numeric)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "%u key columns, the table has %u", key_count, table_numeric);
+    if (string_count != J->string_count)
+        return make_status(YTGPU_ERR_INVALID_ARGUMENT, "%u string key columns, the table has %u", string_count, J->string_count);
     if (!known_kind(kind)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "unknown join kind %d", kind);
     const bool rows_only = kind == YTGPU_JOIN_SEMI || kind == YTGPU_JOIN_ANTI;
     if (rows_only && out_foreign)
@@ -601,7 +661,8 @@ Status join_table_probe_impl(Context* ctx, const JoinTable* J, const ytgpu_colum
     if (out_mem != YTGPU_MEM_DEVICE && out_mem != YTGPU_MEM_HOST)
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "out_mem must be YTGPU_MEM_DEVICE or YTGPU_MEM_HOST");
     u64 np = 0;
-    YTGPU_TRY(check_side(primary_keys, key_count, "primary", kMaxPrimaryRows, &np));
+    if (key_count) YTGPU_TRY(check_side(primary_keys, key_count, "primary", kMaxPrimaryRows, &np));
+    YTGPU_TRY(check_string_side(strings, string_count, key_count != 0, "primary", kMaxPrimaryRows, &np));
     for (u32 k = 0; k < key_count; ++k)
         if (primary_keys[k].value_type != J->types[k])
             return make_status(YTGPU_ERR_INVALID_ARGUMENT, "key %u: primary type 0x%x differs from the table's type 0x%x (no implicit widening)",
@@ -613,7 +674,17 @@ Status join_table_probe_impl(Context* ctx, const JoinTable* J, const ytgpu_colum
     KeyColumns KP;
     bool primary_direct = false;
     YTGPU_TRY(stage_keys(ctx, primary_keys, key_count, &sp, &KP, &primary_direct));
-    return probe_table(ctx, *J, KP, primary_direct, np, kind, out_primary, out_foreign, capacity, out_count, out_mem);
+    DevBuf<u64> ids[kMaxGroupKeys];
+    DevBuf<u32> null_bits[kMaxGroupKeys];
+    KP.count = key_count + string_count;
+    for (u32 c = 0; c < string_count; ++c) {
+        YTGPU_TRY(ids[c].allocate(ctx, np));
+        if (strings[c].null_bytemap) YTGPU_TRY(null_bits[c].allocate(ctx, (np + 31) / 32));
+        YTGPU_TRY(string_dict_lookup(ctx, J->dicts[c], strings[c], np, ids[c].p, null_bits[c].p));
+        KP.col[key_count + c] = id_column(ids[c].p, null_bits[c].p, np);
+        primary_direct = primary_direct && !strings[c].null_bytemap;
+    }
+    return probe_table(ctx, *J, KP, primary_direct, np, kind, out_primary, out_foreign, capacity, out_count, out_mem, string_count != 0);
 }
 
 // The row indexes of a gather, on the device.
@@ -757,7 +828,7 @@ int ytgpu_join_table_build(ytgpu_context* h, const ytgpu_column_view* foreign_ke
     if (!h) return fill_error(err, make_status(YTGPU_ERR_INVALID_ARGUMENT, "null context"));
     CtxLock lock(h);
     JoinTable* t = nullptr;
-    const int code = fill_error(err, join_table_build_impl(as_context(h), foreign_keys, key_count, nulls, &t));
+    const int code = fill_error(err, join_table_build_impl(as_context(h), foreign_keys, key_count, nullptr, 0, nulls, &t));
     if (out) *out = reinterpret_cast<ytgpu_join_table*>(t);
     return code;
 }
@@ -767,8 +838,31 @@ int ytgpu_join_table_probe(ytgpu_context* h, const ytgpu_join_table* table, cons
                            int out_mem, ytgpu_error* err) {
     if (!h) return fill_error(err, make_status(YTGPU_ERR_INVALID_ARGUMENT, "null context"));
     CtxLock lock(h);
-    return fill_error(err, join_table_probe_impl(as_context(h), reinterpret_cast<const JoinTable*>(table), primary_keys, key_count, kind,
-                                                 out_primary_rows, out_foreign_rows, capacity, out_count, out_mem));
+    return fill_error(err, join_table_probe_impl(as_context(h), reinterpret_cast<const JoinTable*>(table), primary_keys, key_count, nullptr, 0,
+                                                 kind, out_primary_rows, out_foreign_rows, capacity, out_count, out_mem));
+}
+
+int ytgpu_join_table_build_strings(ytgpu_context* h, const ytgpu_column_view* foreign_keys, uint32_t key_count,
+                                   const ytgpu_string_column* foreign_string_keys, uint32_t string_key_count, int nulls,
+                                   ytgpu_join_table** out, ytgpu_error* err) {
+    if (!h) return fill_error(err, make_status(YTGPU_ERR_INVALID_ARGUMENT, "null context"));
+    CtxLock lock(h);
+    JoinTable* t = nullptr;
+    const int code = fill_error(err, join_table_build_impl(as_context(h), foreign_keys, key_count, foreign_string_keys, string_key_count,
+                                                           nulls, &t));
+    if (out) *out = reinterpret_cast<ytgpu_join_table*>(t);
+    return code;
+}
+
+int ytgpu_join_table_probe_strings(ytgpu_context* h, const ytgpu_join_table* table, const ytgpu_column_view* primary_keys,
+                                   uint32_t key_count, const ytgpu_string_column* primary_string_keys, uint32_t string_key_count,
+                                   int kind, uint32_t* out_primary_rows, uint32_t* out_foreign_rows, uint64_t capacity,
+                                   uint64_t* out_count, int out_mem, ytgpu_error* err) {
+    if (!h) return fill_error(err, make_status(YTGPU_ERR_INVALID_ARGUMENT, "null context"));
+    CtxLock lock(h);
+    return fill_error(err, join_table_probe_impl(as_context(h), reinterpret_cast<const JoinTable*>(table), primary_keys, key_count,
+                                                 primary_string_keys, string_key_count, kind, out_primary_rows, out_foreign_rows, capacity,
+                                                 out_count, out_mem));
 }
 
 int ytgpu_join_table_destroy(ytgpu_join_table* table, ytgpu_error* err) {

@@ -18,11 +18,15 @@
 //               more pass over the rows finds the largest zig-zag difference (the bit width of the offsets); then part
 //               sizes and data offsets (segments are laid out 8-byte aligned);
 //   4. pack   : one thread per OUTPUT word of the bit-packed vectors / bitmaps; string bytes are copied by whole warps.
+//
+// The same insert, over a whole column as one segment, gives ytgpu_string_value_ids and the string dictionary of
+// string_dict.cuh, which keeps its table and looks other strings up in it with the same hash and slot words.
 #include <algorithm>
 #include <vector>
 
 #include "context.cuh"
 #include "scan.cuh"
+#include "string_dict.cuh"
 
 using namespace ytgpu;
 
@@ -91,15 +95,28 @@ __global__ void __launch_bounds__(256) segment_of_row_kernel(const u64* __restri
     }
 }
 
-__device__ __forceinline__ bool same_string(const Input& in, u64 a, u64 b) {
-    const u32 len = in.lengths[a];
-    if (in.lengths[b] != len) return false;
-    const u8* pa = in.heap + in.starts[a];
-    const u8* pb = in.heap + in.starts[b];
+__device__ __forceinline__ bool same_bytes(const u8* pa, const u8* pb, u32 len) {
     for (u32 i = 0; i < len; ++i)
         if (pa[i] != pb[i]) return false;
     return true;
 }
+
+__device__ __forceinline__ bool same_string(const Input& in, u64 a, u64 b) {
+    const u32 len = in.lengths[a];
+    if (in.lengths[b] != len) return false;
+    return same_bytes(in.heap + in.starts[a], in.heap + in.starts[b], len);
+}
+
+// The hash of a value's bytes: FNV-1a seeded with the length, then mix64.  Its top 32 bits are the value's fingerprint, its
+// low bits under a table's mask the value's first slot.  The insert and the dictionary lookup both hash through here.
+__device__ __forceinline__ u64 string_hash(const u8* p, u32 len) {
+    u64 hsh = 0xcbf29ce484222325ull ^ len;
+    for (u32 k = 0; k < len; ++k) hsh = (hsh ^ p[k]) * 0x100000001b3ull;
+    return mix64(hsh);
+}
+
+// A slot word: the fingerprint, and the row (inside its segment) of the value the slot holds.
+__device__ __forceinline__ u64 slot_word(u32 fp, u32 row) { return ((u64)fp << 32) | (u64)row; }
 
 // Every segment has its own table: a power of two >= 2 x the segment's rows, at least 8 slots.  table_at[s] <- its slot
 // count, and table_at[nseg] <- 0 so that the exclusive scan turns table_at into the first slots plus the total.  Sizing by
@@ -128,12 +145,9 @@ __global__ void __launch_bounds__(256) insert_kernel(const Input in, const u64* 
             const u64 begin = seg_start[s];
             const u32 i = (u32)(g - begin);
             const u32 len = in.lengths[g];
-            const u8* p = in.heap + in.starts[g];
-            u64 hsh = 0xcbf29ce484222325ull ^ len;
-            for (u32 k = 0; k < len; ++k) hsh = (hsh ^ p[k]) * 0x100000001b3ull;
-            const u64 mx = mix64(hsh);
+            const u64 mx = string_hash(in.heap + in.starts[g], len);
             const u32 fp = (u32)(mx >> 32);
-            const u64 want = ((u64)fp << 32) | (u64)i;
+            const u64 want = slot_word(fp, i);
             u64* slots = table + table_at[s];
             const u32 mask = (u32)(table_at[s + 1] - table_at[s]) - 1;
             u32 h = (u32)mx & mask;
@@ -650,44 +664,75 @@ __global__ void __launch_bounds__(256) value_ids_kernel(const Input in, const u6
     }
 }
 
+// A string column on the device: HOST columns are uploaded.
+struct StagedInput {
+    Input in{};
+    u64 heap_bytes = 0;
+    DevBuf<u8> heap, nulls;
+    DevBuf<u64> starts;
+    DevBuf<u32> lengths;
+};
+
+Status stage_input(Context* ctx, const u8* heap, u64 heap_bytes, const u64* starts, const u32* lengths, const u8* null_bytemap, u64 n,
+                   int mem, StagedInput* s) {
+    s->in = Input{heap, starts, lengths, null_bytemap, n};
+    s->heap_bytes = heap_bytes;
+    if (mem != YTGPU_MEM_HOST) return Status{};
+    YTGPU_TRY(s->heap.allocate(ctx, heap_bytes));
+    YTGPU_TRY(copy_in(ctx, s->heap.p, heap, heap_bytes, YTGPU_MEM_HOST));
+    YTGPU_TRY(s->starts.allocate(ctx, n));
+    YTGPU_TRY(copy_in(ctx, s->starts.p, starts, n * 8, YTGPU_MEM_HOST));
+    YTGPU_TRY(s->lengths.allocate(ctx, n));
+    YTGPU_TRY(copy_in(ctx, s->lengths.p, lengths, n * 4, YTGPU_MEM_HOST));
+    s->in.heap = s->heap.p;
+    s->in.starts = s->starts.p;
+    s->in.lengths = s->lengths.p;
+    if (null_bytemap) {
+        YTGPU_TRY(s->nulls.allocate(ctx, n));
+        YTGPU_TRY(copy_in(ctx, s->nulls.p, null_bytemap, n, YTGPU_MEM_HOST));
+        s->in.nulls = s->nulls.p;
+    }
+    return Status{};
+}
+
+u64 value_table_slots(u64 n) {
+    u64 cap = 8;
+    while (cap < 2 * n) cap <<= 1;
+    return cap;
+}
+
+// The insert over the n rows of `in` as one segment, then the ids.  bounds (device, 4 words) = {0, n, 0, cap}: the
+// segment's rows, then its table's slots.  table (cap words) is left as the insert leaves it.
+Status insert_value_ids(Context* ctx, int timer_class, const Input& in, const u64* bounds, u64* table, u64 cap, u64* out_ids, u8* out_null) {
+    const u64 n = in.n;
+    DevBuf<u32> seg_of_row, slot_of_row, max_len;
+    YTGPU_TRY(seg_of_row.allocate(ctx, n));
+    YTGPU_TRY(slot_of_row.allocate(ctx, n));
+    YTGPU_TRY(max_len.allocate(ctx, 1));
+    YTGPU_CUDA_TRY(cudaMemsetAsync(table, 0xff, cap * 8, ctx->stream));
+    YTGPU_CUDA_TRY(cudaMemsetAsync(seg_of_row.p, 0, n * 4, ctx->stream));  // one segment: every row belongs to segment 0
+    YTGPU_CUDA_TRY(cudaMemsetAsync(max_len.p, 0, 4, ctx->stream));
+    KernelTimer t(ctx, timer_class, 2);
+    insert_kernel<<<(u32)((n + kRowsPerBlock - 1) / kRowsPerBlock), 256, 0, ctx->stream>>>(in, bounds, seg_of_row.p, table, bounds + 2,
+                                                                                         slot_of_row.p, max_len.p);
+    value_ids_kernel<<<grid_for(n, 256, 8), 256, 0, ctx->stream>>>(in, table, (u32)cap, slot_of_row.p, out_ids, out_null);
+    YTGPU_CUDA_TRY(cudaGetLastError());
+    return Status{};
+}
+
 Status string_value_ids_impl(Context* ctx, const u8* heap, u64 heap_bytes, const u64* starts, const u32* lengths, const u8* null_bytemap, u64 n,
                              u64* out_ids, u8* out_null, int mem) {
     if (n == 0) return Status{};
     if (!starts || !lengths || !out_ids || (heap_bytes && !heap)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null argument");
     if (n > (1ull << 30)) return make_status(YTGPU_ERR_UNSUPPORTED, "at most 2^30 rows per call");
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
-    DevBuf<u8> hstage, nstage, onull;
-    DevBuf<u64> sstage, oids;
-    DevBuf<u32> lstage;
-    Input in{heap, starts, lengths, null_bytemap, n};
-    if (mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(hstage.allocate(ctx, heap_bytes));
-        YTGPU_TRY(copy_in(ctx, hstage.p, heap, heap_bytes, YTGPU_MEM_HOST));
-        YTGPU_TRY(sstage.allocate(ctx, n));
-        YTGPU_TRY(copy_in(ctx, sstage.p, starts, n * 8, YTGPU_MEM_HOST));
-        YTGPU_TRY(lstage.allocate(ctx, n));
-        YTGPU_TRY(copy_in(ctx, lstage.p, lengths, n * 4, YTGPU_MEM_HOST));
-        in.heap = hstage.p;
-        in.starts = sstage.p;
-        in.lengths = lstage.p;
-        if (null_bytemap) {
-            YTGPU_TRY(nstage.allocate(ctx, n));
-            YTGPU_TRY(copy_in(ctx, nstage.p, null_bytemap, n, YTGPU_MEM_HOST));
-            in.nulls = nstage.p;
-        }
-    }
-    u32 cap = 8;
-    while ((u64)cap < 2 * n) cap <<= 1;
-    DevBuf<u64> table, seg_start;
-    DevBuf<u32> seg_of_row, slot_of_row, max_len;
+    StagedInput staged;
+    YTGPU_TRY(stage_input(ctx, heap, heap_bytes, starts, lengths, null_bytemap, n, mem, &staged));
+    const u64 cap = value_table_slots(n);
+    DevBuf<u8> onull;
+    DevBuf<u64> table, seg_start, oids;
     YTGPU_TRY(table.allocate(ctx, cap));
-    YTGPU_TRY(seg_start.allocate(ctx, 4));  // the segment's rows [0, n), then its table's slots [0, cap)
-    YTGPU_TRY(seg_of_row.allocate(ctx, n));
-    YTGPU_TRY(slot_of_row.allocate(ctx, n));
-    YTGPU_TRY(max_len.allocate(ctx, 1));
-    YTGPU_CUDA_TRY(cudaMemsetAsync(table.p, 0xff, (u64)cap * 8, ctx->stream));
-    YTGPU_CUDA_TRY(cudaMemsetAsync(seg_of_row.p, 0, n * 4, ctx->stream));  // one segment: every row belongs to segment 0
-    YTGPU_CUDA_TRY(cudaMemsetAsync(max_len.p, 0, 4, ctx->stream));
+    YTGPU_TRY(seg_start.allocate(ctx, 4));
     const u64 bounds[4] = {0, n, 0, cap};
     YTGPU_CUDA_TRY(cudaMemcpyAsync(seg_start.p, bounds, 32, cudaMemcpyHostToDevice, ctx->stream));
     u64* dids = out_ids;
@@ -700,13 +745,7 @@ Status string_value_ids_impl(Context* ctx, const u8* heap, u64 heap_bytes, const
             dnull = onull.p;
         }
     }
-    {
-        KernelTimer t(ctx, KC_GROUPBY, 2);
-        insert_kernel<<<(u32)((n + kRowsPerBlock - 1) / kRowsPerBlock), 256, 0, ctx->stream>>>(in, seg_start.p, seg_of_row.p, table.p, seg_start.p + 2,
-                                                                                             slot_of_row.p, max_len.p);
-        value_ids_kernel<<<grid_for(n, 256, 8), 256, 0, ctx->stream>>>(in, table.p, cap, slot_of_row.p, dids, dnull);
-        YTGPU_CUDA_TRY(cudaGetLastError());
-    }
+    YTGPU_TRY(insert_value_ids(ctx, KC_GROUPBY, staged.in, seg_start.p, table.p, cap, dids, dnull));
     if (mem == YTGPU_MEM_HOST) {
         YTGPU_TRY(copy_out(ctx, out_ids, dids, n * 8, YTGPU_MEM_HOST));
         if (out_null) YTGPU_TRY(copy_out(ctx, out_null, dnull, n, YTGPU_MEM_HOST));
@@ -715,7 +754,166 @@ Status string_value_ids_impl(Context* ctx, const u8* heap, u64 heap_bytes, const
     return Status{};
 }
 
+// ---- the string dictionary (string_dict.cuh) ----
+__device__ __forceinline__ bool in_heap(u64 start, u32 len, u64 heap_bytes) { return start <= heap_bytes && len <= heap_bytes - start; }
+
+// Build, step 1: each row's length in the dictionary's heap, at n the 0 that makes the scan's last word the total.  A NULL
+// row and a value outside its heap (which sets the error bit) take no bytes.
+__global__ void __launch_bounds__(256) dict_lengths_kernel(const Input in, u64 heap_bytes, u64* __restrict__ out, u32* err_word) {
+    u32 bad = 0;
+    for (u64 g = (u64)blockIdx.x * blockDim.x + threadIdx.x; g <= in.n; g += (u64)gridDim.x * blockDim.x) {
+        u64 len = 0;
+        if (g < in.n && !is_null(in, g)) {
+            const u32 l = in.lengths[g];
+            if (in_heap(in.starts[g], l, heap_bytes)) len = l;
+            else bad = 1;
+        }
+        out[g] = len;
+    }
+    if (bad) atomicOr(err_word, (u32)DE_STRING_OUT_OF_HEAP);
+}
+
+// Build, step 2, after the scan of step 1 (at[g] = value g's start in the dictionary's heap): each warp takes 32 rows,
+// writes their lengths and null bits, and copies their bytes one value after the other with the whole warp.
+__global__ void __launch_bounds__(256) dict_copy_kernel(const Input in, const u64* __restrict__ at, u8* __restrict__ heap,
+                                                        u32* __restrict__ lengths, u32* __restrict__ null_bits) {
+    const u32 lane = threadIdx.x & 31;
+    const u64 warps = ((u64)gridDim.x * blockDim.x) >> 5;
+    for (u64 base = (u64)blockIdx.x * blockDim.x + threadIdx.x - lane; base < in.n; base += warps * 32) {
+        const u64 g = base + lane;
+        u32 len = 0;
+        if (g < in.n) {
+            len = (u32)(at[g + 1] - at[g]);
+            lengths[g] = len;
+        }
+        if (null_bits) {
+            const u32 m = __ballot_sync(0xffffffffu, g < in.n && is_null(in, g));
+            if (lane == 0) null_bits[base >> 5] = m;
+        }
+        u32 m = __ballot_sync(0xffffffffu, len != 0);
+        while (m) {
+            const int src = __ffs(m) - 1;
+            m &= m - 1;
+            const u64 row = base + src;
+            const u32 l = __shfl_sync(0xffffffffu, len, src);
+            const u8* from = in.heap + in.starts[row];
+            u8* to = heap + at[row];
+            for (u32 k = lane; k < l; k += 32) to[k] = from[k];
+        }
+    }
+}
+
+// The lookup: one thread per row hashes its value as the insert does and walks the kept table from the value's first slot,
+// comparing the fingerprint, then the length and the bytes, until the value's slot or an empty one (the table is at most
+// half full).
+__global__ void __launch_bounds__(256) dict_lookup_kernel(const Input dict, const u64* __restrict__ slots, u32 mask, const Input in,
+                                                          u64 heap_bytes, u64* __restrict__ ids, u32* __restrict__ null_bits, u32* err_word) {
+    const u32 lane = threadIdx.x & 31;
+    u32 bad = 0;
+    for (u64 base = (u64)blockIdx.x * blockDim.x + threadIdx.x - lane; base < in.n; base += (u64)gridDim.x * blockDim.x) {
+        const u64 g = base + lane;
+        const bool nul = g < in.n && is_null(in, g);
+        if (g < in.n) {
+            u64 id = 0;
+            if (!nul) {
+                id = kStringDictMiss;
+                const u64 start = in.starts[g];
+                const u32 len = in.lengths[g];
+                if (!in_heap(start, len, heap_bytes)) {
+                    bad = 1;
+                } else {
+                    const u8* p = in.heap + start;
+                    const u64 mx = string_hash(p, len);
+                    const u32 fp = (u32)(mx >> 32);
+                    u32 h = (u32)mx & mask;
+                    for (;;) {
+                        const u64 w = slots[h];
+                        if (w == kEmptySlot) break;
+                        const u32 row = (u32)w;
+                        if ((u32)(w >> 32) == fp && dict.lengths[row] == len && same_bytes(dict.heap + dict.starts[row], p, len)) {
+                            id = row;
+                            break;
+                        }
+                        h = (h + 1) & mask;
+                    }
+                }
+            }
+            ids[g] = id;
+        }
+        if (null_bits) {
+            const u32 m = __ballot_sync(0xffffffffu, nul);
+            if (lane == 0) null_bits[base >> 5] = m;
+        }
+    }
+    if (bad) atomicOr(err_word, (u32)DE_STRING_OUT_OF_HEAP);
+}
+
 }  // namespace
+
+namespace ytgpu {
+
+Status string_dicts_build(Context* ctx, const ytgpu_string_column* cols, u32 count, u64 n, StringDict* dicts, DevBuf<u64>* ids,
+                          DevBuf<u32>* null_bits) {
+    if (count == 0) return Status{};
+    const u64 cap = value_table_slots(n);
+    for (u32 c = 0; c < count; ++c) YTGPU_TRY(dicts[c].slots.allocate(ctx, cap));
+    if (n == 0) {  // an empty table: every lookup misses
+        for (u32 c = 0; c < count; ++c) YTGPU_CUDA_TRY(cudaMemsetAsync(dicts[c].slots.p, 0xff, cap * 8, ctx->stream));
+        return Status{};
+    }
+    std::vector<StagedInput> staged(count);
+    DevBuf<u64> bounds_dev, sums, totals;
+    YTGPU_TRY(bounds_dev.allocate(ctx, 4));
+    YTGPU_TRY(sums.allocate(ctx, scan_block_count(n + 1)));
+    YTGPU_TRY(totals.allocate(ctx, count));
+    const u64 bounds[4] = {0, n, 0, cap};  // read before the synchronisation below
+    YTGPU_CUDA_TRY(cudaMemcpyAsync(bounds_dev.p, bounds, 32, cudaMemcpyHostToDevice, ctx->stream));
+    for (u32 c = 0; c < count; ++c) {
+        const ytgpu_string_column& s = cols[c];
+        YTGPU_TRY(stage_input(ctx, s.heap, s.heap_bytes, s.starts, s.lengths, s.null_bytemap, n, s.mem, &staged[c]));
+        YTGPU_TRY(dicts[c].starts.allocate(ctx, n + 1));
+        KernelTimer t(ctx, KC_JOIN, 4);
+        dict_lengths_kernel<<<grid_for(n + 1, 256, 8), 256, 0, ctx->stream>>>(staged[c].in, staged[c].heap_bytes, dicts[c].starts.p,
+                                                                              ctx->dev_err);
+        exclusive_scan_u64(ctx->stream, dicts[c].starts.p, n + 1, sums.p, totals.p + c);
+        YTGPU_CUDA_TRY(cudaGetLastError());
+    }
+    std::vector<u64> bytes(count);
+    YTGPU_CUDA_TRY(cudaMemcpyAsync(bytes.data(), totals.p, (size_t)count * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    YTGPU_TRY(check_device_errors(ctx));  // synchronises: the heap sizes and the bounds checks of every column
+    for (u32 c = 0; c < count; ++c) {
+        StringDict& d = dicts[c];
+        YTGPU_TRY(d.heap.allocate(ctx, bytes[c]));
+        YTGPU_TRY(d.lengths.allocate(ctx, n));
+        YTGPU_TRY(ids[c].allocate(ctx, n));
+        u32* bits = nullptr;
+        if (cols[c].null_bytemap) {
+            YTGPU_TRY(null_bits[c].allocate(ctx, (n + 31) / 32));
+            bits = null_bits[c].p;
+        }
+        {
+            KernelTimer t(ctx, KC_JOIN);
+            dict_copy_kernel<<<grid_for(n, 256, 8), 256, 0, ctx->stream>>>(staged[c].in, d.starts.p, d.heap.p, d.lengths.p, bits);
+            YTGPU_CUDA_TRY(cudaGetLastError());
+        }
+        const Input copy{d.heap.p, d.starts.p, d.lengths.p, staged[c].in.nulls, n};
+        YTGPU_TRY(insert_value_ids(ctx, KC_JOIN, copy, bounds_dev.p, d.slots.p, cap, ids[c].p, nullptr));
+    }
+    return Status{};
+}
+
+Status string_dict_lookup(Context* ctx, const StringDict& dict, const ytgpu_string_column& col, u64 n, u64* ids, u32* null_bits) {
+    StagedInput staged;
+    YTGPU_TRY(stage_input(ctx, col.heap, col.heap_bytes, col.starts, col.lengths, col.null_bytemap, n, col.mem, &staged));
+    const Input d{dict.heap.p, dict.starts.p, dict.lengths.p, nullptr, 0};
+    KernelTimer t(ctx, KC_JOIN);
+    dict_lookup_kernel<<<grid_for(n, 256, 16), 256, 0, ctx->stream>>>(d, dict.slots.p, (u32)dict.slots.n - 1, staged.in, staged.heap_bytes, ids,
+                                                                      col.null_bytemap ? null_bits : nullptr, ctx->dev_err);
+    YTGPU_CUDA_TRY(cudaGetLastError());
+    return Status{};
+}
+
+}  // namespace ytgpu
 
 extern "C" {
 

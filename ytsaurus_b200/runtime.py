@@ -62,6 +62,11 @@ def _string_column(heap, starts, lengths, nulls=None) -> capi.StringColumn:
     return capi.StringColumn(hp, len(heap), parts[0][0], parts[1][0], parts[2][0] if nulls is not None else None, n, mem, 0)
 
 
+def _string_columns(columns):
+    """A ytgpu_string_column array over (heap, starts, lengths, nulls or None) tuples."""
+    return (capi.StringColumn * len(columns))(*[_string_column(*c) for c in columns])
+
+
 class GpuContext:
     """One per device/stream; wraps ytgpu_context (explicit, no thread-local state).
 
@@ -835,12 +840,14 @@ class GpuContext:
         pairs = int(count.value)
         return prim[:pairs], fore[:pairs]
 
-    def join_table(self, foreign_keys, nulls: int = capi.JOIN_NULLS_EQUAL) -> "JoinTable":
+    def join_table(self, foreign_keys, nulls: int = capi.JOIN_NULLS_EQUAL, string_keys=()) -> "JoinTable":
         """ytgpu_join_table_build: a join table over foreign_keys (a list of Column), built once and probed any number of
         times (JoinTable.probe).  nulls: capi.JOIN_NULLS_EQUAL (NULL equals NULL, as hash_join) or
-        capi.JOIN_NULLS_NEVER_MATCH (a tuple with a NULL component matches nothing).  The table owns a copy of the keys:
-        the columns may be freed or overwritten once this returns."""
-        return JoinTable(self, foreign_keys, nulls)
+        capi.JOIN_NULLS_NEVER_MATCH (a tuple with a NULL component matches nothing).  string_keys: string key columns as
+        (heap, starts, lengths, nulls or None) tuples, after the numeric keys in the key tuple (ytgpu_join_table_build_strings);
+        foreign_keys may then be empty.  The table owns a copy of the keys: the columns may be freed or overwritten once
+        this returns."""
+        return JoinTable(self, foreign_keys, nulls, string_keys)
 
     def gather_column(self, column: "Column", rows):
         """ytgpu_gather_column: `column` decoded at rows (uint32; capi.JOIN_NO_ROW gives NULL) -> dict(values, null_bitmap,
@@ -1050,38 +1057,50 @@ class GpuContext:
 class JoinTable:
     """A built join table (ytgpu_join_table); see GpuContext.join_table.  close() or a with block destroys it."""
 
-    def __init__(self, ctx: GpuContext, foreign_keys, nulls: int):
+    def __init__(self, ctx: GpuContext, foreign_keys, nulls: int, string_keys=()):
         self.ctx, self.handle = ctx, None
         views = [c.view() for c in foreign_keys]
         arr = (capi.ColumnView * max(len(views), 1))(*views)
         h = C.c_void_p()
         err = capi.Error()
-        capi.check(ctx.lib.ytgpu_join_table_build(ctx.handle, C.cast(arr, C.c_void_p), len(views), nulls, C.byref(h), C.byref(err)), err)
+        if string_keys:
+            sarr = _string_columns(string_keys)
+            capi.check(ctx.lib.ytgpu_join_table_build_strings(ctx.handle, C.cast(arr, C.c_void_p), len(views), C.cast(sarr, C.c_void_p),
+                                                              len(string_keys), nulls, C.byref(h), C.byref(err)), err)
+        else:
+            capi.check(ctx.lib.ytgpu_join_table_build(ctx.handle, C.cast(arr, C.c_void_p), len(views), nulls, C.byref(h), C.byref(err)), err)
         self.handle = h
         if not hasattr(ctx, "_join_tables"):
             ctx._join_tables = weakref.WeakSet()
         ctx._join_tables.add(self)
 
     def probe(self, primary_keys, kind: int = capi.JOIN_INNER, count_only: bool = False, capacity: int | None = None,
-              out_mem: int | None = None):
-        """ytgpu_join_table_probe with primary_keys (a list of Column).  INNER / LEFT -> (primary rows, foreign rows) as
-        GpuContext.hash_join returns them; SEMI / ANTI -> the ascending primary rows (uint32; int32 tensors in DEVICE
-        memory); with count_only, the count.  The outputs are in out_mem (default: the primary keys' memory).  Without a
-        capacity, SEMI / ANTI size the output for every primary row and INNER / LEFT run a count query first; a capacity
-        below the count raises YtGpuError with .pair_count set."""
+              out_mem: int | None = None, string_keys=()):
+        """ytgpu_join_table_probe with primary_keys (a list of Column), and string_keys as GpuContext.join_table takes them
+        (ytgpu_join_table_probe_strings).  INNER / LEFT -> (primary rows, foreign rows) as GpuContext.hash_join returns
+        them; SEMI / ANTI -> the ascending primary rows (uint32; int32 tensors in DEVICE memory); with count_only, the
+        count.  The outputs are in out_mem (default: the primary keys' memory).  Without a capacity, SEMI / ANTI size the
+        output for every primary row and INNER / LEFT run a count query first; a capacity below the count raises
+        YtGpuError with .pair_count set."""
         if self.handle is None:
             raise ValueError("the join table is closed")
         views = [c.view() for c in primary_keys]
+        sarr = _string_columns(string_keys) if string_keys else None
         if out_mem is None:
-            out_mem = views[0].mem if views else capi.MEM_HOST
+            out_mem = views[0].mem if views else (sarr[0].mem if string_keys else capi.MEM_HOST)
         arr = (capi.ColumnView * max(len(views), 1))(*views)
         rows_only = kind in (capi.JOIN_SEMI, capi.JOIN_ANTI)
         count = C.c_uint64(0)
         err = capi.Error()
 
         def call(prim=None, fore=None, cap=0):
-            code = self.ctx.lib.ytgpu_join_table_probe(self.ctx.handle, self.handle, C.cast(arr, C.c_void_p), len(views), kind,
-                                                       _ptr_mem(prim)[0], _ptr_mem(fore)[0], cap, C.byref(count), out_mem, C.byref(err))
+            if string_keys:
+                code = self.ctx.lib.ytgpu_join_table_probe_strings(self.ctx.handle, self.handle, C.cast(arr, C.c_void_p), len(views),
+                                                                   C.cast(sarr, C.c_void_p), len(string_keys), kind, _ptr_mem(prim)[0],
+                                                                   _ptr_mem(fore)[0], cap, C.byref(count), out_mem, C.byref(err))
+            else:
+                code = self.ctx.lib.ytgpu_join_table_probe(self.ctx.handle, self.handle, C.cast(arr, C.c_void_p), len(views), kind,
+                                                           _ptr_mem(prim)[0], _ptr_mem(fore)[0], cap, C.byref(count), out_mem, C.byref(err))
             if code != capi.OK:
                 e = capi.YtGpuError(code, err.message.decode(errors="replace"), err.cuda_error)
                 e.pair_count = int(count.value)
@@ -1091,7 +1110,7 @@ class JoinTable:
             return int(count.value)
         if capacity is None:
             if rows_only:
-                capacity = views[0].value_count if views else 0
+                capacity = views[0].value_count if views else (sarr[0].row_count if string_keys else 0)
             else:
                 call()
                 capacity = int(count.value)
