@@ -236,29 +236,19 @@ Status combine_all_impl(Context* ctx, const ytgpu_arrow_array* col, const u8* fi
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "device values buffer must be 8-byte aligned");
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
 
-    DevBuf<u64> vstage;
-    DevBuf<u8> nstage, fstage;
-    const u64* vals = static_cast<const u64*>(col->values) + offset;
+    InBuf<u64> vals;
+    InBuf<u8> nulls, flt;
     const u8* validity = col->nullable ? col->validity : nullptr;  // IsNullable ? GetNullCount() : 0
-    const u8* flt = filter;
-    u64 bit_offset = offset;
-    if (col->mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(vstage.allocate(ctx, length));
-        YTGPU_TRY(copy_in(ctx, vstage.p, vals, length * 8, YTGPU_MEM_HOST));
-        vals = vstage.p;
-        if (validity) {
-            const u64 first = offset / 8, bytes = (offset + length + 7) / 8 - first;
-            YTGPU_TRY(nstage.allocate(ctx, bytes));
-            YTGPU_TRY(copy_in(ctx, nstage.p, validity + first, bytes, YTGPU_MEM_HOST));
-            validity = nstage.p;
-            bit_offset = offset % 8;
-        }
-        if (filter) {
-            YTGPU_TRY(fstage.allocate(ctx, length));
-            YTGPU_TRY(copy_in(ctx, fstage.p, filter, length, YTGPU_MEM_HOST));
-            flt = fstage.p;
-        }
+    u64 bit_offset = offset, validity_bytes = 0;
+    if (validity && col->mem == YTGPU_MEM_HOST) {  // upload only the bytes that cover the rows
+        const u64 first = offset / 8;
+        validity += first;
+        validity_bytes = (offset + length + 7) / 8 - first;
+        bit_offset = offset % 8;
     }
+    YTGPU_TRY(vals.stage(ctx, static_cast<const u64*>(col->values) + offset, length, col->mem));
+    YTGPU_TRY(nulls.stage(ctx, validity, validity_bytes, col->mem));
+    YTGPU_TRY(flt.stage(ctx, filter, length, col->mem));
     const u64 groups = (length + kGroup - 1) / kGroup;
     const u32 grid = (u32)std::max<u64>(1, std::min<u64>((groups + kThreads - 1) / kThreads, (u64)kNumSms * 8));
     DevBuf<Partial> partials;
@@ -267,9 +257,9 @@ Status combine_all_impl(Context* ctx, const ytgpu_arrow_array* col, const u8* fi
     YTGPU_TRY(result.allocate(ctx, 1));
     {
         KernelTimer t(ctx, KC_GROUPBY, 2);
-        if (type == YTGPU_TYPE_INT64) YTGPU_TRY((launch<YTGPU_TYPE_INT64>(ctx, vals, validity, bit_offset, length, flt, partials.p, grid, result.p)));
-        else if (type == YTGPU_TYPE_UINT64) YTGPU_TRY((launch<YTGPU_TYPE_UINT64>(ctx, vals, validity, bit_offset, length, flt, partials.p, grid, result.p)));
-        else YTGPU_TRY((launch<YTGPU_TYPE_DOUBLE>(ctx, vals, validity, bit_offset, length, flt, partials.p, grid, result.p)));
+        if (type == YTGPU_TYPE_INT64) YTGPU_TRY((launch<YTGPU_TYPE_INT64>(ctx, vals.p, nulls.p, bit_offset, length, flt.p, partials.p, grid, result.p)));
+        else if (type == YTGPU_TYPE_UINT64) YTGPU_TRY((launch<YTGPU_TYPE_UINT64>(ctx, vals.p, nulls.p, bit_offset, length, flt.p, partials.p, grid, result.p)));
+        else YTGPU_TRY((launch<YTGPU_TYPE_DOUBLE>(ctx, vals.p, nulls.p, bit_offset, length, flt.p, partials.p, grid, result.p)));
     }
     BatchResult br{};
     YTGPU_CUDA_TRY(cudaMemcpyAsync(&br, result.p, sizeof(BatchResult), cudaMemcpyDeviceToHost, ctx->stream));

@@ -217,32 +217,19 @@ Status decode_impl(Context* ctx, const u8* block, u64 block_bytes, u32 nrows, u3
     if ((u64)nrows * 4 > block_bytes) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "block shorter than its offset table");
     if (nrows == 0) return Status{};
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
-    DevBuf<u8> bstage;
-    DevBuf<ytgpu_value> ostage;
-    DevBuf<u32> cstage;
-    const u8* b = block;
-    ytgpu_value* o = out;
-    u32* c = out_counts;
-    if (mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(bstage.allocate(ctx, block_bytes));
-        YTGPU_TRY(copy_in(ctx, bstage.p, block, block_bytes, YTGPU_MEM_HOST));
-        YTGPU_TRY(ostage.allocate(ctx, (size_t)nrows * value_count));
-        b = bstage.p;
-        o = ostage.p;
-        if (out_counts) {
-            YTGPU_TRY(cstage.allocate(ctx, nrows));
-            c = cstage.p;
-        }
-    }
+    InBuf<u8> b;
+    OutBuf<ytgpu_value> o;
+    OutBuf<u32> c;
+    YTGPU_TRY(b.stage(ctx, block, block_bytes, mem));
+    YTGPU_TRY(o.prepare(ctx, out, (size_t)nrows * value_count, mem));
+    YTGPU_TRY(c.prepare(ctx, out_counts, nrows, mem));
     {
         KernelTimer t(ctx, KC_DECODE);
-        decode_block_kernel<<<blocks_for(nrows, 256, 8), 256, 0, ctx->stream>>>(b, block_bytes, nrows, value_count, o, c, ctx->dev_err);
+        decode_block_kernel<<<blocks_for(nrows, 256, 8), 256, 0, ctx->stream>>>(b.p, block_bytes, nrows, value_count, o.p, c.p, ctx->dev_err);
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
-    if (mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(copy_out(ctx, out, o, (size_t)nrows * value_count * 16, YTGPU_MEM_HOST));
-        if (out_counts) YTGPU_TRY(copy_out(ctx, out_counts, c, (size_t)nrows * 4, YTGPU_MEM_HOST));
-    }
+    YTGPU_TRY(o.download(ctx, (size_t)nrows * value_count));
+    YTGPU_TRY(c.download(ctx, nrows));
     // malformed input is reported like ReadRowValue's ThrowUnexpectedValueType
     YTGPU_CUDA_TRY(cudaMemcpyAsync(ctx->host_err, ctx->dev_err, 4, cudaMemcpyDeviceToHost, ctx->stream));
     YTGPU_CUDA_TRY(cudaMemsetAsync(ctx->dev_err, 0, 4, ctx->stream));
@@ -260,32 +247,18 @@ Status encode_impl(Context* ctx, const ytgpu_rowset_view* rows, const u32* row_c
     if (n == 0) return Status{};
     if (n >= (1ull << 32)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "a block holds fewer than 2^32 rows");
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
-    DevBuf<ytgpu_value> vstage;
-    DevBuf<u8> hstage, bstage;
-    DevBuf<u32> cstage;
-    const ytgpu_value* vals = rows->values;
-    const u8* heap = rows->string_heap;
-    const u32* counts = row_counts;
-    if (rows->mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(vstage.allocate(ctx, n * vc));
-        YTGPU_TRY(copy_in(ctx, vstage.p, rows->values, n * vc * 16, YTGPU_MEM_HOST));
-        YTGPU_TRY(hstage.allocate(ctx, rows->string_heap_bytes));
-        YTGPU_TRY(copy_in(ctx, hstage.p, rows->string_heap, rows->string_heap_bytes, YTGPU_MEM_HOST));
-        vals = vstage.p;
-        heap = hstage.p;
-        if (row_counts) {
-            YTGPU_TRY(cstage.allocate(ctx, n));
-            YTGPU_TRY(copy_in(ctx, cstage.p, row_counts, n * 4, YTGPU_MEM_HOST));
-            counts = cstage.p;
-        }
-    }
+    StagedRowset staged;
+    InBuf<u32> counts;
+    YTGPU_TRY(staged.stage(ctx, rows, rows->mem));
+    YTGPU_TRY(counts.stage(ctx, row_counts, n, rows->mem));
+    OutBuf<u8> dst;
     DevBuf<u64> sizes, sums, total;
     const u64 nblocks = (n + kScanBlock - 1) / kScanBlock;
     YTGPU_TRY(sizes.allocate(ctx, n));
     YTGPU_TRY(sums.allocate(ctx, nblocks));
     YTGPU_TRY(total.allocate(ctx, 1));
     KernelTimer t(ctx, KC_DECODE, 5);
-    row_sizes_kernel<<<blocks_for(n, 256, 8), 256, 0, ctx->stream>>>(vals, vc, counts, n, sizes.p);
+    row_sizes_kernel<<<blocks_for(n, 256, 8), 256, 0, ctx->stream>>>(staged.values.p, vc, counts.p, n, sizes.p);
     exclusive_scan_u64(ctx->stream, sizes.p, n, sums.p, total.p);
     YTGPU_CUDA_TRY(cudaGetLastError());
     u64 data_bytes = 0;
@@ -296,14 +269,10 @@ Status encode_impl(Context* ctx, const ytgpu_rowset_view* rows, const u32* row_c
     if (data_bytes >= (1ull << 32)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "block data of %llu bytes does not fit ui32 row offsets", (unsigned long long)data_bytes);
     if (!out_block || bytes > capacity)
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "block needs %llu bytes, capacity is %llu", (unsigned long long)bytes, (unsigned long long)capacity);
-    u8* dst = out_block;
-    if (out_mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(bstage.allocate(ctx, bytes));
-        dst = bstage.p;
-    }
-    encode_rows_kernel<<<blocks_for(n, 256, 8), 256, 0, ctx->stream>>>(vals, vc, counts, heap, n, sizes.p, dst);
+    YTGPU_TRY(dst.prepare(ctx, out_block, bytes, out_mem));
+    encode_rows_kernel<<<blocks_for(n, 256, 8), 256, 0, ctx->stream>>>(staged.values.p, vc, counts.p, staged.heap.p, n, sizes.p, dst.p);
     YTGPU_CUDA_TRY(cudaGetLastError());
-    if (out_mem == YTGPU_MEM_HOST) YTGPU_TRY(copy_out(ctx, out_block, dst, bytes, YTGPU_MEM_HOST));
+    YTGPU_TRY(dst.download(ctx, bytes));
     YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return Status{};
 }

@@ -55,8 +55,7 @@ Status resolve_widths(Context* ctx, const ytgpu_sort_spec* spec, const ytgpu_val
 // point shares.  The buffers live as long as the object (the permutation refers to the scratch).  Keys whose
 // fixed-width normalised form does not fit in kMaxKeyChunks chunks take the refinement sort of long_keys.cu instead.
 struct RowsetSort {
-    DevBuf<ytgpu_value> vals_stage;
-    DevBuf<u8> heap_stage;
+    StagedRowset staged;
     const ytgpu_value* vals = nullptr;
     const u8* heap = nullptr;
     u32 vc = 0;
@@ -86,16 +85,9 @@ struct RowsetSort {
     Status prepare(Context* ctx, const ytgpu_rowset_view* in, const ytgpu_sort_spec* spec) {
         const u64 n = in->row_count;
         vc = in->value_count;
-        vals = in->values;
-        heap = in->string_heap;
-        if (in->mem == YTGPU_MEM_HOST) {
-            YTGPU_TRY(vals_stage.allocate(ctx, n * vc));
-            YTGPU_TRY(copy_in(ctx, vals_stage.p, in->values, n * vc * sizeof(ytgpu_value), YTGPU_MEM_HOST));
-            YTGPU_TRY(heap_stage.allocate(ctx, in->string_heap_bytes));
-            YTGPU_TRY(copy_in(ctx, heap_stage.p, in->string_heap, in->string_heap_bytes, YTGPU_MEM_HOST));
-            vals = vals_stage.p;
-            heap = heap_stage.p;
-        }
+        YTGPU_TRY(staged.stage(ctx, in, in->mem));
+        vals = staged.values.p;
+        heap = staged.heap.p;
         std::vector<ytgpu_key_column> cols;
         YTGPU_TRY(resolve_widths(ctx, spec, vals, vc, n, &cols));
         ytgpu_sort_spec rs{cols.data(), (u32)cols.size()};
@@ -130,26 +122,16 @@ Status sort_rowset_impl(Context* ctx, const ytgpu_rowset_view* in, const ytgpu_s
     const PermRef& perm = rs.perm;
 
     if (out_perm) {
-        if (out_mem == YTGPU_MEM_HOST) {
-            DevBuf<u32> tmp;
-            YTGPU_TRY(tmp.allocate(ctx, n));
-            YTGPU_TRY(materialize_perm(ctx, perm, n, tmp.p));
-            YTGPU_TRY(copy_out(ctx, out_perm, tmp.p, n * 4, YTGPU_MEM_HOST));
-            YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-        } else {
-            YTGPU_TRY(materialize_perm(ctx, perm, n, out_perm));
-        }
+        OutBuf<u32> dst;
+        YTGPU_TRY(dst.prepare(ctx, out_perm, n, out_mem));
+        YTGPU_TRY(materialize_perm(ctx, perm, n, dst.p));
+        YTGPU_TRY(dst.download(ctx, n));
     }
     if (out_values) {
-        if (out_mem == YTGPU_MEM_HOST) {
-            DevBuf<ytgpu_value> tmp;
-            YTGPU_TRY(tmp.allocate(ctx, n * vc));
-            YTGPU_TRY(gather_rows(ctx, reinterpret_cast<const u8*>(vals), perm, reinterpret_cast<u8*>(tmp.p), n, vc * 16));
-            YTGPU_TRY(copy_out(ctx, out_values, tmp.p, n * vc * 16, YTGPU_MEM_HOST));
-            YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-        } else {
-            YTGPU_TRY(gather_rows(ctx, reinterpret_cast<const u8*>(vals), perm, reinterpret_cast<u8*>(out_values), n, vc * 16));
-        }
+        OutBuf<ytgpu_value> dst;
+        YTGPU_TRY(dst.prepare(ctx, out_values, n * vc, out_mem));
+        YTGPU_TRY(gather_rows(ctx, reinterpret_cast<const u8*>(vals), perm, reinterpret_cast<u8*>(dst.p), n, vc * 16));
+        YTGPU_TRY(dst.download(ctx, n * vc));
     }
     if (in->mem == YTGPU_MEM_HOST || out_mem == YTGPU_MEM_HOST) YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return Status{};
@@ -237,7 +219,7 @@ Status join_sorted_impl(Context* ctx, const ytgpu_rowset_view* in, const ytgpu_s
 
     DevBuf<u64> head, keep, sums, totals;
     DevBuf<u8> has_primary;
-    DevBuf<u32> out_dev;
+    OutBuf<u32> dst;
     YTGPU_TRY(head.allocate(ctx, n));
     YTGPU_TRY(keep.allocate(ctx, n));
     YTGPU_TRY(sums.allocate(ctx, scan_block_count(n)));
@@ -247,11 +229,7 @@ Status join_sorted_impl(Context* ctx, const ytgpu_rowset_view* in, const ytgpu_s
     const u32 threads = 256, blocks = (u32)((n + threads - 1) / threads);
     const SortPlan* plan = rs.perm.plan;
     const u32 *pa = rs.perm.idx[0], *pb = rs.perm.idx[1];
-    u32* dst = out_perm;
-    if (out_mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(out_dev.allocate(ctx, n));
-        dst = out_dev.p;
-    }
+    YTGPU_TRY(dst.prepare(ctx, out_perm, n, out_mem));
     {
         KernelTimer t(ctx, KC_HISTOGRAM, 10);
         if (rs.long_keys) {
@@ -265,16 +243,14 @@ Status join_sorted_impl(Context* ctx, const ytgpu_rowset_view* in, const ytgpu_s
         join_mark_kernel<<<blocks, threads, 0, ctx->stream>>>(plan, pa, pb, n, primary_rows, head.p, totals.p, has_primary.p);
         join_keep_kernel<<<blocks, threads, 0, ctx->stream>>>(plan, pa, pb, n, primary_rows, head.p, totals.p, has_primary.p, keep.p);
         exclusive_scan_u64(ctx->stream, keep.p, n, sums.p, totals.p + 1);
-        join_compact_kernel<<<blocks, threads, 0, ctx->stream>>>(plan, pa, pb, n, keep.p, totals.p + 1, dst);
+        join_compact_kernel<<<blocks, threads, 0, ctx->stream>>>(plan, pa, pb, n, keep.p, totals.p + 1, dst.p);
     }
     YTGPU_CUDA_TRY(cudaGetLastError());
     u64 count = 0;
     YTGPU_CUDA_TRY(cudaMemcpyAsync(&count, totals.p + 1, 8, cudaMemcpyDeviceToHost, ctx->stream));
     YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    if (out_mem == YTGPU_MEM_HOST && count) {
-        YTGPU_TRY(copy_out(ctx, out_perm, dst, count * 4, YTGPU_MEM_HOST));
-        YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    }
+    YTGPU_TRY(dst.download(ctx, count));
+    if (out_mem == YTGPU_MEM_HOST && count) YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     *out_count = count;
     return Status{};
 }
@@ -296,26 +272,19 @@ Status sort_fixed_rows_impl(Context* ctx, const ytgpu_fixed_rows_view* in, const
     if (n == 0) return Status{};
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
 
-    DevBuf<u8> in_stage, out_stage;
-    const u8* rows = in->rows;
-    if (in->mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(in_stage.allocate(ctx, n * rb));
-        YTGPU_TRY(copy_in(ctx, in_stage.p, in->rows, n * rb, YTGPU_MEM_HOST));
-        rows = in_stage.p;
-    }
+    InBuf<u8> staged;
+    OutBuf<u8> dst;
+    YTGPU_TRY(staged.stage(ctx, in->rows, n * rb, in->mem));
+    const u8* rows = staged.p;
     ChunkSet chunks;
     YTGPU_TRY(chunks.allocate(ctx, L.nchunks, n));
     SortScratch scratch;
     PermRef perm;
-    u8* dst = out_rows;
     if (out_rows) {
-        if (out_mem == YTGPU_MEM_HOST) {
-            YTGPU_TRY(out_stage.allocate(ctx, n * rb));
-            dst = out_stage.p;
-        }
+        YTGPU_TRY(dst.prepare(ctx, out_rows, n * rb, out_mem));
         // the sort may move the rows itself (three-pass schedule); then the permutation is written only if wanted
         scratch.gather.rows = rows;
-        scratch.gather.out = dst;
+        scratch.gather.out = dst.p;
         scratch.gather.row_bytes = rb;
         scratch.gather.want_perm = out_perm != nullptr;
     }
@@ -323,19 +292,14 @@ Status sort_fixed_rows_impl(Context* ctx, const ytgpu_fixed_rows_view* in, const
     YTGPU_TRY(normalize_fixed_rows(ctx, L, rows, n, rb, chunks.ptrs, scratch.hist.p, &scratch.hist_precomputed));
     YTGPU_TRY(radix_sort_keys(ctx, chunks.cptrs, (int)L.nchunks, n, &scratch, &perm));
     if (out_rows) {
-        if (!scratch.rows_gathered) YTGPU_TRY(gather_rows(ctx, rows, perm, dst, n, rb));
-        if (out_mem == YTGPU_MEM_HOST) YTGPU_TRY(copy_out(ctx, out_rows, dst, n * rb, YTGPU_MEM_HOST));
+        if (!scratch.rows_gathered) YTGPU_TRY(gather_rows(ctx, rows, perm, dst.p, n, rb));
+        YTGPU_TRY(dst.download(ctx, n * rb));
     }
     if (out_perm) {
-        if (out_mem == YTGPU_MEM_HOST) {
-            DevBuf<u32> tmp;
-            YTGPU_TRY(tmp.allocate(ctx, n));
-            YTGPU_TRY(materialize_perm(ctx, perm, n, tmp.p));
-            YTGPU_TRY(copy_out(ctx, out_perm, tmp.p, n * 4, YTGPU_MEM_HOST));
-            YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-        } else {
-            YTGPU_TRY(materialize_perm(ctx, perm, n, out_perm));
-        }
+        OutBuf<u32> perm_dst;
+        YTGPU_TRY(perm_dst.prepare(ctx, out_perm, n, out_mem));
+        YTGPU_TRY(materialize_perm(ctx, perm, n, perm_dst.p));
+        YTGPU_TRY(perm_dst.download(ctx, n));
     }
     if (in->mem == YTGPU_MEM_HOST || out_mem == YTGPU_MEM_HOST) YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return Status{};
@@ -373,22 +337,18 @@ Status merge_sorted_runs_impl(Context* ctx, const ytgpu_rowset_view* in, const y
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
     RowsetSort rs;
     YTGPU_TRY(rs.prepare(ctx, in, spec));
-    DevBuf<u32> tmp;
-    u32* dst = out_perm;
-    if (out_mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(tmp.allocate(ctx, n));
-        dst = tmp.p;
-    }
+    OutBuf<u32> dst;
+    YTGPU_TRY(dst.prepare(ctx, out_perm, n, out_mem));
     bool merged = false;
     if (ctx->opt_merge_path != 0 && !rs.long_keys)  // merge path compares normalised key chunks
-        YTGPU_TRY(merge_sorted_key_runs(ctx, rs.chunks.cptrs, (int)rs.L.nchunks, n, run_offsets, run_count, dst, &merged));
+        YTGPU_TRY(merge_sorted_key_runs(ctx, rs.chunks.cptrs, (int)rs.L.nchunks, n, run_offsets, run_count, dst.p, &merged));
     ctx->last_merge_used_merge_path = merged;
     if (!merged) {
         YTGPU_TRY(rs.sort(ctx, n));
-        YTGPU_TRY(materialize_perm(ctx, rs.perm, n, dst));
+        YTGPU_TRY(materialize_perm(ctx, rs.perm, n, dst.p));
     }
     if (out_mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(copy_out(ctx, out_perm, dst, n * 4, YTGPU_MEM_HOST));
+        YTGPU_TRY(dst.download(ctx, n));
         YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     }
     return Status{};
@@ -551,18 +511,14 @@ Status order_rows_impl(Context* ctx, const ytgpu_column_view* columns, u32 colum
     ctx->last_sort_refine_rounds = 0;
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
 
-    DevBuf<u32> staged_rows;
-    const u32* drows = rows;
-    if (rows && out_mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(staged_rows.allocate(ctx, n));
-        YTGPU_TRY(copy_in(ctx, staged_rows.p, rows, n * 4, YTGPU_MEM_HOST));
-        drows = staged_rows.p;
-    }
+    InBuf<u32> staged_rows;
+    YTGPU_TRY(staged_rows.stage(ctx, rows, n, out_mem));
+    const u32* drows = staged_rows.p;
     // the item columns on the device; each string heap at its offset in one concatenated heap
     std::vector<StagedColumn> staged(item_count);
-    std::vector<DevBuf<u64>> sstarts(item_count);
-    std::vector<DevBuf<u32>> slengths(item_count);
-    std::vector<DevBuf<u8>> snulls(item_count);
+    std::vector<InBuf<u64>> sstarts(item_count);
+    std::vector<InBuf<u32>> slengths(item_count);
+    std::vector<InBuf<u8>> snulls(item_count);
     std::vector<OrderItemDev> host_items(item_count);
     std::vector<ytgpu_key_column> keys(item_count);
     u64 heap_total = 0;
@@ -584,32 +540,22 @@ Status order_rows_impl(Context* ctx, const ytgpu_column_view* columns, u32 colum
         d.heap_base = heap_total;
         d.heap_bytes = s.heap_bytes;
         heap_total += s.heap_bytes;
-        d.starts = s.starts;
-        d.lengths = s.lengths;
-        d.nulls = s.null_bytemap;
-        if (s.mem == YTGPU_MEM_HOST && s.row_count) {
-            YTGPU_TRY(sstarts[k].allocate(ctx, s.row_count));
-            YTGPU_TRY(slengths[k].allocate(ctx, s.row_count));
-            YTGPU_TRY(copy_in(ctx, sstarts[k].p, s.starts, s.row_count * 8, YTGPU_MEM_HOST));
-            YTGPU_TRY(copy_in(ctx, slengths[k].p, s.lengths, s.row_count * 4, YTGPU_MEM_HOST));
-            d.starts = sstarts[k].p;
-            d.lengths = slengths[k].p;
-            if (s.null_bytemap) {
-                YTGPU_TRY(snulls[k].allocate(ctx, s.row_count));
-                YTGPU_TRY(copy_in(ctx, snulls[k].p, s.null_bytemap, s.row_count, YTGPU_MEM_HOST));
-                d.nulls = snulls[k].p;
-            }
-        }
+        const int mem = s.row_count ? s.mem : YTGPU_MEM_DEVICE;  // no rows: the caller's pointers stay
+        YTGPU_TRY(sstarts[k].stage(ctx, s.starts, s.row_count, mem));
+        YTGPU_TRY(slengths[k].stage(ctx, s.lengths, s.row_count, mem));
+        YTGPU_TRY(snulls[k].stage(ctx, s.null_bytemap, s.row_count, mem));
+        d.starts = sstarts[k].p;
+        d.lengths = slengths[k].p;
+        d.nulls = snulls[k].p;
     }
     DevBuf<u8> heap;
     YTGPU_TRY(heap.allocate(ctx, heap_total));
-    for (u32 k = 0; k < item_count; ++k)
+    for (u32 k = 0; k < item_count; ++k)  // each heap lands at its offset in the one sort heap, from either memory space
         if (host_items[k].is_string)
             YTGPU_TRY(copy_in(ctx, heap.p + host_items[k].heap_base, string_columns[items[k].column].heap, host_items[k].heap_bytes,
                               string_columns[items[k].column].mem));
-    DevBuf<OrderItemDev> dev_items;
-    YTGPU_TRY(dev_items.allocate(ctx, item_count));
-    YTGPU_TRY(copy_in(ctx, dev_items.p, host_items.data(), item_count * sizeof(OrderItemDev), YTGPU_MEM_HOST));
+    InBuf<OrderItemDev> dev_items;
+    YTGPU_TRY(dev_items.stage(ctx, host_items.data(), item_count, YTGPU_MEM_HOST));
     DevBuf<ytgpu_value> values;
     YTGPU_TRY(values.allocate(ctx, n * item_count));
     {
@@ -625,19 +571,15 @@ Status order_rows_impl(Context* ctx, const ytgpu_column_view* columns, u32 colum
     RowsetSort rs;
     YTGPU_TRY(rs.run(ctx, &view, &spec));
 
-    DevBuf<u32> out_stage;
-    u32* dst = out_rows;
-    if (out_mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(out_stage.allocate(ctx, window));
-        dst = out_stage.p;
-    }
+    OutBuf<u32> dst;
+    YTGPU_TRY(dst.prepare(ctx, out_rows, window, out_mem));
     {
         KernelTimer t(ctx, KC_GATHER);
         order_window_kernel<<<blocks_for(window, 256, 16), 256, 0, ctx->stream>>>(rs.perm.plan, rs.perm.idx[0], rs.perm.idx[1], drows,
-                                                                                  std::min(offset, n), window, dst);
+                                                                                  std::min(offset, n), window, dst.p);
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
-    if (out_mem == YTGPU_MEM_HOST) YTGPU_TRY(copy_out(ctx, out_rows, dst, window * 4, YTGPU_MEM_HOST));
+    YTGPU_TRY(dst.download(ctx, window));
     YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return Status{};
 }

@@ -99,39 +99,27 @@ Status convert_impl(Context* ctx, const ytgpu_ch_column* col, ytgpu_value* out, 
     d.null_map = col->null_map;
     d.adjust = col->time_adjustment;
     d.rows = n;
-    DevBuf<u8> data_stage, null_stage;
-    DevBuf<u64> off_stage;
-    DevBuf<uint4> out_stage;
-    if (col->mem == YTGPU_MEM_HOST) {
-        if (col->type == YTGPU_CH_STRING) {
-            // the values only carry offsets into the chars: the bytes themselves are not needed on the device
-            YTGPU_TRY(off_stage.allocate(ctx, n));
-            YTGPU_TRY(copy_in(ctx, off_stage.p, col->offsets, n * 8, YTGPU_MEM_HOST));
-            d.offsets = off_stage.p;
-        } else {
-            const size_t bytes = (size_t)n * element_bytes(col->type);
-            YTGPU_TRY(data_stage.allocate(ctx, bytes));
-            YTGPU_TRY(copy_in(ctx, data_stage.p, col->data, bytes, YTGPU_MEM_HOST));
-            d.data = data_stage.p;
-        }
-        if (col->null_map) {
-            YTGPU_TRY(null_stage.allocate(ctx, n));
-            YTGPU_TRY(copy_in(ctx, null_stage.p, col->null_map, n, YTGPU_MEM_HOST));
-            d.null_map = null_stage.p;
-        }
+    InBuf<u8> data, nulls;
+    InBuf<u64> offsets;
+    if (col->type == YTGPU_CH_STRING) {
+        // the values only carry offsets into the chars: the bytes themselves are not needed on the device
+        YTGPU_TRY(offsets.stage(ctx, col->offsets, n, col->mem));
+        d.offsets = offsets.p;
+    } else {
+        YTGPU_TRY(data.stage(ctx, static_cast<const u8*>(col->data), (size_t)n * element_bytes(col->type), col->mem));
+        d.data = data.p;
     }
-    uint4* o = reinterpret_cast<uint4*>(out);
-    if (out_mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(out_stage.allocate(ctx, n));
-        o = out_stage.p;
-    }
+    YTGPU_TRY(nulls.stage(ctx, col->null_map, n, col->mem));
+    d.null_map = nulls.p;
+    OutBuf<uint4> o;
+    YTGPU_TRY(o.prepare(ctx, reinterpret_cast<uint4*>(out), n, out_mem));
     {
         KernelTimer t(ctx, KC_DECODE);
         const unsigned blocks = (unsigned)std::min<u64>((n + 255) / 256, (u64)kNumSms * 16);
-        ch_to_values_kernel<<<blocks, 256, 0, ctx->stream>>>(d, o, ctx->dev_err);
+        ch_to_values_kernel<<<blocks, 256, 0, ctx->stream>>>(d, o.p, ctx->dev_err);
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
-    if (out_mem == YTGPU_MEM_HOST) YTGPU_TRY(copy_out(ctx, out, o, n * 16, YTGPU_MEM_HOST));
+    YTGPU_TRY(o.download(ctx, n));
     Status s = check_device_errors(ctx);  // synchronises the stream
     if (s.ok()) return s;
     const u32 e = *ctx->host_err;

@@ -380,20 +380,11 @@ Status encode_impl(Context* ctx, const u64* values, const u8* null_bytemap, u64 
     const u32 nseg = (u32)nseg64;
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
 
-    DevBuf<u64> vstage;
-    DevBuf<u8> nstage;
-    const u64* raw = values;
-    const u8* nulls = null_bytemap;
-    if (mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(vstage.allocate(ctx, n));
-        YTGPU_TRY(copy_in(ctx, vstage.p, values, n * 8, YTGPU_MEM_HOST));
-        raw = vstage.p;
-        if (null_bytemap) {
-            YTGPU_TRY(nstage.allocate(ctx, n));
-            YTGPU_TRY(copy_in(ctx, nstage.p, null_bytemap, n, YTGPU_MEM_HOST));
-            nulls = nstage.p;
-        }
-    }
+    InBuf<u64> raw;
+    InBuf<u8> staged_nulls;
+    YTGPU_TRY(raw.stage(ctx, values, n, mem));
+    YTGPU_TRY(staged_nulls.stage(ctx, null_bytemap, n, mem));
+    const u8* nulls = staged_nulls.p;
 
     // per-segment table: power of two >= 2 x rows of a segment
     const u64 seg_rows = std::min<u64>(max_values, n);
@@ -421,7 +412,7 @@ Status encode_impl(Context* ctx, const u64* values, const u8* null_bytemap, u64 
     {
         KernelTimer t(ctx, KC_DECODE, 7);
         init_stats_kernel<<<grid_for(nseg, 256, 4), 256, 0, ctx->stream>>>(stats.p, nseg);
-        stats_kernel<<<nseg * blocks_per_seg, kStatThreads, 0, ctx->stream>>>(raw, nulls, n, is_signed, max_values, blocks_per_seg, enc.p,
+        stats_kernel<<<nseg * blocks_per_seg, kStatThreads, 0, ctx->stream>>>(raw.p, nulls, n, is_signed, max_values, blocks_per_seg, enc.p,
                                                                              stats.p, table.p, cap);
         flags_kernel<<<(u32)((n + kRowsPerBlock) / kRowsPerBlock), 256, 0, ctx->stream>>>(enc.p, nulls, n, max_values, table.p, cap, first_of.p,
                                                                                          flags.p);
@@ -443,21 +434,17 @@ Status encode_impl(Context* ctx, const u64* values, const u8* null_bytemap, u64 
                            (unsigned long long)out_capacity);
     YTGPU_CUDA_TRY(cudaMemcpyAsync(out_segments, segs.p, (size_t)nseg * sizeof(ytgpu_integer_segment), cudaMemcpyDeviceToHost, ctx->stream));
 
-    DevBuf<u64> ostage;
-    u64* dst = reinterpret_cast<u64*>(out_data);
-    if (mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(ostage.allocate(ctx, bytes / 8));
-        dst = ostage.p;
-    } else if (reinterpret_cast<uintptr_t>(out_data) & 7) {
+    if (mem != YTGPU_MEM_HOST && (reinterpret_cast<uintptr_t>(out_data) & 7))
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "out_data must be 8-byte aligned");
-    }
+    OutBuf<u64> dst;
+    YTGPU_TRY(dst.prepare(ctx, reinterpret_cast<u64*>(out_data), bytes / 8, mem));
     PackArgs args{enc.p, nulls, first_of.p, flags.p, dict.p, run_start.p, segs.p, work.p, nseg, max_values, bytes / 8};
     {
         KernelTimer t(ctx, KC_DECODE, 1);
-        pack_kernel<<<grid_for(bytes / 8, 256, 8), 256, 0, ctx->stream>>>(args, dst);
+        pack_kernel<<<grid_for(bytes / 8, 256, 8), 256, 0, ctx->stream>>>(args, dst.p);
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
-    if (mem == YTGPU_MEM_HOST) YTGPU_TRY(copy_out(ctx, out_data, dst, bytes, YTGPU_MEM_HOST));
+    YTGPU_TRY(dst.download(ctx, bytes / 8));  // segment data are whole words
     YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return Status{};
 }
@@ -507,32 +494,20 @@ Status convert_impl(Context* ctx, const ytgpu_rowset_view* rows, u32 column, u8 
     const u64 n = rows->row_count;
     if (n == 0) return Status{};
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
-    DevBuf<ytgpu_value> vstage;
-    DevBuf<u64> ostage, bstage;
-    const ytgpu_value* vals = rows->values;
-    if (rows->mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(vstage.allocate(ctx, n * rows->value_count));
-        YTGPU_TRY(copy_in(ctx, vstage.p, rows->values, n * rows->value_count * 16, YTGPU_MEM_HOST));
-        vals = vstage.p;
-    }
     const u64 words = (n + 63) / 64;
-    u64* ov = out_values;
-    u64* ob = reinterpret_cast<u64*>(out_bitmap);
-    if (out_mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(ostage.allocate(ctx, n));
-        YTGPU_TRY(bstage.allocate(ctx, words));
-        ov = ostage.p;
-        ob = bstage.p;
-    }
+    InBuf<ytgpu_value> vals;
+    OutBuf<u64> ov, ob;
+    YTGPU_TRY(vals.stage(ctx, rows->values, n * rows->value_count, rows->mem));
+    YTGPU_TRY(ov.prepare(ctx, out_values, n, out_mem));
+    YTGPU_TRY(ob.prepare(ctx, reinterpret_cast<u64*>(out_bitmap), words, out_mem));
     {
         KernelTimer t(ctx, KC_DECODE, 1);
-        convert_kernel<<<grid_for(words * 32, 256, 8), 256, 0, ctx->stream>>>(vals, n, rows->value_count, column, value_type, ov, ob, ctx->dev_err);
+        convert_kernel<<<grid_for(words * 32, 256, 8), 256, 0, ctx->stream>>>(vals.p, n, rows->value_count, column, value_type, ov.p, ob.p,
+                                                                              ctx->dev_err);
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
-    if (out_mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(copy_out(ctx, out_values, ov, n * 8, YTGPU_MEM_HOST));
-        YTGPU_TRY(copy_out(ctx, out_bitmap, ob, words * 8, YTGPU_MEM_HOST));
-    }
+    YTGPU_TRY(ov.download(ctx, n));
+    YTGPU_TRY(ob.download(ctx, words));
     return check_device_errors(ctx);
 }
 

@@ -585,27 +585,17 @@ Status decode_column_impl(Context* ctx, const ytgpu_column_view* col, u64* out_v
     YTGPU_TRY(stage_column(ctx, col, &sc));
     const u64 n = (u64)col->value_count;
     if (n == 0) return Status{};
-    DevBuf<u64> ov;
-    DevBuf<u8> on;
-    u64* dv = out_values;
-    u8* dn = out_null;
-    if (out_mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(ov.allocate(ctx, n));
-        dv = ov.p;
-        if (out_null) {
-            YTGPU_TRY(on.allocate(ctx, n));
-            dn = on.p;
-        }
-    }
+    OutBuf<u64> dv;
+    OutBuf<u8> dn;
+    YTGPU_TRY(dv.prepare(ctx, out_values, n, out_mem));
+    YTGPU_TRY(dn.prepare(ctx, out_null, n, out_mem));
     {
         KernelTimer t(ctx, KC_DECODE);
-        decode_column_kernel<<<blocks_for(n, 256, 8), 256, 0, ctx->stream>>>(sc.dev, dv, dn);
+        decode_column_kernel<<<blocks_for(n, 256, 8), 256, 0, ctx->stream>>>(sc.dev, dv.p, dn.p);
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
-    if (out_mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(copy_out(ctx, out_values, dv, n * 8, YTGPU_MEM_HOST));
-        if (out_null) YTGPU_TRY(copy_out(ctx, out_null, dn, n, YTGPU_MEM_HOST));
-    }
+    YTGPU_TRY(dv.download(ctx, n));
+    YTGPU_TRY(dn.download(ctx, n));
     if (col->mem == YTGPU_MEM_HOST || out_mem == YTGPU_MEM_HOST) YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return Status{};
 }
@@ -622,17 +612,11 @@ Status decode_column_typed_impl(Context* ctx, const ytgpu_column_view* col, u32 
     const bool is_float32 = col->value_type == YTGPU_TYPE_DOUBLE && col->bit_width == 32;
     if (is_float32 && element_bytes != 4 && element_bytes != 8)
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "a float value vector converts to Float32 or Float64");
-    DevBuf<u8> ov, on;
-    void* dv = out_values;
-    u8* dn = out_null;
-    if (out_mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(ov.allocate(ctx, n * element_bytes));
-        dv = ov.p;
-        if (out_null) {
-            YTGPU_TRY(on.allocate(ctx, n));
-            dn = on.p;
-        }
-    }
+    OutBuf<u8> ov, on;
+    YTGPU_TRY(ov.prepare(ctx, static_cast<u8*>(out_values), n * element_bytes, out_mem));
+    YTGPU_TRY(on.prepare(ctx, out_null, n, out_mem));
+    void* dv = ov.p;
+    u8* dn = on.p;
     {
         KernelTimer t(ctx, KC_DECODE);
         const unsigned blocks = blocks_for(n, 256, 8);
@@ -645,10 +629,8 @@ Status decode_column_typed_impl(Context* ctx, const ytgpu_column_view* col, u32 
         }
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
-    if (out_mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(copy_out(ctx, out_values, dv, n * element_bytes, YTGPU_MEM_HOST));
-        if (out_null) YTGPU_TRY(copy_out(ctx, out_null, dn, n, YTGPU_MEM_HOST));
-    }
+    YTGPU_TRY(ov.download(ctx, n * element_bytes));
+    YTGPU_TRY(on.download(ctx, n));
     if (col->mem == YTGPU_MEM_HOST || out_mem == YTGPU_MEM_HOST) YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return Status{};
 }
@@ -793,28 +775,18 @@ Status groupby_impl(Context* ctx, const ytgpu_column_view* kcol, const ytgpu_col
                            (unsigned long long)total, (unsigned long long)out->capacity);
     if (total == 0) return Status{};
 
-    DevBuf<u64> ok, os, oc, of, omn, omx;
-    DevBuf<u8> osn, okn;
-    u64 *dk = out->keys, *ds = out->sums, *dc = out->counts, *df = out->first_rows, *dmn = out->mins, *dmx = out->maxs;
-    u8 *dsn = out->sum_null, *dkn = out->key_null;
-    if (out_mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(ok.allocate(ctx, total));
-        YTGPU_TRY(os.allocate(ctx, total));
-        YTGPU_TRY(oc.allocate(ctx, total));
-        YTGPU_TRY(osn.allocate(ctx, total));
-        YTGPU_TRY(okn.allocate(ctx, total));
-        if (want_first) YTGPU_TRY(of.allocate(ctx, total));
-        dk = ok.p; ds = os.p; dc = oc.p; dsn = osn.p; dkn = okn.p;
-        df = want_first ? of.p : nullptr;
-        if (out->mins) {
-            YTGPU_TRY(omn.allocate(ctx, total));
-            dmn = omn.p;
-        }
-        if (out->maxs) {
-            YTGPU_TRY(omx.allocate(ctx, total));
-            dmx = omx.p;
-        }
-    }
+    OutBuf<u64> ok, os, oc, of, omn, omx;
+    OutBuf<u8> osn, okn;
+    YTGPU_TRY(ok.prepare(ctx, out->keys, total, out_mem));
+    YTGPU_TRY(os.prepare(ctx, out->sums, total, out_mem));
+    YTGPU_TRY(oc.prepare(ctx, out->counts, total, out_mem));
+    YTGPU_TRY(osn.prepare(ctx, out->sum_null, total, out_mem));
+    YTGPU_TRY(okn.prepare(ctx, out->key_null, total, out_mem));
+    YTGPU_TRY(of.prepare(ctx, out->first_rows, total, out_mem));
+    YTGPU_TRY(omn.prepare(ctx, out->mins, total, out_mem));
+    YTGPU_TRY(omx.prepare(ctx, out->maxs, total, out_mem));
+    u64 *dk = ok.p, *ds = os.p, *dc = oc.p, *df = of.p, *dmn = omn.p, *dmx = omx.p;
+    u8 *dsn = osn.p, *dkn = okn.p;
     SortScratch scratch;
     if (g && g <= (u64)kSmallSortMax) {
         small_sort_groups_kernel<<<1, 1024, 0, ctx->stream>>>((u32)g, ck.p, cs.p, cc.p, csn.p, want_first ? cf.p : nullptr, cmn.p, cmx.p, dk, ds, dc, dsn, dkn, df,
@@ -834,16 +806,14 @@ Status groupby_impl(Context* ctx, const ytgpu_column_view* kcol, const ytgpu_col
         ctx->count_launch();
     }
     YTGPU_CUDA_TRY(cudaGetLastError());
-    if (out_mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(copy_out(ctx, out->keys, dk, total * 8, YTGPU_MEM_HOST));
-        YTGPU_TRY(copy_out(ctx, out->sums, ds, total * 8, YTGPU_MEM_HOST));
-        YTGPU_TRY(copy_out(ctx, out->counts, dc, total * 8, YTGPU_MEM_HOST));
-        YTGPU_TRY(copy_out(ctx, out->sum_null, dsn, total, YTGPU_MEM_HOST));
-        YTGPU_TRY(copy_out(ctx, out->key_null, dkn, total, YTGPU_MEM_HOST));
-        if (want_first) YTGPU_TRY(copy_out(ctx, out->first_rows, df, total * 8, YTGPU_MEM_HOST));
-        if (out->mins) YTGPU_TRY(copy_out(ctx, out->mins, dmn, total * 8, YTGPU_MEM_HOST));
-        if (out->maxs) YTGPU_TRY(copy_out(ctx, out->maxs, dmx, total * 8, YTGPU_MEM_HOST));
-    }
+    YTGPU_TRY(ok.download(ctx, total));
+    YTGPU_TRY(os.download(ctx, total));
+    YTGPU_TRY(oc.download(ctx, total));
+    YTGPU_TRY(osn.download(ctx, total));
+    YTGPU_TRY(okn.download(ctx, total));
+    YTGPU_TRY(of.download(ctx, total));
+    YTGPU_TRY(omn.download(ctx, total));
+    YTGPU_TRY(omx.download(ctx, total));
     YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return Status{};
 }
@@ -876,23 +846,17 @@ int ytgpu_decode_string_offsets(ytgpu_context* h, const uint32_t* encoded, uint3
     auto run = [&]() -> Status {
         YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
         const u64 cnt = (u64)(end_index - start_index + 1);
-        DevBuf<u32> din, dout;
-        const u32* e = encoded;
-        u32* o = out;
-        if (mem == YTGPU_MEM_HOST) {
-            YTGPU_TRY(din.allocate(ctx, (size_t)end_index + 1));
-            YTGPU_TRY(copy_in(ctx, din.p, encoded, (size_t)end_index * 4, YTGPU_MEM_HOST));
-            YTGPU_TRY(dout.allocate(ctx, cnt));
-            e = din.p;
-            o = dout.p;
-        }
+        InBuf<u32> e;
+        OutBuf<u32> o;
+        YTGPU_TRY(e.stage(ctx, encoded, (size_t)end_index, mem));  // the offset of value k reads encoded[k - 1]
+        YTGPU_TRY(o.prepare(ctx, out, cnt, mem));
         {
             KernelTimer t(ctx, KC_DECODE);
-            decode_string_offsets_kernel<<<blocks_for(cnt, 256, 8), 256, 0, ctx->stream>>>(e, avg_length, start_index, end_index, o);
+            decode_string_offsets_kernel<<<blocks_for(cnt, 256, 8), 256, 0, ctx->stream>>>(e.p, avg_length, start_index, end_index, o.p);
             YTGPU_CUDA_TRY(cudaGetLastError());
         }
         if (mem == YTGPU_MEM_HOST) {
-            YTGPU_TRY(copy_out(ctx, out, o, cnt * 4, YTGPU_MEM_HOST));
+            YTGPU_TRY(o.download(ctx, cnt));
             YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
         }
         return Status{};
@@ -909,28 +873,20 @@ int ytgpu_decode_string_pointers_and_lengths(ytgpu_context* h, const uint32_t* e
     auto run = [&]() -> Status {
         if (count == 0) return Status{};
         YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
-        DevBuf<u32> din, dstart;
-        DevBuf<i32> dlen;
-        const u32* e = encoded;
-        u32* os = out_start;
-        i32* ol = out_length;
-        if (mem == YTGPU_MEM_HOST) {
-            YTGPU_TRY(din.allocate(ctx, count));
-            YTGPU_TRY(dstart.allocate(ctx, count));
-            YTGPU_TRY(dlen.allocate(ctx, count));
-            YTGPU_TRY(copy_in(ctx, din.p, encoded, count * 4, YTGPU_MEM_HOST));
-            e = din.p;
-            os = dstart.p;
-            ol = dlen.p;
-        }
+        InBuf<u32> e;
+        OutBuf<u32> os;
+        OutBuf<i32> ol;
+        YTGPU_TRY(e.stage(ctx, encoded, count, mem));
+        YTGPU_TRY(os.prepare(ctx, out_start, count, mem));
+        YTGPU_TRY(ol.prepare(ctx, out_length, count, mem));
         {
             KernelTimer t(ctx, KC_DECODE);
-            decode_string_pointers_kernel<<<blocks_for(count, 256, 8), 256, 0, ctx->stream>>>(e, avg_length, count, os, ol);
+            decode_string_pointers_kernel<<<blocks_for(count, 256, 8), 256, 0, ctx->stream>>>(e.p, avg_length, count, os.p, ol.p);
             YTGPU_CUDA_TRY(cudaGetLastError());
         }
         if (mem == YTGPU_MEM_HOST) {
-            YTGPU_TRY(copy_out(ctx, out_start, os, count * 4, YTGPU_MEM_HOST));
-            YTGPU_TRY(copy_out(ctx, out_length, ol, count * 4, YTGPU_MEM_HOST));
+            YTGPU_TRY(os.download(ctx, count));
+            YTGPU_TRY(ol.download(ctx, count));
             YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
         }
         return Status{};

@@ -195,9 +195,9 @@ __device__ __forceinline__ bool passes(int op, u8 vtype, u64 v, u64 c) {
 // ---- host helpers ----
 struct StagedColumn {
     ColumnDev dev{};
-    DevBuf<u8> values, bitmap;
-    DevBuf<u32> dict;
-    DevBuf<u64> rle;
+    InBuf<u8> values, bitmap;
+    InBuf<u32> dict;
+    InBuf<u64> rle;
 };
 
 Status stage_column(Context* ctx, const ytgpu_column_view* c, StagedColumn* s) {
@@ -233,33 +233,14 @@ Status stage_column(Context* ctx, const ytgpu_column_view* c, StagedColumn* s) {
                              : (c->bit_width == 1 ? (size_t)(c->values_count + 7) / 8 : (size_t)c->values_count * (c->bit_width / 8)));
     const size_t bm_entries = c->null_bitmap ? (size_t)((c->dictionary_indexes || c->rle_indexes) ? d.values_count
                                                         : (u64)(c->start_index + c->value_count)) : 0;
-    if (c->mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(s->values.allocate(ctx, vbytes_exact + 16));
-        YTGPU_CUDA_TRY(cudaMemsetAsync(s->values.p + vbytes_exact, 0, 16, ctx->stream));  // one readable word past the end
-        YTGPU_TRY(copy_in(ctx, s->values.p, c->values, vbytes_exact, YTGPU_MEM_HOST));
-        d.values = d.has_values ? s->values.p : nullptr;
-        if (c->null_bitmap) {
-            size_t bb = (bm_entries + 7) / 8;
-            YTGPU_TRY(s->bitmap.allocate(ctx, bb));
-            YTGPU_TRY(copy_in(ctx, s->bitmap.p, c->null_bitmap, bb, YTGPU_MEM_HOST));
-            d.bitmap = s->bitmap.p;
-        }
-        if (c->dictionary_indexes) {
-            YTGPU_TRY(s->dict.allocate(ctx, c->dictionary_index_count));
-            YTGPU_TRY(copy_in(ctx, s->dict.p, c->dictionary_indexes, c->dictionary_index_count * 4, YTGPU_MEM_HOST));
-            d.dict = s->dict.p;
-        }
-        if (c->rle_indexes) {
-            YTGPU_TRY(s->rle.allocate(ctx, c->rle_count));
-            YTGPU_TRY(copy_in(ctx, s->rle.p, c->rle_indexes, c->rle_count * 8, YTGPU_MEM_HOST));
-            d.rle = s->rle.p;
-        }
-    } else {
-        d.values = d.has_values ? c->values : nullptr;
-        d.bitmap = c->null_bitmap;
-        d.dict = c->dictionary_indexes;
-        d.rle = c->rle_indexes;
-    }
+    YTGPU_TRY(s->values.stage(ctx, static_cast<const u8*>(c->values), vbytes_exact, c->mem, 16));  // one readable word past the end
+    d.values = d.has_values ? s->values.p : nullptr;
+    YTGPU_TRY(s->bitmap.stage(ctx, c->null_bitmap, (bm_entries + 7) / 8, c->mem));
+    d.bitmap = s->bitmap.p;
+    YTGPU_TRY(s->dict.stage(ctx, c->dictionary_indexes, c->dictionary_index_count, c->mem));
+    d.dict = s->dict.p;
+    YTGPU_TRY(s->rle.stage(ctx, c->rle_indexes, c->rle_count, c->mem));
+    d.rle = s->rle.p;
     return Status{};
 }
 

@@ -346,8 +346,8 @@ inline unsigned grid_for(u64 items, unsigned per_block) {
 // A flag source staged on the device (HOST flavour copies the arrays in).
 struct StagedSource {
     FlagSrc dev{};
-    DevBuf<u8> data;
-    DevBuf<u64> rle;
+    InBuf<u8> data;
+    InBuf<u64> rle;
 };
 
 Status validate_source(const ytgpu_flag_source* src, i64 start, i64 end, bool need_rle = false) {
@@ -368,27 +368,21 @@ Status validate_source(const ytgpu_flag_source* src, i64 start, i64 end, bool ne
 }
 
 Status stage_source(Context* ctx, const ytgpu_flag_source* src, int mem, StagedSource* st) {
-    st->dev.kind = src->kind;
-    st->dev.data = src->data;
-    st->dev.data_count = src->data_count;
-    st->dev.rle = src->rle_indexes;
-    st->dev.rle_count = src->rle_indexes ? src->rle_count : 0;
+    const size_t bytes = src->kind == YTGPU_FLAGS_DICTIONARY_ZERO ? (size_t)src->data_count * 4 : (size_t)((src->data_count + 7) >> 3);
+    YTGPU_TRY(st->data.stage(ctx, static_cast<const u8*>(src->data), bytes, mem));
     if (mem == YTGPU_MEM_HOST) {
-        const size_t bytes = src->kind == YTGPU_FLAGS_DICTIONARY_ZERO ? (size_t)src->data_count * 4 : (size_t)((src->data_count + 7) >> 3);
-        YTGPU_TRY(st->data.allocate(ctx, bytes));
-        YTGPU_TRY(copy_in(ctx, st->data.p, src->data, bytes, YTGPU_MEM_HOST));
-        st->dev.data = st->data.p;
-        if (src->rle_indexes) {
-            if (src->rle_indexes[0] != 0) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "rle_indexes[0] != 0");
-            YTGPU_TRY(st->rle.allocate(ctx, src->rle_count));
-            YTGPU_TRY(copy_in(ctx, st->rle.p, src->rle_indexes, (size_t)src->rle_count * 8, YTGPU_MEM_HOST));
-            st->dev.rle = st->rle.p;
-        }
+        if (src->rle_indexes && src->rle_indexes[0] != 0) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "rle_indexes[0] != 0");
     } else if (src->rle_indexes) {
         check_rle_kernel<<<1, 1, 0, ctx->stream>>>(src->rle_indexes, ctx->dev_err);
         YTGPU_CUDA_TRY(cudaGetLastError());
         ctx->count_launch();
     }
+    YTGPU_TRY(st->rle.stage(ctx, src->rle_indexes, src->rle_count, mem));
+    st->dev.kind = src->kind;
+    st->dev.data = st->data.p;
+    st->dev.data_count = src->data_count;
+    st->dev.rle = st->rle.p;
+    st->dev.rle_count = src->rle_indexes ? src->rle_count : 0;
     return Status{};
 }
 
@@ -401,12 +395,9 @@ Status build_map_impl(Context* ctx, const ytgpu_flag_source* src, i64 start, i64
     StagedSource st;
     YTGPU_TRY(stage_source(ctx, src, mem, &st));
     const size_t out_bytes = bitmap ? (size_t)((rows + 7) >> 3) : (size_t)rows;
-    DevBuf<u8> dout;
-    u8* o = dst;
-    if (mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(dout.allocate(ctx, out_bytes));
-        o = dout.p;
-    }
+    OutBuf<u8> out;
+    YTGPU_TRY(out.prepare(ctx, dst, out_bytes, mem));
+    u8* o = out.p;
     {
         KernelTimer t(ctx, KC_DECODE);
         const bool rle = st.dev.rle != nullptr;
@@ -433,7 +424,7 @@ Status build_map_impl(Context* ctx, const ytgpu_flag_source* src, i64 start, i64
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
     if (mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(copy_out(ctx, dst, o, out_bytes, YTGPU_MEM_HOST));
+        YTGPU_TRY(out.download(ctx, out_bytes));
         YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     } else if (st.dev.rle) {
         Status s = check_device_errors(ctx);  // rle_indexes[0] != 0 on the device
@@ -538,22 +529,18 @@ int ytgpu_build_dictionary_indexes(ytgpu_context* h, const uint32_t* dictionary_
             src.data_count = 0;
             YTGPU_TRY(stage_source(ctx, &src, mem, &st));
         }
-        DevBuf<u32> dout;
-        u32* o = dst;
-        if (mem == YTGPU_MEM_HOST) {
-            YTGPU_TRY(dout.allocate(ctx, rows));
-            o = dout.p;
-        }
+        OutBuf<u32> o;
+        YTGPU_TRY(o.prepare(ctx, dst, rows, mem));
         {
             KernelTimer t(ctx, KC_DECODE);
             const u32* idx = dictionary_indexes ? static_cast<const u32*>(st.dev.data) : nullptr;
             if (st.dev.rle) rle_dict_indexes_kernel<<<grid_for((rows + 127) / 128, 8), 256, 0, ctx->stream>>>(idx, st.dev.rle, st.dev.rle_count,
-                                                                                                            (u64)start_index, (u64)end_index, o);
-            else dict_minus_one_kernel<<<grid_for(rows, 256 * 4), 256, 0, ctx->stream>>>(idx + start_index, rows, o);
+                                                                                                            (u64)start_index, (u64)end_index, o.p);
+            else dict_minus_one_kernel<<<grid_for(rows, 256 * 4), 256, 0, ctx->stream>>>(idx + start_index, rows, o.p);
             YTGPU_CUDA_TRY(cudaGetLastError());
         }
         if (mem == YTGPU_MEM_HOST) {
-            YTGPU_TRY(copy_out(ctx, dst, o, (size_t)rows * 4, YTGPU_MEM_HOST));
+            YTGPU_TRY(o.download(ctx, rows));
             YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
         } else if (st.dev.rle) {
             Status s = check_device_errors(ctx);
@@ -584,13 +571,9 @@ int ytgpu_count_total_string_length(ytgpu_context* h, const uint32_t* dictionary
         YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
         StagedSource st;
         YTGPU_TRY(stage_source(ctx, &src, mem, &st));
-        DevBuf<i32> dlen;
-        const i32* lengths = string_lengths;
-        if (mem == YTGPU_MEM_HOST) {
-            YTGPU_TRY(dlen.allocate(ctx, string_count));
-            YTGPU_TRY(copy_in(ctx, dlen.p, string_lengths, (size_t)string_count * 4, YTGPU_MEM_HOST));
-            lengths = dlen.p;
-        }
+        InBuf<i32> dlen;
+        YTGPU_TRY(dlen.stage(ctx, string_lengths, string_count, mem));
+        const i32* lengths = dlen.p;
         static const i32 kNoLengths = 0;
         if (!lengths) lengths = &kNoLengths;  // never read: every index is out of range and reported
         const u64 s = (u64)start_index, e = (u64)end_index;
@@ -612,31 +595,24 @@ int ytgpu_translate_rle_indexes(ytgpu_context* h, const uint64_t* rle_indexes, u
         if (count == 0) return Status{};
         if (!indexes || !out) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null argument");
         YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
-        DevBuf<u64> drle;
-        DevBuf<i64> din, dout;
-        const u64* r = rle_indexes;
-        const i64* q = indexes;
-        i64* o = out;
         if (mem == YTGPU_MEM_HOST) {
             if (rle_indexes[0] != 0) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "rle_indexes[0] != 0");
             for (u64 j = 0; j < count; ++j)
                 if (indexes[j] < 0) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "negative index");
-            YTGPU_TRY(drle.allocate(ctx, rle_count));
-            YTGPU_TRY(din.allocate(ctx, count));
-            YTGPU_TRY(dout.allocate(ctx, count));
-            YTGPU_TRY(copy_in(ctx, drle.p, rle_indexes, (size_t)rle_count * 8, YTGPU_MEM_HOST));
-            YTGPU_TRY(copy_in(ctx, din.p, indexes, (size_t)count * 8, YTGPU_MEM_HOST));
-            r = drle.p;
-            q = din.p;
-            o = dout.p;
         }
+        InBuf<u64> r;
+        InBuf<i64> q;
+        OutBuf<i64> o;
+        YTGPU_TRY(r.stage(ctx, rle_indexes, rle_count, mem));
+        YTGPU_TRY(q.stage(ctx, indexes, count, mem));
+        YTGPU_TRY(o.prepare(ctx, out, count, mem));
         {
             KernelTimer t(ctx, KC_DECODE);
-            translate_rle_kernel<<<grid_for(count, 256), 256, 0, ctx->stream>>>(r, rle_count, q, count, end_flavour, o);
+            translate_rle_kernel<<<grid_for(count, 256), 256, 0, ctx->stream>>>(r.p, rle_count, q.p, count, end_flavour, o.p);
             YTGPU_CUDA_TRY(cudaGetLastError());
         }
         if (mem == YTGPU_MEM_HOST) {
-            YTGPU_TRY(copy_out(ctx, out, o, (size_t)count * 8, YTGPU_MEM_HOST));
+            YTGPU_TRY(o.download(ctx, count));
             YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
         }
         return Status{};

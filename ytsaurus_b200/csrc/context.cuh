@@ -131,6 +131,55 @@ inline Status copy_out(Context* ctx, void* dst, const void* src_dev, size_t byte
     return Status{};
 }
 
+// A caller's input in `mem` space, readable on the device: the caller's pointer unless `mem` is HOST, in which case a
+// device copy uploaded on the context stream. A null pointer stays null. `tail` zeroed elements after the copy let kernels
+// read whole words past the end of the input.
+template <class T>
+struct InBuf {
+    DevBuf<T> buf;
+    const T* p = nullptr;
+    Status stage(Context* ctx, const T* src, size_t count, int mem, size_t tail = 0) {
+        p = src;
+        if (mem != YTGPU_MEM_HOST || !src) return Status{};
+        YTGPU_TRY(buf.allocate(ctx, count + tail));
+        if (tail) YTGPU_CUDA_TRY(cudaMemsetAsync(buf.p + count, 0, tail * sizeof(T), ctx->stream));
+        YTGPU_TRY(copy_in(ctx, buf.p, src, count * sizeof(T), YTGPU_MEM_HOST));
+        p = buf.p;
+        return Status{};
+    }
+};
+
+// A caller's output in `mem` space, written on the device: the caller's buffer unless `mem` is HOST, in which case a
+// device scratch buffer that download() copies into the caller's. A null pointer stays null. The copy is asynchronous:
+// the caller synchronises the stream before it returns.
+template <class T>
+struct OutBuf {
+    DevBuf<T> buf;
+    T* dst = nullptr;
+    T* p = nullptr;
+    Status prepare(Context* ctx, T* out, size_t count, int mem) {
+        dst = p = out;
+        if (mem != YTGPU_MEM_HOST || !out) return Status{};
+        YTGPU_TRY(buf.allocate(ctx, count));
+        p = buf.p;
+        return Status{};
+    }
+    Status download(Context* ctx, size_t count) {
+        if (p == dst) return Status{};
+        return copy_out(ctx, dst, p, count * sizeof(T), YTGPU_MEM_HOST);
+    }
+};
+
+// A rowset's values and string heap, readable on the device (see InBuf).
+struct StagedRowset {
+    InBuf<ytgpu_value> values;
+    InBuf<u8> heap;
+    Status stage(Context* ctx, const ytgpu_rowset_view* r, int mem) {
+        YTGPU_TRY(values.stage(ctx, r->values, r->row_count * r->value_count, mem));
+        return heap.stage(ctx, r->string_heap, r->string_heap_bytes, mem);
+    }
+};
+
 inline int fill_error(ytgpu_error* err, const Status& s) {
     if (err) {
         err->code = s.code;

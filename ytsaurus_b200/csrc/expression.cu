@@ -1651,21 +1651,20 @@ Status evaluate_expression_impl(Context* ctx, const ytgpu_column_view* columns, 
 
     const u64 words = (n + 63) / 64 * 2;  // 32-bit bitmap words
     const bool host = out_mem == YTGPU_MEM_HOST;
-    DevBuf<u64> tvalues, tstarts, scan_sums;
-    DevBuf<u32> tnulls, tselection, tlengths;
+    DevBuf<u64> tstarts, scan_sums;
+    DevBuf<u32> tlengths;
     DevBuf<u8> tnull_bytes, theap;
     DevBuf<unsigned long long> result;
+    InBuf<u32> dselection;
+    OutBuf<u64> values;
+    OutBuf<u32> nulls;
     u64* dvalues = out_values;
     u32* dnulls = reinterpret_cast<u32*>(out_null_bitmap);
-    const u32* dselection = reinterpret_cast<const u32*>(selection);
-    if (host && selection) {
-        YTGPU_TRY(tselection.allocate(ctx, words));
-        YTGPU_TRY(copy_in(ctx, tselection.p, selection, words * 4, YTGPU_MEM_HOST));
-        dselection = tselection.p;
-    }
+    YTGPU_TRY(dselection.stage(ctx, reinterpret_cast<const u32*>(selection), words, out_mem));
     u64* dstarts = nullptr;
     u32* dlengths = nullptr;
     u8* dnull_bytes = nullptr;
+    // A string result is sized in one pass and filled in a second, so its scratch depends on more than out_mem.
     if (string_result) {  // the size pass writes the caller's DEVICE outputs only when they are filled too
         const bool direct = !host && sr->heap;
         dstarts = direct ? sr->starts : nullptr;
@@ -1680,11 +1679,11 @@ Status evaluate_expression_impl(Context* ctx, const ytgpu_column_view* columns, 
             dnull_bytes = tnull_bytes.p;
         }
         YTGPU_TRY(scan_sums.allocate(ctx, scan_block_count(n)));
-    } else if (host) {
-        YTGPU_TRY(tvalues.allocate(ctx, n));
-        YTGPU_TRY(tnulls.allocate(ctx, words));
-        dvalues = tvalues.p;
-        dnulls = tnulls.p;
+    } else {
+        YTGPU_TRY(values.prepare(ctx, out_values, n, out_mem));
+        YTGPU_TRY(nulls.prepare(ctx, dnulls, words, out_mem));
+        dvalues = values.p;
+        dnulls = nulls.p;
     }
     YTGPU_TRY(result.allocate(ctx, 3));
     YTGPU_CUDA_TRY(cudaMemsetAsync(result.p, 0, 24, ctx->stream));
@@ -1694,7 +1693,7 @@ Status evaluate_expression_impl(Context* ctx, const ytgpu_column_view* columns, 
     A.node_count = (u32)P.nodes.size();
     A.columns = blob.at<ColumnDev>(o_cols);
     A.column_count = (u32)cols.scalars.size();
-    A.selection = dselection;
+    A.selection = dselection.p;
     A.n = n;
     A.values = dvalues;
     A.nulls = dnulls;
@@ -1751,10 +1750,8 @@ Status evaluate_expression_impl(Context* ctx, const ytgpu_column_view* columns, 
     }
     unsigned long long res[3] = {0, 0, 0};  // the one host read: NULL count, error bits and the heap size
     YTGPU_CUDA_TRY(cudaMemcpyAsync(res, result.p, string_result ? 24 : 16, cudaMemcpyDeviceToHost, ctx->stream));
-    if (host && !string_result) {
-        YTGPU_TRY(copy_out(ctx, out_values, dvalues, n * 8, YTGPU_MEM_HOST));
-        YTGPU_TRY(copy_out(ctx, out_null_bitmap, dnulls, words * 4, YTGPU_MEM_HOST));
-    }
+    YTGPU_TRY(values.download(ctx, n));
+    YTGPU_TRY(nulls.download(ctx, words));
     YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     if (res[1] & kErrOutOfHeap) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "a string value of an expression column leaves its heap");
     if (res[1] & kErrNonAscii)

@@ -383,19 +383,15 @@ Status evaluate_filter_impl(Context* ctx, const ytgpu_column_view* columns, u32 
     const u64 words = (n + 63) / 64 * 2;  // 32-bit bitmap words
     const bool host = out_mem == YTGPU_MEM_HOST;
     DevBuf<u32> tbitmap;
-    DevBuf<u8> tbytemap;
     DevBuf<u64> word_counts, scan_sums, scan_total;
     DevBuf<unsigned long long> result;
     u32* dbitmap = reinterpret_cast<u32*>(out_bitmap);
-    if (!out_bitmap || host) {
+    if (!out_bitmap || host) {  // the kernel writes the bitmap even when the caller asks for none
         YTGPU_TRY(tbitmap.allocate(ctx, words));
         dbitmap = tbitmap.p;
     }
-    u8* dbytemap = out_bytemap;
-    if (out_bytemap && host) {
-        YTGPU_TRY(tbytemap.allocate(ctx, n));
-        dbytemap = tbytemap.p;
-    }
+    OutBuf<u8> bytemap;
+    YTGPU_TRY(bytemap.prepare(ctx, out_bytemap, n, out_mem));
     if (out_rows) YTGPU_TRY(word_counts.allocate(ctx, words));
     YTGPU_TRY(result.allocate(ctx, 2));
     YTGPU_CUDA_TRY(cudaMemsetAsync(result.p, 0, 16, ctx->stream));
@@ -417,9 +413,9 @@ Status evaluate_filter_impl(Context* ctx, const ytgpu_column_view* columns, u32 
     A.pattern_bytes = (u32)((P.patterns.size() + 15) & ~(size_t)15);  // staged in 16-byte units, as the blob pads them
     A.n = n;
     A.bitmap = dbitmap;
-    A.bytemap = dbytemap;
+    A.bytemap = bytemap.p;
     A.word_counts = out_rows ? word_counts.p : nullptr;
-    A.bytemap_vec = dbytemap && (reinterpret_cast<uintptr_t>(dbytemap) & 15) == 0;
+    A.bytemap_vec = bytemap.p && (reinterpret_cast<uintptr_t>(bytemap.p) & 15) == 0;
     A.result = result.p;
     // shared memory in the kernel's order; every part is a multiple of 8 bytes (NodeDev 24, ColumnDev / StringDev 8-aligned)
     const bool patterns = !P.patterns.empty();
@@ -447,25 +443,21 @@ Status evaluate_filter_impl(Context* ctx, const ytgpu_column_view* columns, u32 
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "%llu rows selected, rows_capacity is %llu", (unsigned long long)selected,
                            (unsigned long long)rows_capacity);
 
-    DevBuf<u32> trows;
+    OutBuf<u32> rows;
     if (out_rows && selected) {
-        u32* drows = out_rows;
-        if (host) {
-            YTGPU_TRY(trows.allocate(ctx, selected));
-            drows = trows.p;
-        }
+        YTGPU_TRY(rows.prepare(ctx, out_rows, selected, out_mem));
         YTGPU_TRY(scan_sums.allocate(ctx, scan_block_count(words)));
         YTGPU_TRY(scan_total.allocate(ctx, 1));
         {
             KernelTimer t(ctx, KC_DECODE, 4);
             exclusive_scan_u64(ctx->stream, word_counts.p, words, scan_sums.p, scan_total.p);
-            filter_rows_kernel<<<blocks, kFilterThreads, 0, ctx->stream>>>(dbitmap, word_counts.p, words, drows);
+            filter_rows_kernel<<<blocks, kFilterThreads, 0, ctx->stream>>>(dbitmap, word_counts.p, words, rows.p);
             YTGPU_CUDA_TRY(cudaGetLastError());
         }
-        if (host) YTGPU_TRY(copy_out(ctx, out_rows, drows, selected * 4, YTGPU_MEM_HOST));
+        YTGPU_TRY(rows.download(ctx, selected));
     }
     if (host && out_bitmap) YTGPU_TRY(copy_out(ctx, out_bitmap, dbitmap, words * 4, YTGPU_MEM_HOST));
-    if (host && out_bytemap) YTGPU_TRY(copy_out(ctx, out_bytemap, dbytemap, n, YTGPU_MEM_HOST));
+    YTGPU_TRY(bytemap.download(ctx, n));
     if (host) YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return Status{};
 }

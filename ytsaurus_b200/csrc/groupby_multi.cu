@@ -576,64 +576,42 @@ Status groupby_multi_impl(Context* ctx, const ytgpu_column_view* key_columns, u3
     YTGPU_TRY(radix_sort_chunks(ctx, cptr, 1, g, &scratch, &perm));
     YTGPU_TRY(slot_sorted.allocate(ctx, g));
 
-    const bool host = out_mem == YTGPU_MEM_HOST;
-    std::vector<DevBuf<u64>> tk(key_count), tv(aggregate_count);
-    std::vector<DevBuf<u8>> tkn(key_count), tvn(aggregate_count);
-    DevBuf<u64> tcounts, tfirst;
+    std::vector<OutBuf<u64>> tk(key_count), tv(aggregate_count);
+    std::vector<OutBuf<u8>> tkn(key_count), tvn(aggregate_count);
+    OutBuf<u64> tcounts, tfirst;
     KeyOutputs O{};
     for (u32 k = 0; k < key_count; ++k) {
         if (!out->keys[k] || !out->key_null[k]) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null key output %u", k);
-        O.keys[k] = out->keys[k];
-        O.key_null[k] = out->key_null[k];
-        if (host) {
-            YTGPU_TRY(tk[k].allocate(ctx, g));
-            YTGPU_TRY(tkn[k].allocate(ctx, g));
-            O.keys[k] = tk[k].p;
-            O.key_null[k] = tkn[k].p;
-        }
+        YTGPU_TRY(tk[k].prepare(ctx, out->keys[k], g, out_mem));
+        YTGPU_TRY(tkn[k].prepare(ctx, out->key_null[k], g, out_mem));
+        O.keys[k] = tk[k].p;
+        O.key_null[k] = tkn[k].p;
     }
-    u64 *dcounts = out->counts, *dfirst = out->first_rows;
-    if (host && out->counts) {
-        YTGPU_TRY(tcounts.allocate(ctx, g));
-        dcounts = tcounts.p;
-    }
-    if (host && out->first_rows) {
-        YTGPU_TRY(tfirst.allocate(ctx, g));
-        dfirst = tfirst.p;
-    }
+    YTGPU_TRY(tcounts.prepare(ctx, out->counts, g, out_mem));
+    YTGPU_TRY(tfirst.prepare(ctx, out->first_rows, g, out_mem));
     const u32 gblocks = (u32)((g + threads - 1) / threads);
-    mg_emit_keys_kernel<<<gblocks, threads, 0, ctx->stream>>>(K, perm.plan, perm.idx[0], perm.idx[1], g, cslot.p, T.first.p, T.counts.p, O, dcounts,
-                                                             dfirst, slot_sorted.p);
+    mg_emit_keys_kernel<<<gblocks, threads, 0, ctx->stream>>>(K, perm.plan, perm.idx[0], perm.idx[1], g, cslot.p, T.first.p, T.counts.p, O, tcounts.p,
+                                                             tfirst.p, slot_sorted.p);
     ctx->count_launch();
     for (u32 a = 0; a < aggregate_count; ++a) {
         if (!out->values[a] || !out->value_null[a]) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null aggregate output %u", a);
-        u64* dv = out->values[a];
-        u8* dn = out->value_null[a];
-        if (host) {
-            YTGPU_TRY(tv[a].allocate(ctx, g));
-            YTGPU_TRY(tvn[a].allocate(ctx, g));
-            dv = tv[a].p;
-            dn = tvn[a].p;
-        }
+        YTGPU_TRY(tv[a].prepare(ctx, out->values[a], g, out_mem));
+        YTGPU_TRY(tvn[a].prepare(ctx, out->value_null[a], g, out_mem));
         const ytgpu_aggregate& A = aggregates[a];
         const bool row_result = is_string(A.column) && A.op != YTGPU_AGG_COUNT;
         const ColumnDev col = is_string(A.column) ? ColumnDev{} : sv[A.column].dev;
-        mg_finalize_kernel<<<gblocks, threads, 0, ctx->stream>>>(A.op, col, 0, g, slot_sorted.p, states[a], dv, dn, row_result);
+        mg_finalize_kernel<<<gblocks, threads, 0, ctx->stream>>>(A.op, col, 0, g, slot_sorted.p, states[a], tv[a].p, tvn[a].p, row_result);
         ctx->count_launch();
-        if (host) {
-            YTGPU_TRY(copy_out(ctx, out->values[a], dv, g * 8, YTGPU_MEM_HOST));
-            YTGPU_TRY(copy_out(ctx, out->value_null[a], dn, g, YTGPU_MEM_HOST));
-        }
+        YTGPU_TRY(tv[a].download(ctx, g));
+        YTGPU_TRY(tvn[a].download(ctx, g));
     }
     YTGPU_CUDA_TRY(cudaGetLastError());
-    if (host) {
-        for (u32 k = 0; k < key_count; ++k) {
-            YTGPU_TRY(copy_out(ctx, out->keys[k], O.keys[k], g * 8, YTGPU_MEM_HOST));
-            YTGPU_TRY(copy_out(ctx, out->key_null[k], O.key_null[k], g, YTGPU_MEM_HOST));
-        }
-        if (out->counts) YTGPU_TRY(copy_out(ctx, out->counts, dcounts, g * 8, YTGPU_MEM_HOST));
-        if (out->first_rows) YTGPU_TRY(copy_out(ctx, out->first_rows, dfirst, g * 8, YTGPU_MEM_HOST));
+    for (u32 k = 0; k < key_count; ++k) {
+        YTGPU_TRY(tk[k].download(ctx, g));
+        YTGPU_TRY(tkn[k].download(ctx, g));
     }
+    YTGPU_TRY(tcounts.download(ctx, g));
+    YTGPU_TRY(tfirst.download(ctx, g));
     YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return Status{};
 }

@@ -466,7 +466,7 @@ Status probe_table(Context* ctx, const JoinTable& J, const KeyColumns& KP, bool 
             YTGPU_CUDA_TRY(cudaGetLastError());
         }
         // the list has at most np rows: with that much DEVICE capacity it goes straight to the output, and the count is
-        // the one read-back
+        // the one read-back; with less, it is staged and copied out once its length is known, in either memory space
         DevBuf<u32> staged;
         u32* dst = out_primary;
         if (out_primary && (host || capacity < np)) {
@@ -526,25 +526,18 @@ Status probe_table(Context* ctx, const JoinTable& J, const KeyColumns& KP, bool 
     if (!J.listed) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "the table was built without its per-key row lists");
 
     // step 5
-    DevBuf<u32> tp, tf;
-    u32 *dp = out_primary, *df = out_foreign;
-    if (host) {
-        YTGPU_TRY(tp.allocate(ctx, pairs));
-        YTGPU_TRY(tf.allocate(ctx, pairs));
-        dp = tp.p;
-        df = tf.p;
-    }
+    OutBuf<u32> dp, df;
+    YTGPU_TRY(dp.prepare(ctx, out_primary, pairs, out_mem));
+    YTGPU_TRY(df.prepare(ctx, out_foreign, pairs, out_mem));
     {
         KernelTimer t(ctx, KC_JOIN);
         const u64 tiles = (pairs + kWriteTile - 1) / kWriteTile;
         hj_write_pairs_kernel<<<(u32)tiles, kWriteThreads, 0, ctx->stream>>>(offsets.p, np, pairs, probe_slot.p, J.slot_start.p,
-                                                                             J.rows_by_slot.p, dp, df);
+                                                                             J.rows_by_slot.p, dp.p, df.p);
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
-    if (host) {
-        YTGPU_TRY(copy_out(ctx, out_primary, dp, pairs * 4, YTGPU_MEM_HOST));
-        YTGPU_TRY(copy_out(ctx, out_foreign, df, pairs * 4, YTGPU_MEM_HOST));
-    }
+    YTGPU_TRY(dp.download(ctx, pairs));
+    YTGPU_TRY(df.download(ctx, pairs));
     YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return Status{};
 }
@@ -687,18 +680,6 @@ Status join_table_probe_impl(Context* ctx, const JoinTable* J, const ytgpu_colum
     return probe_table(ctx, *J, KP, primary_direct, np, kind, out_primary, out_foreign, capacity, out_count, out_mem, string_count != 0);
 }
 
-// The row indexes of a gather, on the device.
-Status stage_rows(Context* ctx, const u32* rows, u64 count, int mem, DevBuf<u32>* staged, const u32** dev) {
-    if (mem != YTGPU_MEM_HOST) {
-        *dev = rows;
-        return Status{};
-    }
-    YTGPU_TRY(staged->allocate(ctx, count));
-    YTGPU_TRY(copy_in(ctx, staged->p, rows, count * 4, YTGPU_MEM_HOST));
-    *dev = staged->p;
-    return Status{};
-}
-
 Status gather_column_impl(Context* ctx, const ytgpu_column_view* column, const u32* rows, u64 count, u64* out_values, u8* out_null_bitmap,
                           u64* out_null_count, int out_mem) {
     if (!column) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null column");
@@ -712,33 +693,23 @@ Status gather_column_impl(Context* ctx, const ytgpu_column_view* column, const u
     if (count == 0) return Status{};
     StagedColumn sc;
     YTGPU_TRY(stage_column(ctx, column, &sc));
-    DevBuf<u32> staged_rows;
-    const u32* drows = nullptr;
-    YTGPU_TRY(stage_rows(ctx, rows, count, out_mem, &staged_rows, &drows));
+    InBuf<u32> drows;
+    YTGPU_TRY(drows.stage(ctx, rows, count, out_mem));  // the row indexes live in out_mem
     const u64 words = (count + 63) / 64;
-    const bool host = out_mem == YTGPU_MEM_HOST;
-    DevBuf<u64> tv, tb;
+    OutBuf<u64> dv, db;
     DevBuf<unsigned long long> nulls;
-    u64* dv = out_values;
-    u32* db = reinterpret_cast<u32*>(out_null_bitmap);
-    if (host) {
-        YTGPU_TRY(tv.allocate(ctx, count));
-        YTGPU_TRY(tb.allocate(ctx, words));
-        dv = tv.p;
-        db = reinterpret_cast<u32*>(tb.p);
-    }
+    YTGPU_TRY(dv.prepare(ctx, out_values, count, out_mem));
+    YTGPU_TRY(db.prepare(ctx, reinterpret_cast<u64*>(out_null_bitmap), words, out_mem));
     YTGPU_TRY(nulls.allocate(ctx, 1));
     YTGPU_CUDA_TRY(cudaMemsetAsync(nulls.p, 0, 8, ctx->stream));
     {
         KernelTimer t(ctx, KC_JOIN);
-        hj_gather_kernel<<<blocks_for(words * 64, 256, 16), 256, 0, ctx->stream>>>(sc.dev, (u64)column->value_count, drows, count, dv, db,
-                                                                                   nulls.p, ctx->dev_err);
+        hj_gather_kernel<<<blocks_for(words * 64, 256, 16), 256, 0, ctx->stream>>>(sc.dev, (u64)column->value_count, drows.p, count, dv.p,
+                                                                                   reinterpret_cast<u32*>(db.p), nulls.p, ctx->dev_err);
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
-    if (host) {
-        YTGPU_TRY(copy_out(ctx, out_values, dv, count * 8, YTGPU_MEM_HOST));
-        YTGPU_TRY(copy_out(ctx, out_null_bitmap, db, words * 8, YTGPU_MEM_HOST));
-    }
+    YTGPU_TRY(dv.download(ctx, count));
+    YTGPU_TRY(db.download(ctx, words));
     unsigned long long null_count = 0;
     YTGPU_CUDA_TRY(cudaMemcpyAsync(&null_count, nulls.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
     YTGPU_TRY(check_device_errors(ctx));  // synchronises
@@ -760,53 +731,30 @@ Status gather_string_column_impl(Context* ctx, const ytgpu_string_column* column
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
     if (count == 0) return Status{};
     // the heap is never read: only starts, lengths and the null bytemap move
-    DevBuf<u64> cs;
-    DevBuf<u32> cl;
-    DevBuf<u8> cn;
-    const u64* ds = column->starts;
-    const u32* dl = column->lengths;
-    const u8* dn = column->null_bytemap;
-    if (column->mem == YTGPU_MEM_HOST && n) {
-        YTGPU_TRY(cs.allocate(ctx, n));
-        YTGPU_TRY(cl.allocate(ctx, n));
-        YTGPU_TRY(copy_in(ctx, cs.p, column->starts, n * 8, YTGPU_MEM_HOST));
-        YTGPU_TRY(copy_in(ctx, cl.p, column->lengths, n * 4, YTGPU_MEM_HOST));
-        ds = cs.p;
-        dl = cl.p;
-        if (dn) {
-            YTGPU_TRY(cn.allocate(ctx, n));
-            YTGPU_TRY(copy_in(ctx, cn.p, column->null_bytemap, n, YTGPU_MEM_HOST));
-            dn = cn.p;
-        }
-    }
-    DevBuf<u32> staged_rows;
-    const u32* drows = nullptr;
-    YTGPU_TRY(stage_rows(ctx, rows, count, out_mem, &staged_rows, &drows));
-    const bool host = out_mem == YTGPU_MEM_HOST;
-    DevBuf<u64> ts;
-    DevBuf<u32> tl;
-    DevBuf<u8> tn;
-    u64* os = out_starts;
-    u32* ol = out_lengths;
-    u8* on = out_null_bytemap;
-    if (host) {
-        YTGPU_TRY(ts.allocate(ctx, count));
-        YTGPU_TRY(tl.allocate(ctx, count));
-        YTGPU_TRY(tn.allocate(ctx, count));
-        os = ts.p;
-        ol = tl.p;
-        on = tn.p;
-    }
+    InBuf<u64> ds;
+    InBuf<u32> dl;
+    InBuf<u8> dn;
+    const int mem = n ? column->mem : YTGPU_MEM_DEVICE;  // no rows: the caller's pointers stay
+    YTGPU_TRY(ds.stage(ctx, column->starts, n, mem));
+    YTGPU_TRY(dl.stage(ctx, column->lengths, n, mem));
+    YTGPU_TRY(dn.stage(ctx, column->null_bytemap, n, mem));
+    InBuf<u32> drows;
+    YTGPU_TRY(drows.stage(ctx, rows, count, out_mem));  // the row indexes live in out_mem
+    OutBuf<u64> os;
+    OutBuf<u32> ol;
+    OutBuf<u8> on;
+    YTGPU_TRY(os.prepare(ctx, out_starts, count, out_mem));
+    YTGPU_TRY(ol.prepare(ctx, out_lengths, count, out_mem));
+    YTGPU_TRY(on.prepare(ctx, out_null_bytemap, count, out_mem));
     {
         KernelTimer t(ctx, KC_JOIN);
-        hj_gather_strings_kernel<<<blocks_for(count, 256, 16), 256, 0, ctx->stream>>>(ds, dl, dn, n, drows, count, os, ol, on, ctx->dev_err);
+        hj_gather_strings_kernel<<<blocks_for(count, 256, 16), 256, 0, ctx->stream>>>(ds.p, dl.p, dn.p, n, drows.p, count, os.p, ol.p, on.p,
+                                                                                       ctx->dev_err);
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
-    if (host) {
-        YTGPU_TRY(copy_out(ctx, out_starts, os, count * 8, YTGPU_MEM_HOST));
-        YTGPU_TRY(copy_out(ctx, out_lengths, ol, count * 4, YTGPU_MEM_HOST));
-        YTGPU_TRY(copy_out(ctx, out_null_bytemap, on, count, YTGPU_MEM_HOST));
-    }
+    YTGPU_TRY(os.download(ctx, count));
+    YTGPU_TRY(ol.download(ctx, count));
+    YTGPU_TRY(on.download(ctx, count));
     return check_device_errors(ctx);  // synchronises
 }
 

@@ -459,7 +459,7 @@ struct PartitionRun {
     bool key_words = false;  // the layout does not fit kMaxKeyChunks: partition_words_kernel over `wbounds`
     WordBounds wbounds{};
     DevBuf<unsigned long long> hist;
-    DevBuf<i32> index;
+    OutBuf<i32> index;
     DevBuf<u64> chunk;
 };
 
@@ -550,7 +550,8 @@ Status prepare_params(Context* ctx, const ytgpu_partition_spec* spec, bool fixed
 }
 
 Status finish_outputs(Context* ctx, PartitionRun& run, u64 n, u32 Pn, i32* out_index, u64* out_histogram, int out_mem) {
-    if (out_index && out_mem == YTGPU_MEM_HOST) YTGPU_TRY(copy_out(ctx, out_index, run.index.p, n * 4, YTGPU_MEM_HOST));
+    YTGPU_TRY(run.index.download(ctx, n));
+    // the kernels count into a zeroed scratch histogram, which is copied out in either memory space
     if (out_histogram) YTGPU_TRY(copy_out(ctx, out_histogram, run.hist.p, (size_t)Pn * 8, out_mem));
     return Status{};
 }
@@ -562,25 +563,16 @@ Status partition_rowset_impl(Context* ctx, const ytgpu_rowset_view* in, const yt
     if (!in) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null rowset");
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
     const u64 n = in->row_count;
-    DevBuf<ytgpu_value> vstage;
-    DevBuf<u8> hstage;
-    const ytgpu_value* vals = in->values;
-    const u8* heap = in->string_heap;
-    if (in->mem == YTGPU_MEM_HOST && n) {
-        YTGPU_TRY(vstage.allocate(ctx, n * in->value_count));
-        YTGPU_TRY(copy_in(ctx, vstage.p, in->values, n * in->value_count * 16, YTGPU_MEM_HOST));
-        YTGPU_TRY(hstage.allocate(ctx, in->string_heap_bytes));
-        YTGPU_TRY(copy_in(ctx, hstage.p, in->string_heap, in->string_heap_bytes, YTGPU_MEM_HOST));
-        vals = vstage.p;
-        heap = hstage.p;
-    }
+    StagedRowset staged;
+    YTGPU_TRY(staged.stage(ctx, in, n ? in->mem : YTGPU_MEM_DEVICE));  // no rows: the caller's pointers stay
+    const ytgpu_value* vals = staged.values.p;
     PartParams P;
     PartitionRun run;
     YTGPU_TRY(prepare_params(ctx, spec, false, in->value_count, vals, n, &P, &run));
     ctx->last_partition_key_words = run.key_words;
     P.values = vals;
     P.value_count = in->value_count;
-    P.heap = heap;
+    P.heap = staged.heap.p;
     P.n = n;
     const u32 Pn = P.partition_count;
     if (out_histogram) {
@@ -588,14 +580,8 @@ Status partition_rowset_impl(Context* ctx, const ytgpu_rowset_view* in, const yt
         YTGPU_CUDA_TRY(cudaMemsetAsync(run.hist.p, 0, (size_t)Pn * 8, ctx->stream));
         P.histogram = run.hist.p;
     }
-    if (out_index) {
-        if (out_mem == YTGPU_MEM_HOST) {
-            YTGPU_TRY(run.index.allocate(ctx, n));
-            P.out_index = run.index.p;
-        } else {
-            P.out_index = out_index;
-        }
-    }
+    YTGPU_TRY(run.index.prepare(ctx, out_index, n, out_mem));
+    P.out_index = run.index.p;
     const bool slabs = (out_slab_values || out_slab_perm) && n;
     if (slabs) {
         YTGPU_TRY(run.chunk.allocate(ctx, n));
@@ -610,25 +596,17 @@ Status partition_rowset_impl(Context* ctx, const ytgpu_rowset_view* in, const yt
         const u64* cptr[1] = {run.chunk.p};
         YTGPU_TRY(radix_sort_chunks(ctx, cptr, 1, n, &scratch, &perm));
         const u32 rb = in->value_count * 16;
-        DevBuf<u8> vout;
-        DevBuf<u32> pout;
+        OutBuf<u8> vout;
+        OutBuf<u32> pout;
         if (out_slab_values) {
-            u8* dst = reinterpret_cast<u8*>(out_slab_values);
-            if (out_mem == YTGPU_MEM_HOST) {
-                YTGPU_TRY(vout.allocate(ctx, n * rb));
-                dst = vout.p;
-            }
-            YTGPU_TRY(gather_rows(ctx, reinterpret_cast<const u8*>(vals), perm, dst, n, rb));
-            if (out_mem == YTGPU_MEM_HOST) YTGPU_TRY(copy_out(ctx, out_slab_values, dst, n * rb, YTGPU_MEM_HOST));
+            YTGPU_TRY(vout.prepare(ctx, reinterpret_cast<u8*>(out_slab_values), n * rb, out_mem));
+            YTGPU_TRY(gather_rows(ctx, reinterpret_cast<const u8*>(vals), perm, vout.p, n, rb));
+            YTGPU_TRY(vout.download(ctx, n * rb));
         }
         if (out_slab_perm) {
-            u32* dst = out_slab_perm;
-            if (out_mem == YTGPU_MEM_HOST) {
-                YTGPU_TRY(pout.allocate(ctx, n));
-                dst = pout.p;
-            }
-            YTGPU_TRY(materialize_perm(ctx, perm, n, dst));
-            if (out_mem == YTGPU_MEM_HOST) YTGPU_TRY(copy_out(ctx, out_slab_perm, dst, n * 4, YTGPU_MEM_HOST));
+            YTGPU_TRY(pout.prepare(ctx, out_slab_perm, n, out_mem));
+            YTGPU_TRY(materialize_perm(ctx, perm, n, pout.p));
+            YTGPU_TRY(pout.download(ctx, n));
         }
         if (out_mem == YTGPU_MEM_HOST) YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));  // the staging buffers die here
     }
@@ -643,20 +621,16 @@ Status partition_fixed_impl(Context* ctx, const ytgpu_fixed_rows_view* in, const
     const u64 n = in->row_count;
     const u32 rb = in->row_bytes;
     if (rb == 0 || rb % 16 != 0) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "row_bytes (%u) must be a positive multiple of 16", rb);
-    DevBuf<u8> rstage, ostage;
-    const u8* rows = in->rows;
-    if (in->mem == YTGPU_MEM_HOST && n) {
-        YTGPU_TRY(rstage.allocate(ctx, n * rb));
-        YTGPU_TRY(copy_in(ctx, rstage.p, in->rows, n * rb, YTGPU_MEM_HOST));
-        rows = rstage.p;
-    }
+    InBuf<u8> rows;
+    YTGPU_TRY(rows.stage(ctx, in->rows, n * rb, n ? in->mem : YTGPU_MEM_DEVICE));  // no rows: the caller's pointer stays
+    OutBuf<u8> slabs;
     PartParams P;
     PartitionRun run;
     YTGPU_TRY(prepare_params(ctx, spec, true, 0, nullptr, n, &P, &run));
     for (u32 c = 0; c < P.layout.ncols; ++c)
         if ((u64)P.layout.col[c].index + P.layout.col[c].payload_bytes > rb)
             return make_status(YTGPU_ERR_INVALID_ARGUMENT, "key column %u exceeds the row", c);
-    P.rows = rows;
+    P.rows = rows.p;
     P.row_bytes = rb;
     P.n = n;
     const u32 Pn = P.partition_count;
@@ -665,14 +639,8 @@ Status partition_fixed_impl(Context* ctx, const ytgpu_fixed_rows_view* in, const
         YTGPU_CUDA_TRY(cudaMemsetAsync(run.hist.p, 0, (size_t)Pn * 8, ctx->stream));
         P.histogram = run.hist.p;
     }
-    if (out_index) {
-        if (out_mem == YTGPU_MEM_HOST) {
-            YTGPU_TRY(run.index.allocate(ctx, n));
-            P.out_index = run.index.p;
-        } else {
-            P.out_index = out_index;
-        }
-    }
+    YTGPU_TRY(run.index.prepare(ctx, out_index, n, out_mem));
+    P.out_index = run.index.p;
     if (out_slab_rows) {
         YTGPU_TRY(run.chunk.allocate(ctx, n));
         P.out_chunk = run.chunk.p;
@@ -684,13 +652,9 @@ Status partition_fixed_impl(Context* ctx, const ytgpu_fixed_rows_view* in, const
         PermRef perm;
         const u64* cptr[1] = {run.chunk.p};
         YTGPU_TRY(radix_sort_chunks(ctx, cptr, 1, n, &scratch, &perm));
-        u8* dst = out_slab_rows;
-        if (out_mem == YTGPU_MEM_HOST) {
-            YTGPU_TRY(ostage.allocate(ctx, n * rb));
-            dst = ostage.p;
-        }
-        YTGPU_TRY(gather_rows(ctx, rows, perm, dst, n, rb));
-        if (out_mem == YTGPU_MEM_HOST) YTGPU_TRY(copy_out(ctx, out_slab_rows, dst, n * rb, YTGPU_MEM_HOST));
+        YTGPU_TRY(slabs.prepare(ctx, out_slab_rows, n * rb, out_mem));
+        YTGPU_TRY(gather_rows(ctx, rows.p, perm, slabs.p, n, rb));
+        YTGPU_TRY(slabs.download(ctx, n * rb));
     }
     YTGPU_TRY(finish_outputs(ctx, run, n, Pn, out_index, out_histogram, out_mem));
     return check_device_errors(ctx);
@@ -719,31 +683,17 @@ Status fingerprint_impl(Context* ctx, const ytgpu_rowset_view* in, u32 k, u64* o
     const u64 n = in->row_count;
     if (n == 0) return Status{};
     k = std::min(k, in->value_count);
-    DevBuf<ytgpu_value> vstage;
-    DevBuf<u8> hstage;
-    DevBuf<u64> ostage;
-    const ytgpu_value* vals = in->values;
-    const u8* heap = in->string_heap;
-    if (in->mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(vstage.allocate(ctx, n * in->value_count));
-        YTGPU_TRY(copy_in(ctx, vstage.p, in->values, n * in->value_count * 16, YTGPU_MEM_HOST));
-        YTGPU_TRY(hstage.allocate(ctx, in->string_heap_bytes));
-        YTGPU_TRY(copy_in(ctx, hstage.p, in->string_heap, in->string_heap_bytes, YTGPU_MEM_HOST));
-        vals = vstage.p;
-        heap = hstage.p;
-    }
-    u64* dst = out;
-    if (out_mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(ostage.allocate(ctx, n));
-        dst = ostage.p;
-    }
+    StagedRowset staged;
+    OutBuf<u64> dst;
+    YTGPU_TRY(staged.stage(ctx, in, in->mem));
+    YTGPU_TRY(dst.prepare(ctx, out, n, out_mem));
     {
         KernelTimer t(ctx, KC_PARTITION);
         u32 blocks = (u32)std::min<u64>((n + 255) / 256, (u64)kNumSms * 8);
-        fingerprint_rows_kernel<<<blocks, 256, 0, ctx->stream>>>(vals, in->value_count, heap, n, k, dst, ctx->dev_err);
+        fingerprint_rows_kernel<<<blocks, 256, 0, ctx->stream>>>(staged.values.p, in->value_count, staged.heap.p, n, k, dst.p, ctx->dev_err);
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
-    if (out_mem == YTGPU_MEM_HOST) YTGPU_TRY(copy_out(ctx, out, dst, n * 8, YTGPU_MEM_HOST));
+    YTGPU_TRY(dst.download(ctx, n));
     return check_device_errors(ctx);
 }
 

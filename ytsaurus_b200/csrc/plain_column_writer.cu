@@ -123,36 +123,21 @@ Status encode_plain_impl(Context* ctx, bool boolean, const void* values, const u
         }
     }
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
-    DevBuf<u8> vstage, nstage;
-    DevBuf<u64> ostage;
-    const void* dv = values;
-    const u8* dn = null_bytemap;
-    const u64 vbytes = boolean ? n : n * 8;
-    if (mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(vstage.allocate(ctx, vbytes));
-        YTGPU_TRY(copy_in(ctx, vstage.p, values, vbytes, YTGPU_MEM_HOST));
-        dv = vstage.p;
-        if (null_bytemap) {
-            YTGPU_TRY(nstage.allocate(ctx, n));
-            YTGPU_TRY(copy_in(ctx, nstage.p, null_bytemap, n, YTGPU_MEM_HOST));
-            dn = nstage.p;
-        }
-    } else if (reinterpret_cast<uintptr_t>(out_data) & 7) {
+    InBuf<u8> dv, dn;
+    YTGPU_TRY(dv.stage(ctx, static_cast<const u8*>(values), boolean ? n : n * 8, mem));
+    YTGPU_TRY(dn.stage(ctx, null_bytemap, n, mem));
+    if (mem != YTGPU_MEM_HOST && (reinterpret_cast<uintptr_t>(out_data) & 7))
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "out_data must be 8-byte aligned");
-    }
-    u64* dst = reinterpret_cast<u64*>(out_data);
-    if (mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(ostage.allocate(ctx, total_words));
-        dst = ostage.p;
-    }
+    OutBuf<u64> dst;
+    YTGPU_TRY(dst.prepare(ctx, reinterpret_cast<u64*>(out_data), total_words, mem));
     {
         KernelTimer t(ctx, KC_DECODE, 1);
         const u32 grid = (u32)std::max<u64>(1, std::min<u64>((total_words + 255) / 256, (u64)kNumSms * 8));
-        plain_pack_kernel<<<grid, 256, 0, ctx->stream>>>(L, boolean ? nullptr : reinterpret_cast<const u64*>(dv),
-                                                        boolean ? reinterpret_cast<const u8*>(dv) : nullptr, dn, total_words, dst);
+        plain_pack_kernel<<<grid, 256, 0, ctx->stream>>>(L, boolean ? nullptr : reinterpret_cast<const u64*>(dv.p),
+                                                        boolean ? dv.p : nullptr, dn.p, total_words, dst.p);
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
-    if (mem == YTGPU_MEM_HOST) YTGPU_TRY(copy_out(ctx, out_data, dst, bytes, YTGPU_MEM_HOST));
+    YTGPU_TRY(dst.download(ctx, total_words));
     YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return Status{};
 }
@@ -192,42 +177,24 @@ Status extract_column_impl(Context* ctx, const ytgpu_rowset_view* rows, u32 colu
     const u64 n = rows->row_count;
     if (n == 0) return Status{};
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
-    DevBuf<ytgpu_value> vstage;
-    DevBuf<u64> pstage;
-    DevBuf<u32> lstage;
-    DevBuf<u8> nstage;
-    const ytgpu_value* vals = rows->values;
-    if (rows->mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(vstage.allocate(ctx, n * rows->value_count));
-        YTGPU_TRY(copy_in(ctx, vstage.p, rows->values, n * rows->value_count * 16, YTGPU_MEM_HOST));
-        vals = vstage.p;
-    }
-    u64* dp = out_payload;
-    u32* dl = out_lengths;
-    u8* dn = out_null;
-    if (out_mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(pstage.allocate(ctx, n));
-        dp = pstage.p;
-        if (out_lengths) {
-            YTGPU_TRY(lstage.allocate(ctx, n));
-            dl = lstage.p;
-        }
-        if (out_null) {
-            YTGPU_TRY(nstage.allocate(ctx, n));
-            dn = nstage.p;
-        }
-    }
+    InBuf<ytgpu_value> vals;
+    OutBuf<u64> dp;
+    OutBuf<u32> dl;
+    OutBuf<u8> dn;
+    YTGPU_TRY(vals.stage(ctx, rows->values, n * rows->value_count, rows->mem));
+    YTGPU_TRY(dp.prepare(ctx, out_payload, n, out_mem));
+    YTGPU_TRY(dl.prepare(ctx, out_lengths, n, out_mem));
+    YTGPU_TRY(dn.prepare(ctx, out_null, n, out_mem));
     {
         KernelTimer t(ctx, KC_DECODE, 1);
         const u32 grid = (u32)std::max<u64>(1, std::min<u64>((n + 255) / 256, (u64)kNumSms * 8));
-        extract_column_kernel<<<grid, 256, 0, ctx->stream>>>(vals, n, rows->value_count, column, value_type, dp, dl, dn, ctx->dev_err);
+        extract_column_kernel<<<grid, 256, 0, ctx->stream>>>(vals.p, n, rows->value_count, column, value_type, dp.p, dl.p, dn.p,
+                                                             ctx->dev_err);
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
-    if (out_mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(copy_out(ctx, out_payload, dp, n * 8, YTGPU_MEM_HOST));
-        if (out_lengths) YTGPU_TRY(copy_out(ctx, out_lengths, dl, n * 4, YTGPU_MEM_HOST));
-        if (out_null) YTGPU_TRY(copy_out(ctx, out_null, dn, n, YTGPU_MEM_HOST));
-    }
+    YTGPU_TRY(dp.download(ctx, n));
+    YTGPU_TRY(dl.download(ctx, n));
+    YTGPU_TRY(dn.download(ctx, n));
     return check_device_errors(ctx);
 }
 

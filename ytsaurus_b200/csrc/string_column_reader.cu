@@ -84,14 +84,9 @@ Status decode_string_segment_impl(Context* ctx, const ytgpu_string_segment* seg,
     if (mem != YTGPU_MEM_HOST && (reinterpret_cast<uintptr_t>(data) & 7))
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "segment data must be 8-byte aligned");
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
-    DevBuf<u8> stage;
-    const u8* dev = data;
-    if (mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(stage.allocate(ctx, seg->data_bytes + 16));
-        YTGPU_CUDA_TRY(cudaMemsetAsync(stage.p + seg->data_bytes, 0, 16, ctx->stream));  // one readable word past the end
-        YTGPU_TRY(copy_in(ctx, stage.p, data, seg->data_bytes, YTGPU_MEM_HOST));
-        dev = stage.p;
-    }
+    InBuf<u8> staged;
+    YTGPU_TRY(staged.stage(ctx, data, seg->data_bytes, mem, 16));  // one readable word past the end
+    const u8* dev = staged.p;
     // the structured parts, in writer order (ytgpu.h): sizes from the descriptor, checked against the vectors' own headers
     const int nstruct = seg->type == 3 || seg->type == 1 ? 2 : 3;
     u64 header[3] = {0, 0, 0};
@@ -143,32 +138,21 @@ Status decode_string_segment_impl(Context* ctx, const ytgpu_string_segment* seg,
         stored = S.row_indexes.size;
         if (stored == 0 || S.ids.size != stored) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "string segment: DictionaryRle sizes");
     }
-    DevBuf<u32> ostart, olen;
-    DevBuf<u8> onull;
-    u32 *ds = out_start, *dl = out_length;
-    u8* dn = out_null;
-    if (mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(ostart.allocate(ctx, rows));
-        YTGPU_TRY(olen.allocate(ctx, rows));
-        ds = ostart.p;
-        dl = olen.p;
-        if (out_null) {
-            YTGPU_TRY(onull.allocate(ctx, rows));
-            dn = onull.p;
-        }
-    }
+    OutBuf<u32> ds, dl;
+    OutBuf<u8> dn;
+    YTGPU_TRY(ds.prepare(ctx, out_start, rows, mem));
+    YTGPU_TRY(dl.prepare(ctx, out_length, rows, mem));
+    YTGPU_TRY(dn.prepare(ctx, out_null, rows, mem));
     {
         KernelTimer t(ctx, KC_DECODE, 1);
         const u32 grid = (u32)std::max<u64>(1, std::min<u64>((rows + 255) / 256, (u64)kNumSms * 8));
-        decode_string_segment_kernel<<<grid, 256, 0, ctx->stream>>>(S, ds, dl, dn);
+        decode_string_segment_kernel<<<grid, 256, 0, ctx->stream>>>(S, ds.p, dl.p, dn.p);
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
-    if (mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(copy_out(ctx, out_start, ds, rows * 4, YTGPU_MEM_HOST));
-        YTGPU_TRY(copy_out(ctx, out_length, dl, rows * 4, YTGPU_MEM_HOST));
-        if (out_null) YTGPU_TRY(copy_out(ctx, out_null, dn, rows, YTGPU_MEM_HOST));
-        YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    }
+    YTGPU_TRY(ds.download(ctx, rows));
+    YTGPU_TRY(dl.download(ctx, rows));
+    YTGPU_TRY(dn.download(ctx, rows));
+    if (mem == YTGPU_MEM_HOST) YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return Status{};
 }
 

@@ -27,6 +27,7 @@
 #include "context.cuh"
 #include "scan.cuh"
 #include "string_dict.cuh"
+#include "strings.cuh"
 
 using namespace ytgpu;
 
@@ -53,6 +54,9 @@ struct Input {
     const u8* nulls;
     u64 n;
 };
+
+// A column staged by stage_strings, as the kernels here take it.
+Input input_of(const StagedStrings& s, u64 n) { return Input{s.dev.heap, s.dev.starts, s.dev.lengths, s.dev.nulls, n}; }
 
 __device__ __forceinline__ bool is_null(const Input& in, u64 g) { return in.nulls && in.nulls[g]; }
 
@@ -520,26 +524,9 @@ Status encode_string_impl(Context* ctx, const u8* heap, u64 heap_bytes, const u6
     if (n >= (1ull << 32)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "one call encodes fewer than 2^32 rows");
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
 
-    DevBuf<u8> hstage, nstage;
-    DevBuf<u64> sstage;
-    DevBuf<u32> lstage;
-    Input in{heap, starts, lengths, null_bytemap, n};
-    if (mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(hstage.allocate(ctx, heap_bytes));
-        YTGPU_TRY(copy_in(ctx, hstage.p, heap, heap_bytes, YTGPU_MEM_HOST));
-        YTGPU_TRY(sstage.allocate(ctx, n));
-        YTGPU_TRY(copy_in(ctx, sstage.p, starts, n * 8, YTGPU_MEM_HOST));
-        YTGPU_TRY(lstage.allocate(ctx, n));
-        YTGPU_TRY(copy_in(ctx, lstage.p, lengths, n * 4, YTGPU_MEM_HOST));
-        in.heap = hstage.p;
-        in.starts = sstage.p;
-        in.lengths = lstage.p;
-        if (null_bytemap) {
-            YTGPU_TRY(nstage.allocate(ctx, n));
-            YTGPU_TRY(copy_in(ctx, nstage.p, null_bytemap, n, YTGPU_MEM_HOST));
-            in.nulls = nstage.p;
-        }
-    }
+    StagedStrings staged;
+    YTGPU_TRY(stage_strings(ctx, ytgpu_string_column{heap, heap_bytes, starts, lengths, null_bytemap, n, mem, 0}, &staged));
+    const Input in = input_of(staged, n);
 
     // 0. prefix sums of the non-null lengths, segment cuts
     DevBuf<u64> P, sums, totals, seg_start;
@@ -631,23 +618,19 @@ Status encode_string_impl(Context* ctx, const u8* heap, u64 heap_bytes, const u6
     YTGPU_CUDA_TRY(cudaMemcpyAsync(out_segments, segs.p, (size_t)nseg * sizeof(ytgpu_string_segment), cudaMemcpyDeviceToHost, ctx->stream));
 
     // 4.
-    DevBuf<u8> ostage;
-    u8* dst = out_data;
-    if (mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(ostage.allocate(ctx, bytes + 8));
-        dst = ostage.p;
-    } else if (reinterpret_cast<uintptr_t>(out_data) & 7) {
+    if (mem != YTGPU_MEM_HOST && (reinterpret_cast<uintptr_t>(out_data) & 7))
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "out_data must be 8-byte aligned");
-    }
-    YTGPU_CUDA_TRY(cudaMemsetAsync(dst, 0, bytes, ctx->stream));  // the alignment gaps between segments
+    OutBuf<u8> dst;
+    YTGPU_TRY(dst.prepare(ctx, out_data, bytes + 8, mem));
+    YTGPU_CUDA_TRY(cudaMemsetAsync(dst.p, 0, bytes, ctx->stream));  // the alignment gaps between segments
     PackArgs args{in, S, first_of.p, dict_row.p, run_row.p, work.p, segs.p, nseg, layout[1]};
     {
         KernelTimer t(ctx, KC_DECODE, 2);
-        pack_words_kernel<<<grid_for(layout[1], 256, 8), 256, 0, ctx->stream>>>(args, dst);
-        copy_strings_kernel<<<grid_for(n, 256, 8), 256, 0, ctx->stream>>>(args, seg_of_row.p, dst);
+        pack_words_kernel<<<grid_for(layout[1], 256, 8), 256, 0, ctx->stream>>>(args, dst.p);
+        copy_strings_kernel<<<grid_for(n, 256, 8), 256, 0, ctx->stream>>>(args, seg_of_row.p, dst.p);
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
-    if (mem == YTGPU_MEM_HOST) YTGPU_TRY(copy_out(ctx, out_data, dst, bytes, YTGPU_MEM_HOST));
+    YTGPU_TRY(dst.download(ctx, bytes));
     YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return Status{};
 }
@@ -662,37 +645,6 @@ __global__ void __launch_bounds__(256) value_ids_kernel(const Input in, const u6
         out_ids[g] = slot == kNone ? 0 : (u64)(u32)table[slot];
         if (out_null) out_null[g] = slot == kNone ? 1 : 0;
     }
-}
-
-// A string column on the device: HOST columns are uploaded.
-struct StagedInput {
-    Input in{};
-    u64 heap_bytes = 0;
-    DevBuf<u8> heap, nulls;
-    DevBuf<u64> starts;
-    DevBuf<u32> lengths;
-};
-
-Status stage_input(Context* ctx, const u8* heap, u64 heap_bytes, const u64* starts, const u32* lengths, const u8* null_bytemap, u64 n,
-                   int mem, StagedInput* s) {
-    s->in = Input{heap, starts, lengths, null_bytemap, n};
-    s->heap_bytes = heap_bytes;
-    if (mem != YTGPU_MEM_HOST) return Status{};
-    YTGPU_TRY(s->heap.allocate(ctx, heap_bytes));
-    YTGPU_TRY(copy_in(ctx, s->heap.p, heap, heap_bytes, YTGPU_MEM_HOST));
-    YTGPU_TRY(s->starts.allocate(ctx, n));
-    YTGPU_TRY(copy_in(ctx, s->starts.p, starts, n * 8, YTGPU_MEM_HOST));
-    YTGPU_TRY(s->lengths.allocate(ctx, n));
-    YTGPU_TRY(copy_in(ctx, s->lengths.p, lengths, n * 4, YTGPU_MEM_HOST));
-    s->in.heap = s->heap.p;
-    s->in.starts = s->starts.p;
-    s->in.lengths = s->lengths.p;
-    if (null_bytemap) {
-        YTGPU_TRY(s->nulls.allocate(ctx, n));
-        YTGPU_TRY(copy_in(ctx, s->nulls.p, null_bytemap, n, YTGPU_MEM_HOST));
-        s->in.nulls = s->nulls.p;
-    }
-    return Status{};
 }
 
 u64 value_table_slots(u64 n) {
@@ -726,30 +678,21 @@ Status string_value_ids_impl(Context* ctx, const u8* heap, u64 heap_bytes, const
     if (!starts || !lengths || !out_ids || (heap_bytes && !heap)) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "null argument");
     if (n > (1ull << 30)) return make_status(YTGPU_ERR_UNSUPPORTED, "at most 2^30 rows per call");
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
-    StagedInput staged;
-    YTGPU_TRY(stage_input(ctx, heap, heap_bytes, starts, lengths, null_bytemap, n, mem, &staged));
+    StagedStrings staged;
+    YTGPU_TRY(stage_strings(ctx, ytgpu_string_column{heap, heap_bytes, starts, lengths, null_bytemap, n, mem, 0}, &staged));
     const u64 cap = value_table_slots(n);
-    DevBuf<u8> onull;
-    DevBuf<u64> table, seg_start, oids;
+    OutBuf<u64> ids;
+    OutBuf<u8> nulls;
+    DevBuf<u64> table, seg_start;
     YTGPU_TRY(table.allocate(ctx, cap));
     YTGPU_TRY(seg_start.allocate(ctx, 4));
     const u64 bounds[4] = {0, n, 0, cap};
     YTGPU_CUDA_TRY(cudaMemcpyAsync(seg_start.p, bounds, 32, cudaMemcpyHostToDevice, ctx->stream));
-    u64* dids = out_ids;
-    u8* dnull = out_null;
-    if (mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(oids.allocate(ctx, n));
-        dids = oids.p;
-        if (out_null) {
-            YTGPU_TRY(onull.allocate(ctx, n));
-            dnull = onull.p;
-        }
-    }
-    YTGPU_TRY(insert_value_ids(ctx, KC_GROUPBY, staged.in, seg_start.p, table.p, cap, dids, dnull));
-    if (mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(copy_out(ctx, out_ids, dids, n * 8, YTGPU_MEM_HOST));
-        if (out_null) YTGPU_TRY(copy_out(ctx, out_null, dnull, n, YTGPU_MEM_HOST));
-    }
+    YTGPU_TRY(ids.prepare(ctx, out_ids, n, mem));
+    YTGPU_TRY(nulls.prepare(ctx, out_null, n, mem));
+    YTGPU_TRY(insert_value_ids(ctx, KC_GROUPBY, input_of(staged, n), seg_start.p, table.p, cap, ids.p, nulls.p));
+    YTGPU_TRY(ids.download(ctx, n));
+    YTGPU_TRY(nulls.download(ctx, n));
     YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));  // bounds[] lives on this frame
     return Status{};
 }
@@ -861,7 +804,7 @@ Status string_dicts_build(Context* ctx, const ytgpu_string_column* cols, u32 cou
         for (u32 c = 0; c < count; ++c) YTGPU_CUDA_TRY(cudaMemsetAsync(dicts[c].slots.p, 0xff, cap * 8, ctx->stream));
         return Status{};
     }
-    std::vector<StagedInput> staged(count);
+    std::vector<StagedStrings> staged(count);
     DevBuf<u64> bounds_dev, sums, totals;
     YTGPU_TRY(bounds_dev.allocate(ctx, 4));
     YTGPU_TRY(sums.allocate(ctx, scan_block_count(n + 1)));
@@ -870,10 +813,10 @@ Status string_dicts_build(Context* ctx, const ytgpu_string_column* cols, u32 cou
     YTGPU_CUDA_TRY(cudaMemcpyAsync(bounds_dev.p, bounds, 32, cudaMemcpyHostToDevice, ctx->stream));
     for (u32 c = 0; c < count; ++c) {
         const ytgpu_string_column& s = cols[c];
-        YTGPU_TRY(stage_input(ctx, s.heap, s.heap_bytes, s.starts, s.lengths, s.null_bytemap, n, s.mem, &staged[c]));
+        YTGPU_TRY(stage_strings(ctx, s, &staged[c]));  // the key columns hold n rows each
         YTGPU_TRY(dicts[c].starts.allocate(ctx, n + 1));
         KernelTimer t(ctx, KC_JOIN, 4);
-        dict_lengths_kernel<<<grid_for(n + 1, 256, 8), 256, 0, ctx->stream>>>(staged[c].in, staged[c].heap_bytes, dicts[c].starts.p,
+        dict_lengths_kernel<<<grid_for(n + 1, 256, 8), 256, 0, ctx->stream>>>(input_of(staged[c], n), s.heap_bytes, dicts[c].starts.p,
                                                                               ctx->dev_err);
         exclusive_scan_u64(ctx->stream, dicts[c].starts.p, n + 1, sums.p, totals.p + c);
         YTGPU_CUDA_TRY(cudaGetLastError());
@@ -893,21 +836,21 @@ Status string_dicts_build(Context* ctx, const ytgpu_string_column* cols, u32 cou
         }
         {
             KernelTimer t(ctx, KC_JOIN);
-            dict_copy_kernel<<<grid_for(n, 256, 8), 256, 0, ctx->stream>>>(staged[c].in, d.starts.p, d.heap.p, d.lengths.p, bits);
+            dict_copy_kernel<<<grid_for(n, 256, 8), 256, 0, ctx->stream>>>(input_of(staged[c], n), d.starts.p, d.heap.p, d.lengths.p, bits);
             YTGPU_CUDA_TRY(cudaGetLastError());
         }
-        const Input copy{d.heap.p, d.starts.p, d.lengths.p, staged[c].in.nulls, n};
+        const Input copy{d.heap.p, d.starts.p, d.lengths.p, staged[c].dev.nulls, n};
         YTGPU_TRY(insert_value_ids(ctx, KC_JOIN, copy, bounds_dev.p, d.slots.p, cap, ids[c].p, nullptr));
     }
     return Status{};
 }
 
 Status string_dict_lookup(Context* ctx, const StringDict& dict, const ytgpu_string_column& col, u64 n, u64* ids, u32* null_bits) {
-    StagedInput staged;
-    YTGPU_TRY(stage_input(ctx, col.heap, col.heap_bytes, col.starts, col.lengths, col.null_bytemap, n, col.mem, &staged));
+    StagedStrings staged;
+    YTGPU_TRY(stage_strings(ctx, col, &staged));  // col holds n rows
     const Input d{dict.heap.p, dict.starts.p, dict.lengths.p, nullptr, 0};
     KernelTimer t(ctx, KC_JOIN);
-    dict_lookup_kernel<<<grid_for(n, 256, 16), 256, 0, ctx->stream>>>(d, dict.slots.p, (u32)dict.slots.n - 1, staged.in, staged.heap_bytes, ids,
+    dict_lookup_kernel<<<grid_for(n, 256, 16), 256, 0, ctx->stream>>>(d, dict.slots.p, (u32)dict.slots.n - 1, input_of(staged, n), col.heap_bytes, ids,
                                                                       col.null_bytemap ? null_bits : nullptr, ctx->dev_err);
     YTGPU_CUDA_TRY(cudaGetLastError());
     return Status{};

@@ -216,50 +216,35 @@ Status convert_impl(Context* ctx, const ytgpu_string_column_view* col, const u8*
     YTGPU_CUDA_TRY(cudaSetDevice(ctx->device));
 
     StringColumnDev c{};
-    c.offsets = col->offsets;
     c.string_count = col->string_count;
     c.avg = col->avg_length;
     c.chars = col->chars;
     c.chars_bytes = col->chars_bytes;
-    c.dict = col->dictionary_indexes;
     c.dict_count = col->dictionary_index_count;
-    c.rle = col->rle_indexes;
     c.rle_count = col->rle_indexes ? col->rle_count : 0;
     c.start = (u64)col->start_index;
     c.count = n;
-    c.filter = filter_hint;
-    DevBuf<u32> off_stage, dict_stage;
-    DevBuf<u64> rle_stage;
-    DevBuf<u8> chars_stage, filter_stage;
     if (col->mem == YTGPU_MEM_HOST) {
         if (col->rle_indexes && col->rle_indexes[0] != 0) return make_status(YTGPU_ERR_INVALID_ARGUMENT, "rle_indexes[0] != 0");
-        YTGPU_TRY(off_stage.allocate(ctx, col->string_count));
-        YTGPU_TRY(copy_in(ctx, off_stage.p, col->offsets, (size_t)col->string_count * 4, YTGPU_MEM_HOST));
-        c.offsets = off_stage.p;
-        if (out_chars) {  // the size query does not read the bytes
-            YTGPU_TRY(chars_stage.allocate(ctx, col->chars_bytes));
-            YTGPU_TRY(copy_in(ctx, chars_stage.p, col->chars, (size_t)col->chars_bytes, YTGPU_MEM_HOST));
-            c.chars = chars_stage.p;
-        }
-        if (col->dictionary_indexes) {
-            YTGPU_TRY(dict_stage.allocate(ctx, col->dictionary_index_count));
-            YTGPU_TRY(copy_in(ctx, dict_stage.p, col->dictionary_indexes, (size_t)col->dictionary_index_count * 4, YTGPU_MEM_HOST));
-            c.dict = dict_stage.p;
-        }
-        if (col->rle_indexes) {
-            YTGPU_TRY(rle_stage.allocate(ctx, col->rle_count));
-            YTGPU_TRY(copy_in(ctx, rle_stage.p, col->rle_indexes, (size_t)col->rle_count * 8, YTGPU_MEM_HOST));
-            c.rle = rle_stage.p;
-        }
-        if (filter_hint) {
-            YTGPU_TRY(filter_stage.allocate(ctx, n));
-            YTGPU_TRY(copy_in(ctx, filter_stage.p, filter_hint, n, YTGPU_MEM_HOST));
-            c.filter = filter_stage.p;
-        }
     } else if (col->rle_indexes) {
         check_rle_first_kernel<<<1, 1, 0, ctx->stream>>>(col->rle_indexes, ctx->dev_err);
         ctx->count_launch();
     }
+    InBuf<u32> offsets, dict;
+    InBuf<u64> rle;
+    InBuf<u8> chars, filter;
+    YTGPU_TRY(offsets.stage(ctx, col->offsets, col->string_count, col->mem));
+    c.offsets = offsets.p;
+    if (out_chars) {  // the size query does not read the bytes
+        YTGPU_TRY(chars.stage(ctx, col->chars, col->chars_bytes, col->mem));
+        c.chars = chars.p;
+    }
+    YTGPU_TRY(dict.stage(ctx, col->dictionary_indexes, col->dictionary_index_count, col->mem));
+    c.dict = dict.p;
+    YTGPU_TRY(rle.stage(ctx, col->rle_indexes, col->rle_count, col->mem));
+    c.rle = rle.p;
+    YTGPU_TRY(filter.stage(ctx, filter_hint, n, col->mem));
+    c.filter = filter.p;
 
     DevBuf<u32> src_start;
     DevBuf<u64> pos, sums, total;
@@ -288,27 +273,19 @@ Status convert_impl(Context* ctx, const ytgpu_string_column_view* col, const u8*
     if (out_capacity < total_host)
         return make_status(YTGPU_ERR_INVALID_ARGUMENT, "out_chars holds %llu bytes, %llu are needed", (unsigned long long)out_capacity,
                            (unsigned long long)total_host);
-    DevBuf<u8> chars_out;
-    DevBuf<u64> offs_out;
-    u8* oc = out_chars;
-    u64* oo = out_offsets;
-    if (out_mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(chars_out.allocate(ctx, total_host));
-        YTGPU_TRY(offs_out.allocate(ctx, n));
-        oc = chars_out.p;
-        oo = offs_out.p;
-    }
+    OutBuf<u8> oc;
+    OutBuf<u64> oo;
+    YTGPU_TRY(oc.prepare(ctx, out_chars, total_host, out_mem));
+    YTGPU_TRY(oo.prepare(ctx, out_offsets, n, out_mem));
     {
         KernelTimer t(ctx, KC_GATHER, 2);
-        end_offsets_kernel<<<grid_for(n, 256), 256, 0, ctx->stream>>>(pos.p, total.p, n, oo);
-        copy_chars_kernel<<<grid_for(n, 256), 256, 0, ctx->stream>>>(c.chars, src_start.p, pos.p, total.p, n, oc);
+        end_offsets_kernel<<<grid_for(n, 256), 256, 0, ctx->stream>>>(pos.p, total.p, n, oo.p);
+        copy_chars_kernel<<<grid_for(n, 256), 256, 0, ctx->stream>>>(c.chars, src_start.p, pos.p, total.p, n, oc.p);
         YTGPU_CUDA_TRY(cudaGetLastError());
     }
-    if (out_mem == YTGPU_MEM_HOST) {
-        YTGPU_TRY(copy_out(ctx, out_chars, oc, total_host, YTGPU_MEM_HOST));
-        YTGPU_TRY(copy_out(ctx, out_offsets, oo, n * 8, YTGPU_MEM_HOST));
-        YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    }
+    YTGPU_TRY(oc.download(ctx, total_host));
+    YTGPU_TRY(oo.download(ctx, n));
+    if (out_mem == YTGPU_MEM_HOST) YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return Status{};
 }
 

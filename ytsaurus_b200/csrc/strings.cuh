@@ -308,38 +308,24 @@ inline Status add_in_list(u32 k, u8 vtype, const u64* e, u32 count, const u8* co
 // A string column on the device (HOST inputs are uploaded).
 struct StagedStrings {
     StringDev dev{};
-    DevBuf<u8> heap, nulls;
-    DevBuf<u64> starts;
-    DevBuf<u32> lengths;
+    InBuf<u8> heap, nulls;
+    InBuf<u64> starts;
+    InBuf<u32> lengths;
 };
 
 Status stage_strings(Context* ctx, const ytgpu_string_column& c, StagedStrings* s) {
-    StringDev& d = s->dev;
-    d.heap_bytes = c.heap_bytes;
-    d.present = 1;
-    if (c.mem != YTGPU_MEM_HOST) {
-        d.heap = c.heap;
-        d.starts = c.starts;
-        d.lengths = c.lengths;
-        d.nulls = c.null_bytemap;
-        return Status{};
-    }
     const u64 n = c.row_count;
-    YTGPU_TRY(s->heap.allocate(ctx, c.heap_bytes));
-    YTGPU_TRY(copy_in(ctx, s->heap.p, c.heap, c.heap_bytes, YTGPU_MEM_HOST));
-    YTGPU_TRY(s->starts.allocate(ctx, n));
-    YTGPU_TRY(copy_in(ctx, s->starts.p, c.starts, n * 8, YTGPU_MEM_HOST));
-    YTGPU_TRY(s->lengths.allocate(ctx, n));
-    YTGPU_TRY(copy_in(ctx, s->lengths.p, c.lengths, n * 4, YTGPU_MEM_HOST));
+    YTGPU_TRY(s->heap.stage(ctx, c.heap, c.heap_bytes, c.mem));
+    YTGPU_TRY(s->starts.stage(ctx, c.starts, n, c.mem));
+    YTGPU_TRY(s->lengths.stage(ctx, c.lengths, n, c.mem));
+    YTGPU_TRY(s->nulls.stage(ctx, c.null_bytemap, n, c.mem));
+    StringDev& d = s->dev;
     d.heap = s->heap.p;
+    d.heap_bytes = c.heap_bytes;
     d.starts = s->starts.p;
     d.lengths = s->lengths.p;
-    d.nulls = nullptr;
-    if (c.null_bytemap) {
-        YTGPU_TRY(s->nulls.allocate(ctx, n));
-        YTGPU_TRY(copy_in(ctx, s->nulls.p, c.null_bytemap, n, YTGPU_MEM_HOST));
-        d.nulls = s->nulls.p;
-    }
+    d.nulls = s->nulls.p;
+    d.present = 1;
     return Status{};
 }
 
