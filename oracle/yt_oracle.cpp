@@ -1245,8 +1245,8 @@ static inline u64 zigzag_encode64(i64 n) { return ((u64)n << 1) ^ (u64)(n >> 63)
 u64 yto_varuint_encode(u64 v, u8* out) { return put_varuint(out, v); }
 u64 yto_zigzag_encode64(i64 v) { return zigzag_encode64(v); }
 
-// row_value_counts (nullable): values of row r actually written (<= ncols).  Returns bytes written or 0
-// when `cap` is too small.
+// row_value_counts (nullable): values of row r actually written, clamped to ncols as the device encoder does.
+// Returns bytes written or 0 when `cap` is too small.
 u64 yto_block_encode(const Value* v, const char* heap, size_t nrows, u32 ncols, const u32* row_value_counts,
                      u8* out, u64 cap) {
     std::vector<u8> data;
@@ -1255,7 +1255,7 @@ u64 yto_block_encode(const Value* v, const char* heap, size_t nrows, u32 ncols, 
     auto put = [&](u64 x) { size_t n = put_varuint(tmp, x); data.insert(data.end(), tmp, tmp + n); };
     for (size_t r = 0; r < nrows; ++r) {
         offsets[r] = (u32)data.size();
-        u32 cnt = row_value_counts ? row_value_counts[r] : ncols;
+        u32 cnt = row_value_counts ? std::min(row_value_counts[r], ncols) : ncols;
         put(cnt);
         for (u32 c = 0; c < cnt; ++c) {
             const Value& x = v[r * ncols + c];
@@ -1305,7 +1305,7 @@ int yto_block_decode(const u8* block, u64 block_bytes, u32 nrows, u32 value_coun
             u64 id, type;
             if (!(n = get_varuint(p, end, &id))) return 20;
             p += n;
-            if (!(n = get_varuint(p, end, &type))) return 20;
+            if (!(n = get_varuint(p, end, &type)) || type > 0xff) return 20;
             p += n;
             o = Value{(u16)id, (u8)type, 0, 0, 0};
             switch ((u8)type) {
@@ -1319,7 +1319,7 @@ int yto_block_decode(const u8* block, u64 block_bytes, u32 nrows, u32 value_coun
                     u64 len;
                     if (!(n = get_varuint(p, end, &len))) return 20;
                     p += n;
-                    if (p + len > end) return 20;
+                    if (len >= (1ull << 32) || len > (u64)(end - p)) return 20;  // p + len wraps for a length near 2^64
                     o.length = (u32)len;
                     o.data = (u64)(p - block);
                     p += len;

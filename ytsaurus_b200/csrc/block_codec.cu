@@ -83,7 +83,7 @@ __global__ void __launch_bounds__(256) decode_block_kernel(const u8* __restrict_
             u32 length = 0;
             if (!(n = get_varuint(p, end, &id))) { bad = true; --c; continue; }
             p += n;
-            if (!(n = get_varuint(p, end, &type))) { bad = true; --c; continue; }
+            if (!(n = get_varuint(p, end, &type)) || type > 0xff) { bad = true; --c; continue; }
             p += n;
             switch ((u8)type) {
                 case YTGPU_TYPE_INT64:
@@ -108,8 +108,9 @@ __global__ void __launch_bounds__(256) decode_block_kernel(const u8* __restrict_
                 case YTGPU_TYPE_STRING:
                 case YTGPU_TYPE_ANY:
                 case YTGPU_TYPE_COMPOSITE: {
+                    // a varuint32 length; compared with the bytes left, as p + n + len wraps for a length near 2^64
                     u64 len = 0;
-                    if (!(n = get_varuint(p, end, &len)) || p + n + len > end) { bad = true; break; }
+                    if (!(n = get_varuint(p, end, &len)) || len >= (1ull << 32) || len > (u64)(end - p - n)) { bad = true; break; }
                     p += n;
                     length = (u32)len;
                     payload = (u64)(p - block);
