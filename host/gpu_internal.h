@@ -158,4 +158,19 @@ inline ytgpu_column_view ArrowColumnView(const TArrowColumn& a) {
     return v;
 }
 
+// Element i of an Arrow binary / utf8 array is [Offsets[Offset + i], Offsets[Offset + i + 1]): the offsets of the window
+// must not decrease (nor start below 0).
+inline void CheckOffsets(const TArrowColumn& a, const char* side) {
+    using NYT::NTableClient::TErrorException;
+    const int32_t* o = a.Offsets + a.Offset;
+    if (o[0] < 0) throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, std::string(side) + " string key: a negative offset");
+    for (int64_t i = 0; i < a.Length; ++i)
+        if (o[i + 1] < o[i]) throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, std::string(side) + " string key: decreasing offsets");
+}
+
+inline bool IsValid(const TArrowColumn& a, int64_t i) {
+    const int64_t bit = a.Offset + i;
+    return !a.Validity || ((a.Validity[bit >> 3] >> (bit & 7)) & 1);
+}
+
 }  // namespace NYql::NMiniKQL::NDetail

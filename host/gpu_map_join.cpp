@@ -35,19 +35,8 @@ struct TLeftStrings {
     ytgpu_string_column Column{};
 };
 
-// Element i of an Arrow binary / utf8 array is [Offsets[Offset + i], Offsets[Offset + i + 1]): the offsets of the window
-// must not decrease (nor start below 0).
-void CheckOffsets(const TArrowColumn& a, const char* side) {
-    const int32_t* o = a.Offsets + a.Offset;
-    if (o[0] < 0) throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, std::string(side) + " string key: a negative offset");
-    for (int64_t i = 0; i < a.Length; ++i)
-        if (o[i + 1] < o[i]) throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, std::string(side) + " string key: decreasing offsets");
-}
-
-bool IsValid(const TArrowColumn& a, int64_t i) {
-    const int64_t bit = a.Offset + i;
-    return !a.Validity || ((a.Validity[bit >> 3] >> (bit & 7)) & 1);
-}
+using NDetail::CheckOffsets;
+using NDetail::IsValid;
 
 class TGpuBlockMapJoin : public IBlockMapJoin {
 public:

@@ -589,6 +589,65 @@ int ytgpu_scan_filter_groupby_multi_strings(ytgpu_context* ctx, const ytgpu_colu
                                             const ytgpu_string_column* string_columns, uint32_t string_count,
                                             ytgpu_error* err);
 
+/* ---- GROUP BY table: kept on the device and updated block by block ----
+ * The one-shot GROUP BY above needs every row of a query in one call.  A GROUP BY table accumulates blocks instead: it is
+ * created with the key and value types and the aggregate list, each _update folds one block of rows into it, and _result
+ * returns the groups so far.  The contract: updates over blocks B1 .. Bm, each with its own predicate, then _result, give
+ * exactly what ytgpu_scan_filter_groupby_multi_strings gives over the rows of B1 ++ .. ++ Bm with each block's predicate
+ * applied to its own rows: the same groups, the same first-seen order, first_rows as GLOBAL row numbers (the rows of the
+ * earlier updates plus the row's index in its block, 64-bit), COUNT(*) and every aggregate with the semantics stated above
+ * (NULLs, wrap-around, AggLess for doubles, the first row winning an ARGMIN / ARGMAX tie).  Two exceptions, as for the
+ * one-shot call: double SUM / AVG add in any order, and a +-0 MIN / MAX compares by value.
+ * Keys.  The key tuple is the key_count numeric keys (INT64 / UINT64 / DOUBLE / BOOLEAN, any encoding the GROUP BY calls
+ * take) followed by the string_key_count string keys (flat string columns, HOST or DEVICE): 1 .. 8 components, key_count
+ * may be 0.  Keys compare as GROUP BY keys: (is-null, payload), doubles by bit pattern, NULL equals NULL; strings by length
+ * and bytes, "" is not NULL.  The table owns its keys: the caller may free a block's buffers once _update returns.
+ * Create.  value_types: the types of the value_count value columns every update passes; aggregates over them only (at most
+ * 32; string-valued aggregates are UNSUPPORTED).  group_count_hint sizes the table (0 = unknown); it grows by doubling.
+ * Update.  At most 2^30 rows, checked from the views before any access (UNSUPPORTED); all columns of one length; key and
+ * value counts and types must be the table's (INVALID_ARGUMENT); predicate as for the one-shot call.  The table holds fewer
+ * than 2^30 groups: an update whose new groups would reach 2^30 together with the table's is UNSUPPORTED.  A refused
+ * update leaves the groups and states as they were (a non-NULL string outside its heap is INVALID_ARGUMENT, with no byte
+ * outside the heap read, and is found before anything changes).  Updates may follow a refusal.  The string dictionaries
+ * keep every distinct non-NULL value an update passed, including the values of rows its predicate dropped and of a block
+ * refused for its group count: their memory is bounded by the distinct values seen, not by the groups, and no result
+ * shows the extra values.
+ * Result.  out as for the one-shot call, with out->keys / key_null for the numeric keys only; string_out[s] per string
+ * key: starts / lengths / null_bytemap [capacity] and a heap of heap_capacity bytes, value o at heap + starts[o] (a NULL
+ * key has start, length 0).  Capacity protocol: group_count and every heap_bytes are written; a capacity below the group
+ * count, or a heap_capacity below heap_bytes, is INVALID_ARGUMENT with nothing written to the outputs, so capacity 0 is
+ * the count query.  _result does not
+ * change the table: updates may continue after it.  The outputs are in out_mem.
+ * Memory.  Per group: 8 B per key component, 4 B of null mask, 16 B of COUNT(*) and first row and 32 B per aggregate, in
+ * arrays whose capacity doubles (so up to twice that per group held), and 8 to 16 B of slot table; per string value
+ * kept: its bytes, 12 B of start and length (capacity doubling too) and 16 to 32 B of slots.
+ * Synchronisations.  Update: one for the block's group count, one for its count of new groups (which sizes the growth),
+ * and a closing one; with string keys, one for the bounds checks and one per string key for the number and bytes of new
+ * values; the assign step's error word as in the one-shot call.  Result: one for the sort's plan (from 2^18 groups), one for the byte totals and group
+ * count, and a closing one.  Errors: a table of another context is INVALID_ARGUMENT; destroy(NULL) is a no-op; destroy a
+ * table before its context. */
+typedef struct ytgpu_groupby_table ytgpu_groupby_table;
+
+typedef struct ytgpu_groupby_string_keys {
+    uint8_t* heap;           /* [heap_capacity]: the emitted values' bytes, in output order */
+    uint64_t heap_capacity;  /* in */
+    uint64_t heap_bytes;     /* out: bytes the values need */
+    uint64_t* starts;        /* [capacity] */
+    uint32_t* lengths;       /* [capacity] */
+    uint8_t* null_bytemap;   /* [capacity]: 1 = NULL */
+} ytgpu_groupby_string_keys;
+
+int ytgpu_groupby_table_create(ytgpu_context* ctx, const uint8_t* key_types, uint32_t key_count, uint32_t string_key_count,
+                               const uint8_t* value_types, uint32_t value_count, const ytgpu_aggregate* aggregates,
+                               uint32_t aggregate_count, uint64_t group_count_hint, ytgpu_groupby_table** out, ytgpu_error* err);
+int ytgpu_groupby_table_update(ytgpu_context* ctx, ytgpu_groupby_table* table, const ytgpu_column_view* key_columns,
+                               uint32_t key_count, const ytgpu_string_column* string_keys, uint32_t string_key_count,
+                               const ytgpu_column_view* value_columns, uint32_t value_count, const ytgpu_predicate* predicate,
+                               int32_t predicate_column, ytgpu_error* err);
+int ytgpu_groupby_table_result(ytgpu_context* ctx, const ytgpu_groupby_table* table, ytgpu_groupby_multi_result* out,
+                               ytgpu_groupby_string_keys* string_out, uint32_t string_key_count, int out_mem, ytgpu_error* err);
+int ytgpu_groupby_table_destroy(ytgpu_groupby_table* table, ytgpu_error* err);
+
 /* ---- hash JOIN: inner, left, left semi and left only equi-joins over key tuples ----
  * The join of YT QL's JoinOpHelper (library/query/engine/cg_routines/registry.cpp), which collects the primary rows' join
  * keys, fetches the foreign rows and joins them row by row through a hash lookup keyed on the join key.  Here the foreign

@@ -123,6 +123,7 @@ EXPORTED_SYMBOLS = [
     "ytgpu_hash_join", "ytgpu_gather_column", "ytgpu_gather_string_column", "ytgpu_order_rows",
     "ytgpu_join_table_build", "ytgpu_join_table_probe", "ytgpu_join_table_destroy",
     "ytgpu_join_table_build_strings", "ytgpu_join_table_probe_strings",
+    "ytgpu_groupby_table_create", "ytgpu_groupby_table_update", "ytgpu_groupby_table_result", "ytgpu_groupby_table_destroy",
 ]
 
 FLAGS_DICTIONARY_ZERO, FLAGS_BITMAP = 0, 1
@@ -239,6 +240,11 @@ class GroupByMultiResult(C.Structure):
     _fields_ = [("group_count", C.c_uint64), ("capacity", C.c_uint64), ("keys", C.POINTER(C.c_void_p)),
                 ("key_null", C.POINTER(C.c_void_p)), ("values", C.POINTER(C.c_void_p)), ("value_null", C.POINTER(C.c_void_p)),
                 ("counts", C.c_void_p), ("first_rows", C.c_void_p)]
+
+
+class GroupByStringKeys(C.Structure):
+    _fields_ = [("heap", C.c_void_p), ("heap_capacity", C.c_uint64), ("heap_bytes", C.c_uint64), ("starts", C.c_void_p),
+                ("lengths", C.c_void_p), ("null_bytemap", C.c_void_p)]
 
 
 class ArrowArray(C.Structure):
@@ -393,6 +399,13 @@ def load() -> C.CDLL:
                                                    C.POINTER(C.c_void_p), C.POINTER(Error)]
     lib.ytgpu_join_table_probe_strings.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_int,
                                                    C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.c_int, C.POINTER(Error)]
+    lib.ytgpu_groupby_table_create.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p,
+                                               C.c_uint32, C.c_uint64, C.POINTER(C.c_void_p), C.POINTER(Error)]
+    lib.ytgpu_groupby_table_update.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p,
+                                               C.c_uint32, C.c_void_p, C.c_int32, C.POINTER(Error)]
+    lib.ytgpu_groupby_table_result.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(GroupByMultiResult), C.c_void_p, C.c_uint32, C.c_int,
+                                               C.POINTER(Error)]
+    lib.ytgpu_groupby_table_destroy.argtypes = [C.c_void_p, C.POINTER(Error)]
     lib.ytgpu_gather_column.argtypes = [C.c_void_p, C.POINTER(ColumnView), C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
                                         C.POINTER(C.c_uint64), C.c_int, C.POINTER(Error)]
     lib.ytgpu_gather_string_column.argtypes = [C.c_void_p, C.POINTER(StringColumn), C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,

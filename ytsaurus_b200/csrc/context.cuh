@@ -92,6 +92,20 @@ struct DevBuf {
     }
 };
 
+// Grows *b to at least `want` elements, doubling from its size (at least 16), and keeps its first `keep` elements; a
+// buffer already that large is left as it is.  Stream-ordered, no synchronisation.
+template <class T>
+Status grow_buf(Context* ctx, DevBuf<T>* b, size_t keep, size_t want) {
+    if (b->p && b->n >= want) return Status{};
+    size_t cap = b->n > 16 ? b->n : 16;
+    while (cap < want) cap <<= 1;
+    DevBuf<T> nb;
+    YTGPU_TRY(nb.allocate(ctx, cap));
+    if (keep) YTGPU_CUDA_TRY(cudaMemcpyAsync(nb.p, b->p, keep * sizeof(T), cudaMemcpyDeviceToDevice, ctx->stream));
+    *b = static_cast<DevBuf<T>&&>(nb);
+    return Status{};
+}
+
 // Scoped CUDA-event span around one or more launches of a kernel class.
 struct KernelTimer {
     Context* ctx;

@@ -323,19 +323,6 @@ Status check_string_side(const ytgpu_string_column* strings, u32 count, bool hav
     return Status{};
 }
 
-// A string key's ids as a key column: plain 64-bit values, with a null bitmap only when the strings have NULLs.
-ColumnDev id_column(const u64* ids, const u32* null_bits, u64 n) {
-    ColumnDev c{};
-    c.count = (i64)n;
-    c.values = ids;
-    c.values_count = n;
-    c.bitmap = reinterpret_cast<const u8*>(null_bits);
-    c.bit_width = 64;
-    c.has_values = 1;
-    c.value_type = YTGPU_TYPE_UINT64;
-    return c;
-}
-
 bool known_kind(int kind) {
     return kind == YTGPU_JOIN_INNER || kind == YTGPU_JOIN_LEFT || kind == YTGPU_JOIN_SEMI || kind == YTGPU_JOIN_ANTI;
 }

@@ -73,6 +73,19 @@ __device__ __forceinline__ u64 hash_tuple(const KeyColumns& K, const KeyTuple& t
     return h ^ (h >> 29);
 }
 
+// A string key's dictionary ids as a key column: plain 64-bit values, with a null bitmap only when the strings have NULLs.
+ColumnDev id_column(const u64* ids, const u32* null_bits, u64 n) {
+    ColumnDev c{};
+    c.count = (i64)n;
+    c.values = ids;
+    c.values_count = n;
+    c.bitmap = reinterpret_cast<const u8*>(null_bits);
+    c.bit_width = 64;
+    c.has_values = 1;
+    c.value_type = YTGPU_TYPE_UINT64;
+    return c;
+}
+
 // Small tables (<= kSmemSlots slots, i.e. up to ~1000 expected groups): COUNT(*), the non-null counts and the sums are
 // accumulated in shared memory per CTA and flushed once — 10^8 rows otherwise mean 10^8 global atomics on a thousand
 // addresses.  The kernels run grid-stride with a fixed grid so that a CTA flushes once.

@@ -791,6 +791,72 @@ __global__ void __launch_bounds__(256) dict_lookup_kernel(const Input dict, cons
     if (bad) atomicOr(err_word, (u32)DE_STRING_OUT_OF_HEAP);
 }
 
+// Append, step 1: flags[g] = 1 at the first row of each value the dictionary lacks (its lookup missed and the block's
+// value-ids insert names the row itself), new_bytes[g] = that value's length; at n, the 0s that make the scans' last words
+// the totals.
+__global__ void __launch_bounds__(256) dict_new_values_kernel(const Input in, const u64* __restrict__ ids, const u64* __restrict__ first_row,
+                                                              u64* __restrict__ flags, u64* __restrict__ new_bytes) {
+    for (u64 g = (u64)blockIdx.x * blockDim.x + threadIdx.x; g <= in.n; g += (u64)gridDim.x * blockDim.x) {
+        const bool fresh = g < in.n && !is_null(in, g) && ids[g] == kStringDictMiss && first_row[g] == g;
+        flags[g] = fresh ? 1 : 0;
+        new_bytes[g] = fresh ? in.lengths[g] : 0;
+    }
+}
+
+// Inserts value id's slot word into a dictionary's slots (at most half full, so an empty slot is always found).  The
+// values are distinct: no comparison, a CAS on an empty slot only.
+__device__ __forceinline__ void dict_insert_slot(u64* slots, u32 mask, const u8* p, u32 len, u32 id) {
+    const u64 mx = string_hash(p, len);
+    u32 h = (u32)mx & mask;
+    const unsigned long long want = slot_word((u32)(mx >> 32), id);
+    while (atomicCAS((unsigned long long*)&slots[h], (unsigned long long)kEmptySlot, want) != (unsigned long long)kEmptySlot) h = (h + 1) & mask;
+}
+
+// Append, step 2 (rank, at: the scans of step 1): each new value gets id count + rank, its bytes at bytes + at, and its slot.
+// Each warp takes 32 rows and copies their new values' bytes one after the other with the whole warp, as dict_copy_kernel.
+__global__ void __launch_bounds__(256) dict_append_kernel(const Input in, const u64* __restrict__ rank, const u64* __restrict__ at, u64 count,
+                                                          u64 bytes, u8* __restrict__ heap, u64* __restrict__ starts, u32* __restrict__ lengths,
+                                                          u64* slots, u32 mask, u64* __restrict__ ids) {
+    const u32 lane = threadIdx.x & 31;
+    const u64 warps = ((u64)gridDim.x * blockDim.x) >> 5;
+    for (u64 base = (u64)blockIdx.x * blockDim.x + threadIdx.x - lane; base < in.n; base += warps * 32) {
+        const u64 g = base + lane;
+        const bool fresh = g < in.n && rank[g + 1] != rank[g];
+        u32 len = 0;
+        if (fresh) {
+            const u64 id = count + rank[g];
+            len = in.lengths[g];
+            starts[id] = bytes + at[g];
+            lengths[id] = len;
+            dict_insert_slot(slots, mask, in.heap + in.starts[g], len, (u32)id);
+            ids[g] = id;
+        }
+        u32 m = __ballot_sync(0xffffffffu, len != 0);
+        while (m) {
+            const int src = __ffs(m) - 1;
+            m &= m - 1;
+            const u64 row = base + src;
+            const u32 l = __shfl_sync(0xffffffffu, len, src);
+            const u8* from = in.heap + in.starts[row];
+            u8* to = heap + bytes + at[row];
+            for (u32 k = lane; k < l; k += 32) to[k] = from[k];
+        }
+    }
+}
+
+// Append, step 3: the other rows of a new value take the id of its first row (set by step 2).
+__global__ void __launch_bounds__(256) dict_map_new_kernel(const Input in, const u64* __restrict__ first_row, u64* ids) {
+    for (u64 g = (u64)blockIdx.x * blockDim.x + threadIdx.x; g < in.n; g += (u64)gridDim.x * blockDim.x)
+        if (!is_null(in, g) && ids[g] == kStringDictMiss) ids[g] = ids[first_row[g]];
+}
+
+// The slots of a grown dictionary, from its kept values.
+__global__ void __launch_bounds__(256) dict_rehash_kernel(const u8* __restrict__ heap, const u64* __restrict__ starts, const u32* __restrict__ lengths,
+                                                          u64 count, u64* slots, u32 mask) {
+    for (u64 id = (u64)blockIdx.x * blockDim.x + threadIdx.x; id < count; id += (u64)gridDim.x * blockDim.x)
+        dict_insert_slot(slots, mask, heap + starts[id], lengths[id], (u32)id);
+}
+
 }  // namespace
 
 namespace ytgpu {
@@ -853,6 +919,63 @@ Status string_dict_lookup(Context* ctx, const StringDict& dict, const ytgpu_stri
     dict_lookup_kernel<<<grid_for(n, 256, 16), 256, 0, ctx->stream>>>(d, dict.slots.p, (u32)dict.slots.n - 1, input_of(staged, n), col.heap_bytes, ids,
                                                                       col.null_bytemap ? null_bits : nullptr, ctx->dev_err);
     YTGPU_CUDA_TRY(cudaGetLastError());
+    return Status{};
+}
+
+Status string_dict_append(Context* ctx, StringDict* dict, u64* count, u64* bytes, const ytgpu_string_column& col, u64 n, u64* ids) {
+    if (n == 0) return Status{};
+    StagedStrings staged;
+    YTGPU_TRY(stage_strings(ctx, col, &staged));
+    const Input in = input_of(staged, n);
+    // the block's own value ids: the first row of each value
+    const u64 cap = value_table_slots(n);
+    DevBuf<u64> table, bounds_dev, first_row, rank, at, sums, totals;
+    YTGPU_TRY(table.allocate(ctx, cap));
+    YTGPU_TRY(bounds_dev.allocate(ctx, 4));
+    YTGPU_TRY(first_row.allocate(ctx, n));
+    YTGPU_TRY(rank.allocate(ctx, n + 1));
+    YTGPU_TRY(at.allocate(ctx, n + 1));
+    YTGPU_TRY(sums.allocate(ctx, scan_block_count(n + 1)));
+    YTGPU_TRY(totals.allocate(ctx, 2));
+    const u64 bounds[4] = {0, n, 0, cap};  // read before the synchronisation below
+    YTGPU_CUDA_TRY(cudaMemcpyAsync(bounds_dev.p, bounds, 32, cudaMemcpyHostToDevice, ctx->stream));
+    YTGPU_TRY(insert_value_ids(ctx, KC_GROUPBY, in, bounds_dev.p, table.p, cap, first_row.p, nullptr));
+    {
+        KernelTimer t(ctx, KC_GROUPBY, 7);
+        dict_new_values_kernel<<<grid_for(n + 1, 256, 8), 256, 0, ctx->stream>>>(in, ids, first_row.p, rank.p, at.p);
+        exclusive_scan_u64(ctx->stream, rank.p, n + 1, sums.p, totals.p);
+        exclusive_scan_u64(ctx->stream, at.p, n + 1, sums.p, totals.p + 1);
+        YTGPU_CUDA_TRY(cudaGetLastError());
+    }
+    u64 added[2] = {0, 0};
+    YTGPU_CUDA_TRY(cudaMemcpyAsync(added, totals.p, 16, cudaMemcpyDeviceToHost, ctx->stream));
+    YTGPU_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    if (added[0] == 0) return Status{};  // every value was there already: the lookup's ids are final
+    const u64 c = *count + added[0], b = *bytes + added[1];
+    YTGPU_TRY(grow_buf(ctx, &dict->heap, *bytes, b));
+    YTGPU_TRY(grow_buf(ctx, &dict->starts, *count, c));
+    YTGPU_TRY(grow_buf(ctx, &dict->lengths, *count, c));
+    if (dict->slots.n < 2 * c) {
+        u64 slots = dict->slots.n;
+        while (slots < 2 * c) slots <<= 1;
+        YTGPU_TRY(dict->slots.allocate(ctx, slots));
+        YTGPU_CUDA_TRY(cudaMemsetAsync(dict->slots.p, 0xff, slots * 8, ctx->stream));
+        if (*count) {
+            KernelTimer t(ctx, KC_GROUPBY);
+            dict_rehash_kernel<<<grid_for(*count, 256, 8), 256, 0, ctx->stream>>>(dict->heap.p, dict->starts.p, dict->lengths.p, *count, dict->slots.p,
+                                                                                (u32)slots - 1);
+            YTGPU_CUDA_TRY(cudaGetLastError());
+        }
+    }
+    {
+        KernelTimer t(ctx, KC_GROUPBY, 2);
+        dict_append_kernel<<<grid_for(n, 256, 8), 256, 0, ctx->stream>>>(in, rank.p, at.p, *count, *bytes, dict->heap.p, dict->starts.p,
+                                                                         dict->lengths.p, dict->slots.p, (u32)dict->slots.n - 1, ids);
+        dict_map_new_kernel<<<grid_for(n, 256, 8), 256, 0, ctx->stream>>>(in, first_row.p, ids);
+        YTGPU_CUDA_TRY(cudaGetLastError());
+    }
+    *count = c;
+    *bytes = b;
     return Status{};
 }
 

@@ -34,4 +34,13 @@ Status string_dicts_build(Context* ctx, const ytgpu_string_column* cols, u32 cou
 // nothing; the caller reads that word.  No synchronisation.
 Status string_dict_lookup(Context* ctx, const StringDict& dict, const ytgpu_string_column& col, u64 rows, u64* ids, u32* null_bits);
 
+// A growing dictionary (the GROUP BY table's, groupby_table.cu) uses the same layout with dense ids: value id is
+// lengths[id] bytes at heap + starts[id] for id < *count, *bytes heap bytes are in use, and the slot words are
+// (fingerprint << 32) | id; string_dict_lookup reads it as it reads a built one.  An empty one has 8 empty slots.
+// string_dict_append adds the values of `col` (n rows, HOST or DEVICE, every non-NULL value inside its heap: the caller
+// looked the column up first and read the device error word) that the dictionary lacks, in first-row order, growing its
+// buffers by doubling and rehashing its slots from the kept bytes.  ids: in, string_dict_lookup's result over col; out,
+// every non-NULL row's id (NULL rows keep 0).  Synchronises once, for the count and bytes of the new values.
+Status string_dict_append(Context* ctx, StringDict* dict, u64* count, u64* bytes, const ytgpu_string_column& col, u64 n, u64* ids);
+
 }  // namespace ytgpu

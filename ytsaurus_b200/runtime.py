@@ -93,6 +93,8 @@ class GpuContext:
         if getattr(self, "handle", None):
             for table in list(getattr(self, "_join_tables", ())):  # a join table is destroyed before its context
                 table.close()
+            for table in list(getattr(self, "_groupby_tables", ())):
+                table.close()
             self.lib.ytgpu_context_destroy(self.handle)
             self.handle = None
 
@@ -849,6 +851,13 @@ class GpuContext:
         this returns."""
         return JoinTable(self, foreign_keys, nulls, string_keys)
 
+    def groupby_table(self, key_types, string_key_count, value_types, aggregates, hint: int = 0) -> "GroupByTable":
+        """ytgpu_groupby_table_create: a GROUP BY table updated block by block (GroupByTable.update) whose result
+        (GroupByTable.result) is the one-shot scan_filter_groupby_multi over all the blocks' rows.  key_types: the numeric
+        keys' EValueTypes, followed in the key tuple by string_key_count string keys; value_types: the value columns every
+        update passes; aggregates [(op, column[, by_column])] over them."""
+        return GroupByTable(self, key_types, string_key_count, value_types, aggregates, hint)
+
     def gather_column(self, column: "Column", rows):
         """ytgpu_gather_column: `column` decoded at rows (uint32; capi.JOIN_NO_ROW gives NULL) -> dict(values, null_bitmap,
         null_count, column) in the rows' memory flavour, laid out as evaluate_expression's result: `column` is a Column over
@@ -1128,6 +1137,120 @@ class JoinTable:
             if getattr(self.ctx, "handle", None):
                 err = capi.Error()
                 capi.check(self.ctx.lib.ytgpu_join_table_destroy(self.handle, C.byref(err)), err)
+            self.handle = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class GroupByTable:
+    """A GROUP BY table (ytgpu_groupby_table); see GpuContext.groupby_table.  close() or a with block destroys it."""
+
+    def __init__(self, ctx: GpuContext, key_types, string_key_count: int, value_types, aggregates, hint: int = 0):
+        self.ctx, self.handle = ctx, None
+        self.numeric, self.strings, self.aggregate_count = len(key_types), string_key_count, len(aggregates)
+        kt = (C.c_uint8 * max(len(key_types), 1))(*[int(t) for t in key_types])
+        vt = (C.c_uint8 * max(len(value_types), 1))(*[int(t) for t in value_types])
+        aggs = (capi.Aggregate * max(len(aggregates), 1))()
+        for i, a in enumerate(aggregates):
+            aggs[i].op, aggs[i].column = a[0], a[1]
+            aggs[i].by_column = a[2] if len(a) > 2 else -1
+        h = C.c_void_p()
+        err = capi.Error()
+        capi.check(ctx.lib.ytgpu_groupby_table_create(ctx.handle, C.cast(kt, C.c_void_p), len(key_types), string_key_count,
+                                                      C.cast(vt, C.c_void_p), len(value_types), C.cast(aggs, C.c_void_p),
+                                                      len(aggregates), hint, C.byref(h), C.byref(err)), err)
+        self.handle = h
+        if not hasattr(ctx, "_groupby_tables"):
+            ctx._groupby_tables = weakref.WeakSet()
+        ctx._groupby_tables.add(self)
+
+    def update(self, key_cols, value_cols, string_keys=(), predicate=None, predicate_column: int = -1):
+        """ytgpu_groupby_table_update with key_cols and value_cols (lists of Column) and string_keys as (heap, starts,
+        lengths, nulls or None) tuples; predicate (op, constant) over value_cols[predicate_column]."""
+        if self.handle is None:
+            raise ValueError("the GROUP BY table is closed")
+        kviews = [c.view() for c in key_cols]
+        vviews = [c.view() for c in value_cols]
+        karr = (capi.ColumnView * max(len(kviews), 1))(*kviews)
+        varr = (capi.ColumnView * max(len(vviews), 1))(*vviews)
+        sarr = _string_columns(string_keys) if string_keys else None
+        pred = None
+        if predicate is not None:
+            op, const = predicate
+            pred = capi.Predicate(op, 0, const & 0xFFFFFFFFFFFFFFFF)
+        err = capi.Error()
+        capi.check(self.ctx.lib.ytgpu_groupby_table_update(
+            self.ctx.handle, self.handle, C.cast(karr, C.c_void_p), len(kviews), C.cast(sarr, C.c_void_p) if sarr is not None else None,
+            len(string_keys), C.cast(varr, C.c_void_p), len(vviews), C.cast(C.pointer(pred), C.c_void_p) if pred is not None else None,
+            predicate_column, C.byref(err)), err)
+
+    def _call_result(self, res, skeys, out_mem):
+        err = capi.Error()
+        sarr = (capi.GroupByStringKeys * max(self.strings, 1))(*skeys)
+        code = self.ctx.lib.ytgpu_groupby_table_result(self.ctx.handle, self.handle, C.byref(res), C.cast(sarr, C.c_void_p), self.strings,
+                                                       out_mem, C.byref(err))
+        return code, err, [int(sarr[s].heap_bytes) for s in range(self.strings)]
+
+    def result(self, count_only: bool = False, out_mem: int = capi.MEM_HOST, capacity: int | None = None, heap_capacity=None):
+        """ytgpu_groupby_table_result -> dict(keys=[...], key_null=[...], values=[...], value_null=[...], count, first_row,
+        string_keys=[(heap, starts, lengths, nulls)]) in first-seen order, in out_mem; with count_only, the group count.
+        Without capacities a count query sizes the outputs first; a capacity below the need raises YtGpuError with
+        .group_count and .heap_bytes set."""
+        if self.handle is None:
+            raise ValueError("the GROUP BY table is closed")
+        zero = [capi.GroupByStringKeys() for _ in range(self.strings)]
+        empty = (C.c_void_p * 1)()
+        if count_only or capacity is None or heap_capacity is None:
+            res = capi.GroupByMultiResult(0, 0, empty, empty, empty, empty, None, None)
+            code, err, heap_bytes = self._call_result(res, zero, out_mem)
+            if code not in (capi.OK, capi.ERR_INVALID_ARGUMENT) or (code != capi.OK and res.group_count == 0):
+                capi.check(code, err)
+            if count_only:
+                return int(res.group_count)
+            capacity = int(res.group_count) if capacity is None else capacity
+            heap_capacity = heap_bytes if heap_capacity is None else heap_capacity
+        out = self.ctx._out
+        cap = max(capacity, 1)
+        keys = [out((cap,), np.uint64, out_mem) for _ in range(self.numeric)]
+        kn = [out((cap,), np.uint8, out_mem) for _ in range(self.numeric)]
+        vals = [out((cap,), np.uint64, out_mem) for _ in range(self.aggregate_count)]
+        vn = [out((cap,), np.uint8, out_mem) for _ in range(self.aggregate_count)]
+        counts = out((cap,), np.uint64, out_mem)
+        first = out((cap,), np.uint64, out_mem)
+        sout = [(out((max(hc, 1),), np.uint8, out_mem), out((cap,), np.uint64, out_mem), out((cap,), np.uint32, out_mem),
+                 out((cap,), np.uint8, out_mem)) for hc in heap_capacity]
+
+        def ptrs(arrs):
+            return (C.c_void_p * max(len(arrs), 1))(*[_ptr_mem(a)[0] for a in arrs])
+        pk, pkn, pv, pvn = ptrs(keys), ptrs(kn), ptrs(vals), ptrs(vn)
+        res = capi.GroupByMultiResult(0, capacity, pk, pkn, pv, pvn, _ptr_mem(counts)[0], _ptr_mem(first)[0])
+        skeys = [capi.GroupByStringKeys(_ptr_mem(h)[0], hc, 0, _ptr_mem(st)[0], _ptr_mem(ln)[0], _ptr_mem(nl)[0])
+                 for (h, st, ln, nl), hc in zip(sout, heap_capacity)]
+        code, err, heap_bytes = self._call_result(res, skeys, out_mem)
+        if code != capi.OK:
+            e = capi.YtGpuError(code, err.message.decode(errors="replace"), err.cuda_error)
+            e.group_count, e.heap_bytes = int(res.group_count), heap_bytes
+            raise e
+        g = int(res.group_count)
+        strings = [(h[:hb], st[:g], ln[:g], nl[:g]) for (h, st, ln, nl), hb in zip(sout, heap_bytes)]
+        return dict(keys=[k[:g] for k in keys], key_null=[k[:g] for k in kn], values=[v[:g] for v in vals],
+                    value_null=[v[:g] for v in vn], count=counts[:g], first_row=first[:g], string_keys=strings)
+
+    def close(self):
+        if self.handle is not None:
+            if getattr(self.ctx, "handle", None):
+                err = capi.Error()
+                capi.check(self.ctx.lib.ytgpu_groupby_table_destroy(self.handle, C.byref(err)), err)
             self.handle = None
 
     def __enter__(self):
