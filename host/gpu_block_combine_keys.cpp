@@ -45,7 +45,7 @@ private:
     size_t Capacity_ = 0;
 };
 
-//! One staged column: numeric values with a null bytemap turned into Arrow validity bits, or a string key's heap,
+//! One staged column: numeric values with a null bytemap turned into Arrow validity bits, or a string column's heap,
 //! starts, lengths and null bytemap.
 struct TStaged {
     TPinned<uint64_t> Values;
@@ -88,7 +88,8 @@ public:
         ytgpu_context* ctx = GetGpuContext();
         ytgpu_error err{};
         const uint32_t strings = (uint32_t)StringKeys_.size(), numeric = (uint32_t)NumericKeys_.size(), aggs = (uint32_t)Aggregates_.size();
-        std::vector<ytgpu_groupby_string_keys> sout(strings);
+        const uint32_t valueStrings = StringValued_, outputs = strings + valueStrings;
+        std::vector<ytgpu_groupby_string_keys> sout(outputs);  // the string keys, then the string-valued aggregates
         uint64_t* none[1] = {nullptr};
         uint8_t* noneb[1] = {nullptr};
         ytgpu_groupby_multi_result q{};
@@ -96,7 +97,8 @@ public:
         q.key_null = noneb;
         q.values = none;
         q.value_null = noneb;
-        const int code = ytgpu_groupby_table_result(ctx, Table_, &q, sout.data(), strings, YTGPU_MEM_HOST, &err);
+        const int code = ytgpu_groupby_table_result_strings(ctx, Table_, &q, sout.data(), strings, sout.data() + strings, valueStrings,
+                                                            YTGPU_MEM_HOST, &err);
         if (code != YTGPU_OK && !(code == YTGPU_ERR_INVALID_ARGUMENT && q.group_count > 0)) ThrowFrom(err);  // capacity 0: the count
         const uint64_t g = q.group_count;
         r.Keys.assign(numeric, std::vector<uint64_t>(g));
@@ -107,6 +109,9 @@ public:
             r.StringKeyBytes.assign(strings, std::string());
             r.StringKeyOffsets.assign(strings, std::vector<int32_t>(1, 0));
             r.StringKeyValid.assign(strings, std::vector<uint8_t>());
+            r.StringValueBytes.assign(valueStrings, std::string());
+            r.StringValueOffsets.assign(valueStrings, std::vector<int32_t>(1, 0));
+            r.StringValueValid.assign(valueStrings, std::vector<uint8_t>());
             return r;
         }
         std::vector<uint64_t*> keys(numeric + 1), values(aggs + 1);
@@ -119,10 +124,10 @@ public:
             values[a] = r.Values[a].data();
             valueNull[a] = r.ValueValid[a].data();
         }
-        std::vector<std::vector<uint8_t>> heaps(strings), nulls(strings);
-        std::vector<std::vector<uint64_t>> starts(strings);
-        std::vector<std::vector<uint32_t>> lengths(strings);
-        for (uint32_t s = 0; s < strings; ++s) {
+        std::vector<std::vector<uint8_t>> heaps(outputs), nulls(outputs);
+        std::vector<std::vector<uint64_t>> starts(outputs);
+        std::vector<std::vector<uint32_t>> lengths(outputs);
+        for (uint32_t s = 0; s < outputs; ++s) {
             heaps[s].resize(std::max<uint64_t>(sout[s].heap_bytes, 1));
             starts[s].resize(g);
             lengths[s].resize(g);
@@ -139,21 +144,25 @@ public:
         out.key_null = keyNull.data();
         out.values = values.data();
         out.value_null = valueNull.data();
-        if (ytgpu_groupby_table_result(ctx, Table_, &out, sout.data(), strings, YTGPU_MEM_HOST, &err) != YTGPU_OK) ThrowFrom(err);
+        if (ytgpu_groupby_table_result_strings(ctx, Table_, &out, sout.data(), strings, sout.data() + strings, valueStrings, YTGPU_MEM_HOST,
+                                               &err) != YTGPU_OK)
+            ThrowFrom(err);
         for (auto& v : r.KeyValid)
             for (uint8_t& b : v) b = !b;  // null bytemap -> validity
         for (auto& v : r.ValueValid)
             for (uint8_t& b : v) b = !b;
-        for (uint32_t s = 0; s < strings; ++s) {
+        for (uint32_t s = 0; s < outputs; ++s) {
+            const bool key = s < strings;
             if (sout[s].heap_bytes > (uint64_t)INT32_MAX)
-                throw TErrorException(YTGPU_ERR_UNSUPPORTED, "string key " + std::to_string(s) + ": more than 2^31 - 1 bytes of keys in 32-bit Arrow offsets");
-            r.StringKeyBytes.emplace_back(reinterpret_cast<const char*>(heaps[s].data()), sout[s].heap_bytes);
+                throw TErrorException(YTGPU_ERR_UNSUPPORTED, std::string(key ? "string key " : "string value ") + std::to_string(key ? s : s - strings) +
+                                                                 ": more than 2^31 - 1 bytes in 32-bit Arrow offsets");
+            (key ? r.StringKeyBytes : r.StringValueBytes).emplace_back(reinterpret_cast<const char*>(heaps[s].data()), sout[s].heap_bytes);
             std::vector<int32_t> offsets(g + 1, 0);
             for (uint64_t o = 0; o < g; ++o) offsets[o + 1] = offsets[o] + (int32_t)lengths[s][o];  // starts are in output order
-            r.StringKeyOffsets.push_back(std::move(offsets));
+            (key ? r.StringKeyOffsets : r.StringValueOffsets).push_back(std::move(offsets));
             std::vector<uint8_t> valid(g);
             for (uint64_t o = 0; o < g; ++o) valid[o] = !nulls[s][o];
-            r.StringKeyValid.push_back(std::move(valid));
+            (key ? r.StringKeyValid : r.StringValueValid).push_back(std::move(valid));
         }
         return r;
     }
@@ -172,10 +181,12 @@ private:
             if (IsString(a)) CheckOffsets(a, "block");
         }
         for (size_t v = 0; v < values.size(); ++v) {
-            if (!IsNumber(values[v].ValueType))
-                throw TErrorException(YTGPU_ERR_UNSUPPORTED, "value " + std::to_string(v) + ": INT64, UINT64 and DOUBLE values");
-            if (values[v].Length != keys[0].Length || values[v].Offset < 0)
+            const TArrowColumn& a = values[v];
+            if (!IsNumber(a.ValueType) && !(IsString(a) && a.Offsets))
+                throw TErrorException(YTGPU_ERR_UNSUPPORTED, "value " + std::to_string(v) + ": INT64, UINT64, DOUBLE and STRING values with 32-bit offsets");
+            if (a.Length != keys[0].Length || a.Offset < 0)
                 throw TErrorException(YTGPU_ERR_INVALID_ARGUMENT, "value column " + std::to_string(v) + " differs in length from the keys");
+            if (IsString(a)) CheckOffsets(a, "block");
         }
         if (!Table_) return;
         if (keys.size() != KeyTypes_.size() || values.size() != ValueTypes_.size())
@@ -198,19 +209,37 @@ private:
                 numericTypes.push_back(keys[k].ValueType);
             }
         }
-        for (const TArrowColumn& v : values) ValueTypes_.push_back(v.ValueType);
+        // the table's value columns are the numeric values in their order, then the string values in theirs
+        std::vector<uint8_t> numericValueTypes;
+        for (size_t v = 0; v < values.size(); ++v) {
+            ValueTypes_.push_back(values[v].ValueType);
+            if (IsString(values[v])) StringValues_.push_back(v);
+            else {
+                NumericValues_.push_back(v);
+                numericValueTypes.push_back(values[v].ValueType);
+            }
+        }
+        std::vector<int32_t> index(values.size());
+        for (size_t i = 0; i < NumericValues_.size(); ++i) index[NumericValues_[i]] = (int32_t)i;
+        for (size_t i = 0; i < StringValues_.size(); ++i) index[StringValues_[i]] = (int32_t)(NumericValues_.size() + i);
+        auto remap = [&](int32_t c) { return c >= 0 && (size_t)c < values.size() ? index[c] : c; };
         std::vector<ytgpu_aggregate> aggs;
-        for (const TAggregateItem& a : Aggregates_)
-            aggs.push_back(ytgpu_aggregate{(int32_t)a.Function, a.Column, a.ByColumn, 0});  // EAggregateFunction follows ytgpu_agg_op
+        StringValued_ = 0;
+        for (const TAggregateItem& a : Aggregates_) {
+            aggs.push_back(ytgpu_aggregate{(int32_t)a.Function, remap(a.Column), remap(a.ByColumn), 0});  // EAggregateFunction follows ytgpu_agg_op
+            if (a.Column >= 0 && (size_t)a.Column < values.size() && IsString(values[a.Column]) && aggs.back().op != YTGPU_AGG_COUNT) ++StringValued_;
+        }
         ytgpu_error err{};
         ytgpu_groupby_table* t = nullptr;
-        if (ytgpu_groupby_table_create(GetGpuContext(), numericTypes.data(), (uint32_t)numericTypes.size(), (uint32_t)StringKeys_.size(),
-                                       ValueTypes_.data(), (uint32_t)ValueTypes_.size(), aggs.data(), (uint32_t)aggs.size(), Hint_, &t,
-                                       &err) != YTGPU_OK) {
+        if (ytgpu_groupby_table_create_strings(GetGpuContext(), numericTypes.data(), (uint32_t)numericTypes.size(), (uint32_t)StringKeys_.size(),
+                                               numericValueTypes.data(), (uint32_t)numericValueTypes.size(), (uint32_t)StringValues_.size(),
+                                               aggs.data(), (uint32_t)aggs.size(), Hint_, &t, &err) != YTGPU_OK) {
             KeyTypes_.clear();
             StringKeys_.clear();
             NumericKeys_.clear();
             ValueTypes_.clear();
+            NumericValues_.clear();
+            StringValues_.clear();
             ThrowFrom(err);
         }
         Table_ = t;
@@ -237,13 +266,7 @@ private:
                 if (IsValid(a, from + i)) bits[at >> 3] |= (uint8_t)(1u << (at & 7));
             }
         };
-        for (size_t k = 0; k < keys.size(); ++k) {
-            const TArrowColumn& a = keys[k];
-            TStaged& s = Keys_[k];
-            if (!IsString(a)) {
-                numeric(a, s);
-                continue;
-            }
+        auto strings = [&](const TArrowColumn& a, TStaged& s) {
             s.Starts.Reserve(BlockCombineHashedKeysStageRows);
             s.Lengths.Reserve(BlockCombineHashedKeysStageRows);
             s.Nulls.Reserve(BlockCombineHashedKeysStageRows);
@@ -258,8 +281,13 @@ private:
                 s.Nulls.Data()[at] = IsValid(a, from + i) ? 0 : 1;
             }
             s.HeapBytes += bytes;
-        }
-        for (size_t v = 0; v < values.size(); ++v) numeric(values[v], Values_[v]);
+        };
+        auto stage = [&](const TArrowColumn& a, TStaged& s) {
+            if (IsString(a)) strings(a, s);
+            else numeric(a, s);
+        };
+        for (size_t k = 0; k < keys.size(); ++k) stage(keys[k], Keys_[k]);
+        for (size_t v = 0; v < values.size(); ++v) stage(values[v], Values_[v]);
         Staged_ += (uint64_t)count;
     }
 
@@ -279,11 +307,7 @@ private:
             v.mem = YTGPU_MEM_HOST;
             return v;
         };
-        std::vector<ytgpu_column_view> keys, values;
-        std::vector<ytgpu_string_column> strings;
-        for (size_t k : NumericKeys_) keys.push_back(view(Keys_[k], KeyTypes_[k]));
-        for (size_t k : StringKeys_) {
-            TStaged& s = Keys_[k];
+        auto stringView = [&](TStaged& s) {
             ytgpu_string_column c{};
             c.heap = s.Heap.Data();
             c.heap_bytes = s.HeapBytes;
@@ -292,14 +316,21 @@ private:
             c.null_bytemap = s.Nulls.Data();
             c.row_count = Staged_;
             c.mem = YTGPU_MEM_HOST;
-            strings.push_back(c);
-        }
-        for (size_t v = 0; v < Values_.size(); ++v) values.push_back(view(Values_[v], ValueTypes_[v]));
+            return c;
+        };
+        std::vector<ytgpu_column_view> keys, values;
+        std::vector<ytgpu_string_column> strings, stringValues;
+        for (size_t k : NumericKeys_) keys.push_back(view(Keys_[k], KeyTypes_[k]));
+        for (size_t k : StringKeys_) strings.push_back(stringView(Keys_[k]));
+        for (size_t v : NumericValues_) values.push_back(view(Values_[v], ValueTypes_[v]));
+        for (size_t v : StringValues_) stringValues.push_back(stringView(Values_[v]));
         ytgpu_error err{};
-        const int code = ytgpu_groupby_table_update(GetGpuContext(), Table_, keys.data(), (uint32_t)keys.size(), strings.data(),
-                                                    (uint32_t)strings.size(), values.data(), (uint32_t)values.size(), nullptr, -1, &err);
+        const int code = ytgpu_groupby_table_update_strings(GetGpuContext(), Table_, keys.data(), (uint32_t)keys.size(), strings.data(),
+                                                            (uint32_t)strings.size(), values.data(), (uint32_t)values.size(),
+                                                            stringValues.data(), (uint32_t)stringValues.size(), nullptr, -1, &err);
         Staged_ = 0;
         for (TStaged& s : Keys_) s.HeapBytes = 0;
+        for (TStaged& s : Values_) s.HeapBytes = 0;
         if (code != YTGPU_OK) ThrowFrom(err);
     }
 
@@ -307,7 +338,8 @@ private:
     const uint64_t Hint_;
     ytgpu_groupby_table* Table_ = nullptr;
     std::vector<uint8_t> KeyTypes_, ValueTypes_;
-    std::vector<size_t> NumericKeys_, StringKeys_;
+    std::vector<size_t> NumericKeys_, StringKeys_, NumericValues_, StringValues_;
+    uint32_t StringValued_ = 0;  // aggregates whose result is a string
     std::vector<TStaged> Keys_, Values_;
     uint64_t Staged_ = 0;
 };

@@ -495,16 +495,21 @@ std::unique_ptr<IBlockCombineHashed> CreateGpuBlockCombineHashed(uint64_t groupC
 //! BlockCombineHashed over a key TUPLE with a list of aggregates (mkql_block_agg.cpp:1234-1400), on one GPU GROUP BY table
 //! (ytgpu_groupby_table_*) that stays on the device for the whole input.
 //!   * Keys: INT64, UINT64, DOUBLE, and STRING as an Arrow binary / utf8 array with 32-bit Offsets; 1..8 columns.  The key
-//!     tuple is the numeric keys in their order, then the string keys in theirs.  Values: INT64, UINT64 or DOUBLE columns;
-//!     TAggregateItem::Column / ByColumn index them.  Types and counts come from the first block; a later block that
-//!     differs is INVALID_ARGUMENT, as are decreasing or negative offsets; any other type is UNSUPPORTED.  The checks run
-//!     before a block is staged, so a refused block changes nothing.
+//!     tuple is the numeric keys in their order, then the string keys in theirs.  Values: INT64, UINT64 or DOUBLE columns,
+//!     and STRING as an Arrow binary / utf8 array with 32-bit Offsets; TAggregateItem::Column / ByColumn index them.  A
+//!     STRING value takes MIN, MAX, FIRST, COUNT, and ARGMIN / ARGMAX as the value, the bound or both (that YQL's block
+//!     MIN / MAX take String / Utf8 arguments is recalled, not read).  Types and counts come from the first block; a later
+//!     block that differs is INVALID_ARGUMENT, as are decreasing or negative offsets; any other type, and a STRING column
+//!     without offsets, is UNSUPPORTED.  The checks run before a block is staged, so a refused block changes nothing.
 //!   * NULL keys form one group (SQL GROUP BY); doubles group by bit pattern; strings by their bytes.  Groups come out in
 //!     first-seen order, the aggregates with the semantics of ytgpu_scan_filter_groupby_multi (header).
 //!   * Blocks are copied into pinned host staging and folded into the table once BlockCombineHashedKeysStageRows rows are
 //!     staged, and at Finish: an update has fixed launch and synchronisation costs that small YQL blocks would pay each.
 //!   * Result: Keys / KeyValid per numeric key, StringKeyBytes / StringKeyOffsets (Arrow layout, groups + 1 offsets) /
 //!     StringKeyValid per string key, Values / ValueValid per aggregate (bit patterns of the result type; AVG a double).
+//!     A string-valued aggregate (MIN / MAX / FIRST of a STRING value, ARGMIN / ARGMAX whose Column is one) has its global
+//!     input row in Values and its bytes in StringValueBytes / StringValueOffsets / StringValueValid, one per such
+//!     aggregate in aggregate order.
 constexpr uint64_t BlockCombineHashedKeysStageRows = 1ull << 20;  // from bench_groupby_table.py's block-size legs (DESIGN.md 7)
 struct IBlockCombineHashedKeys {
     virtual ~IBlockCombineHashedKeys() = default;
@@ -517,6 +522,9 @@ struct IBlockCombineHashedKeys {
         std::vector<std::vector<uint8_t>> StringKeyValid;
         std::vector<std::vector<uint64_t>> Values;
         std::vector<std::vector<uint8_t>> ValueValid;
+        std::vector<std::string> StringValueBytes;
+        std::vector<std::vector<int32_t>> StringValueOffsets;
+        std::vector<std::vector<uint8_t>> StringValueValid;
     };
     virtual TResult Finish() = 0;
 };

@@ -603,7 +603,7 @@ int ytgpu_scan_filter_groupby_multi_strings(ytgpu_context* ctx, const ytgpu_colu
  * may be 0.  Keys compare as GROUP BY keys: (is-null, payload), doubles by bit pattern, NULL equals NULL; strings by length
  * and bytes, "" is not NULL.  The table owns its keys: the caller may free a block's buffers once _update returns.
  * Create.  value_types: the types of the value_count value columns every update passes; aggregates over them only (at most
- * 32; string-valued aggregates are UNSUPPORTED).  group_count_hint sizes the table (0 = unknown); it grows by doubling.
+ * 32; string-valued aggregates are UNSUPPORTED here and take ytgpu_groupby_table_create_strings below).  group_count_hint sizes the table (0 = unknown); it grows by doubling.
  * Update.  At most 2^30 rows, checked from the views before any access (UNSUPPORTED); all columns of one length; key and
  * value counts and types must be the table's (INVALID_ARGUMENT); predicate as for the one-shot call.  The table holds fewer
  * than 2^30 groups: an update whose new groups would reach 2^30 together with the table's is UNSUPPORTED.  A refused
@@ -647,6 +647,46 @@ int ytgpu_groupby_table_update(ytgpu_context* ctx, ytgpu_groupby_table* table, c
 int ytgpu_groupby_table_result(ytgpu_context* ctx, const ytgpu_groupby_table* table, ytgpu_groupby_multi_result* out,
                                ytgpu_groupby_string_keys* string_out, uint32_t string_key_count, int out_mem, ytgpu_error* err);
 int ytgpu_groupby_table_destroy(ytgpu_groupby_table* table, ytgpu_error* err);
+
+/* GROUP BY tables with string-valued aggregates: MIN / MAX / FIRST / COUNT of a string column and ARGMIN / ARGMAX whose
+ * `column`, `by_column` or both are strings, with the semantics of ytgpu_scan_filter_groupby_multi_strings (QL string
+ * order, the first row winning a tie).  The table keeps the bytes of every selected string, so the caller may free a
+ * block once _update returns.  The calls above are these with string_value_count = 0.
+ * Create.  An aggregate's `column` and `by_column` index value_types ++ string_value_count string value columns (index
+ * value_count + i is string value i).  SUM / AVG of a string is UNSUPPORTED; an index past both is INVALID_ARGUMENT.
+ * Update.  string_values: string_value_count flat string columns (HOST or DEVICE) of the block's length; a count that
+ * differs from the table's is INVALID_ARGUMENT.  Every non-NULL value of a string column the aggregates read is
+ * bounds-checked, the rows the predicate drops included: one outside its heap is INVALID_ARGUMENT, no byte outside the
+ * heap is read, and it is found before the table (its string key dictionaries included) changes.  The predicate column
+ * is a value column.
+ * Result.  values[a] of a string-valued aggregate (MIN, MAX or FIRST of a string, ARGMIN / ARGMAX whose `column` is a
+ * string) is the GLOBAL row number of the selected row, exactly the row index the one-shot call returns over the
+ * concatenated blocks (MIN / MAX: the smallest row holding the value); value_null as for scalars.  value_string_out[j],
+ * one per string-valued aggregate in aggregate order (string_aggregate_count of them, else INVALID_ARGUMENT), carries the
+ * values' bytes in the layout of string_out, under the same capacity protocol: every heap_bytes is written, and a short
+ * capacity is INVALID_ARGUMENT with nothing written.
+ * Memory.  Per group and string-valued aggregate, 12 B of start and length per kept string (one for MIN / MAX / FIRST,
+ * one or two for ARGMIN / ARGMAX: the value and a string bound) in the group-indexed arrays, and the strings' bytes in the
+ * aggregate's own heap.  A replaced string's bytes stay there until the heap's used bytes exceed 2 x its live bytes (and
+ * 1 MiB): it is then compacted in group-id order into a buffer of the live bytes.  After every update an aggregate's heap
+ * holds at most max(2 x live bytes, 1 MiB); during an update, that plus the update's replacements, in a buffer of up to
+ * twice its used bytes, plus the compacted copy.
+ * Synchronisations.  None more per update: the bytes the replacements append and free are read in the same copy as the
+ * count of new groups (string values alone add the bounds-check synchronisation of string keys).  Result: the value
+ * heaps' byte totals are read in the same copy as the key heaps'. */
+int ytgpu_groupby_table_create_strings(ytgpu_context* ctx, const uint8_t* key_types, uint32_t key_count, uint32_t string_key_count,
+                                       const uint8_t* value_types, uint32_t value_count, uint32_t string_value_count,
+                                       const ytgpu_aggregate* aggregates, uint32_t aggregate_count, uint64_t group_count_hint,
+                                       ytgpu_groupby_table** out, ytgpu_error* err);
+int ytgpu_groupby_table_update_strings(ytgpu_context* ctx, ytgpu_groupby_table* table, const ytgpu_column_view* key_columns,
+                                       uint32_t key_count, const ytgpu_string_column* string_keys, uint32_t string_key_count,
+                                       const ytgpu_column_view* value_columns, uint32_t value_count,
+                                       const ytgpu_string_column* string_values, uint32_t string_value_count,
+                                       const ytgpu_predicate* predicate, int32_t predicate_column, ytgpu_error* err);
+int ytgpu_groupby_table_result_strings(ytgpu_context* ctx, const ytgpu_groupby_table* table, ytgpu_groupby_multi_result* out,
+                                       ytgpu_groupby_string_keys* string_out, uint32_t string_key_count,
+                                       ytgpu_groupby_string_keys* value_string_out, uint32_t string_aggregate_count, int out_mem,
+                                       ytgpu_error* err);
 
 /* ---- hash JOIN: inner, left, left semi and left only equi-joins over key tuples ----
  * The join of YT QL's JoinOpHelper (library/query/engine/cg_routines/registry.cpp), which collects the primary rows' join

@@ -124,6 +124,7 @@ EXPORTED_SYMBOLS = [
     "ytgpu_join_table_build", "ytgpu_join_table_probe", "ytgpu_join_table_destroy",
     "ytgpu_join_table_build_strings", "ytgpu_join_table_probe_strings",
     "ytgpu_groupby_table_create", "ytgpu_groupby_table_update", "ytgpu_groupby_table_result", "ytgpu_groupby_table_destroy",
+    "ytgpu_groupby_table_create_strings", "ytgpu_groupby_table_update_strings", "ytgpu_groupby_table_result_strings",
 ]
 
 FLAGS_DICTIONARY_ZERO, FLAGS_BITMAP = 0, 1
@@ -406,6 +407,12 @@ def load() -> C.CDLL:
     lib.ytgpu_groupby_table_result.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(GroupByMultiResult), C.c_void_p, C.c_uint32, C.c_int,
                                                C.POINTER(Error)]
     lib.ytgpu_groupby_table_destroy.argtypes = [C.c_void_p, C.POINTER(Error)]
+    lib.ytgpu_groupby_table_create_strings.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32,
+                                                       C.c_void_p, C.c_uint32, C.c_uint64, C.POINTER(C.c_void_p), C.POINTER(Error)]
+    lib.ytgpu_groupby_table_update_strings.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p,
+                                                       C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_int32, C.POINTER(Error)]
+    lib.ytgpu_groupby_table_result_strings.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(GroupByMultiResult), C.c_void_p, C.c_uint32,
+                                                       C.c_void_p, C.c_uint32, C.c_int, C.POINTER(Error)]
     lib.ytgpu_gather_column.argtypes = [C.c_void_p, C.POINTER(ColumnView), C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
                                         C.POINTER(C.c_uint64), C.c_int, C.POINTER(Error)]
     lib.ytgpu_gather_string_column.argtypes = [C.c_void_p, C.POINTER(StringColumn), C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,

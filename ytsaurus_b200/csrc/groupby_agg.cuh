@@ -1,6 +1,7 @@
 // groupby_agg.cuh — the aggregate states and kernels of the GROUP BY over key tuples, shared by the one-shot call
-// (groupby_multi.cu) and the GROUP BY table (groupby_table.cu): the per-row accumulation into slot-indexed states, the
-// compaction of occupied slots and the finalisation of one aggregate's result column.  TU-local, as key_tuple.cuh.
+// (groupby_multi.cu) and the GROUP BY table (groupby_table.cu): the per-row accumulation into slot-indexed states (over
+// scalar and string columns), the compaction of occupied slots and the finalisation of one aggregate's result column.
+// TU-local, as key_tuple.cuh.
 #pragma once
 
 #include <algorithm>
@@ -8,6 +9,7 @@
 #include "columnar.cuh"
 #include "context.cuh"
 #include "key_tuple.cuh"
+#include "strings.cuh"
 
 namespace {
 
@@ -172,6 +174,111 @@ __global__ void __launch_bounds__(512) mg_accumulate_kernel(int op, int phase, c
             }
         }
     }
+}
+
+// ---- string-valued aggregates (MIN / MAX / FIRST / COUNT / ARGMIN / ARGMAX with a string column or by_column) ----
+// The selection key of MIN / MAX (the string column itself) or ARGMIN / ARGMAX (by_column, string or scalar).
+struct Selector {
+    ColumnDev by;
+    StringDev bs;
+    bool larger;  // MAX / ARGMAX
+    // (key(a), a) better than (key(b), b): a smaller (larger) key, the smaller row on equal keys.  b holds a selected row,
+    // whose value was checked when it was installed.
+    __device__ __forceinline__ bool better(u64 a, u64 b) const {
+        int c;
+        if (bs.present) {
+            c = string_compare(bs.heap, string_of(bs, a), string_of(bs, b));
+        } else {
+            bool nul;
+            const u64 ea = by_encode(by.value_type, decode_at(by, (i64)a, &nul));
+            const u64 eb = by_encode(by.value_type, decode_at(by, (i64)b, &nul));
+            c = ea < eb ? -1 : (ea > eb ? 1 : 0);
+        }
+        if (larger) c = -c;
+        return c < 0 || (c == 0 && a < b);
+    }
+};
+
+// Lock-free selection: install `cand` while it beats the holder.  A CAS fails only because another thread installed a
+// better row; the inputs are immutable, so comparing against the winner again is enough.
+__device__ __forceinline__ void select_row(unsigned long long* state, u64 cand, const Selector& sel) {
+    u64 cur = __ldcg(state);
+    while (cur == ~0ull || sel.better(cand, cur)) {
+        const u64 old = atomicCAS(state, (unsigned long long)cur, (unsigned long long)cand);
+        if (old == cur) return;
+        cur = old;
+    }
+}
+
+// Step 2 for an aggregate over a string column or by a string column.  State: S.row (selected row, ~0 = none) or, for
+// COUNT, S.nn.  Every non-NULL string of the arguments is bounds-checked, including rows the predicate dropped.
+__global__ void __launch_bounds__(256) mg_accumulate_strings_kernel(int op, const ColumnDev col, const StringDev cs, const ColumnDev by,
+                                                                    const StringDev bs, u64 n, const u32* __restrict__ slot_of_row,
+                                                                    AggState S, u32* err_word) {
+    const bool arg = op == YTGPU_AGG_ARGMIN || op == YTGPU_AGG_ARGMAX;
+    Selector sel;
+    sel.larger = op == YTGPU_AGG_MAX || op == YTGPU_AGG_ARGMAX;
+    if (arg) {
+        sel.by = by;
+        sel.bs = bs;
+    } else {  // MIN / MAX select by the column itself
+        sel.by = col;
+        sel.bs = cs;
+    }
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    const u64 trips = (n + stride - 1) / stride;  // the same for every thread: the warp collectives see whole warps
+    u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    u32 bad = 0;
+    for (u64 t = 0; t < trips; ++t, i += stride) {
+        const bool in = i < n;
+        const u32 slot = in ? slot_of_row[i] : kNoSlot;
+        bool have = false;
+        if (in) {
+            ytgpu_value v;
+            bool nul = true;
+            if (cs.present) have = string_at(cs, i, &v, &bad);
+            else {
+                decode_at(col, (i64)i, &nul);
+                have = !nul;
+            }
+            if (arg) {  // both arguments must be non-null (builtin_function_profiler.cpp:1304-1309)
+                bool bhave;
+                if (bs.present) bhave = string_at(bs, i, &v, &bad);
+                else {
+                    decode_at(by, (i64)i, &nul);
+                    bhave = !nul;
+                }
+                have = have && bhave;
+            }
+        }
+        have = have && slot != kNoSlot;
+        const u32 slot0 = __shfl_sync(0xffffffffu, slot, 0);
+        const bool uniform = __all_sync(0xffffffffu, slot == slot0) && slot0 != kNoSlot;  // sorted / clustered keys
+        if (op == YTGPU_AGG_COUNT) {
+            if (uniform) {
+                const u32 cnt = __popc(__ballot_sync(0xffffffffu, have));
+                if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(&S.nn[slot], (unsigned long long)cnt);
+            } else if (have) {
+                atomicAdd(&S.nn[slot], 1ull);
+            }
+            continue;
+        }
+        if (op == YTGPU_AGG_FIRST) {
+            if (have && i < __ldcg(&S.row[slot])) atomicMin(&S.row[slot], (unsigned long long)i);
+            continue;
+        }
+        u64 cand = have ? i : ~0ull;
+        if (uniform) {  // the warp's best row first: one CAS loop per warp instead of 32 on one address
+#pragma unroll
+            for (int d = 16; d > 0; d >>= 1) {
+                const u64 o = __shfl_xor_sync(0xffffffffu, cand, d);
+                if (o != ~0ull && (cand == ~0ull || sel.better(o, cand))) cand = o;
+            }
+            if ((threadIdx.x & 31) != 0) cand = ~0ull;
+        }
+        if (cand != ~0ull) select_row(&S.row[slot], cand, sel);
+    }
+    if (bad) atomicOr(err_word, (u32)DE_STRING_OUT_OF_HEAP);
 }
 
 // Step 3a: occupied slots -> (first row, slot) pairs, order arbitrary (one atomicAdd per warp).

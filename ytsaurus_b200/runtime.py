@@ -851,12 +851,14 @@ class GpuContext:
         this returns."""
         return JoinTable(self, foreign_keys, nulls, string_keys)
 
-    def groupby_table(self, key_types, string_key_count, value_types, aggregates, hint: int = 0) -> "GroupByTable":
-        """ytgpu_groupby_table_create: a GROUP BY table updated block by block (GroupByTable.update) whose result
+    def groupby_table(self, key_types, string_key_count, value_types, aggregates, hint: int = 0,
+                      string_value_count: int = 0) -> "GroupByTable":
+        """ytgpu_groupby_table_create_strings: a GROUP BY table updated block by block (GroupByTable.update) whose result
         (GroupByTable.result) is the one-shot scan_filter_groupby_multi over all the blocks' rows.  key_types: the numeric
         keys' EValueTypes, followed in the key tuple by string_key_count string keys; value_types: the value columns every
-        update passes; aggregates [(op, column[, by_column])] over them."""
-        return GroupByTable(self, key_types, string_key_count, value_types, aggregates, hint)
+        update passes, followed by string_value_count string value columns; aggregates [(op, column[, by_column])] over
+        them (column len(value_types) + i is string value i)."""
+        return GroupByTable(self, key_types, string_key_count, value_types, aggregates, hint, string_value_count)
 
     def gather_column(self, column: "Column", rows):
         """ytgpu_gather_column: `column` decoded at rows (uint32; capi.JOIN_NO_ROW gives NULL) -> dict(values, null_bitmap,
@@ -1155,9 +1157,12 @@ class JoinTable:
 class GroupByTable:
     """A GROUP BY table (ytgpu_groupby_table); see GpuContext.groupby_table.  close() or a with block destroys it."""
 
-    def __init__(self, ctx: GpuContext, key_types, string_key_count: int, value_types, aggregates, hint: int = 0):
+    def __init__(self, ctx: GpuContext, key_types, string_key_count: int, value_types, aggregates, hint: int = 0,
+                 string_value_count: int = 0):
         self.ctx, self.handle = ctx, None
         self.numeric, self.strings, self.aggregate_count = len(key_types), string_key_count, len(aggregates)
+        # string-valued aggregates: MIN / MAX / FIRST of a string, ARGMIN / ARGMAX whose column is a string
+        self.value_strings = sum(1 for a in aggregates if a[1] >= len(value_types) and a[0] != capi.AGG_COUNT)
         kt = (C.c_uint8 * max(len(key_types), 1))(*[int(t) for t in key_types])
         vt = (C.c_uint8 * max(len(value_types), 1))(*[int(t) for t in value_types])
         aggs = (capi.Aggregate * max(len(aggregates), 1))()
@@ -1166,17 +1171,18 @@ class GroupByTable:
             aggs[i].by_column = a[2] if len(a) > 2 else -1
         h = C.c_void_p()
         err = capi.Error()
-        capi.check(ctx.lib.ytgpu_groupby_table_create(ctx.handle, C.cast(kt, C.c_void_p), len(key_types), string_key_count,
-                                                      C.cast(vt, C.c_void_p), len(value_types), C.cast(aggs, C.c_void_p),
-                                                      len(aggregates), hint, C.byref(h), C.byref(err)), err)
+        capi.check(ctx.lib.ytgpu_groupby_table_create_strings(ctx.handle, C.cast(kt, C.c_void_p), len(key_types), string_key_count,
+                                                              C.cast(vt, C.c_void_p), len(value_types), string_value_count,
+                                                              C.cast(aggs, C.c_void_p), len(aggregates), hint, C.byref(h), C.byref(err)), err)
         self.handle = h
         if not hasattr(ctx, "_groupby_tables"):
             ctx._groupby_tables = weakref.WeakSet()
         ctx._groupby_tables.add(self)
 
-    def update(self, key_cols, value_cols, string_keys=(), predicate=None, predicate_column: int = -1):
-        """ytgpu_groupby_table_update with key_cols and value_cols (lists of Column) and string_keys as (heap, starts,
-        lengths, nulls or None) tuples; predicate (op, constant) over value_cols[predicate_column]."""
+    def update(self, key_cols, value_cols, string_keys=(), predicate=None, predicate_column: int = -1, string_values=()):
+        """ytgpu_groupby_table_update_strings with key_cols and value_cols (lists of Column) and string_keys and
+        string_values as (heap, starts, lengths, nulls or None) tuples; predicate (op, constant) over
+        value_cols[predicate_column]."""
         if self.handle is None:
             raise ValueError("the GROUP BY table is closed")
         kviews = [c.view() for c in key_cols]
@@ -1184,35 +1190,40 @@ class GroupByTable:
         karr = (capi.ColumnView * max(len(kviews), 1))(*kviews)
         varr = (capi.ColumnView * max(len(vviews), 1))(*vviews)
         sarr = _string_columns(string_keys) if string_keys else None
+        varr_s = _string_columns(string_values) if string_values else None
         pred = None
         if predicate is not None:
             op, const = predicate
             pred = capi.Predicate(op, 0, const & 0xFFFFFFFFFFFFFFFF)
         err = capi.Error()
-        capi.check(self.ctx.lib.ytgpu_groupby_table_update(
+        capi.check(self.ctx.lib.ytgpu_groupby_table_update_strings(
             self.ctx.handle, self.handle, C.cast(karr, C.c_void_p), len(kviews), C.cast(sarr, C.c_void_p) if sarr is not None else None,
-            len(string_keys), C.cast(varr, C.c_void_p), len(vviews), C.cast(C.pointer(pred), C.c_void_p) if pred is not None else None,
-            predicate_column, C.byref(err)), err)
+            len(string_keys), C.cast(varr, C.c_void_p), len(vviews), C.cast(varr_s, C.c_void_p) if varr_s is not None else None,
+            len(string_values), C.cast(C.pointer(pred), C.c_void_p) if pred is not None else None, predicate_column, C.byref(err)), err)
 
-    def _call_result(self, res, skeys, out_mem):
+    def _call_result(self, res, skeys, svals, out_mem):
         err = capi.Error()
         sarr = (capi.GroupByStringKeys * max(self.strings, 1))(*skeys)
-        code = self.ctx.lib.ytgpu_groupby_table_result(self.ctx.handle, self.handle, C.byref(res), C.cast(sarr, C.c_void_p), self.strings,
-                                                       out_mem, C.byref(err))
-        return code, err, [int(sarr[s].heap_bytes) for s in range(self.strings)]
+        varr = (capi.GroupByStringKeys * max(self.value_strings, 1))(*svals)
+        code = self.ctx.lib.ytgpu_groupby_table_result_strings(self.ctx.handle, self.handle, C.byref(res), C.cast(sarr, C.c_void_p),
+                                                               self.strings, C.cast(varr, C.c_void_p), self.value_strings, out_mem,
+                                                               C.byref(err))
+        return code, err, [int(sarr[s].heap_bytes) for s in range(self.strings)] + [int(varr[s].heap_bytes) for s in range(self.value_strings)]
 
     def result(self, count_only: bool = False, out_mem: int = capi.MEM_HOST, capacity: int | None = None, heap_capacity=None):
-        """ytgpu_groupby_table_result -> dict(keys=[...], key_null=[...], values=[...], value_null=[...], count, first_row,
-        string_keys=[(heap, starts, lengths, nulls)]) in first-seen order, in out_mem; with count_only, the group count.
-        Without capacities a count query sizes the outputs first; a capacity below the need raises YtGpuError with
-        .group_count and .heap_bytes set."""
+        """ytgpu_groupby_table_result_strings -> dict(keys=[...], key_null=[...], values=[...], value_null=[...], count,
+        first_row, string_keys=[(heap, starts, lengths, nulls)], string_values=[(heap, starts, lengths, nulls)]) in
+        first-seen order, in out_mem; with count_only, the group count.  string_values: one per string-valued aggregate,
+        in aggregate order.  heap_capacity: one per string key, then one per string value.  Without capacities a count
+        query sizes the outputs first; a capacity below the need raises YtGpuError with .group_count and .heap_bytes
+        (keys, then values) set."""
         if self.handle is None:
             raise ValueError("the GROUP BY table is closed")
-        zero = [capi.GroupByStringKeys() for _ in range(self.strings)]
+        zero = [capi.GroupByStringKeys() for _ in range(self.strings + self.value_strings)]
         empty = (C.c_void_p * 1)()
         if count_only or capacity is None or heap_capacity is None:
             res = capi.GroupByMultiResult(0, 0, empty, empty, empty, empty, None, None)
-            code, err, heap_bytes = self._call_result(res, zero, out_mem)
+            code, err, heap_bytes = self._call_result(res, zero[:self.strings], zero[self.strings:], out_mem)
             if code not in (capi.OK, capi.ERR_INVALID_ARGUMENT) or (code != capi.OK and res.group_count == 0):
                 capi.check(code, err)
             if count_only:
@@ -1236,7 +1247,7 @@ class GroupByTable:
         res = capi.GroupByMultiResult(0, capacity, pk, pkn, pv, pvn, _ptr_mem(counts)[0], _ptr_mem(first)[0])
         skeys = [capi.GroupByStringKeys(_ptr_mem(h)[0], hc, 0, _ptr_mem(st)[0], _ptr_mem(ln)[0], _ptr_mem(nl)[0])
                  for (h, st, ln, nl), hc in zip(sout, heap_capacity)]
-        code, err, heap_bytes = self._call_result(res, skeys, out_mem)
+        code, err, heap_bytes = self._call_result(res, skeys[:self.strings], skeys[self.strings:], out_mem)
         if code != capi.OK:
             e = capi.YtGpuError(code, err.message.decode(errors="replace"), err.cuda_error)
             e.group_count, e.heap_bytes = int(res.group_count), heap_bytes
@@ -1244,7 +1255,8 @@ class GroupByTable:
         g = int(res.group_count)
         strings = [(h[:hb], st[:g], ln[:g], nl[:g]) for (h, st, ln, nl), hb in zip(sout, heap_bytes)]
         return dict(keys=[k[:g] for k in keys], key_null=[k[:g] for k in kn], values=[v[:g] for v in vals],
-                    value_null=[v[:g] for v in vn], count=counts[:g], first_row=first[:g], string_keys=strings)
+                    value_null=[v[:g] for v in vn], count=counts[:g], first_row=first[:g], string_keys=strings[:self.strings],
+                    string_values=strings[self.strings:])
 
     def close(self):
         if self.handle is not None:
